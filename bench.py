@@ -4,8 +4,8 @@
 Headline workload (BASELINE.json configs[1]): 64 channels of 4FSK-2k RX (RRC + clock recovery + Viterbi), 1 Msps per
 channel, per GPU (weak scaling: every rank runs its own 64 channels; channels are independent, so there is no data-path
 collective).  One STEP = CALLS_PER_STEP streaming qrl_rx_work calls, each over a [64][2^22] gr_complex slab resident in
-HBM (2.1 GB per call, far beyond the 126 MB L2), i.e. 268 s of air time per channel per step -- long enough that the
-K timed steps the driver asks for cover more than a second of device time.
+HBM (2.1 GB per call, far beyond the 50 MB L2 of an H100), i.e. 268 s of air time per channel per step (about 94 ms of device
+time on an H100).
 
   python bench.py --gpus N --steps K --warmup W            our CUDA path: device-resident `value`, host-buffer `e2e`,
                                                            plus a `configs` block with the other BASELINE configurations
@@ -42,14 +42,14 @@ def headline_config(world):
     """Identical in both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "channels_per_gpu": CHANNELS, "samples_per_channel_per_call": T_CALL,
             "calls_per_step": CALLS_PER_STEP, "samples_per_channel_per_step": T_CALL * CALLS_PER_STEP,
-            "l2": "inputs 2.1 GB per call > 126 MB L2, no flush", "parallelism": "channel-sharded x%d, no data-path collective" % world}
+            "l2": "inputs 2.1 GB per call > 50 MB L2, no flush", "parallelism": "channel-sharded x%d, no data-path collective" % world}
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return json.load(open(p)).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def host_cores():
@@ -251,19 +251,41 @@ def timed_calls(fn, k, stream, torch, warm=2):
 
 
 
-def latency_bound_block(kernel, what, stage_ms_per_call, items_per_channel_per_call, clocks, chain_cycles, chain_source):
+def latency_bound_block(kernel, what, stage_ms_per_call, items_per_channel_per_call, clocks):
     """SURVEY 8d: the loop stages are latency bound -- what is reported for them is cycles of the loop-carried chain per item, live from the
-    stage's CUDA-event time and the SM clock sampled under load, beside the chain's own schedule (the same recurrence alone in a
-    kernel, tools/microbench/lone_warp.cu / ncu of the single launch: it runs at the sum of ptxas' stall counts)."""
+    stage's CUDA-event time and the SM clock sampled under load."""
     try:
-        mhz = (clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1965
-        cyc = stage_ms_per_call * 1e-3 * mhz * 1e6 / items_per_channel_per_call
+        mhz = (clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz")
+        cyc = stage_ms_per_call * 1e-3 * mhz * 1e6 / items_per_channel_per_call if mhz else None
         return {"kernel": kernel, "bound": "latency (loop-carried dependency chain, one warp per 32 channels)", "what": what,
                 "items_per_channel_per_call": items_per_channel_per_call, "stage_ms_per_call": stage_ms_per_call, "sm_mhz": mhz,
-                "cycles_per_item_in_step": cyc, "chain_cycles_alone": chain_cycles, "frac_of_chain_schedule": chain_cycles / cyc if cyc > 0 else None,
-                "chain_source": chain_source}
+                "cycles_per_item_in_step": cyc}
     except Exception as e:  # noqa: BLE001
         return {"kernel": kernel, "error": "%s: %s" % (type(e).__name__, e)}
+
+DUMP_BYTES_MAX = 64 << 20
+
+
+def dump_outputs(blk, out_dir):
+    """Writes what the last work() call left on every output port of `blk`, as a caller reads it (RxBlock.read_port), to
+    out_dir/port<p>.npy: float32, the channels' outputs back to back (complex samples as [n, 2], bits as 0.0 / 1.0), with
+    out_dir/port<p>_counts.npy (float64) the per-channel lengths.  When all channels together exceed DUMP_BYTES_MAX, a fixed seeded
+    sample of channels is written instead; out_dir/channels.npy (float64) lists the channels that were."""
+    ports = [blk.read_port(p) for p in range(blk.nports)]
+    per_ch = np.array([sum(len(ports[p][c]) * (8 if ports[p][c].dtype == np.complex64 else 4) for p in range(blk.nports))
+                       for c in range(blk.n_channels)])
+    chans = np.random.default_rng(0).permutation(blk.n_channels)
+    n = int(np.searchsorted(np.cumsum(per_ch[chans]), DUMP_BYTES_MAX, side="right"))
+    chans = np.sort(chans[:n])
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "channels.npy"), chans.astype(np.float64))
+    for p, port in enumerate(ports):
+        parts = [port[c] for c in chans]
+        cat = np.concatenate(parts) if parts else np.zeros(0, port[0].dtype)
+        arr = np.ascontiguousarray(cat).view(np.float32).reshape(-1, 2) if cat.dtype == np.complex64 else cat.astype(np.float32)
+        np.save(os.path.join(out_dir, "port%d.npy" % p), arr)
+        np.save(os.path.join(out_dir, "port%d_counts.npy" % p), np.array([len(x) for x in parts], np.float64))
+
 
 def rx_stage_ms(L, blk, names=("stage1_fir", "chan_filter", "demod_or_loop", "symbol_sync_or_audio", "viterbi", "soft_epilogue")):
     out = {}
@@ -335,6 +357,9 @@ def rx_config_block(q, torch, dev, name, make, make_args, okind, oargs, X, alg_b
     C, T = X.shape
     peak, _ = peaks()
     stream = torch.cuda.current_stream()
+    # the library allocates with cudaMalloc: give it back what torch's caching allocator keeps from building the inputs
+    # (4096-channel QPSK: ~37 GB of handle next to 26 GB of cached intermediates does not fit an 80 GB card)
+    torch.cuda.empty_cache()
     blk = make(*make_args, n_channels=C, max_samples=T, device=dev.index)
     blk.set_stream(stream.cuda_stream)
     blk.work_device(X.data_ptr(), T, T)
@@ -400,6 +425,7 @@ def tx_config_block(q, torch, dev, cores, cpu_seconds):
     C, n = 64, 1024
     rng = np.random.default_rng(5000)
     stream = torch.cuda.current_stream()
+    torch.cuda.empty_cache()
     tx = q.make_gr_mod_4fsk(25, 1000000, 1700, 3500, True, n_channels=C, max_items=n)
     tx.set_stream(stream.cuda_stream)
     data_h = rng.integers(0, 256, (C, n), dtype=np.uint8)
@@ -828,6 +854,8 @@ def run_ours(args):
     sampler.join()
     ms = e0.elapsed_time(e1)
     launches = blk.launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(blk, args.dump_outputs)
     stage = rx_stage_ms(L, blk)
     L.qrl_rx_profile(blk._h, 0)
     t_ms = torch.tensor([ms], device=dev, dtype=torch.float64)
@@ -1029,12 +1057,6 @@ def run_ours(args):
     launches_per_call = max(1, fir_n // n_calls)
     alg_bytes = ALG_BYTES_PER_SAMPLE * C * T / launches_per_call
     achieved = alg_bytes / fir_avg_s / 1e9 if fir_avg_s > 0 else 0.0
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "fir_traffic_bytes.json")
-    if os.path.exists(tp):      # ncu --set full capture (profiles/): DRAM bytes per input sample x samples per launch
-        tj = json.load(open(tp))
-        traffic = tj.get("per_sample") * C * T / launches_per_call
-        traffic_src = tj.get("source")
 
     cpu_line = None
     if world == 1 and not args.no_cpu:
@@ -1061,7 +1083,7 @@ def run_ours(args):
                 "numa": numa, "sc16_ingest": e2e_sc16},
         "gpu_launches": int(launches),
         "roofline": {"kernel": "fir_decim_poly_kernel<50,9,8,128,8>", "bound": "hbm", "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                     "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": alg_bytes, "avg_launch_ms": fir_avg_s * 1e3,
                      "launches_per_call": launches_per_call,
                      "whole_chain_frac": ALG_BYTES_PER_SAMPLE * C * T * n_calls / (ms_max * 1e-3) / 1e9 / peak},
@@ -1071,15 +1093,13 @@ def run_ours(args):
     }
     line["latency_bound"] = latency_bound_block(
         "symsync_kernel<1,SL_RECT4,EPI_EXT_4FSK_FM,512,2,1,LOOP_SYMSYNC,2>", "symbol_sync_ff recurrence (MMSE interpolation -> TED -> loop filter), the stage that IS the step",
-        line["stage_ms_per_call"].get("symbol_sync_or_audio", 0.0), T / 500.0, line["clocks"], 203.0,
-        "ncu --set full of one launch over the whole call, profiles/r02_final2_ncu_full_summary.csv: 891.7 us for 8613 symbols")
+        line["stage_ms_per_call"].get("symbol_sync_or_audio", 0.0), T / 500.0, line["clocks"])
     try:
         c3 = configs.get("cfg3_qpsk250k_256ch")
         if isinstance(c3, dict) and "stage_ms_per_call" in c3:
             c3["latency_bound"] = latency_bound_block(
                 "agc_costas_kernel<128,2,4,1>", "agc2_cc -> costas_loop_cc(order 4, snr) per sample at 500 ksps, the stage that bounds the QPSK chain",
-                c3["stage_ms_per_call"].get("demod_or_loop", 0.0), c3["samples_per_channel_per_call"] / 2.0, line["clocks"], 202.6,
-                "the Costas recurrence alone in a kernel, tools/microbench/lone_warp.cu, profiles/r02_t_symsync_prefetch_costas_select.txt")
+                c3["stage_ms_per_call"].get("demod_or_loop", 0.0), c3["samples_per_channel_per_call"] / 2.0, line["clocks"])
     except Exception:  # noqa: BLE001
         pass
     if cpu_line:
@@ -1099,6 +1119,7 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline legs (profiling runs)")
     ap.add_argument("--no-parity", action="store_true", help="skip the full-size parity spot checks")
     ap.add_argument("--headline-only", action="store_true", help="config 2 only (no `configs` block)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the port outputs of the last timed call to DIR/*.npy (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

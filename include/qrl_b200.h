@@ -1,5 +1,5 @@
 /*
- * qrl_b200.h -- C ABI of libqrl_b200.so: batched-channel, B200-native replacements for the per-mode
+ * qrl_b200.h -- C ABI of libqrl_b200.so: batched-channel, H100-native replacements for the per-mode
  * GNU Radio hier-blocks that QRadioLink's gr_demod_base / gr_mod_base connect between the SDR
  * source/sink and the gr_*_sink / gr_*_source boundary blocks.
  *

@@ -136,7 +136,7 @@ private:
     std::mutex _mutex;
 };
 
-// ---- batched demodulator: n_channels instances of one reference hier block on one B200
+// ---- batched demodulator: n_channels instances of one reference hier block on one GPU
 class gr_demod_b200 {
 public:
     gr_demod_b200(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,

@@ -1,6 +1,6 @@
-"""qradiolink_b200 -- B200-native batched-channel replacement for QRadioLink's per-mode GNU Radio
+"""qradiolink_b200 -- H100-native batched-channel replacement for QRadioLink's per-mode GNU Radio
 demod/mod hier-blocks (src/gr/gr_demod_*.cpp, gr_mod_*.cpp).  The arithmetic runs in hand-written
-sm_100a CUDA kernels behind the C ABI in include/qrl_b200.h (libqrl_b200.so); this package is the
+sm_90a CUDA kernels behind the C ABI in include/qrl_b200.h (libqrl_b200.so); this package is the
 Python host side: a ctypes binding plus mirrors of the reference's factory functions and sink blocks.
 
 There is no CPU fallback: importing works anywhere (so the CPU test tier can check the ABI), but

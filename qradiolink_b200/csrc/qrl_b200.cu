@@ -363,9 +363,8 @@ bool make_sm_partition(qrl_rx* h, unsigned loop_sms, int prio, bool fec_on_par_d
     CUstream a = nullptr, b = nullptr, c = nullptr, d = nullptr;
     if (pStream(&a, h->g_loop, CU_STREAM_NON_BLOCKING, prio) != CUDA_SUCCESS) return false;
     // FEC (Viterbi) stream.  Up to 64 channels the step is the latency of the lone recurrence warps and the decoder runs on the wide
-    // partition, off their SMs (64 ch x 2^22: 0.925 ms per call against 0.941 next to the loop kernels); with more channels the step is
-    // the sum of the parallel stages and the decoder stays in the loop partition, out of their way (256 ch: 2.23 ms against 2.35).
-    // profiles/r02_y_256ch_stage_times.txt; QRL_FEC_ON_PAR=0/1 forces either.
+    // partition, off their SMs; with more channels the step is the sum of the parallel stages and the decoder stays in the loop
+    // partition, out of their way.  QRL_FEC_ON_PAR=0/1 forces either.
     bool fec_on_par = fec_on_par_default;
     if (const char* e = getenv("QRL_FEC_ON_PAR")) fec_on_par = e[0] == '1';
     if (pStream(&b, fec_on_par ? h->g_par : h->g_loop, CU_STREAM_NON_BLOCKING, prio) != CUDA_SUCCESS) return false;
@@ -482,7 +481,7 @@ int qrl_device_count(void)
     if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
     return n;
 }
-const char* qrl_version(void) { return "qrl_b200 0.1 (sm_100a)"; }
+const char* qrl_version(void) { return "qrl_b200 0.1 (sm_90a)"; }
 const char* qrl_last_error(const void* handle)
 {
     if (handle) return static_cast<const HandleBase*>(handle)->err.c_str();
@@ -856,8 +855,10 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         }
         // (an FP64 instruction occupies an SM's FP64 pipe for ~64 cycles whatever its lane count, so two recurrences only overlap on
         // DIFFERENT SMs: both kernels then ask for more than half an SM's shared memory, which keeps their CTAs one per SM and apart, and
-        // the split is used while 2 C CTAs fit the machine)
-        if (kind == QRL_DEMOD_NBFM && 2 * h->C <= 140 && !getenv("QRL_NBFM_NO_SPLIT")) {
+        // the split is used while each kernel's C CTAs fit the SMs at once -- on an H100 it is faster up to 128 channels, slower at 160)
+        int n_sm = 0;
+        if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess) { set_err(h, "SM count query failed"); return fail(QRL_ECUDA); }
+        if (kind == QRL_DEMOD_NBFM && h->C <= n_sm && !getenv("QRL_NBFM_NO_SPLIT")) {
             if ((rc = make_ring(h, &h->raud, sizeof(float), h->n1max * 2 / 5 + 64))) return fail(rc);
             if ((rc = dev_alloc(h, &h->d_nb2, h->C))) return fail(rc);
             h->zero_list.emplace_back(h->d_nb2, sizeof(NbfmDeemphState) * h->C);
@@ -952,9 +953,8 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         // per SM) on all SMs, next to the parallel stages, on priority streams.
         h->many = big_ctas > 44 || (analog_kind && h->C > 64);
         if (const char* e = getenv("QRL_MANY_CHANNELS")) h->many = e[0] == '1';
-        // QPSK (per-sample loops, 2 loop CTAs per 32 channels + a heavy Viterbi load): measured faster WITHOUT a private partition
-        // (256 channels: 62.3 ms per 2^20-sample call on priority streams, 66.8 ms with a 24-SM partition -- the decoder gets the whole
-        // machine (38.9 -> 12.9 ms) and the loop CTAs spread over more SMs); QRL_QPSK_PARTITION=1 brings the partition back.
+        // QPSK (per-sample loops, 2 loop CTAs per 32 channels + a heavy Viterbi load): runs WITHOUT a private partition, so that the
+        // decoder gets the whole machine and the loop CTAs spread over more SMs; QRL_QPSK_PARTITION=1 brings the partition back.
         bool want_partition = kind != QRL_DEMOD_QPSK;
         if (const char* e = getenv("QRL_QPSK_PARTITION")) { if (kind == QRL_DEMOD_QPSK) want_partition = e[0] == '1'; }
         if (h->many || !want_partition || !make_sm_partition(h, loop_sms, hi, !analog_kind && groups <= 2)) {
@@ -1334,8 +1334,8 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     CK(cudaStreamWaitEvent(h->s_fec, h->ev_start, 0));
     if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
     cudaStream_t sp = h->par();
-    // overlapped calls keep the pipeline full across calls: two big slices are enough and cost least (a symbol-sync launch has
-    // ~20 us of start-up: measured 0.941 ms per 64 x 2^22 call with 2 slices, 0.963 with 3, 0.988 with 4, 1.45 with 1)
+    // overlapped calls keep the pipeline full across calls: two big slices are enough and cost least (every symbol-sync launch pays
+    // its own start-up)
     int nsub = (h->overlap && !h->nsub_forced) ? 2 : h->nsub;
     if (T < 32768L * nsub) nsub = static_cast<int>(std::max<long>(1, T / 32768));
     const long long k_call0 = h->n1;
@@ -2920,8 +2920,11 @@ int qrl_fir_decim_ccf_device(const float* taps, int ntaps, int D, const float* x
     HandleBase* h = nullptr;
     CK(cudaMalloc(&d_taps, sizeof(float) * ntaps));
     cudaError_t e = cudaMemcpyAsync(d_taps, taps, sizeof(float) * ntaps, cudaMemcpyHostToDevice, st);
+    int dev = 0, n_sm = 0;
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     if (e == cudaSuccess) {
-        dim3 g(static_cast<unsigned>(std::min<long long>((nout + 7) / 8, 148LL * 16)), static_cast<unsigned>(C));
+        dim3 g(static_cast<unsigned>(std::min<long long>((nout + 7) / 8, n_sm * 16LL)), static_cast<unsigned>(C));
         fir_decim_generic_kernel<<<g, 256, 0, st>>>(d_taps, ntaps, D, reinterpret_cast<const float2*>(x_dev), T, x_stride,
                                                     reinterpret_cast<float2*>(y_dev), y_stride, nout);
         e = cudaGetLastError();

@@ -1,4 +1,4 @@
-// qrl_design.hpp -- host-side filter / table / loop-gain design for the B200 path.
+// qrl_design.hpp -- host-side filter / table / loop-gain design for the GPU path.
 //
 // These are the construction-time computations the reference performs through GNU Radio's
 // gr::filter::firdes, gr::fft::window, gr::calculate_deemph_taps and the control-loop constructors

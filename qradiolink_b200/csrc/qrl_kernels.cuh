@@ -1,4 +1,4 @@
-// qrl_kernels.cuh -- sm_100a device code for the batched-channel IQ DSP hot path.
+// qrl_kernels.cuh -- sm_90a device code for the batched-channel IQ DSP hot path.
 //
 // Numerics contract (see DESIGN.md "Numerics"): compiled with -fmad=false; every fused multiply-add is
 // an explicit fmaf(); FIR dot products follow ONE fixed order (polyphase branch r = j mod D accumulated
@@ -199,7 +199,7 @@ fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long l
 
     float* outc = reinterpret_cast<float*>(out_ring + static_cast<long long>(c) * ring_stride);
     for (int b = warp; b < NOUT / K; b += NWARPS) {
-        float2 acc[K];                                // (re, im) pairs: one FFMA2 per tap and output
+        float2 acc[K];                                // (re, im) pairs: one ffma2() (two FFMA) per tap and output
 #pragma unroll
         for (int i = 0; i < K; i++) acc[i] = make_float2(0.0f, 0.0f);
 #pragma unroll
@@ -299,7 +299,7 @@ fir_decim2_kernel(const float2* __restrict__ iq, long long iq_stride, long long 
     }
     __syncthreads();
     // thread t: outputs kbase + K t + i ; newest sample of output i at window index (NTP-1) + D (K t + i)
-    float2 s0[K], s1[K];                                 // branch chains j even / j odd, (re, im) pairs: FFMA2
+    float2 s0[K], s1[K];                                 // branch chains j even / j odd, (re, im) pairs: ffma2()
 #pragma unroll
     for (int i = 0; i < K; i++) { s0[i] = make_float2(0.0f, 0.0f); s1[i] = make_float2(0.0f, 0.0f); }
     const int t = threadIdx.x;
@@ -405,7 +405,7 @@ __global__ void fir_ccf_ring_kernel(const float2* __restrict__ in, unsigned in_m
 // Register-tiled form of fir_ccf_ring_kernel (round 2): one CTA = NT * K consecutive outputs of one channel.  The tile's samples
 // (+ ntaps - 1 of history) and the taps sit in shared memory; thread t owns K consecutive outputs and walks the samples oldest
 // first, so every sample is loaded once (one LDS.64) and meets K taps that slide through a register window (one broadcast LDS.32
-// per step): 2 LDS per K FFMA2 instead of 2 loads per FFMA2.  Per output the accumulation order is the ring kernel's (tap index
+// per step): 2 LDS per K ffma2() instead of 2 loads per ffma2().  Per output the accumulation order is the ring kernel's (tap index
 // descending = oldest sample first): results are bit-identical.  Sample index i lives at i + i / 16 (one pad slot per 16): the K-strided
 // LDS.64 of a half-warp then hit distinct bank pairs.
 template <int K, int NT>
@@ -1284,8 +1284,7 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
     const bool active = c < C;
     // tap-major copy of the MMSE bank: mm[k * 132 + imu] (a lane's 8 taps are 8 scalar loads in the order the
     // oldest-first FMA chain consumes them; random imu across lanes spreads over all 32 banks)
-    // (all of a thread's table entries are loaded before the first store: one L2 latency per launch instead of one per entry -- the
-    // fill used to be 6 us of every launch, profiles/r02_w_symsync_launch_phases.txt)
+    // (all of a thread's table entries are loaded before the first store: one L2 latency per launch instead of one per entry)
     constexpr int NT = 64 + 32 * NEPI, TPT = (129 * 8 + NT - 1) / NT;
     float tv[TPT];
 #pragma unroll
@@ -3063,9 +3062,8 @@ interp_fir_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long
 // at once.  Each input sample is loaded once (a broadcast LDS: the lanes of a group read the same address) and feeds
 // R accumulators, so consecutive FFMAs share an operand (register reuse) instead of streaming 2 new operands each:
 // 2 NT FFMA per output as before, about twice the FP32 issue rate.  Same accumulation order (oldest sample first).
-// (round 2 experiment, profiles/README.md: several tiles per CTA with a double-buffered window measured 8 % SLOWER on B200 -- 131.6 vs
-// 121.9 us per launch, the window fill competes with the FFMA stream for the LSU -- and keeping the taps resident across tiles costs
-// an occupancy step (64 registers); the one-tile form below stays)
+// (several tiles per CTA with a double-buffered window were tried and were slower -- the window fill competes with the FFMA stream
+// for the LSU -- and keeping the taps resident across tiles costs an occupancy step (64 registers); the one-tile form below stays)
 template <int L, int NT, int R, int G>
 __global__ void __launch_bounds__(L * G)
 interp_fir_ccf_rt_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride, long long m0, long long m1,
@@ -3087,7 +3085,7 @@ interp_fir_ccf_rt_kernel(const float2* __restrict__ in_ring, unsigned in_mask, l
     float h[NT];
 #pragma unroll
     for (int k = 0; k < NT; k++) h[k] = arms[p * NT + k];
-    float2 acc[R];                                              // (re, im) pairs: one FFMA2 per tap and output
+    float2 acc[R];                                              // (re, im) pairs: one ffma2() (two FFMA) per tap and output
 #pragma unroll
     for (int r = 0; r < R; r++) acc[r] = make_float2(0.0f, 0.0f);
     const float2* s = xs + q * R;                               // s[j] = x[tile0 + qR - (NT-1) + j]

@@ -14,7 +14,7 @@
 // (float)cos / (float)sin of the double angle.  Results are bit-identical to the oracle.
 //
 // Bound: 16 bytes of HBM traffic per wideband sample (8 read + 8 written) against 2*tpf + 4*M FFMA per sample
-// (110 for the reference's M = 10, 341-tap prototype): FP32-issue bound on B200, HBM roofline reported beside it.
+// (110 for the reference's M = 10, 341-tap prototype): FP32-issue bound, HBM roofline reported beside it.
 // There is NO CPU fallback.
 #include "../../include/qrl_b200.h"
 #include "qrl_tma.cuh"
@@ -86,14 +86,14 @@ pfb_chan_kernel(const float* __restrict__ bt /*[M][TPF]*/, const float* __restri
     {
         // thread -> (branch k, output group q).  The LDS.64 below touch float2 index R M q + (M - 1 - k) + const: a half-warp (16 consecutive
         // tids) is conflict-free when those are distinct mod 16.  With q = tid / M the group stride R M = 90 = 10 (mod 16) collides with
-        // the k run of the neighbouring group (2-way conflicts on every load, ncu r02_b: 4 wavefronts instead of 2); visiting the groups
+        // the k run of the neighbouring group (2-way conflicts on every load: 4 wavefronts instead of 2); visiting the groups
         // in the order 7 q' makes the stride 630 = 6 = -10 (mod 16), i.e. the index is 9 - tid (mod 16): distinct for any 16 consecutive tids.
         const int k = tid % M, qlin = tid / M;
         const int q = (M == 10 && R == 9 && G == 32) ? ((7 * qlin) & 31) : qlin;
         float h[TPF];
 #pragma unroll
         for (int t = 0; t < TPF; t++) h[t] = bt[k * TPF + t];
-        float2 acc[R];                                              // (re, im) pairs: one FFMA2 per tap and output
+        float2 acc[R];                                              // (re, im) pairs: one ffma2() (two FFMA) per tap and output
 #pragma unroll
         for (int r = 0; r < R; r++) acc[r] = make_float2(0.0f, 0.0f);
         const float2* s = win + woff + (q * R) * M + (M - 1 - k);  // s[j*M] = stream sample at time (q*R - (TPF-1) + j)
@@ -124,7 +124,7 @@ pfb_chan_kernel(const float* __restrict__ bt /*[M][TPF]*/, const float* __restri
 #pragma unroll
                 for (int k = 0; k < M; k++) {
                     const float2 u = ub[k * TMP + m];
-                    // re += u.x wr; re += -u.y wi; im += u.x wi; im += u.y wr  ==  o += u.x (wr, wi); o += u.y (-wi, wr)   (two FFMA2;
+                    // re += u.x wr; re += -u.y wi; im += u.x wi; im += u.y wr  ==  o += u.x (wr, wi); o += u.y (-wi, wr)   (two ffma2();
                     // fma(-a, b, c) and fma(a, -b, c) are the same operation)
                     ffma2_sp(o, u.x, wr[k], wi[k]);
                     ffma2_sp(o, u.y, -wi[k], wr[k]);
@@ -232,7 +232,7 @@ pfb_synth_kernel(const float* __restrict__ bt, const float* __restrict__ w,
         float h[TPF];
 #pragma unroll
         for (int t = 0; t < TPF; t++) h[t] = bt[br * TPF + t];
-        float2 acc[R];                                              // (re, im) pairs: one FFMA2 per tap and output
+        float2 acc[R];                                              // (re, im) pairs: one ffma2() (two FFMA) per tap and output
 #pragma unroll
         for (int r = 0; r < R; r++) acc[r] = make_float2(0.0f, 0.0f);
         const float2* s = vb + br * VP + q * R;                     // s[j] = v_br[n0 + qR - (TPF-1) + j]

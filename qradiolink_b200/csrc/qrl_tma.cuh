@@ -1,4 +1,4 @@
-// qrl_tma.cuh -- TMA 1-D bulk copy (cp.async.bulk -> UBLKCP), mbarrier and shared-memory address helpers (sm_100a).
+// qrl_tma.cuh -- TMA 1-D bulk copy (cp.async.bulk -> UBLKCP), mbarrier and shared-memory address helpers (sm_90a).
 // Header-only, shared by the translation units of libqrl_b200.so.
 #pragma once
 #include <cuda_runtime.h>
@@ -26,17 +26,12 @@ template <int OFF> __device__ __forceinline__ float2 lds_f32x2(uint32_t a)
     float2 v; asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+%3];" : "=f"(v.x), "=f"(v.y) : "r"(a), "n"(OFF)); return v;
 }
 __device__ __forceinline__ void sts_f32x2(uint32_t a, float x, float y) { asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(x), "f"(y) : "memory"); }
-// Packed FP32 pair FMA (sm_100: FFMA2, one issue slot for two IEEE fma): acc.x = fma(s, v.x, acc.x), acc.y = fma(s, v.y, acc.y).
-// Each half is a correctly rounded single fma, so results are bit-identical to two fmaf() calls; a complex sample times a
-// real tap is exactly this shape (the scalar operand is broadcast by the instruction: FFMA2 Rd, Rs.F32, Rv.F32x2, Rd.F32x2).
+// FP32 pair FMA: acc.x = fma(s, v.x, acc.x), acc.y = fma(s, v.y, acc.y), a complex sample times a real tap.  sm_90 has no
+// packed FP32 FMA, so this is two correctly rounded single FFMAs (the numerics contract asks for exactly these roundings).
 __device__ __forceinline__ void ffma2(float2& acc, float s, float2 v)
 {
-    unsigned long long a, b, c;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(a) : "f"(s));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(v.x), "f"(v.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(c) : "f"(acc.x), "f"(acc.y));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(c) : "l"(a), "l"(b));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(acc.x), "=f"(acc.y) : "l"(c));
+    acc.x = fmaf(s, v.x, acc.x);
+    acc.y = fmaf(s, v.y, acc.y);
 }
 // acc.x = fma(s, p.x, acc.x), acc.y = fma(s, p.y, acc.y) with a per-half multiplier pair p (DFT butterflies: s * (wr, wi))
 __device__ __forceinline__ void ffma2_sp(float2& acc, float s, float px, float py)

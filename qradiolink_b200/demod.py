@@ -18,7 +18,7 @@ from .lib import KIND, PARAM, QrlError, check, load_library
 
 
 class RxBlock:
-    """n_channels instances of one reference demod hier-block, batched on one B200."""
+    """n_channels instances of one reference demod hier-block, batched on one GPU."""
 
     def __init__(self, kind, sps, samp_rate, carrier_freq, filter_width, flag=0, n_channels=1,
                  max_samples=1 << 20, device=0):

@@ -1,9 +1,7 @@
 """GPU tier: DMR receive chain (gr_demod_dmr.cpp: x3/125 rational resampler to 24 ksps, quadrature demod, 0.2 roll-off symbol
 filter tapped as float port 3, symbol sync with the PLAIN Mueller & Mueller detector, x0.9, phase modulator, hard bits) against the
 CPU oracle: all four ports, ragged chunks.
-
-STATUS: first run on a B200 at the start of round 2 (tools/gpu_checklist.sh: compute-sanitizer memcheck 0 errors, all tests green,
-profiles/r02_a_checklist_summary.txt); part of the normal GPU tier since."""
+"""
 import numpy as np
 import pytest
 

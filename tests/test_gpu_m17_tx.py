@@ -1,8 +1,6 @@
 """GPU tier: M17 modulator (gr_mod_m17.cpp: bytes -> dibits -> map -> RRC x5 -> x0.66666666 -> frequency modulator -> 24 ksps low-pass
 -> x0.9 -> x125 / 3 rational interpolator) against the CPU oracle, state carried across calls, then CUDA TX -> CUDA M17 RX.
-
-STATUS: first run on a B200 at the start of round 2 (tools/gpu_checklist.sh: compute-sanitizer memcheck 0 errors, all tests green,
-profiles/r02_a_checklist_summary.txt); part of the normal GPU tier since."""
+"""
 import numpy as np
 import pytest
 

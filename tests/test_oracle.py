@@ -1,5 +1,5 @@
 """CPU tier: pin the ORACLE itself (the known-answer tests the reference never had, SURVEY.md section 4 / 8c)."""
-import ctypes as C
+import json
 import os
 
 import numpy as np
@@ -75,19 +75,21 @@ def test_sincos_and_atan(oracle):
 
 
 def test_deemph_taps_against_compiled_reference(oracle):
-    """oracle/_ref = /root/reference/src/gr/emphasis.cpp compiled as-is (the only stand-alone piece)."""
-    so = os.path.join(ROOT, "oracle", "_ref", "libqrl_ref_emphasis.so")
-    if not os.path.exists(so):
-        pytest.skip("oracle/_ref not built (reference tree absent)")
-    R = C.CDLL(so)
+    """oracle/_ref = the reference's src/gr/emphasis.cpp compiled as-is (the only stand-alone piece); where it was not built (the
+    reference tree is absent), the taps it gave, committed in tests/golden/golden_v1.json."""
+    from tests.golden import cases
+    R = cases.load_ref_emphasis()
+    G = json.load(open(os.path.join(ROOT, "tests", "golden", "golden_v1.json")))["emphasis"]
     for fs, tau in ((20000, 50e-6), (8000, 50e-6), (48000, 75e-6)):
-        a = np.zeros(2); b = np.zeros(2)
-        R.ref_deemph_taps(C.c_int(fs), C.c_double(tau), a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p))
+        if R is not None:
+            wd, wp = cases.ref_deemph(R, fs, tau), cases.ref_preemph(R, fs, tau)
+        else:
+            wd = [float.fromhex(x) for x in G["deemph_%d_%g" % (fs, tau)]]
+            wp = [float.fromhex(x) for x in G["preemph_%d_%g" % (fs, tau)]]
         oa, ob = oracle.deemph_taps(fs, tau)
-        assert np.array_equal(a, oa) and np.array_equal(b, ob)
-        R.ref_preemph_taps(C.c_int(fs), C.c_double(tau), C.c_double(-1.0), a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p))
+        assert list(oa) + list(ob) == wd
         oa, ob = oracle.preemph_taps(fs, tau)
-        assert np.array_equal(a, oa) and np.array_equal(b, ob)
+        assert list(oa) + list(ob) == wp
 
 
 def test_fir_orders_and_scipy(oracle):

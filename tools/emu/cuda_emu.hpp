@@ -31,7 +31,7 @@ struct uint4 { unsigned x, y, z, w; };
 static inline uint2 make_uint2(unsigned x, unsigned y) { return uint2{ x, y }; }
 static inline float2 make_float2(float x, float y) { return float2{ x, y }; }
 namespace qrl {
-// qrl_tma.cuh's fma.rn.f32x2 (FFMA2) helpers = two independent correctly rounded fma
+// qrl_tma.cuh's ffma2 helpers = two independent correctly rounded fma
 inline void ffma2(float2& acc, float s, float2 v) { acc.x = std::fmaf(s, v.x, acc.x); acc.y = std::fmaf(s, v.y, acc.y); }
 inline void ffma2_sp(float2& acc, float s, float px, float py) { acc.x = std::fmaf(s, px, acc.x); acc.y = std::fmaf(s, py, acc.y); }
 }

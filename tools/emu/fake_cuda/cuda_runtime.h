@@ -19,12 +19,15 @@ typedef emuStream* cudaStream_t;
 typedef emuEvent* cudaEvent_t;
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaFuncAttributeMaxDynamicSharedMemorySize = 8, cudaEnableDefault = 0 };
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
 enum cudaDriverEntryPointQueryResult { cudaDriverEntryPointSuccess = 0, cudaDriverEntryPointSymbolNotFound = 1 };
 
 static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulated CUDA error"; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
+static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
+static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = 132; return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetStreamPriorityRange(int* lo, int* hi) { *lo = 0; *hi = -1; return cudaSuccess; }
 static inline cudaError_t cudaMalloc(void** p, size_t n)
 {

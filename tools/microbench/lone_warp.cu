@@ -1,8 +1,7 @@
-// lone_warp.cu -- what does a LONE warp pay per dependent instruction on sm_100a?
+// lone_warp.cu -- what does a LONE warp pay per dependent instruction on sm_90a (H100)?
 // (measurement tool behind DESIGN.md's latency floors: the symbol-sync and Costas recurrences run one warp per 32 channels,
-// so their time is (items per channel) x (cycles of the loop-carried chain); ptxas schedules a dependent FFMA 4 cycles behind
-// its producer, the kernels measure ~6.4)
-//   build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -fmad=false -I../../qradiolink_b200/csrc
+// so their time is (items per channel) x (cycles of the loop-carried chain))
+//   build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false -I../../qradiolink_b200/csrc
 //          -o lone_warp lone_warp.cu
 //   run  : ./lone_warp            (prints cycles per operation / per Costas item for a few occupancy shapes)
 #include <cstdio>

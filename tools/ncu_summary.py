@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Summarise `ncu --set full` reports into a small CSV for profiles/:  python tools/ncu_summary.py out.csv rep1.ncu-rep rep2.ncu-rep ...
-One row per (report, metric) for the metrics the roofline discussion uses; the .ncu-rep files themselves stay in gpurun_out/ (scratch)."""
+"""Summarise `ncu --set full` reports into a small CSV:  python tools/ncu_summary.py out.csv rep1.ncu-rep rep2.ncu-rep ...
+One row per (report, metric) for the metrics the roofline discussion uses."""
 import csv
 import subprocess
 import sys
