@@ -50,6 +50,10 @@ enum qrl_kind {
                                  look-back beyond its declared history is DEFINED as the stream's own older items (zeros at the start) */
     QRL_DEMOD_WBFM = 9,       /* gr_demod_wbfm.cpp:28-70 (SURVEY 8f row 3); ports: IQ at 200 ksps, float audio at 8 ksps */
     QRL_DEMOD_GMSK = 8,       /* gr_demod_gmsk.cpp:30-134 (SURVEY 8f row 3); sps 10 / 5 / 1 = GMSK1K / 2K / 10K; 4 ports like 2FSK */
+    QRL_DEMOD_FREEDV = 13,    /* gr_demod_freedv.cpp:31-81 up to the input of freedv_rx_ss (codec2 runs on the host): created with
+                                 qrl_rx_create_freedv.  Ports: 0 = IQ at 8 ksps (sps x the input level: the stage-1 low-pass has a DC gain of
+                                 sps, the reference's taps); 1 = INT16 modem samples at 8 ksps (item size 2), the float_to_short(1, 32768)
+                                 output that freedv_rx_ss consumes -- unlike the reference's port 1, which is float speech behind the vocoder */
     QRL_MOD_4FSK = 101, QRL_MOD_QPSK = 102, QRL_MOD_NBFM = 103, QRL_MOD_BPSK = 104, QRL_MOD_2FSK = 105,
     QRL_MOD_SSB = 106,
     QRL_MOD_GMSK = 107,       /* gr_mod_gmsk.cpp:30-100 (sps 50 / 100 / 10 = GMSK2K / 1K / 10K) */
@@ -57,6 +61,8 @@ enum qrl_kind {
     QRL_MOD_DSSS = 110,       /* gr_mod_dsss.cpp:27-93 (make_gr_mod_dsss(25, 1e6, 1700, 200), gr_mod_base.cpp:170): one input byte = 208 chips = 10^6 output items, so
                                  max_items is small (the output buffer holds max_items x 8 MB per channel) */
     QRL_MOD_AM = 111,         /* gr_mod_am.cpp:25-72 (make_gr_mod_am(125, 1e6, 1700, 5000), gr_mod_base.cpp:167): float audio at 8 ksps in, like NBFM / SSB */
+    QRL_MOD_FREEDV = 112,     /* gr_mod_freedv.cpp:27-85 behind freedv_tx_ss: created with qrl_tx_create_freedv; items: int16 modem samples at
+                                 8 ksps (what freedv_tx_ss produces), sps gr_complex outputs per item in every call */
     QRL_MOD_DMR = 109         /* gr_mod_dmr.cpp:27-93 (the M17 modulator's structure with the DMR pulse, deviation 0.85 and
                                  gr_zero_idle_bursts in place of the IF low-pass; see qrl_tx_zero_samples) */
 };
@@ -96,6 +102,13 @@ const char* qrl_last_error(const void* handle);
  * n_channels independent channels; max_samples = largest T a single qrl_rx_work call will carry. */
 int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
                   int n_channels, long max_samples, int device, qrl_rx** out);
+/* gr_demod_freedv (make_gr_demod_freedv(sps, samp_rate, carrier_freq, filter_width, low_cutoff, mode, sb), gr_demod_freedv.cpp:31-81;
+ * instances gr_demod_base.cpp:229-249) as a QRL_DEMOD_FREEDV handle.  The codec2 `mode` only matters to the vocoder behind port 1 and is not
+ * taken here.  QRL_EINVAL unless samp_rate / sps == 8000 and 0 <= low_cutoff < filter_width <= 4000.  Setters: QRL_PARAM_AGC_ATTACK /
+ * _DECAY (the agc2_ff rates, :85-93), QRL_PARAM_CARRIER_OFFSET_HZ; QRL_PARAM_SQUELCH_DB is codec2's setting (:95-98) and, like
+ * FILTER_WIDTH and OVERLAP_CALLS, returns QRL_EINVAL. */
+int qrl_rx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
+                         int n_channels, long max_samples, int device, qrl_rx** out);
 int qrl_rx_destroy(qrl_rx* h);
 /* run all kernels of this handle on an existing CUDA stream (cudaStream_t); NULL = the handle's own stream */
 int qrl_rx_set_stream(qrl_rx* h, void* cuda_stream);
@@ -144,10 +157,16 @@ int qrl_rx_profile_read(qrl_rx* h, int stage, double* ms_total, long* n_launches
 /* ---- TX ---- */
 int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
                   int n_channels, long max_items, int device, qrl_tx** out);
+/* gr_mod_freedv (make_gr_mod_freedv(sps, samp_rate, carrier_freq, filter_width, low_cutoff, mode, sb), gr_mod_freedv.cpp:27-85; instances
+ * gr_mod_base.cpp:181-203) as a QRL_MOD_FREEDV handle: qrl_tx_work takes [n_channels][n] int16 modem samples at 8 ksps and produces
+ * n x sps gr_complex per channel.  Arguments checked as for qrl_rx_create_freedv; QRL_PARAM_BB_GAIN is the one setter. */
+int qrl_tx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
+                         int n_channels, long max_items, int device, qrl_tx** out);
 int qrl_tx_destroy(qrl_tx* h);
 int qrl_tx_set_stream(qrl_tx* h, void* cuda_stream);
 int qrl_tx_set_param(qrl_tx* h, int channel, int key, double value);
-/* in: [n_channels][n] bytes (digital) ; produces [n_channels][n_out] gr_complex at 1 Msps */
+/* in: [n_channels][n] bytes (digital), float audio (NBFM / SSB / AM) or int16 modem samples (FreeDV); produces [n_channels][n_out]
+ * gr_complex at 1 Msps */
 int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device);
 int qrl_tx_sync(qrl_tx* h);
 int qrl_tx_read(qrl_tx* h, float* dst, long cap, long* n_out, int dst_on_device);
@@ -163,7 +182,8 @@ long qrl_tx_launch_count(const qrl_tx* h);
  * the first 62 items of a scheduler window (its lookup is bounded by the current window); here results do not depend on chunking. */
 int qrl_tx_zero_samples(qrl_tx* h, int channel, long long byte_offset, long n_samples);
 /* per-stage device timing of the modulator (like qrl_rx_profile): stage 0 = bit chain (scrambler / encoder / mapper),
- * 1 = pulse shaping + frequency modulator, 2 = final interpolating FIR (the HBM-write-bound kernel) */
+ * 1 = pulse shaping + frequency modulator, 2 = final interpolating FIR (the HBM-write-bound kernel); FreeDV: 0 = int16 conversion +
+ * side-band filter, 1 = feedforward AGC, 2 = x sps interpolator */
 int qrl_tx_profile(qrl_tx* h, int enable);
 int qrl_tx_profile_read(qrl_tx* h, int stage, double* ms_total, long* n_launches);
 

@@ -5,6 +5,8 @@
 //   make_gr_demod_qpsk(sps, samp_rate, carrier_freq, filter_width)          src/gr/gr_demod_qpsk.h:48-50
 //   make_gr_demod_nbfm(sps, samp_rate, carrier_freq, filter_width)          src/gr/gr_demod_nbfm.h:38-39
 //   make_gr_demod_{bpsk,2fsk,ssb,am,gmsk}(...)                              src/gr/gr_demod_<mode>.h
+//   make_gr_demod_freedv / make_gr_mod_freedv(sps, samp_rate, carrier_freq, filter_width, low_cutoff, mode, sb)
+//                                                                             up to the codec2 modem boundary (int16 at 8 ksps)
 //   make_gr_mod_4fsk / make_gr_mod_qpsk                                     src/gr/gr_mod_4fsk.h:46-48
 //   gr_bit_sink / gr_audio_sink / gr_const_sink  get_data() semantics       src/gr/gr_bit_sink.cpp:45-84 ...
 //
@@ -139,11 +141,14 @@ private:
 // ---- batched demodulator: n_channels instances of one reference hier block on one GPU
 class gr_demod_b200 {
 public:
+    // low_cutoff: QRL_DEMOD_FREEDV only (qrl_rx_create_freedv)
     gr_demod_b200(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
-                  int n_channels, long max_samples, int device)
+                  int n_channels, long max_samples, int device, int low_cutoff = 0)
         : _C(n_channels)
     {
-        const int rc = qrl_rx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, n_channels, max_samples, device, &_h);
+        const int rc = kind == QRL_DEMOD_FREEDV
+            ? qrl_rx_create_freedv(sps, samp_rate, carrier_freq, filter_width, low_cutoff, flag, n_channels, max_samples, device, &_h)
+            : qrl_rx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, n_channels, max_samples, device, &_h);
         if (rc != QRL_OK) throw std::runtime_error(std::string("qrl_rx_create: ") + qrl_last_error(nullptr));
         _nports = qrl_rx_num_ports(_h);
         for (int p = 0; p < _nports; p++) {
@@ -191,6 +196,7 @@ public:
     }
     const char* last_error() const { return qrl_last_error(_h); }
     qrl_rx* handle() { return _h; }
+    int mode = 0;       // make_gr_demod_freedv: the codec2 mode, for the adapter that runs freedv_rx behind port 1
 
 private:
     qrl_rx* _h = nullptr;
@@ -241,6 +247,15 @@ inline gr_demod_b200_sptr make_gr_demod_m17(int sps = 125, int samp_rate = 10000
 inline gr_demod_b200_sptr make_gr_demod_dsss(int sps = 25, int samp_rate = 1000000, int carrier_freq = 1700, int filter_width = 150,
                                              int n_channels = 1, long max_samples = 1 << 20, int device = 0)     // instance gr_demod_base.cpp:218
 { return std::make_shared<gr_demod_b200>(QRL_DEMOD_DSSS, sps, samp_rate, carrier_freq, filter_width, 0, n_channels, max_samples, device); }
+// src/gr/gr_demod_freedv.h:40-41 up to the input of freedv_rx_ss: port 0 = IQ at 8 ksps, port 1 = int16 modem samples (short)
+inline gr_demod_b200_sptr make_gr_demod_freedv(int sps = 125, int samp_rate = 8000, int carrier_freq = 1700, int filter_width = 2000,
+                                               int low_cutoff = 200, int mode = 0, int sb = 0,
+                                               int n_channels = 1, long max_samples = 1 << 20, int device = 0)
+{
+    auto b = std::make_shared<gr_demod_b200>(QRL_DEMOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb, n_channels, max_samples, device, low_cutoff);
+    b->mode = mode;
+    return b;
+}
 inline gr_demod_b200_sptr make_gr_demod_dmr(int sps = 5, int samp_rate = 1000000,
                                             int n_channels = 1, long max_samples = 1 << 20, int device = 0)      // src/gr/gr_demod_dmr.h:42
 { return std::make_shared<gr_demod_b200>(QRL_DEMOD_DMR, sps, samp_rate, 0, 5000, 0, n_channels, max_samples, device); }
@@ -248,10 +263,15 @@ inline gr_demod_b200_sptr make_gr_demod_dmr(int sps = 5, int samp_rate = 1000000
 // ---- batched modulator
 class gr_mod_b200 {
 public:
-    gr_mod_b200(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int n_channels, long max_items, int device)
+    // low_cutoff: QRL_MOD_FREEDV only (qrl_tx_create_freedv)
+    gr_mod_b200(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int n_channels, long max_items, int device,
+                int low_cutoff = 0)
         : _C(n_channels)
     {
-        if (qrl_tx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, n_channels, max_items, device, &_h) != QRL_OK)
+        const int rc = kind == QRL_MOD_FREEDV
+            ? qrl_tx_create_freedv(sps, samp_rate, carrier_freq, filter_width, low_cutoff, flag, n_channels, max_items, device, &_h)
+            : qrl_tx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, n_channels, max_items, device, &_h);
+        if (rc != QRL_OK)
             throw std::runtime_error(std::string("qrl_tx_create: ") + qrl_last_error(nullptr));
     }
     ~gr_mod_b200() { qrl_tx_destroy(_h); }
@@ -262,15 +282,17 @@ public:
     // gr_mod_dmr: the "zero_samples" tag gr_dmr_source attaches to a byte of the stream (gr_dmr_source.cpp:148)
     int zero_samples(int channel, long long byte_offset, long n_samples) { return qrl_tx_zero_samples(_h, channel, byte_offset, n_samples); }
     // what gr_byte_source::set_data hands over: [channels][n] frame bytes -> [channels][n_out] gr_complex at 1 Msps
-    int work(const unsigned char* bytes, long n, long stride, std::vector<gr_complex>& out, long* n_out)
+    // (gr_mod_freedv: [channels][n] int16 modem samples, what freedv_tx_ss produces)
+    int work(const void* items, long n, long stride, std::vector<gr_complex>& out, long* n_out)
     {
-        if (qrl_tx_work(_h, bytes, n, stride, 0) != QRL_OK) return WORK_DONE;
+        if (qrl_tx_work(_h, items, n, stride, 0) != QRL_OK) return WORK_DONE;
         float* d; long st, no;
         qrl_tx_out_device(_h, &d, &st, &no);
         out.resize(static_cast<size_t>(no) * _C);
         if (qrl_tx_read(_h, reinterpret_cast<float*>(out.data()), no, n_out, 0) != QRL_OK) return WORK_DONE;
         return static_cast<int>(*n_out);
     }
+    int mode = 0;       // make_gr_mod_freedv: the codec2 mode, for the adapter that runs freedv_tx in front of the block
 private:
     qrl_tx* _h = nullptr;
     int _C;
@@ -300,6 +322,15 @@ inline gr_mod_b200_sptr make_gr_mod_am(int sps = 125, int samp_rate = 1000000, i
 inline gr_mod_b200_sptr make_gr_mod_dsss(int sps = 25, int samp_rate = 1000000, int carrier_freq = 1700, int filter_width = 200,
                                          int n_channels = 1, long max_items = 8, int device = 0)                  // instance gr_mod_base.cpp:170
 { return std::make_shared<gr_mod_b200>(QRL_MOD_DSSS, sps, samp_rate, carrier_freq, filter_width, 0, n_channels, max_items, device); }
+// src/gr/gr_mod_freedv.h:39-40 behind freedv_tx_ss: work() takes int16 modem samples at 8 ksps, sps outputs per sample
+inline gr_mod_b200_sptr make_gr_mod_freedv(int sps = 125, int samp_rate = 8000, int carrier_freq = 1700, int filter_width = 2000,
+                                           int low_cutoff = 200, int mode = 0, int sb = 0,
+                                           int n_channels = 1, long max_items = 4096, int device = 0)
+{
+    auto b = std::make_shared<gr_mod_b200>(QRL_MOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb, n_channels, max_items, device, low_cutoff);
+    b->mode = mode;
+    return b;
+}
 inline gr_mod_b200_sptr make_gr_mod_dmr(int sps = 125, int samp_rate = 1000000, int carrier_freq = 1700, int filter_width = 5000,
                                         int n_channels = 1, long max_items = 4096, int device = 0)               // src/gr/gr_mod_dmr.h:37-38
 { return std::make_shared<gr_mod_b200>(QRL_MOD_DMR, sps, samp_rate, carrier_freq, filter_width, 0, n_channels, max_items, device); }

@@ -161,6 +161,9 @@ struct qrl_rx : HandleBase {
     float* d_bank_taps = nullptr; int nt_bank = 0;
     float* d_symf_taps = nullptr; int nt_symf = 0;
     Ring rbank;                    // bank output (complex for 4FSK, float for 2FSK), channel-major
+    // FreeDV: agc2_ff + audio band-pass + int16 conversion behind the side-band filter (AGC output ring: rstr)
+    FreedvRxParams fdp{};
+    FreedvRxState* d_fdv = nullptr;
     // SSB audio chain
     SsbParams ssbp{};
     SsbState* d_ssb = nullptr;
@@ -488,8 +491,37 @@ const char* qrl_last_error(const void* handle)
     return g_err.c_str();
 }
 
+// gr_demod_freedv / gr_mod_freedv factory arguments the reference does not check itself: the chain only holds together at 8 ksps
+static int check_freedv_args(const char* who, int sps, int samp_rate, int filter_width, int low_cutoff)
+{
+    if (sps <= 0 || samp_rate / sps != 8000) { set_err(nullptr, std::string(who) + ": samp_rate / sps must be 8000 (the codec2 modem rate)"); return QRL_EINVAL; }
+    if (low_cutoff < 0 || low_cutoff >= filter_width || filter_width > 4000) {
+        set_err(nullptr, std::string(who) + ": need 0 <= low_cutoff < filter_width <= 4000 (the side band of an 8 ksps stream)");
+        return QRL_EINVAL;
+    }
+    return QRL_OK;
+}
+
+static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+                     int n_channels, long max_samples, int device, qrl_rx** out);
+
 int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
                   int n_channels, long max_samples, int device, qrl_rx** out)
+{
+    if (kind == QRL_DEMOD_FREEDV) { set_err(nullptr, "qrl_rx_create: QRL_DEMOD_FREEDV takes a low cutoff: use qrl_rx_create_freedv"); return QRL_EINVAL; }
+    return rx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, 0, n_channels, max_samples, device, out);
+}
+
+int qrl_rx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
+                         int n_channels, long max_samples, int device, qrl_rx** out)
+{
+    int rc = check_freedv_args("qrl_rx_create_freedv", sps, samp_rate, filter_width, low_cutoff);
+    if (rc) return rc;
+    return rx_create(QRL_DEMOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_samples, device, out);
+}
+
+static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+                     int n_channels, long max_samples, int device, qrl_rx** out)
 {
     if (!out || n_channels <= 0 || max_samples <= 0) { set_err(nullptr, "qrl_rx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
@@ -710,6 +742,14 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         taps2 = flag ? complex_band_pass_2(1, tsr, -filter_width, -200, 200, 90, WIN_BLACKMAN_HARRIS)
                      : complex_band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
         h->nports = 2;
+    } else if (kind == QRL_DEMOD_FREEDV) {
+        // gr_demod_freedv.cpp:40-54; flag = sb (0 USB, 1 LSB); sps = decimation to 8 ksps.  The stage-1 taps are low_pass(sps, ...): DC gain sps
+        tsr = 8000; sym_sps = 2;
+        taps1 = low_pass(sps, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
+        h->D1 = sps;
+        taps2 = flag ? complex_band_pass_2(1, tsr, -filter_width, -low_cutoff, 200, 90, WIN_BLACKMAN_HARRIS)
+                     : complex_band_pass_2(1, tsr, low_cutoff, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
+        h->nports = 2;
     } else if (kind == QRL_DEMOD_WBFM) {
         // gr_demod_wbfm.cpp:35-54
         tsr = 200000; sym_sps = 2;
@@ -763,7 +803,7 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
     if ((rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C))) return fail(rc);
     h->n1max = h->Tmax * h->L1 / h->D1 + 2;
     // ---- rings
-    h->ntaps2 = static_cast<int>(taps2.size()) / ((kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM) ? 2 : 1);
+    h->ntaps2 = static_cast<int>(taps2.size()) / ((kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM || kind == QRL_DEMOD_FREEDV) ? 2 : 1);
     h->ntaps3 = static_cast<int>(taps3.size());
     {
         std::vector<float> t2(std::max<size_t>(taps2.size(), 512), 0.0f);     // room for set_filter_width redesigns
@@ -784,6 +824,16 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         if ((rc = make_ring(h, &h->rclip, sizeof(float2), h->n1max + 16))) return fail(rc);
         if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->ssbp.nt_audio + 16))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_ssb, h->C))) return fail(rc);
+    } else if (kind == QRL_DEMOD_FREEDV) {
+        // gr_demod_freedv.cpp:57-77: agc2_ff(1e-1, 1e-3, 0.5, 1) (max gain 65536) -> band_pass_2(1, 8000, 200, 3500, 200, 90, BH) -> x0.1 ->
+        // float_to_short(1, 32768); the feedforward_agc_cc of :56 is never connected
+        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
+        std::vector<float> audio_f = band_pass_2(1, tsr, 200, 3500, 200, 90, WIN_BLACKMAN_HARRIS);
+        if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return fail(rc);
+        h->fdp.attack = 1e-1f; h->fdp.decay = 1e-3f; h->fdp.ref = 0.5f; h->fdp.max_gain = 65536.0f;
+        h->fdp.nt_audio = static_cast<int>(audio_f.size());
+        if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->fdp.nt_audio + 16))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_fdv, h->C))) return fail(rc);
     } else if (kind == QRL_DEMOD_WBFM) {
         // gr_demod_wbfm.cpp:39-64: the analog audio kernel in mode 2
         if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
@@ -944,7 +994,8 @@ int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         const int groups = (h->C + 31) / 32;
         // analog blocks: one CTA per channel whose thread 0 runs the double-precision recurrences (squelch power, de-emphasis): they want
         // an SM (its FP64 pipe) each, up to half the machine
-        const bool analog_kind = kind == QRL_DEMOD_NBFM || kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM || kind == QRL_DEMOD_WBFM;
+        const bool analog_kind = kind == QRL_DEMOD_NBFM || kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM || kind == QRL_DEMOD_WBFM ||
+                                 kind == QRL_DEMOD_FREEDV;
         const int big_ctas = (kind == QRL_DEMOD_QPSK) ? 2 * groups : (analog_kind ? (h->nbfm_split ? 2 * h->C : std::min(h->C, 44)) : groups);
         unsigned loop_sms = static_cast<unsigned>(std::min(48, 8 * ((big_ctas + 4 + 7) / 8)));
         if (const char* e = getenv("QRL_LOOP_SMS")) { int v = atoi(e); if (v >= 8 && v <= 64) loop_sms = static_cast<unsigned>(v); }
@@ -1034,6 +1085,11 @@ int qrl_rx_reset(qrl_rx* h)
     if (h->d_ssb) {
         for (int c = 0; c < h->C; c++) { std::memset(&sb[c], 0, sizeof(SsbState)); sb[c].sq_state = SQ_MUTED; sb[c].gain = 1.0f; }
         CK(cudaMemcpyAsync(h->d_ssb, sb.data(), sizeof(SsbState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    }
+    std::vector<FreedvRxState> fdv(h->C);
+    if (h->d_fdv) {
+        for (auto& f : fdv) { f.n_in = 0; f.gain = 1.0f; f.pad_ = 0; }           // agc2_ff::make(..., gain = 1)
+        CK(cudaMemcpyAsync(h->d_fdv, fdv.data(), sizeof(FreedvRxState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
     std::vector<NbfmState> nb(h->C);
     if (h->d_nb) {
@@ -1178,6 +1234,15 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
         return QRL_OK;
     }
     if (key == QRL_PARAM_GAIN && ssb) { h->if_gain = static_cast<float>(value); return QRL_OK; }      // gr_demod_ssb::set_gain (:118-121): _if_gain->set_k
+    if (h->kind == QRL_DEMOD_FREEDV) {
+        // gr_demod_freedv::set_agc_attack / set_agc_decay (:85-93): the agc2_ff rates, from the next sample on
+        if (key == QRL_PARAM_AGC_ATTACK) { h->fdp.attack = static_cast<float>(value); return QRL_OK; }
+        if (key == QRL_PARAM_AGC_DECAY) { h->fdp.decay = static_cast<float>(value); return QRL_OK; }
+        if (key == QRL_PARAM_SQUELCH_DB) {
+            set_err(h, "qrl_rx_set_param: gr_demod_freedv::set_squelch is codec2's (freedv_rx_ss::set_squelch_thresh), behind port 1");
+            return QRL_EINVAL;
+        }
+    }
     if (key == QRL_PARAM_CTCSS && nbfm) {
         // gr_demod_nbfm::set_ctcss (:97-121).  0: tone squelch out of the graph, low-pass audio filter (only when it was in: the first
         // disconnect of :101 throws otherwise and the rest is skipped).  f: ctcss_squelch_ff::set_frequency(f) (new Goertzel filters at
@@ -1436,6 +1501,27 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
                 static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
                 h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
+            h->launches++;
+            h->prof_end(pe);
+            continue;
+        }
+        if (h->kind == QRL_DEMOD_FREEDV) {
+            if (n_new > 0) {
+                pe = h->prof_begin(1, sp);
+                fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
+                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
+                    static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                    h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
+                h->launches++;
+                h->prof_end(pe);
+            }
+            CK(cudaEventRecord(h->ev_a[i], sp));
+            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof_begin(3, h->s_loop);
+            freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
+                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
+                static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
+                reinterpret_cast<short*>(h->d_port1), 4 * h->port1_cap, h->d_port1_cnt, static_cast<int>(4 * h->port1_cap));
             h->launches++;
             h->prof_end(pe);
             continue;
@@ -1907,6 +1993,7 @@ int qrl_rx_port_itemsize(const qrl_rx* h, int port)
 {
     if (!h || port < 0 || port >= h->nports) return QRL_EINVAL;
     if (port == 0) return 8;
+    if (port == 1 && h->kind == QRL_DEMOD_FREEDV) return 2;        // int16 modem samples
     if (port == 1) return (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_SSB || h->kind == QRL_DEMOD_AM || h->kind == QRL_DEMOD_WBFM) ? 4 : 8;
     if (port == 3 && h->dmr) return 4;
     return 1;
@@ -1919,6 +2006,7 @@ int qrl_rx_port_device(qrl_rx* h, int port, void** data, long* cap, int** counts
     else if (port == 1) {
         *data = h->d_port1; *counts = h->d_port1_cnt;
         *cap = (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_SSB || h->kind == QRL_DEMOD_AM || h->kind == QRL_DEMOD_WBFM) ? 2 * h->port1_cap : h->port1_cap;      // float view of the same buffer
+        if (h->kind == QRL_DEMOD_FREEDV) *cap = 4 * h->port1_cap;                                                                   // int16 view
     }
     else if (port == 2) { *data = h->d_port2; *cap = h->port2_cap; *counts = h->d_port2_cnt; }
     else if (h->dmr) { *data = h->d_port3f; *cap = h->port0_cap; *counts = nullptr; }      // one float per port-0 sample
@@ -2029,6 +2117,9 @@ struct qrl_tx : HandleBase {
     bool dsss_tx = false;
     // gr_mod_am: audio ring d_ra -> 8 ksps complex ring d_if -> x sps (ring d_rc at the output rate) -> output filter (taps d_cfilt) -> d_out
     bool am_tx = false; float am_dc = 0.0f;
+    // gr_mod_freedv: int16 in (d_short_in) -> complex ring d_rs2 -> side-band filter (taps d_cfilt) -> ring d_rc -> feedforward AGC -> ring d_if
+    // (same geometry) -> x sps (arms d_arms2) -> d_out
+    bool freedv_tx = false; short* d_short_in = nullptr;
     // gr_mod_nbfm::set_ctcss: multiply_const_ff gain and the CTCSS tone source (fxpt_nco phase / increment, advanced per sample with the tone on)
     float audio_gain = 0.99f; bool tone_on = false; unsigned tone_phase = 0, tone_inc = 0;
     // gr_mod_dmr: the m17 path with gr_zero_idle_bursts in place of the IF low-pass (a delay of history - 1 items + "zero_samples" tags)
@@ -2085,8 +2176,26 @@ static std::vector<float> make_arms(const std::vector<float>& taps, int L, int n
     return a;
 }
 
+static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+                     int n_channels, long max_items, int device, qrl_tx** out);
+
 int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
                   int n_channels, long max_items, int device, qrl_tx** out)
+{
+    if (kind == QRL_MOD_FREEDV) { set_err(nullptr, "qrl_tx_create: QRL_MOD_FREEDV takes a low cutoff: use qrl_tx_create_freedv"); return QRL_EINVAL; }
+    return tx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, 0, n_channels, max_items, device, out);
+}
+
+int qrl_tx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
+                         int n_channels, long max_items, int device, qrl_tx** out)
+{
+    int rc = check_freedv_args("qrl_tx_create_freedv", sps, samp_rate, filter_width, low_cutoff);
+    if (rc) return rc;
+    return tx_create(QRL_MOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_items, device, out);
+}
+
+static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+                     int n_channels, long max_items, int device, qrl_tx** out)
 {
     (void)carrier_freq;
     if (!out || n_channels <= 0 || max_items <= 0) { set_err(nullptr, "qrl_tx_create: bad argument"); return QRL_EINVAL; }
@@ -2152,6 +2261,21 @@ int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
         h->L1 = 1; h->nt1 = 1; t1 = { 1.0f };
         h->amplif = 0.9f;
+    } else if (kind == QRL_MOD_FREEDV) {
+        // gr_mod_freedv.cpp:34-85 (sps = final interpolation, 125; flag = sb): side-band filter complex_band_pass_2(1, 8000, lo, fw, 250, 90, BH)
+        // (LSB: (-fw, -lo)), feedforward_agc_cc(512, 1), rational_resampler_ccf(sps, 1, low_pass(sps, fs, fw, 1200)) (Hamming), x0.98, x bb gain
+        h->freedv_tx = true; h->amplif = 0.98f;
+        std::vector<float> sb = flag ? complex_band_pass_2(1, 8000, -filter_width, -low_cutoff, 250, 90, WIN_BLACKMAN_HARRIS)
+                                     : complex_band_pass_2(1, 8000, low_cutoff, filter_width, 250, 90, WIN_BLACKMAN_HARRIS);
+        h->nt_cfilt = static_cast<int>(sb.size() / 2);
+        if ((rc = upload_floats(h, &h->d_cfilt, sb))) return fail(rc);
+        t2 = low_pass(sps, samp_rate, filter_width, 1200, WIN_HAMMING);
+        h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
+        t1 = { 1.0f }; h->L1 = 1; h->nt1 = 1;
+        if (h->L2 != 125 || h->nt2 != 17) {     // the register-tiled x125 instance (2007 taps, 17 per arm) is the one built
+            set_err(h, "make_gr_mod_freedv: interpolator shape not built (sps " + std::to_string(sps) + ", " + std::to_string(t2.size()) + " taps)");
+            return fail(QRL_EINVAL);
+        }
     } else if (kind == QRL_MOD_BPSK) {
         // gr_mod_bpsk.cpp:44-56
         t1 = root_raised_cosine(sps, sps, 1, 0.35, 11 * sps);
@@ -2274,6 +2398,15 @@ int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
         for (auto& a : an) { std::memset(&a, 0, sizeof a); a.agc = 1.0f; }               // agc2_ff::make(1e-2, 1e-4, 1, 1): initial gain 1
         if (cudaMemcpy(h->d_an, an.data(), sizeof(TxAnalogState) * h->C, cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "state upload failed"); return fail(QRL_ECUDA); }
     }
+    if (h->freedv_tx) {
+        // three 8 ksps complex rings of one geometry: the 512-item AGC window and the filters' history stay behind the newest call
+        max_sym = max_items;
+        unsigned cap = pow2_at_least(max_items + 1024); h->rc_mask = cap - 1; h->rc_stride = cap; h->if_mask = cap - 1; h->if_stride = cap;
+        if ((rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(cap) * h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap) * h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap) * h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_short_in, static_cast<size_t>(max_items) * h->C))) return fail(rc);
+    }
     if (h->dsss_tx) {
         max_sym = 16LL * 13 * max_items;                               // chips per call
         unsigned cap1 = pow2_at_least(max_sym * h->L1 + h->nt_cfilt + 128); h->if_mask = cap1 - 1; h->if_stride = cap1;
@@ -2299,14 +2432,14 @@ int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter
     const bool qpsk = kind == QRL_MOD_QPSK || kind == QRL_MOD_BPSK || h->dsss_tx;      // complex symbols (QPSK / BPSK: single interpolation stage)
     { unsigned cap = pow2_at_least(max_sym + 64); h->sym_mask = cap - 1; h->sym_stride = cap;
       if ((rc = dev_alloc(h, &h->d_sym, static_cast<size_t>(cap) * h->C * (qpsk ? 2 : 1)))) return fail(rc); }
-    if (!qpsk) {
+    if (!qpsk && !h->freedv_tx) {
         unsigned cap = pow2_at_least(max_sym * (analog ? 1 : h->L1) + 128 + h->zi_delay_items); h->if_mask = cap - 1; h->if_stride = cap;
         if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap) * h->C))) return fail(rc);
     }
     h->out_stride = analog ? max_sym * h->L2 : max_sym * h->L1 * (qpsk ? 1 : h->L2);
     if (h->m17) h->out_stride = (4LL * max_items * h->L1 * h->L2 + h->M2 - 1) / h->M2 + 8;
     if (h->dsss_tx) h->out_stride = ((max_sym * h->L1 * 50 + 12) / 13 + 1) * 50;
-    if (h->am_tx) h->out_stride = static_cast<long long>(max_items) * h->L2;
+    if (h->am_tx || h->freedv_tx) h->out_stride = static_cast<long long>(max_items) * h->L2;
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
     std::vector<TxBitState> st(h->C);
     for (auto& x : st) { x.scr_reg = 0x7F; x.enc_state = 0; x.diff_prev = 0; x.phase_q = 0; }
@@ -2430,6 +2563,42 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
     if (n == 0) return QRL_OK;
     CK(cudaSetDevice(h->device));
     if (on_device) { int rc = check_device_ptr(h, in, "qrl_tx_work"); if (rc) return rc; }
+    if (h->freedv_tx) {
+        // `in` = [C][n] int16 modem samples at 8 ksps; every stage is one item per thread (no recurrence), all on the handle's stream
+        const short* s = static_cast<const short*>(in);
+        long long sstride = stride;
+        if (!on_device) {
+            CK(cudaMemcpy2DAsync(h->d_short_in, sizeof(short) * h->max_items, in, sizeof(short) * stride, sizeof(short) * n, h->C,
+                                 cudaMemcpyHostToDevice, h->stream));
+            s = h->d_short_in; sstride = h->max_items;
+        }
+        const long long a0 = h->n_audio, a1 = h->n_audio + n;
+        const int TB = 256;
+        cudaEvent_t pe = h->prof_begin(0, h->stream);
+        short_to_complex_ring_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + TB - 1) / TB, 1024)), h->C), TB, 0, h->stream>>>(
+            s, sstride, n, static_cast<float>(1.0 / 32765.0), h->d_rs2, h->rc_mask, h->rc_stride, a0);
+        fir_ccc_ring_kernel<<<dim3(static_cast<unsigned>((n + TB - 1) / TB), h->C), TB, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(
+            h->d_rs2, h->rc_mask, h->rc_stride, h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, 1.0f, a0, a1, nullptr, 0, 0);
+        h->prof_end(pe);
+        constexpr int AN = 512, ATILE = 3584, ANT = 256;
+        pe = h->prof_begin(1, h->stream);
+        ffagc_kernel<AN, ATILE, ANT><<<dim3(static_cast<unsigned>((n + ATILE - 1) / ATILE), h->C), ANT, 0, h->stream>>>(
+            h->d_rc, h->rc_mask, h->rc_stride, a0, a1, 1.0f, h->d_if, h->if_mask, h->if_stride);
+        h->prof_end(pe);
+        {   // the HBM-write-bound stage (8 B per output sample): register-tiled, x0.98 and x bb_gain fused (the one shape tx_create accepts)
+            constexpr int L = 125, NT = 17, R = 8, G = 4;
+            dim3 g(static_cast<unsigned>((n + R * G - 1) / (R * G)), h->C);
+            pe = h->prof_begin(2, h->stream);
+            interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, a0, a1, h->d_arms2,
+                h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
+            h->prof_end(pe);
+        }
+        h->launches += 4;
+        h->n_audio = a1;
+        h->n_out_last = static_cast<long>(n * h->L2);
+        CK(cudaGetLastError());
+        return QRL_OK;
+    }
     if (h->am_tx) {
         // `in` = [C][n] float audio at 8 ksps
         const float* au = static_cast<const float*>(in);

@@ -3751,4 +3751,143 @@ __global__ void tx_zero_ranges_kernel(float2* __restrict__ ring, unsigned mask, 
     for (long long a = a0 + threadIdx.x; a < a1; a += blockDim.x) ring[c * stride + (a & mask)] = make_float2(0.0f, 0.0f);
 }
 
+// ================================================================================================
+// FreeDV up to the codec2 modem boundary (gr_demod_freedv.cpp:31-81, gr_mod_freedv.cpp:27-85).  Arithmetic and orders as
+// tests/freedv_oracle.c (qo_freedv_rx_work / qo_freedv_tx_work).
+// ================================================================================================
+struct FreedvRxState { long long n_in; float gain; int pad_; };
+struct FreedvRxParams { float attack, decay, ref, max_gain; int nt_audio; };
+
+// RX behind the side-band filter, 8 ksps, one CTA per channel: complex_to_real -> agc2_ff (the per-sample recurrence on thread 0 over
+// shared-memory chunks; the fabsf form of the AM chain) into a float ring, then over the CTA band_pass_2(1, 8000, 200, 3500, 200, 90) in direct form (oldest tap
+// first) -> x0.1 -> float_to_short(1, 32768) (x scale, clip, rintf) -> port 1 (int16 modem samples for freedv_rx_ss)
+__global__ void __launch_bounds__(128)
+freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
+                      const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long avail_in,
+                      float* __restrict__ agc_ring, unsigned agc_mask, long long agc_stride, const float* __restrict__ audio_taps,
+                      short* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap)
+{
+    extern __shared__ float fdv_taps[];
+    const int c = blockIdx.x;
+    __shared__ FreedvRxState st;
+    for (int k = threadIdx.x; k < p.nt_audio; k += blockDim.x) fdv_taps[k] = audio_taps[k];
+    if (threadIdx.x == 0) st = states[c];
+    __syncthreads();
+    const long long a0 = st.n_in;
+    const int cnt0 = port1_cnt[c];
+    __syncthreads();      // every thread holds a0 before thread 0 advances st.n_in
+    const float2* x = in + static_cast<long long>(c) * in_stride;
+    float* g = agc_ring + static_cast<long long>(c) * agc_stride;
+    // the recurrence walks shared-memory chunks: the CTA stages the real parts, thread 0 runs the gain over them in place, the CTA
+    // stores the AGC output (one global round trip per chunk instead of one per sample on the dependent chain)
+    constexpr int CHUNK = 1024;
+    __shared__ float buf[CHUNK];
+    float gain = st.gain;
+    for (long long b0 = a0; b0 < avail_in; b0 += CHUNK) {
+        const int nb = static_cast<int>(avail_in - b0 < CHUNK ? avail_in - b0 : CHUNK);
+        for (int j = threadIdx.x; j < nb; j += blockDim.x) buf[j] = x[(b0 + j) & in_mask].x;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int j = 0; j < nb; j++) {
+                const float out = buf[j] * gain;
+                const float tmp = fabsf(out) - p.ref;
+                const float rate = (fabsf(tmp) > gain) ? p.attack : p.decay;
+                gain = gain - tmp * rate;
+                if (gain < 0.0f) gain = 10e-5f;
+                if (p.max_gain > 0.0f && gain > p.max_gain) gain = p.max_gain;
+                buf[j] = out;
+            }
+        }
+        __syncthreads();
+        for (int j = threadIdx.x; j < nb; j += blockDim.x) g[(b0 + j) & agc_mask] = buf[j];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { st.gain = gain; st.n_in = avail_in; }
+    __syncthreads();
+    short* o = port1 + static_cast<long long>(c) * port1_stride;
+    for (long long a = a0 + threadIdx.x; a < avail_in; a += blockDim.x) {
+        float acc = 0.0f;
+        for (int k = p.nt_audio - 1; k >= 0; k--) {
+            const long long n = a - k;
+            acc = fmaf(fdv_taps[k], n >= 0 ? g[n & agc_mask] : 0.0f, acc);
+        }
+        float v = acc * 0.1f;
+        v = v * 32768.0f;
+        v = v > 32767.0f ? 32767.0f : (v < -32768.0f ? -32768.0f : v);
+        const long long idx = cnt0 + (a - a0);
+        if (idx < port1_cap) o[idx] = static_cast<short>(rintf(v));
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        port1_cnt[c] = cnt0 + static_cast<int>(avail_in - a0);
+        states[c] = st;
+    }
+}
+
+// TX front: int16 modem samples -> short_to_float(1, scale) (x (float)(1 / scale)) -> float_to_complex -> complex ring at absolute a0..
+__global__ void short_to_complex_ring_kernel(const short* __restrict__ in, long long in_stride, long long n, float inv,
+                                             float2* __restrict__ ring, unsigned mask, long long stride, long long a0)
+{
+    const int c = blockIdx.y;
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const float v = static_cast<float>(in[static_cast<long long>(c) * in_stride + i]) * inv;
+        ring[static_cast<long long>(c) * stride + ((a0 + i) & mask)] = make_float2(v, 0.0f);
+    }
+}
+
+// analog::feedforward_agc_cc(N, ref): y[m] = (ref / max(1e-4, max_{k=m-N+1..m} env(x[k]))) x[m-N+1], env(z) = max(|re|, |im|), zero
+// history; input and output are channel-major complex rings at absolute positions.  A CTA takes TILE outputs: the envelope of the
+// TILE + N - 1 inputs they see goes to shared memory, split into blocks of N; per block the prefix and suffix maxima (van Herk /
+// Gil-Werman) give every window maximum as max(suffix at its first item, prefix at its last item): two loads per output instead of N.
+// Each thread scans CH consecutive items, then combines the chunk totals of its block.  Max is exact, so the order does not matter.
+template <int N, int TILE, int NT>
+__global__ void __launch_bounds__(NT)
+ffagc_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long m0, long long m1, float ref,
+             float2* __restrict__ out, unsigned out_mask, long long out_stride)
+{
+    constexpr int SPAN = TILE + N;                  // local item i = absolute input tile0 - (N - 1) + i; the last item is padding
+    constexpr int CH = SPAN / NT;                   // items per thread
+    constexpr int CPB = N / CH;                     // chunks per block of N
+    static_assert(TILE % N == 0 && SPAN % NT == 0 && N % CH == 0, "ffagc tiling");
+    __shared__ float pre[SPAN], suf[SPAN], tot[NT];
+    const int c = blockIdx.y;
+    const long long tile0 = m0 + static_cast<long long>(blockIdx.x) * TILE;
+    const long long s0 = tile0 - (N - 1);
+    const float2* x = in + static_cast<long long>(c) * in_stride;
+    for (int i = threadIdx.x; i < SPAN; i += NT) {
+        const long long a = s0 + i;
+        float e = 0.0f;                             // envelopes are >= 0: 0 is neutral (history and the items past m1)
+        if (a >= 0 && a < m1) { const float2 v = x[a & in_mask]; e = fmaxf(fabsf(v.x), fabsf(v.y)); }
+        pre[i] = e;
+    }
+    __syncthreads();
+    const int b = threadIdx.x * CH;
+    float pl[CH], sl[CH];
+    float run = 0.0f;
+#pragma unroll
+    for (int j = 0; j < CH; j++) { run = fmaxf(run, pre[b + j]); pl[j] = run; }
+    tot[threadIdx.x] = run;
+    run = 0.0f;
+#pragma unroll
+    for (int j = CH - 1; j >= 0; j--) { run = fmaxf(run, pre[b + j]); sl[j] = run; }
+    __syncthreads();
+    const int k0 = (threadIdx.x / CPB) * CPB;
+    float before = 0.0f, after = 0.0f;
+    for (int k = k0; k < threadIdx.x; k++) before = fmaxf(before, tot[k]);
+    for (int k = threadIdx.x + 1; k < k0 + CPB; k++) after = fmaxf(after, tot[k]);
+#pragma unroll
+    for (int j = 0; j < CH; j++) { pre[b + j] = fmaxf(pl[j], before); suf[b + j] = fmaxf(sl[j], after); }
+    __syncthreads();
+    float2* o = out + static_cast<long long>(c) * out_stride;
+    for (int i = threadIdx.x; i < TILE; i += NT) {
+        const long long m = tile0 + i;
+        if (m >= m1) break;
+        const float mx = fmaxf(fmaxf(suf[i], pre[i + N - 1]), 1e-4f);
+        const float gain = ref / mx;
+        const long long a = m - (N - 1);
+        const float2 v = a >= 0 ? x[a & in_mask] : make_float2(0.0f, 0.0f);
+        o[m & out_mask] = make_float2(v.x * gain, v.y * gain);
+    }
+}
+
 }  // namespace qrl

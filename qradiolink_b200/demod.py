@@ -21,12 +21,16 @@ class RxBlock:
     """n_channels instances of one reference demod hier-block, batched on one GPU."""
 
     def __init__(self, kind, sps, samp_rate, carrier_freq, filter_width, flag=0, n_channels=1,
-                 max_samples=1 << 20, device=0):
+                 max_samples=1 << 20, device=0, low_cutoff=None):
         self._L = load_library()
         self.kind, self.n_channels, self.max_samples = kind, int(n_channels), int(max_samples)
         self._h = C.c_void_p()
-        rc = self._L.qrl_rx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
-                                   self.n_channels, self.max_samples, device, C.byref(self._h))
+        if kind == KIND.DEMOD_FREEDV:
+            rc = self._L.qrl_rx_create_freedv(sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
+                                              self.n_channels, self.max_samples, device, C.byref(self._h))
+        else:
+            rc = self._L.qrl_rx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
+                                       self.n_channels, self.max_samples, device, C.byref(self._h))
         if rc != 0:
             # constructor failures surface like the std::runtime_error RadioController::toggleRX catches
             raise QrlError("qrl_rx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
@@ -140,7 +144,7 @@ class RxBlock:
     def read_port(self, port):
         """Returns a list (one entry per channel) of what the last work() produced on `port`."""
         isz = self._itemsize[port]
-        dt = {8: np.complex64, 4: np.float32, 1: np.uint8}[isz]
+        dt = {8: np.complex64, 4: np.float32, 2: np.int16, 1: np.uint8}[isz]
         cap = C.c_long()
         data = C.c_void_p()
         cnts = C.c_void_p()
@@ -219,6 +223,16 @@ def make_gr_demod_am(sps, samp_rate, carrier_freq, filter_width, n_channels=1, *
 
 def make_gr_demod_nbfm(sps, samp_rate, carrier_freq, filter_width, n_channels=1, **kw):
     return RxBlock(KIND.DEMOD_NBFM, sps, samp_rate, carrier_freq, filter_width, 0, n_channels, **kw)
+
+
+def make_gr_demod_freedv(sps=125, samp_rate=8000, carrier_freq=1700, filter_width=2000, low_cutoff=200, mode=0, sb=0, n_channels=1, **kw):
+    """src/gr/gr_demod_freedv.h:40-41 (defaults as there; instances gr_demod_base.cpp:229-249, e.g. (125, 1e6, 1700, 2500, 200, MODE_1600,
+    0)) up to the input of codec2's freedv_rx_ss.  Ports: 0 = IQ at 8 ksps (sps x the input level: the reference's stage-1 taps), 1 = int16
+    modem samples at 8 ksps, the samples freedv_rx_ss consumes (the reference's port 1 is float speech behind the vocoder).  `mode` is
+    codec2's and only kept as an attribute for the adapter that runs the vocoder."""
+    blk = RxBlock(KIND.DEMOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, int(sb), n_channels, low_cutoff=low_cutoff, **kw)
+    blk.mode = mode
+    return blk
 
 
 # ------------------------------------------------------------------ sink blocks (per channel)

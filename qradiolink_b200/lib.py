@@ -13,7 +13,9 @@ class QrlError(RuntimeError):
 
 class KIND:
     DEMOD_NBFM, DEMOD_4FSK, DEMOD_QPSK, DEMOD_BPSK, DEMOD_2FSK, DEMOD_SSB, DEMOD_AM, DEMOD_GMSK, DEMOD_WBFM, DEMOD_M17, DEMOD_DMR, DEMOD_DSSS = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12
+    DEMOD_FREEDV = 13
     MOD_4FSK, MOD_QPSK, MOD_NBFM, MOD_BPSK, MOD_2FSK, MOD_SSB, MOD_GMSK, MOD_M17, MOD_DMR, MOD_DSSS, MOD_AM = 101, 102, 103, 104, 105, 106, 107, 108, 109, 110, 111
+    MOD_FREEDV = 112
 
 
 class PARAM:
@@ -27,6 +29,7 @@ SYMBOLS = {
     "qrl_version": (C.c_char_p, []),
     "qrl_last_error": (C.c_char_p, [_vp]),
     "qrl_rx_create": (_i, [_i] * 7 + [_l, _i, C.POINTER(_vp)]),
+    "qrl_rx_create_freedv": (_i, [_i] * 7 + [_l, _i, C.POINTER(_vp)]),
     "qrl_rx_destroy": (_i, [_vp]),
     "qrl_rx_set_stream": (_i, [_vp, _vp]),
     "qrl_rx_set_param": (_i, [_vp, _i, _i, _d]),
@@ -46,6 +49,7 @@ SYMBOLS = {
     "qrl_rx_profile": (_i, [_vp, _i]),
     "qrl_rx_profile_read": (_i, [_vp, _i, C.POINTER(_d), C.POINTER(_l)]),
     "qrl_tx_create": (_i, [_i] * 7 + [_l, _i, C.POINTER(_vp)]),
+    "qrl_tx_create_freedv": (_i, [_i] * 7 + [_l, _i, C.POINTER(_vp)]),
     "qrl_tx_destroy": (_i, [_vp]),
     "qrl_tx_set_stream": (_i, [_vp, _vp]),
     "qrl_tx_set_param": (_i, [_vp, _i, _i, _d]),

@@ -10,12 +10,16 @@ from .lib import KIND, PARAM, QrlError, check, load_library
 
 class TxBlock:
     def __init__(self, kind, sps, samp_rate, carrier_freq, filter_width, flag=0, n_channels=1,
-                 max_items=1 << 12, device=0):
+                 max_items=1 << 12, device=0, low_cutoff=None):
         self._L = load_library()
         self.n_channels, self.max_items = int(n_channels), int(max_items)
         self._h = C.c_void_p()
-        rc = self._L.qrl_tx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
-                                   self.n_channels, self.max_items, device, C.byref(self._h))
+        if kind == KIND.MOD_FREEDV:
+            rc = self._L.qrl_tx_create_freedv(sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
+                                              self.n_channels, self.max_items, device, C.byref(self._h))
+        else:
+            rc = self._L.qrl_tx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
+                                       self.n_channels, self.max_items, device, C.byref(self._h))
         if rc != 0:
             raise QrlError("qrl_tx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
 
@@ -71,6 +75,20 @@ class TxBlock:
         check(self._L.qrl_tx_work(self._h, audio.ctypes.data_as(C.c_void_p), n, n, 0), self._h, "qrl_tx_work")
         dptr, stride, nout = C.c_void_p(), C.c_long(), C.c_long()
         check(self._L.qrl_tx_out_device(self._h, C.byref(dptr), C.byref(stride), C.byref(nout)), self._h, "tx_out_device")
+        out = np.zeros((self.n_channels, max(1, nout.value)), np.complex64)
+        n2 = C.c_long()
+        check(self._L.qrl_tx_read(self._h, out.ctypes.data_as(C.c_void_p), max(1, nout.value), C.byref(n2), 0), self._h, "qrl_tx_read")
+        return out[:, :n2.value]
+
+    def work_modem(self, samples):
+        """FreeDV: int16 [n_channels, n] modem samples at 8 ksps (what freedv_tx_ss produces) -> complex64 [n_channels, n x sps]."""
+        samples = np.ascontiguousarray(samples, np.int16)
+        if samples.ndim == 1:
+            samples = samples[None, :]
+        n = samples.shape[1]
+        check(self._L.qrl_tx_work(self._h, samples.ctypes.data_as(C.c_void_p), n, n, 0), self._h, "qrl_tx_work")
+        nout = C.c_long()
+        check(self._L.qrl_tx_out_device(self._h, None, None, C.byref(nout)), self._h, "tx_out_device")
         out = np.zeros((self.n_channels, max(1, nout.value)), np.complex64)
         n2 = C.c_long()
         check(self._L.qrl_tx_read(self._h, out.ctypes.data_as(C.c_void_p), max(1, nout.value), C.byref(n2), 0), self._h, "qrl_tx_read")
@@ -141,3 +159,11 @@ def make_gr_mod_dmr(sps=125, samp_rate=1000000, carrier_freq=1700, filter_width=
     """src/gr/gr_mod_dmr.h:37-38 (defaults as there); items: frame bytes, 4 symbols per byte.  TxBlock.zero_samples is the
     "zero_samples" stream tag gr_dmr_source attaches to the bytes of an idle burst (gr_zero_idle_bursts)."""
     return TxBlock(KIND.MOD_DMR, sps, samp_rate, carrier_freq, filter_width, 0, n_channels, **kw)
+
+
+def make_gr_mod_freedv(sps=125, samp_rate=8000, carrier_freq=1700, filter_width=2000, low_cutoff=200, mode=0, sb=0, n_channels=1, **kw):
+    """src/gr/gr_mod_freedv.h:39-40 (defaults as there; instances gr_mod_base.cpp:181-203, e.g. (125, 1e6, 1700, 2500, 200, MODE_1600, 0))
+    behind codec2's freedv_tx_ss: feed int16 modem samples with TxBlock.work_modem.  `mode` is kept as an attribute for the adapter."""
+    blk = TxBlock(KIND.MOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, int(sb), n_channels, low_cutoff=low_cutoff, **kw)
+    blk.mode = mode
+    return blk
