@@ -1372,32 +1372,50 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         h->launches++;
         x = h->d_rot_buf; xstride = h->Tmax;
     }
+    // A call of a different length moves the slice boundaries, the symbol-sync scratch regions and the number of slices; the
+    // per-slice fences below (ev_v[i], ev_c[q]) pair slice i of this call with slice i of the previous one, so such a call joins the
+    // previous call's tail first (no overlap across that one seam).
+    const bool seam = h->overlap && h->prev_T != T && h->prev_T >= 0;
+    // Overlapped 4FSK calls launch stage 1 of the whole call BEFORE waiting for the tail of call k-2.  Stage 1 writes only the
+    // stage-1 ring and its history, which nothing behind the channel filter reads (the channel filter runs on the same stream), so it
+    // does not touch the double-buffered ports that tail still owns.  Waiting first put the FIR (about 0.8 ms at 64 x 2^22) behind
+    // call k-2's last Viterbi slice, on the loop that sets the step; now it runs under that tail.
+    const bool early_fir = h->overlap && !h->fir_group_forced && h->kind == QRL_DEMOD_4FSK && !seam;
     if (h->overlap) {
-        // this call writes the buffers call k-2 used: wait for that call's tail, then they are free
         h->call_parity ^= 1;
-        for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
-        // The per-slice fences below (ev_v[i], ev_c[q]) pair slice i of this call with slice i of the previous one: that only
-        // holds while both calls are cut the same way.  A call of a different length moves the slice boundaries, the symbol-sync
-        // scratch regions and the number of slices, so it joins the previous call's tail first (no overlap across that one seam).
-        if (h->prev_T != T && h->prev_T >= 0)
-            for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity ^ 1][j], 0));
         std::swap(h->d_port0, h->alt_port0); std::swap(h->d_port1, h->alt_port1); std::swap(h->d_port2, h->alt_port2);
         std::swap(h->d_port1_cnt, h->alt_port1_cnt); std::swap(h->d_port2_cnt, h->alt_port2_cnt);
         if (h->d_port3) { std::swap(h->d_port3, h->alt_port3); std::swap(h->d_port3_cnt, h->alt_port3_cnt); }
         h->d_port1f = reinterpret_cast<float*>(h->d_port1);
     }
-    CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
-    CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
-    if (h->d_port3_cnt) CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
-
     // The call is cut into nsub time slices.  Per slice the parallel stages (decimating FIR, channel filter,
     // demod + RRC) run on the caller's stream; the sequential loop stage of slice i runs on s_loop and the
     // FEC stage on s_fec, overlapping the parallel stages of slices i+1.. (channels stay independent).
-    CK(cudaEventRecord(h->ev_start, h->stream));
-    CK(cudaStreamWaitEvent(h->s_loop, h->ev_start, 0));
-    CK(cudaStreamWaitEvent(h->s_loop2, h->ev_start, 0));
-    CK(cudaStreamWaitEvent(h->s_fec, h->ev_start, 0));
-    if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
+    bool began = false;
+    auto begin_call = [&]() -> int {
+        began = true;
+        if (h->overlap) {
+            // this call writes the buffers call k-2 used: wait for that call's tail, then they are free
+            for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
+            if (seam) for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity ^ 1][j], 0));
+        }
+        CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
+        CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+        if (h->d_port3_cnt) CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
+        CK(cudaEventRecord(h->ev_start, h->stream));
+        CK(cudaStreamWaitEvent(h->s_loop, h->ev_start, 0));
+        CK(cudaStreamWaitEvent(h->s_loop2, h->ev_start, 0));
+        CK(cudaStreamWaitEvent(h->s_fec, h->ev_start, 0));
+        if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
+        return QRL_OK;
+    };
+    if (early_fir) {
+        // stage 1 still follows everything the caller queued on its stream before this call (its input)
+        CK(cudaEventRecord(h->ev_start, h->stream));
+        if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
+    } else {
+        int rc = begin_call(); if (rc) return rc;
+    }
     cudaStream_t sp = h->par();
     // overlapped calls keep the pipeline full across calls: two big slices are enough and cost least (every symbol-sync launch pays
     // its own start-up)
@@ -1444,6 +1462,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
             h->hist_cur ^= 1;
             h->n_in = Ng; h->n1 = kg1;
         }
+        if (!began) { int rc2 = begin_call(); if (rc2) return rc2; }
         // ---- the stages behind it advance slice by slice
         const long long N = h->n_in_s + Ti;
         const long long k0 = h->n1_s;
@@ -1898,6 +1917,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         h->prof_end(pe);
         if (h->overlap) CK(cudaEventRecord(h->ev_v[i], h->s_fec));
     }
+    if (!began) { int rc = begin_call(); if (rc) return rc; }     // every slice was empty
     if (h->kind == QRL_DEMOD_DSSS) {          // port 0 holds 5200 sps items (13 / 50 of the stage-1 items counted in the loop)
         const long long o_end = (h->n1_s * 13 + 49) / 50;
         h->port0_n = static_cast<long>(o_end - h->ds_o_call0);

@@ -1210,6 +1210,22 @@ __device__ __forceinline__ float qrl_ge1(float a, float b)     // (a >= b) ? 1.0
     asm("set.ge.f32.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
     return r;
 }
+// (x >= t) ? a : b as one FSETP + one select.  In PTX so that the compiler keeps the select where it is written: a plain ?: lets it
+// move an operation from both arms behind the select (p ? a*h : b*h -> (p ? a : b) * h) or turn "v + (p ? k : 0)" into predicated
+// adds, either of which puts operations back on a loop-carried chain that the select was meant to keep them off.
+__device__ __forceinline__ float qrl_sel_ge(float x, float t, float a, float b)
+{
+    float r;
+    asm("{ .reg .pred p; setp.ge.f32 p, %1, %2; selp.f32 %0, %3, %4, p; }" : "=f"(r) : "f"(x), "f"(t), "f"(a), "f"(b));
+    return r;
+}
+// (a >= b) ? 0xffffffff : 0 in one FSET (an integer mask: AND-ed with a constant it never becomes a predicated add)
+__device__ __forceinline__ uint32_t qrl_ge_mask(float a, float b)
+{
+    uint32_t r;
+    asm("set.ge.u32.f32 %0, %1, %2;" : "=r"(r) : "f"(a), "f"(b));
+    return r;
+}
 __device__ __forceinline__ float qrl_slice_rect4(float re)
 {
     // -1.5 + [re >= -1] + [re >= -2^-24] + [re >= 1 - 2^-23]  (all partial sums exact)
@@ -1473,18 +1489,28 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
                     xs4 = lds_f32<ROWF * 16>(xa); xs5 = lds_f32<ROWF * 20>(xa); xs6 = lds_f32<ROWF * 24>(xa); xs7 = lds_f32<ROWF * 28>(xa);
                 };
                 if (ofm <= lim) load_xs();
+                // Tap address of the next symbol, carried from one symbol to the next.  rint(mu * 128) is the magic-number FFMA
+                // fmaf(mu, 128, M), M = 1.5 * 2^23, whose low mantissa bits are the bank row.  Inside a symbol it is taken from ph
+                // instead of from mu = ph - n0 - s12: fmaf(ph, 128, M - 128 n0) == fmaf(mu, 128, M) + 128 s12 exactly for ph in
+                // [n0, n0 + 3) (the product is exact, both addends are integers and 128 s12 is even, so ties round alike), and the
+                // 128 s12 rows come off the address through two compare masks on ph that run beside the FFMA (tests/test_symsync_chain.py
+                // checks every float of the window).  ph -> m0 -> s12 -> mu no longer stands in front of the tap load.
+                constexpr uint32_t TROW = REP ? 512u : 48u;                        // bytes per bank row
+                const float q_mph = (12582912.0f - 128.0f * p.fl0) + zf;
+                uint32_t ta = mm2_b + __float_as_uint(fmaf(mu, k128, 12582912.0f)) * TROW;
                 // one symbol; returns true when the lane fell out of the in-lock stride window (generic step taken).
                 // ws_tag = true: the loop constants make that impossible (see window_sure), the check is compiled out.
                 auto body_t = [&](auto ws_tag, float& n, const float h1, const float h2, float& dn, const float dh1, const float dh2) -> bool {
                     constexpr bool WS = decltype(ws_tag)::value;
-                    const uint32_t ta = mm2_b + __float_as_uint(fmaf(mu, k128, 12582912.0f)) * (REP ? 512u : 48u);
                     const float ofn = ofm + q_f0;
                     const uint32_t xn = xb + (__float_as_uint(ofn) << 7);
                     const float r0 = lds_f32<0>(xn), r1 = lds_f32<ROWF * 4>(xn), r2 = lds_f32<ROWF * 8>(xn), r3 = lds_f32<ROWF * 12>(xn),
                                 r4 = lds_f32<ROWF * 16>(xn), r5 = lds_f32<ROWF * 20>(xn), r6 = lds_f32<ROWF * 24>(xn), r7 = lds_f32<ROWF * 28>(xn),
                                 r8 = lds_f32<ROWF * 32>(xn), r9 = lds_f32<ROWF * 36>(xn);
-                    const float kd = -1.5f - dh2;
                     const float4 ta0 = lds_f32x4<0>(ta), ta1 = lds_f32x4<REP ? 256 : 16>(ta);   // taps[7..4], taps[3..0]
+                    // br * h1 of the TED for each of the four decisions (br = dn - dh2 is exact), formed while the taps load; the
+                    // slicer's three thresholds then only pick one, beside (yr - h2) * dh1 (same multiply, same operands: same bits)
+                    const float pb0 = (-1.5f - dh2) * h1, pb1 = (-0.5f - dh2) * h1, pb2 = (0.5f - dh2) * h1, pb3 = (1.5f - dh2) * h1;
                     float yr = fmaf(ta0.x, xs0, 0.0f);                            // oldest sample first
                     yr = fmaf(ta0.y, xs1, yr);
                     yr = fmaf(ta0.z, xs2, yr);
@@ -1496,19 +1522,22 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
                     n = yr;
                     // slicer levels are +-0.5, +-1.5: the sums below are exact in any order (two-level tree)
                     const float s1 = qrl_ge1(yr, -1.0f), s23 = qrl_ge1(yr, -5.9604644775390625e-8f) + qrl_ge1(yr, 0.99999988079071044921875f);
-                    const float br = (s1 + kd) + s23;                             // dn - dh2
                     dn = (s1 - 1.5f) + s23;
-                    const float u = (yr - h2) * dh1 - br * h1;
+                    const float pb = qrl_sel_ge(yr, -5.9604644775390625e-8f, qrl_sel_ge(yr, 0.99999988079071044921875f, pb3, pb2),
+                                                qrl_sel_ge(yr, -1.0f, pb1, pb0));            // (dn - dh2) * h1
+                    const float u = (yr - h2) * dh1 - pb;
                     const float e2x = fminf(fmaxf(u, -2.0f), 2.0f);               // 2 * err
                     avg_period = avg_period + k_hb * e2x;
                     avg_period = fminf(fmaxf(avg_period, q_minp), q_maxp);
                     inst_period = avg_period + k_ha * e2x;
                     const float ph = mu + inst_period;
-                    const float m0 = ph - q_f0;
+                    const float m0 = ph - q_f0;                                   // exact for ph >= n0
                     sts_f32(syp, yr);
                     syp += ROWF * 4;
-                    const float s12 = qrl_ge1(m0, 1.0f) + qrl_ge1(m0, 2.0f);     // == [ph >= n0+1] + [ph >= n0+2] (m0 exact)
-                    const bool g1 = m0 >= 1.0f, g2 = m0 >= 2.0f;
+                    const bool g1 = ph >= q_f1, g2 = ph >= q_f2;                  // == m0 >= 1, m0 >= 2
+                    ta = mm2_b + __float_as_uint(fmaf(ph, k128, q_mph)) * TROW + (qrl_ge_mask(ph, q_f1) & (0u - 128u * TROW))
+                                                                               + (qrl_ge_mask(ph, q_f2) & (0u - 128u * TROW));
+                    const float s12 = qrl_ge1(ph, q_f1) + qrl_ge1(ph, q_f2);
                     mu = m0 - s12;
                     ofm = ofn + s12;
                     xs0 = g2 ? r2 : (g1 ? r1 : r0); xs1 = g2 ? r3 : (g1 ? r2 : r1); xs2 = g2 ? r4 : (g1 ? r3 : r2); xs3 = g2 ? r5 : (g1 ? r4 : r3);
@@ -1517,6 +1546,7 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
                         if (__builtin_expect(__float_as_uint(m0) >= 0x40400000u, 0)) {    // ph not in [n0, n0+3): generic floor
                             const float2 g = symsync_generic_step(ph);
                             mu = g.x;
+                            ta = mm2_b + __float_as_uint(fmaf(mu, k128, 12582912.0f)) * TROW;
                             ofm = (ofn - q_f0) + g.y;
                             if (ofm <= lim) load_xs();
                             return true;

@@ -9,7 +9,8 @@ What the rewrite does to the sources (nothing else is touched):
   * `kernel<<<grid, block, smem, stream>>>(args);`  ->  `emu::launch(dim3(grid), dim3(block), smem, [&] { kernel(args); });`
   * `extern __shared__ T name[];`                   ->  `EMU_DYN_SMEM(T, name);`
   * qrl_tma.cuh (inline PTX: mbarrier, cp.async.bulk, shared-memory loads by address) -> tools/emu/qrl_tma_emu.hpp
-  * the two other inline-PTX spots of qrl_kernels.cuh: `set.ge.f32.f32` (qrl_ge1) and one `cp.async.bulk.wait_group.read 1`
+  * the other inline-PTX spots of qrl_kernels.cuh: `set.ge.f32.f32` (qrl_ge1), `setp.ge.f32` + `selp.f32` (qrl_sel_ge),
+    `set.ge.u32.f32` (qrl_ge_mask) and one `cp.async.bulk.wait_group.read 1`
 """
 import os
 import re
@@ -101,7 +102,7 @@ def rewrite(src):
     src = re.sub(r"extern\s+__shared__\s+(?:__align__\(\d+\)\s+)?([\w ]+?)\s+(\w+)\[\];", r"EMU_DYN_SMEM(\1, \2);", src)
     # inline PTX outside qrl_tma.cuh
     src = re.sub(r'asm volatile\("cp\.async\.bulk\.wait_group\.read 1;" ::: "memory"\);', "/* cp.async.bulk.wait_group.read 1 */;", src)
-    src = re.sub(r"__device__ __forceinline__ float qrl_ge1\(float a, float b\)[^{]*\{.*?\n\}\n", "/* qrl_ge1: tools/emu/qrl_tma_emu.hpp */\n", src, flags=re.S)
+    src = re.sub(r"__device__ __forceinline__ \w+ (qrl_ge1|qrl_sel_ge|qrl_ge_mask)\([^)]*\)[^{]*\{.*?\n\}\n", r"/* \1: tools/emu/qrl_tma_emu.hpp */\n", src, flags=re.S)
     assert "asm" not in re.sub(r"//[^\n]*", "", src).replace("__restrict__", ""), "inline asm left in a rewritten source"
     return src, n
 

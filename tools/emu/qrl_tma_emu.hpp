@@ -67,4 +67,8 @@ inline unsigned long long globaltimer_ns() { return 0; }   // profiling build on
 
 // (a >= b) ? 1.0f : 0.0f  (set.ge.f32.f32 in qrl_kernels.cuh)
 inline float qrl_ge1(float a, float b) { return a >= b ? 1.0f : 0.0f; }
+// (x >= t) ? a : b  (setp.ge.f32 + selp.f32 in qrl_kernels.cuh)
+inline float qrl_sel_ge(float x, float t, float a, float b) { return x >= t ? a : b; }
+// (a >= b) ? 0xffffffff : 0  (set.ge.u32.f32 in qrl_kernels.cuh)
+inline uint32_t qrl_ge_mask(float a, float b) { return a >= b ? 0xffffffffu : 0u; }
 }  // namespace qrl
