@@ -101,6 +101,16 @@ int dev_alloc(HandleBase* h, T** p, size_t n_items, bool zero = true)
     return QRL_OK;
 }
 
+// initial state into a buffer dev_alloc zeroed: the zeroing memset is queued on the handle's (non-blocking) stream, so the copy goes
+// on the same stream behind it -- a plain cudaMemcpy on the legacy stream is not ordered against it and can be overwritten by it
+int upload_state(HandleBase* h, void* dst, const void* src, size_t bytes)
+{
+    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) { set_err(h, std::string("state upload: ") + cudaGetErrorString(e)); return QRL_ECUDA; }
+    return QRL_OK;
+}
+
 int upload_floats(HandleBase* h, float** p, const std::vector<float>& v)
 {
     int rc = dev_alloc(h, p, v.size(), false);
@@ -2416,7 +2426,7 @@ static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         if ((rc = dev_alloc(h, &h->d_audio_in, static_cast<size_t>(max_items) * h->C))) return fail(rc);
         std::vector<TxAnalogState> an(h->C);
         for (auto& a : an) { std::memset(&a, 0, sizeof a); a.agc = 1.0f; }               // agc2_ff::make(1e-2, 1e-4, 1, 1): initial gain 1
-        if (cudaMemcpy(h->d_an, an.data(), sizeof(TxAnalogState) * h->C, cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "state upload failed"); return fail(QRL_ECUDA); }
+        if ((rc = upload_state(h, h->d_an, an.data(), sizeof(TxAnalogState) * h->C))) return fail(rc);
     }
     if (h->freedv_tx) {
         // three 8 ksps complex rings of one geometry: the 512-item AGC window and the filters' history stay behind the newest call
@@ -2463,7 +2473,7 @@ static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
     std::vector<TxBitState> st(h->C);
     for (auto& x : st) { x.scr_reg = 0x7F; x.enc_state = 0; x.diff_prev = 0; x.phase_q = 0; }
-    if (cudaMemcpy(h->d_bits, st.data(), sizeof(TxBitState) * h->C, cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "state upload failed"); return fail(QRL_ECUDA); }
+    if ((rc = upload_state(h, h->d_bits, st.data(), sizeof(TxBitState) * h->C))) return fail(rc);
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
@@ -3342,7 +3352,7 @@ int qrl_mmdvm_tx_create(int variant, int n_channels, const int* rows, int n_rows
     h->fm_sens = static_cast<float>(2 * kPi * 12500.0f / 24000.0f);
     if ((rc = dev_alloc(h, &h->d_bits, h->C))) return fail(rc);
     { std::vector<TxBitState> st(h->C); for (auto& x : st) { x.scr_reg = 0x7F; x.enc_state = 0; x.diff_prev = 0; x.phase_q = 0; }
-      if (cudaMemcpy(h->d_bits, st.data(), sizeof(TxBitState) * h->C, cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "state upload failed"); return fail(QRL_ECUDA); } }
+      if ((rc = upload_state(h, h->d_bits, st.data(), sizeof(TxBitState) * h->C))) return fail(rc); }
     { const unsigned cap = pow2_at_least(max_in + 64); h->sym_mask = cap - 1; h->sym_stride = cap;
       if ((rc = dev_alloc(h, &h->d_sym, static_cast<size_t>(cap) * h->C))) return fail(rc); }
     { const unsigned cap = pow2_at_least(max_in + std::max(h->nt2, h->nt_arm) + 128); h->if_mask = cap - 1; h->if_stride = cap;
