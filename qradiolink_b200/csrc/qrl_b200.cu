@@ -15,7 +15,6 @@
 #include <algorithm>
 #include <cstring>
 #include <map>
-#include <mutex>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -23,19 +22,6 @@
 using namespace qrl;
 
 namespace {
-
-thread_local std::string g_err;
-std::mutex g_tables_mu;
-bool g_tables_done[16] = { false };     // per device ordinal (mod 16): lookup tables uploaded
-
-#define CK(call)                                                                                     \
-    do {                                                                                             \
-        cudaError_t e__ = (call);                                                                    \
-        if (e__ != cudaSuccess) {                                                                    \
-            set_err(h, std::string(#call) + ": " + cudaGetErrorString(e__));                         \
-            return QRL_ECUDA;                                                                        \
-        }                                                                                            \
-    } while (0)
 
 struct Ring {
     void* d = nullptr;
@@ -52,12 +38,6 @@ unsigned pow2_at_least(long long n)
 
 using HandleBase = QrlHandleBase;       // qrl_handle.hpp: shared by every handle type of the library
 
-void set_err(HandleBase* h, const std::string& s)
-{
-    g_err = s;
-    if (h) h->err = s;
-}
-
 // a device pointer handed to a *_work call must live on the handle's device (a pointer from another GPU would fault inside a kernel
 // long after the call returned)
 int check_device_ptr(HandleBase* h, const void* p, const char* who)
@@ -71,53 +51,18 @@ int check_device_ptr(HandleBase* h, const void* p, const char* who)
     return QRL_OK;
 }
 
+// the atan, tanh, MMSE and sine lookup tables, once per device (keyed by this function)
 int upload_tables(HandleBase* h)
 {
-    std::lock_guard<std::mutex> lk(g_tables_mu);
-    if (g_tables_done[h->device & 15]) return QRL_OK;
-    auto at = atan_table(); auto th = tanh_table(); auto mm = mmse_table(); auto sn = fxpt_sine_table();
-    cudaError_t e = cudaMemcpyToSymbol(d_atan_tab, at.data(), at.size() * 4);
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_tanh_tab, th.data(), th.size() * 4);
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_mmse_tab, mm.data(), mm.size() * 4);
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_sine_tab, sn.data(), sn.size() * 4);
-    if (e != cudaSuccess) { set_err(h, std::string("table upload: ") + cudaGetErrorString(e)); return QRL_ECUDA; }   // retried by the next create
-    g_tables_done[h->device & 15] = true;
-    return QRL_OK;
-}
-
-template <class T>
-int dev_alloc(HandleBase* h, T** p, size_t n_items, bool zero = true)
-{
-    void* q = nullptr;
-    size_t bytes = std::max<size_t>(n_items * sizeof(T), 16);
-    cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) { set_err(h, std::string("cudaMalloc: ") + cudaGetErrorString(e)); return QRL_ENOMEM; }
-    if (zero) {
-        e = cudaMemsetAsync(q, 0, bytes, h->stream);
-        if (e != cudaSuccess) { set_err(h, std::string("cudaMemset: ") + cudaGetErrorString(e)); return QRL_ECUDA; }
-    }
-    h->allocs.push_back(q);
-    *p = static_cast<T*>(q);
-    return QRL_OK;
-}
-
-// initial state into a buffer dev_alloc zeroed: the zeroing memset is queued on the handle's (non-blocking) stream, so the copy goes
-// on the same stream behind it -- a plain cudaMemcpy on the legacy stream is not ordered against it and can be overwritten by it
-int upload_state(HandleBase* h, void* dst, const void* src, size_t bytes)
-{
-    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e != cudaSuccess) { set_err(h, std::string("state upload: ") + cudaGetErrorString(e)); return QRL_ECUDA; }
-    return QRL_OK;
-}
-
-int upload_floats(HandleBase* h, float** p, const std::vector<float>& v)
-{
-    int rc = dev_alloc(h, p, v.size(), false);
-    if (rc) return rc;
-    cudaError_t e = cudaMemcpy(*p, v.data(), v.size() * 4, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { set_err(h, std::string("tap upload: ") + cudaGetErrorString(e)); return QRL_ECUDA; }
-    return QRL_OK;
+    return once_per_device(reinterpret_cast<const void*>(&upload_tables), h->device, [h]() -> int {
+        auto at = atan_table(); auto th = tanh_table(); auto mm = mmse_table(); auto sn = fxpt_sine_table();
+        cudaError_t e = cudaMemcpyToSymbol(d_atan_tab, at.data(), at.size() * 4);
+        if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_tanh_tab, th.data(), th.size() * 4);
+        if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_mmse_tab, mm.data(), mm.size() * 4);
+        if (e == cudaSuccess) e = cudaMemcpyToSymbol(d_sine_tab, sn.data(), sn.size() * 4);
+        if (e != cudaSuccess) { set_err(h, std::string("table upload: ") + cudaGetErrorString(e)); return QRL_ECUDA; }   // retried by the next create
+        return QRL_OK;
+    });
 }
 
 }  // namespace
@@ -233,27 +178,7 @@ struct qrl_rx : HandleBase {
     cudaEvent_t ev_par_done = nullptr;
     int sm_loop = 0, sm_par = 0;
     cudaStream_t par() const { return s_par ? s_par : stream; }
-    // optional per-stage device timing (qrl_rx_profile)
-    bool prof = false;
-    struct ProfRec { int stage; cudaEvent_t a, b; };
-    std::vector<ProfRec> prof_recs; size_t prof_used = 0;
-    double prof_ms[8] = { 0 }; long prof_n[8] = { 0 };
-    cudaStream_t prof_stream = nullptr;
-    cudaEvent_t prof_begin(int stage, cudaStream_t on = nullptr)
-    {
-        prof_stream = on ? on : stream;
-        if (!prof) return nullptr;
-        if (prof_used == prof_recs.size()) {
-            ProfRec r{ stage, nullptr, nullptr };
-            cudaEventCreate(&r.a); cudaEventCreate(&r.b);
-            prof_recs.push_back(r);
-        }
-        ProfRec& r = prof_recs[prof_used];
-        r.stage = stage;
-        cudaEventRecord(r.a, prof_stream);
-        return r.b;
-    }
-    void prof_end(cudaEvent_t b) { if (b) { cudaEventRecord(b, prof_stream); prof_used++; } }
+    StageProfiler prof{ 8 };           // optional per-stage device timing (qrl_rx_profile)
 };
 
 namespace {
@@ -263,18 +188,14 @@ int launch_fir_poly(qrl_rx* h, const float2* iq, long long stride, long long T, 
 {
     constexpr int W = (NOUT + Q - 1) * D;
     const size_t smem = sizeof(float2) * ((W + 3) & ~1);
-    static bool attr_done[16] = { false };
-    if (!attr_done[h->device & 15]) {
-        CK(cudaFuncSetAttribute(fir_decim_poly_kernel<D, Q, K, NOUT, NWARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_done[h->device & 15] = true;
-    }
+    if (int rc = smem_opt_in(h, fir_decim_poly_kernel<D, Q, K, NOUT, NWARPS>, (int)smem)) return rc;
     const long long nout = k1 - k0;
     dim3 grid(static_cast<unsigned>((nout + NOUT - 1) / NOUT), h->C);
     fir_decim_poly_kernel<D, Q, K, NOUT, NWARPS><<<grid, NWARPS * 32, smem, h->par()>>>(
         iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
         static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1, h->rot_fused ? h->d_rot : nullptr);
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -290,7 +211,7 @@ int launch_fir_d2(qrl_rx* h, const float2* iq, long long stride, long long T, lo
         iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
         static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -299,13 +220,12 @@ int launch_fir_resamp_2_25(qrl_rx* h, const float2* iq, long long stride, long l
     constexpr int L = 2, M = 25, NT = 105, NOUT = 512;
     constexpr int SPAN = (NOUT * M + L - 1) / L + NT + 1;
     const size_t smem = sizeof(float2) * SPAN;
-    static bool attr_done[16] = { false };    // per device: function attributes belong to the device's context
-    if (!attr_done[h->device & 15]) { CK(cudaFuncSetAttribute(fir_resamp_ccf_kernel<L, M, NT, NOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr_done[h->device & 15] = true; }
+    if (int rc = smem_opt_in(h, fir_resamp_ccf_kernel<L, M, NT, NOUT>, (int)smem)) return rc;
     dim3 grid(static_cast<unsigned>((k1 - k0 + NOUT - 1) / NOUT), h->C);
     fir_resamp_ccf_kernel<L, M, NT, NOUT><<<grid, 256, smem, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
         static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -319,7 +239,7 @@ int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long
         fir_resamp_hist_generic_kernel<<<grid, 128, 0, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->nt_arm1,
             h->L1, h->D1, static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
         h->launches++;
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     if (h->L1 != 1) { set_err(h, "stage-1 resampler shape not built"); return QRL_EINVAL; }
@@ -336,7 +256,7 @@ int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long
         fir_decim_hist_generic_kernel<<<grid, 128, 0, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->ntaps1, h->D1,
             static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
         h->launches++;
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     set_err(h, "stage-1 resampler shape not built (L=" + std::to_string(h->L1) + ", D=" + std::to_string(h->D1) + ", taps=" + std::to_string(h->ntaps1) + ")");
@@ -388,6 +308,23 @@ bool make_sm_partition(qrl_rx* h, unsigned loop_sms, int prio, bool fec_on_par_d
     h->s_loop = a; h->s_fec = b; h->s_par = c; h->s_loop2 = d; h->s_epi = e2;
     h->sm_loop = static_cast<int>(grp.sm.smCount); h->sm_par = static_cast<int>(rest.sm.smCount);
     return true;
+}
+
+// a carrier-offset change: from input sample n_in on, channel `channel` (every channel for channel < 0) turns by `inc` per sample,
+// the phase kept continuous; returns whether any channel still rotates
+bool retune(std::vector<RotState>& rot, int channel, unsigned inc, long long n_in)
+{
+    bool active = false;
+    for (int c = 0; c < static_cast<int>(rot.size()); c++) {
+        RotState& r = rot[c];
+        if (channel < 0 || c == channel) {
+            r.base = r.base + r.inc * static_cast<unsigned>(n_in - r.n_base);
+            r.n_base = n_in;
+            r.inc = inc;
+        }
+        if (r.inc != 0 || r.base != 0) active = true;
+    }
+    return active;
 }
 
 // interleaved = channel-interleaved layout [ceil(C/32)][slots][32] (allocated for the padded channel count)
@@ -446,8 +383,7 @@ int launch_fir_ccf_c(HandleBase* h, int C_, cudaStream_t st, const float2* in, u
     const int span = TILE + ntaps - 1;
     const size_t smem = sizeof(float) * ((ntaps + 1) & ~1) + sizeof(float2) * (span + (span >> 4) + 2);
     if (smem > 48 * 1024 && smem <= 100 * 1024) {            // long filters (gr_mod_am's 4545-tap output filter): opt in to the larger window once per device
-        static bool big_attr[16] = { false };
-        if (!big_attr[h->device & 15]) { CK(cudaFuncSetAttribute(fir_ccf_ring_tiled_kernel<K, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); big_attr[h->device & 15] = true; }
+        if (int rc = smem_opt_in(h, fir_ccf_ring_tiled_kernel<K, NT>, 100 * 1024)) return rc;
     }
     if (n >= 256 && smem <= 100 * 1024 && ntaps >= K) {      // (the tiled kernel's head / tail phases assume at least K taps)
         dim3 g(static_cast<unsigned>((n + TILE - 1) / TILE), hC->C);
@@ -457,7 +393,7 @@ int launch_fir_ccf_c(HandleBase* h, int C_, cudaStream_t st, const float2* in, u
         fir_ccf_ring_kernel<<<g, 256, sizeof(float) * ntaps, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
     }
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float* out, unsigned out_mask, long long out_stride,
@@ -476,15 +412,11 @@ int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_
         qdemod_fir_fff_kernel<<<g, 256, sizeof(float) * (2 * ntaps + 256), st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, gain, a0, a1, nullptr, 0);
     }
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
 }  // namespace
-
-// =====================================================================================================
-// last-error hook for the other translation units of the library (qrl_pfb.cu)
-void qrl_internal_set_err(const std::string& s) { g_err = s; }
 
 extern "C" {
 
@@ -498,7 +430,7 @@ const char* qrl_version(void) { return "qrl_b200 0.1 (sm_90a)"; }
 const char* qrl_last_error(const void* handle)
 {
     if (handle) return static_cast<const HandleBase*>(handle)->err.c_str();
-    return g_err.c_str();
+    return thread_last_error().c_str();
 }
 
 // gr_demod_freedv / gr_mod_freedv factory arguments the reference does not check itself: the chain only holds together at 8 ksps
@@ -535,7 +467,7 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
 {
     if (!out || n_channels <= 0 || max_samples <= 0) { set_err(nullptr, "qrl_rx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_rx_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_rx_create", device)) return rc;
     // gr_demod_gmsk.cpp:30-134 is the 2FSK (fm) chain without the band-edge FLL, with a plain low-pass as symbol filter and its
     // own clock-loop constants: it runs through the 2FSK code path
     const bool gmsk = (kind == QRL_DEMOD_GMSK);
@@ -550,13 +482,11 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
     if (dmr) { carrier_freq = 0; filter_width = 5000; }
     qrl_rx* h = new qrl_rx();
     h->kind = kind; h->sps = sps; h->samp_rate = samp_rate; h->carrier_freq = carrier_freq;
-    h->filter_width = filter_width; h->flag = flag; h->C = n_channels; h->Tmax = max_samples; h->device = device;
+    h->filter_width = filter_width; h->flag = flag; h->C = n_channels; h->Tmax = max_samples;
     h->gmsk = gmsk; h->m17 = m17; h->dmr = dmr;
-    auto fail = [&](int rc) { std::string e = h->err; qrl_rx_destroy(h); g_err = e; return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { set_err(h, "cudaSetDevice failed"); return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { set_err(h, "stream create failed"); return fail(QRL_ECUDA); }
-    h->own_stream = true;
-    int rc = upload_tables(h);
+    auto fail = [&](int rc) { return create_failed(h, qrl_rx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
 
     std::vector<float> taps1, taps2, taps3;
@@ -1048,22 +978,18 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
 // host-side wait for everything a handle has in flight on its internal streams
 static int rx_join_host(qrl_rx* h)
 {
-    if (h->s_loop) CK(cudaStreamSynchronize(h->s_loop));
-    if (h->s_fec) CK(cudaStreamSynchronize(h->s_fec));
-    if (h->s_loop2) CK(cudaStreamSynchronize(h->s_loop2));
-    if (h->s_epi) CK(cudaStreamSynchronize(h->s_epi));
-    if (h->s_par) CK(cudaStreamSynchronize(h->s_par));
+    if (h->s_loop) QRL_CK(cudaStreamSynchronize(h->s_loop));
+    if (h->s_fec) QRL_CK(cudaStreamSynchronize(h->s_fec));
+    if (h->s_loop2) QRL_CK(cudaStreamSynchronize(h->s_loop2));
+    if (h->s_epi) QRL_CK(cudaStreamSynchronize(h->s_epi));
+    if (h->s_par) QRL_CK(cudaStreamSynchronize(h->s_par));
     return QRL_OK;
 }
 
 int qrl_rx_reset(qrl_rx* h)
 {
     if (!h) return QRL_EINVAL;
-    if (h->s_loop) CK(cudaStreamSynchronize(h->s_loop));
-    if (h->s_fec) CK(cudaStreamSynchronize(h->s_fec));
-    if (h->s_loop2) CK(cudaStreamSynchronize(h->s_loop2));
-    if (h->s_epi) CK(cudaStreamSynchronize(h->s_epi));
-    if (h->s_par) CK(cudaStreamSynchronize(h->s_par));
+    if (int rc = rx_join_host(h)) return rc;
     // all-zero history / rings; loop states at their constructor values
     std::vector<SymSyncState> ss(h->C);
     std::vector<ViterbiState> vs(h->C);
@@ -1073,13 +999,13 @@ int qrl_rx_reset(qrl_rx* h)
         ss[c].mu = (h->ssp.loop_kind == LOOP_CRMM) ? 0.5f : 0.0f;          // clock_recovery_mm_cc(omega, g_omega, mu = 0.5, ...)
         vs[c].rd = 0; vs[c].start_state = 0; vs[c].descr_reg = 0x7F;
     }
-    CK(cudaMemcpyAsync(h->d_ss, ss.data(), sizeof(SymSyncState) * h->C, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_vs, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
-    if (h->d_vs2) CK(cudaMemcpyAsync(h->d_vs2, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
-    if (h->d_port3_cnt) CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
-    CK(cudaMemsetAsync(h->d_hist[0], 0, sizeof(float2) * h->H * h->C, h->stream));
-    CK(cudaMemsetAsync(h->d_hist[1], 0, sizeof(float2) * h->H * h->C, h->stream));
-    for (auto& z : h->zero_list) CK(cudaMemsetAsync(z.first, 0, z.second, h->stream));
+    QRL_CK(cudaMemcpyAsync(h->d_ss, ss.data(), sizeof(SymSyncState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    QRL_CK(cudaMemcpyAsync(h->d_vs, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    if (h->d_vs2) QRL_CK(cudaMemcpyAsync(h->d_vs2, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    if (h->d_port3_cnt) QRL_CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
+    QRL_CK(cudaMemsetAsync(h->d_hist[0], 0, sizeof(float2) * h->H * h->C, h->stream));
+    QRL_CK(cudaMemsetAsync(h->d_hist[1], 0, sizeof(float2) * h->H * h->C, h->stream));
+    for (auto& z : h->zero_list) QRL_CK(cudaMemsetAsync(z.first, 0, z.second, h->stream));
     if (h->d_ds) {
         std::vector<DsssState> ds(h->C);
         for (int c = 0; c < h->C; c++) {
@@ -1087,19 +1013,19 @@ int qrl_rx_reset(qrl_rx* h)
             ds[c].agc = 10.0f;                        // agc2_cc::make(1e-1, 1e-1, 1, 10): initial gain 10 (gr_demod_dsss.cpp:66)
             ds[c].omega = 1.0f; ds[c].mu = 0.5f;      // clock_recovery_mm_cc(1, ..., 0.5, ...)
         }
-        CK(cudaMemcpyAsync(h->d_ds, ds.data(), sizeof(DsssState) * h->C, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_ds, ds.data(), sizeof(DsssState) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         h->ds_o_call0 = 0;
     }
     std::vector<SsbState> sb(h->C);
     if (h->d_ssb) {
         for (int c = 0; c < h->C; c++) { std::memset(&sb[c], 0, sizeof(SsbState)); sb[c].sq_state = SQ_MUTED; sb[c].gain = 1.0f; }
-        CK(cudaMemcpyAsync(h->d_ssb, sb.data(), sizeof(SsbState) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_ssb, sb.data(), sizeof(SsbState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
     std::vector<FreedvRxState> fdv(h->C);
     if (h->d_fdv) {
         for (auto& f : fdv) { f.n_in = 0; f.gain = 1.0f; f.pad_ = 0; }           // agc2_ff::make(..., gain = 1)
-        CK(cudaMemcpyAsync(h->d_fdv, fdv.data(), sizeof(FreedvRxState) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_fdv, fdv.data(), sizeof(FreedvRxState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
     std::vector<NbfmState> nb(h->C);
     if (h->d_nb) {
@@ -1108,16 +1034,16 @@ int qrl_rx_reset(qrl_rx* h)
             nb[c].sq_state = SQ_MUTED; nb[c].envelope = h->nbp.sq_ramp ? 0.0f : 1.0f; nb[c].agc_gain = 1.0f;
             nb[c].c_mute = 1; nb[c].c_state = SQ_MUTED; nb[c].c_env = h->ctc.ramp ? 0.0 : 1.0;      // ctcss_squelch_ff: d_mute(true), squelch_base_ff starts muted
         }
-        CK(cudaMemcpyAsync(h->d_nb, nb.data(), sizeof(NbfmState) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_nb, nb.data(), sizeof(NbfmState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
     std::vector<AgcCostasState> ac(h->C);
     if (h->d_ac) {
         for (int c = 0; c < h->C; c++) { ac[c].pos = 0; ac[c].gain = 1.0f; ac[c].pll.phase = 0.0f; ac[c].pll.freq = 0.0f; }
-        CK(cudaMemcpyAsync(h->d_ac, ac.data(), sizeof(AgcCostasState) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_ac, ac.data(), sizeof(AgcCostasState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
-    CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
-    CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
-    CK(cudaStreamSynchronize(h->stream));   // the staging vectors above go out of scope
+    QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
+    QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));   // the staging vectors above go out of scope
     h->n_in = 0; h->n1 = 0; h->n_in_s = 0; h->n1_s = 0; h->hist_cur = 0; h->port0_n = 0; h->prev_nsub = 0; h->rssi_n = 0;
     return QRL_OK;
 }
@@ -1127,35 +1053,24 @@ int qrl_rx_destroy(qrl_rx* h)
     if (!h) return QRL_OK;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    if (h->s_loop) { cudaStreamSynchronize(h->s_loop); cudaStreamDestroy(h->s_loop); }
-    if (h->s_fec) { cudaStreamSynchronize(h->s_fec); cudaStreamDestroy(h->s_fec); }
-    if (h->s_loop2) { cudaStreamSynchronize(h->s_loop2); cudaStreamDestroy(h->s_loop2); }
-    if (h->s_epi) { cudaStreamSynchronize(h->s_epi); cudaStreamDestroy(h->s_epi); }
-    if (h->s_par) { cudaStreamSynchronize(h->s_par); cudaStreamDestroy(h->s_par); }
+    rx_join_host(h);
+    for (cudaStream_t s : { h->s_loop, h->s_fec, h->s_loop2, h->s_epi, h->s_par }) if (s) cudaStreamDestroy(s);
     // every stream is idle now: the events recorded on them can go
     auto ev_free = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
     for (cudaEvent_t e : { h->ev_start, h->ev_loop_done, h->ev_loop2_done, h->ev_fec_done, h->ev_par_done }) ev_free(e);
     for (int i = 0; i < qrl_rx::kMaxSub; i++) { ev_free(h->ev_a[i]); ev_free(h->ev_b[i]); ev_free(h->ev_c[i]); ev_free(h->ev_v[i]); }
     for (int q = 0; q < 2; q++) for (int j = 0; j < 3; j++) ev_free(h->ev_tail[q][j]);
-    for (auto& r : h->prof_recs) { ev_free(r.a); ev_free(r.b); }
     if (h->g_loop || h->g_par) {
         auto pDestroy = drv<CUresult (*)(CUgreenCtx)>("cuGreenCtxDestroy");
         if (pDestroy) { if (h->g_loop) pDestroy(h->g_loop); if (h->g_par) pDestroy(h->g_par); }
     }
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 
 int qrl_rx_set_stream(qrl_rx* h, void* s)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->own_stream && h->stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (s) h->stream = static_cast<cudaStream_t>(s);
-    else { CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
+    return handle_set_stream(h, s);
 }
 
 int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
@@ -1177,7 +1092,7 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
     if (key == QRL_PARAM_OVERLAP_CALLS) {
         // only the path whose ring reuse is fenced for it: real-symbol 4FSK (external soft-bit epilogue)
         if (!(h->kind == QRL_DEMOD_4FSK && h->flag) || h->dmr) { set_err(h, "QRL_PARAM_OVERLAP_CALLS: not supported for this block"); return QRL_EINVAL; }
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         { int rc = rx_join_host(h); if (rc) return rc; }
         const bool on = value != 0.0;
         if (on && !h->alt_port1) {
@@ -1192,10 +1107,10 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
                 if ((rc = dev_alloc(h, &h->alt_port3_cnt, h->C))) return rc;
             }
             for (int q = 0; q < 2; q++) for (int j = 0; j < 3; j++)
-                if (!h->ev_tail[q][j]) CK(cudaEventCreateWithFlags(&h->ev_tail[q][j], cudaEventDisableTiming));
+                if (!h->ev_tail[q][j]) QRL_CK(cudaEventCreateWithFlags(&h->ev_tail[q][j], cudaEventDisableTiming));
             for (int i = 0; i < qrl_rx::kMaxSub; i++)
-                if (!h->ev_v[i]) CK(cudaEventCreateWithFlags(&h->ev_v[i], cudaEventDisableTiming));
-            CK(cudaStreamSynchronize(h->stream));
+                if (!h->ev_v[i]) QRL_CK(cudaEventCreateWithFlags(&h->ev_v[i], cudaEventDisableTiming));
+            QRL_CK(cudaStreamSynchronize(h->stream));
         }
         h->overlap = on;
         return QRL_OK;
@@ -1204,29 +1119,21 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
         if (channel >= h->C) { set_err(h, "set_param: channel out of range"); return QRL_EINVAL; }
         if (h->rot.empty()) h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
         const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(-value / h->samp_rate * 4294967296.0))));
-        for (int c = 0; c < h->C; c++) {
-            if (channel >= 0 && c != channel) continue;
-            RotState& r = h->rot[c];
-            r.base = r.base + r.inc * static_cast<unsigned>(h->n_in - r.n_base);     // keep the phase continuous
-            r.n_base = h->n_in;
-            r.inc = inc;
-        }
-        h->rot_active = false;
-        for (auto& r : h->rot) if (r.inc != 0 || r.base != 0) h->rot_active = true;
+        h->rot_active = retune(h->rot, channel, inc, h->n_in);
         if (!h->d_rot) { int rc = dev_alloc(h, &h->d_rot, h->C); if (rc) return rc; }
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         if (h->overlap) { int rc = rx_join_host(h); if (rc) return rc; }
-        CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
+        QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
         return QRL_OK;
     }
     // ---- run-time setters of the analog blocks.  Kernel parameters travel by value with every launch, so a plain host-side update is
     // enough for scalars; new taps are uploaded after everything in flight has drained and meet the true sample history (the rings)
     // from the next qrl_rx_work on.
     const bool nbfm = h->kind == QRL_DEMOD_NBFM, ssb = h->kind == QRL_DEMOD_SSB, am = h->kind == QRL_DEMOD_AM, wbfm = h->kind == QRL_DEMOD_WBFM;
-    auto quiesce = [&]() -> int { CK(cudaStreamSynchronize(h->stream)); return rx_join_host(h); };
+    auto quiesce = [&]() -> int { QRL_CK(cudaStreamSynchronize(h->stream)); return rx_join_host(h); };
     auto upload = [&](float* dst, const std::vector<float>& t) -> int {
         int rc = quiesce(); if (rc) return rc;
-        CK(cudaMemcpy(dst, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
+        QRL_CK(cudaMemcpy(dst, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
         return QRL_OK;
     };
     if (key == QRL_PARAM_SQUELCH_DB && (nbfm || ssb || am || wbfm)) {
@@ -1276,9 +1183,9 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
         int rc = quiesce(); if (rc) return rc;
         {   // set_frequency makes new Goertzel objects: their running sums restart (the squelch state machine keeps its state)
             std::vector<NbfmState> stv(h->C);
-            CK(cudaMemcpy(stv.data(), h->d_nb, sizeof(NbfmState) * h->C, cudaMemcpyDeviceToHost));
+            QRL_CK(cudaMemcpy(stv.data(), h->d_nb, sizeof(NbfmState) * h->C, cudaMemcpyDeviceToHost));
             for (auto& x : stv) { x.gl1 = x.gl2 = x.gc1 = x.gc2 = x.gr1 = x.gr2 = 0.0f; x.g_processed = 0; }
-            CK(cudaMemcpy(h->d_nb, stv.data(), sizeof(NbfmState) * h->C, cudaMemcpyHostToDevice));
+            QRL_CK(cudaMemcpy(h->d_nb, stv.data(), sizeof(NbfmState) * h->C, cudaMemcpyHostToDevice));
         }
         if (!h->ctc.on) {
             h->ctc.on = 1;
@@ -1334,7 +1241,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     if (!h || !iq || T < 0) return QRL_EINVAL;
     if (T > h->Tmax) { set_err(h, "qrl_rx_work: T exceeds max_samples given at create"); return QRL_ERANGE; }
     if (T == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     if (on_device) { int rc = check_device_ptr(h, iq, "qrl_rx_work"); if (rc) return rc; }
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
@@ -1355,7 +1262,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 int rc = dev_alloc(h, &h->d_in_sc16, static_cast<size_t>(h->Tmax) * h->C, false);
                 if (rc) return rc;
             }
-            CK(cudaMemcpy2DAsync(h->d_in_sc16, isz * h->Tmax, iq_any, isz * stride, isz * T, h->C, cudaMemcpyHostToDevice, h->stream));
+            QRL_CK(cudaMemcpy2DAsync(h->d_in_sc16, isz * h->Tmax, iq_any, isz * stride, isz * T, h->C, cudaMemcpyHostToDevice, h->stream));
             s = h->d_in_sc16; sstride = h->Tmax;
         }
         dim3 g(static_cast<unsigned>(std::min<long long>((T + 1023) / 1024, 65535)), h->C);
@@ -1365,7 +1272,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         x = h->d_in_staging;
         xstride = h->Tmax;
     } else if (!on_device) {
-        CK(cudaMemcpy2DAsync(h->d_in_staging, sizeof(float2) * h->Tmax, iq, sizeof(float2) * stride,
+        QRL_CK(cudaMemcpy2DAsync(h->d_in_staging, sizeof(float2) * h->Tmax, iq, sizeof(float2) * stride,
                              sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
         x = h->d_in_staging;
         xstride = h->Tmax;
@@ -1406,23 +1313,23 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         began = true;
         if (h->overlap) {
             // this call writes the buffers call k-2 used: wait for that call's tail, then they are free
-            for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
-            if (seam) for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity ^ 1][j], 0));
+            for (int j = 0; j < 3; j++) QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
+            if (seam) for (int j = 0; j < 3; j++) QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity ^ 1][j], 0));
         }
-        CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
-        CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
-        if (h->d_port3_cnt) CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
-        CK(cudaEventRecord(h->ev_start, h->stream));
-        CK(cudaStreamWaitEvent(h->s_loop, h->ev_start, 0));
-        CK(cudaStreamWaitEvent(h->s_loop2, h->ev_start, 0));
-        CK(cudaStreamWaitEvent(h->s_fec, h->ev_start, 0));
-        if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
+        QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
+        QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+        if (h->d_port3_cnt) QRL_CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
+        QRL_CK(cudaEventRecord(h->ev_start, h->stream));
+        QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_start, 0));
+        QRL_CK(cudaStreamWaitEvent(h->s_loop2, h->ev_start, 0));
+        QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_start, 0));
+        if (h->s_par) QRL_CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
         return QRL_OK;
     };
     if (early_fir) {
         // stage 1 still follows everything the caller queued on its stream before this call (its input)
-        CK(cudaEventRecord(h->ev_start, h->stream));
-        if (h->s_par) CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
+        QRL_CK(cudaEventRecord(h->ev_start, h->stream));
+        if (h->s_par) QRL_CK(cudaStreamWaitEvent(h->s_par, h->ev_start, 0));
     } else {
         int rc = begin_call(); if (rc) return rc;
     }
@@ -1454,7 +1361,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
             const long long Ng = h->n_in + Tg;
             const long long kg0 = h->n1;
             const long long kg1 = (Ng * h->L1 + h->D1 - 1) / h->D1;       // outputs i with floor(i M / L) <= N - 1
-            pe = h->prof_begin(0, sp);
+            pe = h->prof.begin(0, sp);
             int rc = stage1(h, xg, xstride, Tg, kg0, kg1);
             if (!rc && h->kind == QRL_DEMOD_SSB && kg1 > kg0) {
                 // gr_demod_ssb's multiply_const_cc(_if_gain) sits between the resampler and the side-band filter: the gain is applied
@@ -1463,7 +1370,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 scale2_ring_kernel<<<gs, 256, 0, sp>>>(static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, kg0, kg1, h->if_gain, 1.0f);
                 h->launches++;
             }
-            h->prof_end(pe);
+            h->prof.end(pe);
             if (rc) return rc;
             dim3 g((h->H + 127) / 128, h->C);
             if (h->rot_fused) frontend_hist_kernel<<<g, 128, 0, sp>>>(h->d_rot, xg, xstride, Tg, h->n_in, h->d_hist[h->hist_cur], h->d_hist[h->hist_cur ^ 1], h->H);
@@ -1486,9 +1393,9 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         dim3 gtile(static_cast<unsigned>((std::max<long long>(n_new, 1) + TB - 1) / TB), h->C);
         const int groups = (h->C + 31) / 32;
         if (h->kind == QRL_DEMOD_DSSS) {
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(3, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(3, h->s_loop);
             dsss_chain_kernel<<<h->C, 256, 0, h->s_loop>>>(h->dsp, h->d_ds, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
                 h->d_ds_arms, h->d_taps2, h->d_ds_taps,
                 static_cast<float2*>(h->ds_a.d), static_cast<float2*>(h->ds_c.d), h->ds_a.mask, h->ds_a.stride,
@@ -1497,10 +1404,10 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
                 static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, nsoft_i);
             h->launches++;
-            h->prof_end(pe);
-            CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-            CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
-            pe = h->prof_begin(4, h->s_fec);
+            h->prof.end(pe);
+            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
+            QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
+            pe = h->prof.begin(4, h->s_fec);
             constexpr int CPB2 = 4;
             viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
                 static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
@@ -1509,65 +1416,65 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
                 h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
             h->launches += 2;
-            h->prof_end(pe);
+            h->prof.end(pe);
             continue;
         }
         if (h->kind == QRL_DEMOD_SSB) {
             if (n_new > 0) {
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
                     static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
                     static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                     h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(3, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(3, h->s_loop);
             ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb,
                 static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
                 static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
                 static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
                 h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
             h->launches++;
-            h->prof_end(pe);
+            h->prof.end(pe);
             continue;
         }
         if (h->kind == QRL_DEMOD_FREEDV) {
             if (n_new > 0) {
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
                     static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
                     static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                     h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(3, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(3, h->s_loop);
             freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
                 static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
                 static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
                 reinterpret_cast<short*>(h->d_port1), 4 * h->port1_cap, h->d_port1_cnt, static_cast<int>(4 * h->port1_cap));
             h->launches++;
-            h->prof_end(pe);
+            h->prof.end(pe);
             continue;
         }
         if (h->kind == QRL_DEMOD_AM) {
             if (n_new > 0) {
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
                     static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
                     static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                     h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(3, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(3, h->s_loop);
             nbfm_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->nbp, h->d_nb,
                 static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1, h->d_env,
                 static_cast<float2*>(h->rg.d), h->rg.mask, h->rg.stride,
@@ -1575,28 +1482,24 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 static_cast<float*>(h->rr.d), h->rr.mask, h->rr.stride,
                 h->d_arm_taps, h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
             h->launches++;
-            h->prof_end(pe);
+            h->prof.end(pe);
             continue;
         }
         if (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_WBFM) {
             if (n_new > 0) {
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 { int rc = launch_fir_ccf(h, sp, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
                                           static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                           h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 0); if (rc) return rc; }
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(3, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(3, h->s_loop);
             const size_t fat = h->nbfm_split ? 120 * 1024 : 0;       // one CTA per SM, and never next to a de-emphasis CTA
             if (h->nbfm_split) {
-                static bool f_attr[16] = { false };
-                if (!f_attr[h->device & 15]) {
-                    CK(cudaFuncSetAttribute(nbfm_audio_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
-                    CK(cudaFuncSetAttribute(nbfm_deemph_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
-                    f_attr[h->device & 15] = true;
-                }
+                int rc;
+                if ((rc = smem_opt_in(h, nbfm_audio_kernel, 120 * 1024)) || (rc = smem_opt_in(h, nbfm_deemph_kernel, 120 * 1024))) return rc;
             }
             nbfm_audio_kernel<<<h->C, 128, fat, h->s_loop>>>(h->nbp, h->d_nb,
                 static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1, h->d_env,
@@ -1607,36 +1510,36 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 h->nbfm_split ? static_cast<float*>(h->raud.d) : nullptr, h->raud.mask, h->raud.stride, h->nbfm_split ? nsoft_i : nullptr,
                 static_cast<float*>(h->rq.d), h->rq.mask, h->rq.stride, h->ctc, h->d_cenv);
             h->launches++;
-            h->prof_end(pe);
+            h->prof.end(pe);
             if (h->nbfm_split) {
-                CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-                CK(cudaStreamWaitEvent(h->s_loop2, h->ev_b[i], 0));
-                pe = h->prof_begin(5, h->s_loop2);
+                QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
+                QRL_CK(cudaStreamWaitEvent(h->s_loop2, h->ev_b[i], 0));
+                pe = h->prof.begin(5, h->s_loop2);
                 nbfm_deemph_kernel<<<h->C, 128, fat, h->s_loop2>>>(h->nbp.b0, h->nbp.b1, h->nbp.a1, h->nbp.out_gain, h->d_nb2,
                     static_cast<const float*>(h->raud.d), h->raud.mask, h->raud.stride, nsoft_i,
                     h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
             continue;
         }
         if (h->kind == QRL_DEMOD_2FSK || h->kind == QRL_DEMOD_BPSK) {
             const bool bpsk = h->kind == QRL_DEMOD_BPSK;
             // ---- FLL (sequential, per sample) on the loop stream: r1 -> rf
-            CK(cudaEventRecord(h->ev_a[i], sp));
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof_begin(1, h->s_loop);
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            pe = h->prof.begin(1, h->s_loop);
             if (!h->gmsk) {
                 fll_kernel<32><<<groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
                     static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
                     static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
                 h->launches++;
             }
-            h->prof_end(pe);
+            h->prof.end(pe);
             const Ring& fin = h->gmsk ? h->r1 : h->rf;             // GMSK: no FLL in front of the channel filter
             if (n_new > 0) {
                 // ---- channel filter / RRC on the FLL output -> port 0 (+ ring: channel-major for 2FSK, interleaved for BPSK)
-                pe = h->prof_begin(2, h->s_loop);
+                pe = h->prof.begin(2, h->s_loop);
                 { int rc = launch_fir_ccf(h, h->s_loop, static_cast<const float2*>(fin.d), fin.mask, fin.stride,
                                           static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                           h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, bpsk ? 1 : 0); if (rc) return rc; }
@@ -1653,16 +1556,15 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                         static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, h->d_symf_taps, h->nt_symf, k0, k1);
                     h->launches += 2;
                 }
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            pe = h->prof_begin(3, h->s_loop);
+            pe = h->prof.begin(3, h->s_loop);
             if (bpsk) {
                 {   // agc2_cc (Costas bypassed): r2 -> r3
                     constexpr int CH = 128, NST = 2;
                     const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
                     auto kern = agc_costas_kernel<CH, NST, 0, 0>;
-                    static bool a_attr[16] = { false };    // per device: function attributes belong to the device's context
-                    if (!a_attr[h->device & 15]) { CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); a_attr[h->device & 15] = true; }
+                    if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
                     kern<<<groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
                         static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
                         static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
@@ -1672,8 +1574,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period) + 3);
                 const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
                 auto kern = symsync_kernel<2, SL_BPSK, EPI_BPSK, CH, NST, NEPI, LOOP_CRMM>;
-                static bool b_attr[16] = { false };    // per device: function attributes belong to the device's context
-                if (!b_attr[h->device & 15]) { CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); b_attr[h->device & 15] = true; }
+                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
                 kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
                     h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
                     h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
@@ -1684,19 +1585,18 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
                 const size_t smem = sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * maxs * 32) + sizeof(int) * 64;
                 auto kern = symsync_kernel<1, SL_BPSK, EPI_REAL1, CH, NST, NEPI>;
-                static bool f_attr[16] = { false };    // per device: function attributes belong to the device's context
-                if (!f_attr[h->device & 15]) { CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); f_attr[h->device & 15] = true; }
+                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
                 kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
                     h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, k1,
                     h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
                     static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
                 h->launches++;
             }
-            h->prof_end(pe);
-            CK(cudaEventRecord(h->ev_b[i], h->s_loop));
+            h->prof.end(pe);
+            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
             // ---- two decoders on the same soft stream, the second behind delay(1)
-            CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
-            pe = h->prof_begin(4, h->s_fec);
+            QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
+            pe = h->prof.begin(4, h->s_fec);
             constexpr int CPB2 = 4;
             viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
                 static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
@@ -1705,17 +1605,17 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
                 h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
             h->launches += 2;
-            h->prof_end(pe);
+            h->prof.end(pe);
             continue;
         }
         if (h->kind == QRL_DEMOD_4FSK) {
             if (n_new > 0) {
                 // ---- stage 2: channel filter -> ring + port 0
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 { int rc = launch_fir_ccf(h, sp, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
                                           static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                           h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 0); if (rc) return rc; }
-                h->prof_end(pe);
+                h->prof.end(pe);
                 // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
                 // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
                 if (h->overlap && h->prev_nsub > 0) {
@@ -1724,9 +1624,9 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                     const long long must = k1 - (static_cast<long long>(h->r4.mask) + 1) + 64;
                     int q = -1;
                     for (int j = 0; j < h->prev_nsub; j++) if (h->prev_k1[j] - 64 < must) q = j;      // not yet safe after slice j alone
-                    if (q >= 0) CK(cudaStreamWaitEvent(sp, h->ev_c[std::min(q + 1, h->prev_nsub - 1)], 0));
+                    if (q >= 0) QRL_CK(cudaStreamWaitEvent(sp, h->ev_c[std::min(q + 1, h->prev_nsub - 1)], 0));
                 }
-                pe = h->prof_begin(2, sp);
+                pe = h->prof.begin(2, sp);
                 if (h->flag) {
                     { int rc = launch_qdemod_fir(h, sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                                  static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
@@ -1746,28 +1646,27 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                                               static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride,
                                               h->d_symf_taps, h->nt_symf, k0, k1, nullptr, 0, 0, 1); if (rc) return rc; }
                 }
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
             // ---- stage 4: symbol sync (+ phase mod + soft bits) on the loop stream
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
             bool ext_recorded = false;
             if (!h->flag) {
-                pe = h->prof_begin(3, h->s_loop);
+                pe = h->prof.begin(3, h->s_loop);
                 constexpr int CH = 128, NST = 3, NEPI = 2;
                 const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
                 const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
                 auto kern = symsync_kernel<2, SL_RECT4, EPI_CPLX, CH, NST, NEPI>;
-                static bool sc_attr[16] = { false };    // per device: function attributes belong to the device's context
-                if (!sc_attr[h->device & 15]) { CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); sc_attr[h->device & 15] = true; }
+                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
                 kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
                     h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
                     h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
                     static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             } else {
-                pe = h->prof_begin(3, h->s_loop);
+                pe = h->prof.begin(3, h->s_loop);
                 // real symbols: lean recurrence + external epilogue (symbols leave the SM by TMA bulk store; the phase
                 // modulator / soft-bit stores run on the wide partition behind it, same stream)
                 auto run_ext = [&](auto ch_tag, auto nst_tag) -> int {
@@ -1781,14 +1680,9 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 auto kern = h->dmr ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>
                           : rep ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 2>
                                 : symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 1>;
-                static bool ss_attr[3][16] = { { false } };   // per (CH, NST) instantiation of this lambda, per variant, per device
-                const int vi = h->dmr ? 2 : (rep ? 1 : 0);
-                if (!ss_attr[vi][h->device & 15]) {
-                    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-                    ss_attr[vi][h->device & 15] = true;
-                }
+                if (int rc = smem_opt_in(h, kern, 224 * 1024)) return rc;
                 // overlapped calls: the previous call's Viterbi of slice i still reads d_nsoft[i], its epilogue scratch region i
-                if (h->overlap) CK(cudaStreamWaitEvent(h->s_loop, h->ev_v[i], 0));
+                if (h->overlap) QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_v[i], 0));
                 // every slice of a call gets its own scratch region and header (the epilogue of slice i overlaps symsync i+1)
                 if (i == 0) h->ss_chunk_off = 0;
                 const int chunk_bound = static_cast<int>(std::min<long long>(h->ss_chunk_cap - h->ss_chunk_off, n_new / symsync_stride(CH, h->ssp.lookahead) + 3));
@@ -1800,11 +1694,11 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                     h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
                     static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i,
                     scratch_i, chunk_bound, static_cast<int>(h->ss_chunk_cap), hdr_i);
-                h->prof_end(pe);
+                h->prof.end(pe);
                 cudaStream_t se = h->s_epi ? h->s_epi : h->s_loop;
-                if (se != h->s_loop || h->overlap) CK(cudaEventRecord(h->ev_c[i], h->s_loop));
-                if (se != h->s_loop) CK(cudaStreamWaitEvent(se, h->ev_c[i], 0));
-                pe = h->prof_begin(5, se);
+                if (se != h->s_loop || h->overlap) QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
+                if (se != h->s_loop) QRL_CK(cudaStreamWaitEvent(se, h->ev_c[i], 0));
+                pe = h->prof.begin(5, se);
                 auto epi = h->dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
                 if (chunk_bound > 0)
                     epi<<<dim3(chunk_bound, groups), dim3(32, 8), 0, se>>>(
@@ -1813,8 +1707,8 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                         static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
                         h->m17 ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
                 h->launches++;
-                h->prof_end(pe);
-                CK(cudaEventRecord(h->ev_b[i], se));
+                h->prof.end(pe);
+                QRL_CK(cudaEventRecord(h->ev_b[i], se));
                 return QRL_OK;
                 };
                 const int rc_ext = h->ss_ch == 512 ? run_ext(std::integral_constant<int, 512>{}, std::integral_constant<int, 2>{})
@@ -1822,44 +1716,40 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 if (rc_ext) return rc_ext;
                 ext_recorded = true;
             }
-            if (!ext_recorded) CK(cudaEventRecord(h->ev_b[i], h->s_loop));
+            if (!ext_recorded) QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
         } else {   // QRL_DEMOD_QPSK
             const float2* shaping_in = static_cast<const float2*>(h->r1.d);
             unsigned shaping_mask = h->r1.mask; long long shaping_stride = h->r1.stride;
             if (h->d_fll) {     // sps > 4: fll_band_edge_cc between resampler and shaping filter (sequential, on the loop stream)
-                CK(cudaEventRecord(h->ev_a[i], sp));
-                CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+                QRL_CK(cudaEventRecord(h->ev_a[i], sp));
+                QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
                 fll_kernel<32><<<groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
                     static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
                     static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
                 h->launches++;
-                CK(cudaEventRecord(h->ev_c[i], h->s_loop));
-                CK(cudaStreamWaitEvent(sp, h->ev_c[i], 0));
+                QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
+                QRL_CK(cudaStreamWaitEvent(sp, h->ev_c[i], 0));
                 shaping_in = static_cast<const float2*>(h->rf.d); shaping_mask = h->rf.mask; shaping_stride = h->rf.stride;
             }
             if (n_new > 0) {
                 // ---- stage 2: RRC shaping filter -> interleaved ring + port 0
-                pe = h->prof_begin(1, sp);
+                pe = h->prof.begin(1, sp);
                 { int rc = launch_fir_ccf(h, sp, shaping_in, shaping_mask, shaping_stride,
                                           static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                           h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 1); if (rc) return rc; }
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_a[i], sp));
+            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
             // ---- stage 3: agc2 + costas "PLL" per sample on the loop stream
-            CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
             {
-                pe = h->prof_begin(2, h->s_loop);
+                pe = h->prof.begin(2, h->s_loop);
                 auto run_ac = [&](auto ch_tag) -> int {
                     constexpr int CH = decltype(ch_tag)::value, NST = 2;      // input stages (2) + hand-off blocks (3): 164 KB at CH = 128
                     const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
                     auto kern = (h->acp.order == 4 && h->acp.use_snr) ? agc_costas_kernel<CH, NST, 4, 1> : agc_costas_kernel<CH, NST>;
-                    static bool ac_attr[16] = { false };    // per CH instantiation, per device: function attributes belong to the device's context
-                    if (!ac_attr[h->device & 15]) {
-                        CK(cudaFuncSetAttribute(agc_costas_kernel<CH, NST, 4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                        CK(cudaFuncSetAttribute(agc_costas_kernel<CH, NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                        ac_attr[h->device & 15] = true;
-                    }
+                    int rc;                                 // both instantiations, whichever this call takes
+                    if ((rc = smem_opt_in(h, agc_costas_kernel<CH, NST, 4, 1>, 200 * 1024)) || (rc = smem_opt_in(h, agc_costas_kernel<CH, NST>, 200 * 1024))) return rc;
                     kern<<<groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
                         static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
                         static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
@@ -1869,13 +1759,13 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 const int rc_ac = h->many ? run_ac(std::integral_constant<int, 32>{}) : run_ac(std::integral_constant<int, 128>{});
                 if (rc_ac) return rc_ac;
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_c[i], h->s_loop));
+            QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
             // ---- stage 4: symbol sync + second Costas + diff phasor + soft bits on the second loop stream
-            CK(cudaStreamWaitEvent(h->s_loop2, h->ev_c[i], 0));
+            QRL_CK(cudaStreamWaitEvent(h->s_loop2, h->ev_c[i], 0));
             {
-                pe = h->prof_begin(3, h->s_loop2);
+                pe = h->prof.begin(3, h->s_loop2);
                 // lean: the prefetching complex recurrence (symbol-sync variant 2, replicated tap bank) with the epilogue split into a
                 // Costas warp and a feed-forward warp over a 3-deep symbol ring (NEPI = 2); else the generic recurrence, one epilogue warp
                 auto run_sq = [&](auto ch_tag, auto nst_tag, auto lean_tag) -> int {
@@ -1886,11 +1776,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                     const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + NB * maxs * 64) + sizeof(int) * 32 * (NB == 2 ? 2 : 4) +
                                         (LEAN ? 129 * 512 : 0);
                     auto kern = symsync_kernel<2, SL_DQPSK, EPI_QPSK, CH, NST, NEPI, LOOP_SYMSYNC, LEAN ? 2 : 0>;
-                    static bool sq_attr[16] = { false };    // per (CH, NST, LEAN) instantiation, per device
-                    if (!sq_attr[h->device & 15]) {
-                        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-                        sq_attr[h->device & 15] = true;
-                    }
+                    if (int rc = smem_opt_in(h, kern, 224 * 1024)) return rc;
                     if (smem > 224 * 1024) { set_err(h, "QPSK symbol sync: window does not fit shared memory"); return QRL_EINVAL; }
                     kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop2>>>(
                         h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
@@ -1908,24 +1794,24 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                                             : run_sq(std::integral_constant<int, 128>{}, std::integral_constant<int, 3>{}, std::false_type{});
                 if (rc_sq) return rc_sq;
                 h->launches++;
-                h->prof_end(pe);
+                h->prof.end(pe);
             }
-            CK(cudaEventRecord(h->ev_b[i], h->s_loop2));
+            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop2));
         }
         // ---- stage 5: Viterbi + descrambler on the FEC stream
-        CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
+        QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
         if (h->m17) {                    // gr_demod_m17 has no FEC: the epilogue wrote the hard bits of port 2 (s_fec joins it at the end)
-            if (h->overlap) CK(cudaEventRecord(h->ev_v[i], h->s_fec));
+            if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[i], h->s_fec));
             continue;
         }
-        pe = h->prof_begin(4, h->s_fec);
+        pe = h->prof.begin(4, h->s_fec);
         constexpr int CPB = 4;    // 4 channels (8 warps) per CTA
         viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
             static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
             h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
         h->launches++;
-        h->prof_end(pe);
-        if (h->overlap) CK(cudaEventRecord(h->ev_v[i], h->s_fec));
+        h->prof.end(pe);
+        if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[i], h->s_fec));
     }
     if (!began) { int rc = begin_call(); if (rc) return rc; }     // every slice was empty
     if (h->kind == QRL_DEMOD_DSSS) {          // port 0 holds 5200 sps items (13 / 50 of the stage-1 items counted in the loop)
@@ -1946,21 +1832,21 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     if (h->overlap) {
         // the caller's stream only waits for the parallel stages (the input has been consumed); the loop / FEC tail runs
         // on under the next call and is joined by qrl_rx_join / qrl_rx_sync / qrl_rx_read_port
-        CK(cudaEventRecord(h->ev_tail[h->call_parity][0], h->s_loop));
-        CK(cudaEventRecord(h->ev_tail[h->call_parity][1], h->s_fec));
-        CK(cudaEventRecord(h->ev_tail[h->call_parity][2], h->s_epi ? h->s_epi : h->s_loop));
-        if (h->s_par) { CK(cudaEventRecord(h->ev_par_done, h->s_par)); CK(cudaStreamWaitEvent(h->stream, h->ev_par_done, 0)); }
-        CK(cudaGetLastError());
+        QRL_CK(cudaEventRecord(h->ev_tail[h->call_parity][0], h->s_loop));
+        QRL_CK(cudaEventRecord(h->ev_tail[h->call_parity][1], h->s_fec));
+        QRL_CK(cudaEventRecord(h->ev_tail[h->call_parity][2], h->s_epi ? h->s_epi : h->s_loop));
+        if (h->s_par) { QRL_CK(cudaEventRecord(h->ev_par_done, h->s_par)); QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_par_done, 0)); }
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
-    CK(cudaEventRecord(h->ev_loop_done, h->s_loop));
-    CK(cudaEventRecord(h->ev_loop2_done, h->s_loop2));
-    CK(cudaStreamWaitEvent(h->stream, h->ev_loop2_done, 0));
-    CK(cudaEventRecord(h->ev_fec_done, h->s_fec));
-    if (h->s_par) { CK(cudaEventRecord(h->ev_par_done, h->s_par)); CK(cudaStreamWaitEvent(h->stream, h->ev_par_done, 0)); }
-    CK(cudaStreamWaitEvent(h->stream, h->ev_loop_done, 0));
-    CK(cudaStreamWaitEvent(h->stream, h->ev_fec_done, 0));
-    CK(cudaGetLastError());
+    QRL_CK(cudaEventRecord(h->ev_loop_done, h->s_loop));
+    QRL_CK(cudaEventRecord(h->ev_loop2_done, h->s_loop2));
+    QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_loop2_done, 0));
+    QRL_CK(cudaEventRecord(h->ev_fec_done, h->s_fec));
+    if (h->s_par) { QRL_CK(cudaEventRecord(h->ev_par_done, h->s_par)); QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_par_done, 0)); }
+    QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_loop_done, 0));
+    QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_fec_done, 0));
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -1968,41 +1854,31 @@ int qrl_rx_join(qrl_rx* h)
 {
     if (!h) return QRL_EINVAL;
     if (!h->overlap) return QRL_OK;
-    for (int j = 0; j < 3; j++) CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
+    for (int j = 0; j < 3; j++) QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity][j], 0));
     return QRL_OK;
 }
 
 int qrl_rx_profile(qrl_rx* h, int enable)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    h->prof = enable != 0;
-    h->prof_used = 0;
-    for (int i = 0; i < 8; i++) { h->prof_ms[i] = 0; h->prof_n[i] = 0; }
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    h->prof.reset(enable != 0);
     return QRL_OK;
 }
 
 int qrl_rx_profile_read(qrl_rx* h, int stage, double* ms_total, long* n_launches)
 {
-    if (!h || stage < 0 || stage >= 8) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
+    if (!h || stage < 0 || stage >= h->prof.stages()) return QRL_EINVAL;
+    QRL_CK(cudaStreamSynchronize(h->stream));
     if (h->overlap) { int rc = rx_join_host(h); if (rc) return rc; }
-    for (size_t i = 0; i < h->prof_used; i++) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, h->prof_recs[i].a, h->prof_recs[i].b) == cudaSuccess) {
-            h->prof_ms[h->prof_recs[i].stage] += ms; h->prof_n[h->prof_recs[i].stage]++;
-        }
-    }
-    h->prof_used = 0;
-    if (ms_total) *ms_total = h->prof_ms[stage];
-    if (n_launches) *n_launches = h->prof_n[stage];
+    h->prof.read(stage, ms_total, n_launches);
     return QRL_OK;
 }
 
 int qrl_rx_sync(qrl_rx* h)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     if (h->overlap) return rx_join_host(h);
     return QRL_OK;
 }
@@ -2011,9 +1887,9 @@ int qrl_rx_rssi(qrl_rx* h, float level, float* rssi_db_host)
 {
     if (!h || !rssi_db_host) return QRL_EINVAL;
     if (!h->rssi_on || !h->d_rssi_db) { set_err(h, "qrl_rx_rssi: enable QRL_PARAM_RSSI first"); return QRL_EINVAL; }
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->s_par) CK(cudaStreamSynchronize(h->s_par));
-    CK(cudaMemcpy(rssi_db_host, h->d_rssi_db, sizeof(float) * h->C, cudaMemcpyDeviceToHost));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    if (h->s_par) QRL_CK(cudaStreamSynchronize(h->s_par));
+    QRL_CK(cudaMemcpy(rssi_db_host, h->d_rssi_db, sizeof(float) * h->C, cudaMemcpyDeviceToHost));
     for (int c = 0; c < h->C; c++) rssi_db_host[c] = (h->rssi_n > 0 ? rssi_db_host[c] : -180.0f) + level;      // add_const_ff(level)
     return QRL_OK;
 }
@@ -2052,10 +1928,10 @@ int qrl_rx_read_port(qrl_rx* h, int port, void* dst, long cap, int* counts, int 
     if (rc) return rc;
     const int isz = qrl_rx_port_itemsize(h, port);
     long maxn = 0;
-    if (h->overlap) { CK(cudaStreamSynchronize(h->stream)); rc = rx_join_host(h); if (rc) return rc; }
+    if (h->overlap) { QRL_CK(cudaStreamSynchronize(h->stream)); rc = rx_join_host(h); if (rc) return rc; }
     if (dcnt) {
-        CK(cudaMemcpyAsync(counts, dcnt, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaMemcpyAsync(counts, dcnt, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         for (int c = 0; c < h->C; c++) { if (counts[c] > scap) counts[c] = static_cast<int>(scap); maxn = std::max<long>(maxn, counts[c]); }
     } else {
         for (int c = 0; c < h->C; c++) counts[c] = static_cast<int>(h->port0_n);
@@ -2063,10 +1939,10 @@ int qrl_rx_read_port(qrl_rx* h, int port, void* dst, long cap, int* counts, int 
     }
     if (dst && maxn > 0) {
         const long w = std::min(maxn, cap);
-        CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * isz, src, static_cast<size_t>(scap) * isz, static_cast<size_t>(w) * isz, h->C,
+        QRL_CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * isz, src, static_cast<size_t>(scap) * isz, static_cast<size_t>(w) * isz, h->C,
                              dst_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, h->stream));
     }
-    CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 
@@ -2176,26 +2052,7 @@ struct qrl_tx : HandleBase {
     cudaStream_t s_bits = nullptr, s_shape = nullptr;
     cudaEvent_t ev_start = nullptr, ev_bits[kTxSub] = { nullptr }, ev_shape[kTxSub] = { nullptr }, ev_shape_done = nullptr, ev_out_done = nullptr;
     // optional per-stage device timing (qrl_tx_profile): 0 = bit chain, 1 = pulse shaping / FM scan, 2 = final interpolator
-    bool prof = false;
-    struct ProfRec { int stage; cudaEvent_t a, b; };
-    std::vector<ProfRec> prof_recs; size_t prof_used = 0;
-    double prof_ms[4] = { 0 }; long prof_n[4] = { 0 };
-    cudaStream_t prof_stream = nullptr;
-    cudaEvent_t prof_begin(int stage, cudaStream_t on)
-    {
-        prof_stream = on;
-        if (!prof) return nullptr;
-        if (prof_used == prof_recs.size()) {
-            ProfRec r{ stage, nullptr, nullptr };
-            cudaEventCreate(&r.a); cudaEventCreate(&r.b);
-            prof_recs.push_back(r);
-        }
-        ProfRec& r = prof_recs[prof_used];
-        r.stage = stage;
-        cudaEventRecord(r.a, prof_stream);
-        return r.b;
-    }
-    void prof_end(cudaEvent_t b) { if (b) { cudaEventRecord(b, prof_stream); prof_used++; } }
+    StageProfiler prof{ 4 };
 };
 
 static std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
@@ -2230,15 +2087,13 @@ static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
     (void)carrier_freq;
     if (!out || n_channels <= 0 || max_items <= 0) { set_err(nullptr, "qrl_tx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_tx_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_tx_create", device)) return rc;
     qrl_tx* h = new qrl_tx();
     h->kind = kind; h->sps = sps; h->samp_rate = samp_rate; h->filter_width = filter_width; h->flag = flag;
-    h->C = n_channels; h->max_items = max_items; h->device = device;
-    auto fail = [&](int rc) { std::string e = h->err; qrl_tx_destroy(h); g_err = e; return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { set_err(h, "cudaSetDevice failed"); return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { set_err(h, "stream create failed"); return fail(QRL_ECUDA); }
-    h->own_stream = true;
-    int rc = upload_tables(h);
+    h->C = n_channels; h->max_items = max_items;
+    auto fail = [&](int rc) { return create_failed(h, qrl_tx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
     std::vector<float> t1, t2;
     if (kind == QRL_MOD_4FSK) {
@@ -2487,21 +2342,13 @@ int qrl_tx_destroy(qrl_tx* h)
     if (h->s_shape) { cudaStreamSynchronize(h->s_shape); cudaStreamDestroy(h->s_shape); }
     for (cudaEvent_t e : { h->ev_start, h->ev_shape_done, h->ev_out_done }) if (e) cudaEventDestroy(e);
     for (int i = 0; i < qrl_tx::kTxSub; i++) { if (h->ev_bits[i]) cudaEventDestroy(h->ev_bits[i]); if (h->ev_shape[i]) cudaEventDestroy(h->ev_shape[i]); }
-    for (auto& r : h->prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
-    for (void* p : h->allocs) cudaFree(p);
     h->zi.release();
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 int qrl_tx_set_stream(qrl_tx* h, void* s)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->own_stream && h->stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (s) h->stream = static_cast<cudaStream_t>(s);
-    else { CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
+    return handle_set_stream(h, s);
 }
 int qrl_tx_set_param(qrl_tx* h, int, int key, double value)
 {
@@ -2520,8 +2367,8 @@ int qrl_tx_set_param(qrl_tx* h, int, int key, double value)
         if (nt1 > 256 || static_cast<int>(tc.size()) > 400 || nt2 > 400 || static_cast<size_t>(h->L2) * nt2 * sizeof(float) > 40 * 1024) {
             set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
         }
-        CK(cudaSetDevice(h->device));
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaSetDevice(h->device));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         float *a1 = nullptr, *cf = nullptr, *a2 = nullptr;
         int rc;
         if ((rc = upload_floats(h, &a1, make_arms(t1, 25, nt1)))) return rc;
@@ -2545,8 +2392,8 @@ int qrl_tx_set_param(qrl_tx* h, int, int key, double value)
             h->tone_inc = static_cast<unsigned>(static_cast<int>(static_cast<float>(x) * 2147483648.0f / static_cast<float>(kPi)));
         }
         if (static_cast<int>(lp.size()) > 400) { set_err(h, "qrl_tx_set_param: audio filter too long"); return QRL_EINVAL; }
-        CK(cudaSetDevice(h->device));
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaSetDevice(h->device));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         float* p = nullptr;
         int rc = upload_floats(h, &p, lp);
         if (rc) return rc;
@@ -2572,8 +2419,8 @@ int qrl_tx_set_param(qrl_tx* h, int, int key, double value)
         if (nt2 > 60 || static_cast<size_t>(h->L2) * nt2 * sizeof(float) > 40 * 1024 || ntc > (h->am_tx ? 8192 : 500)) {
             set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
         }
-        CK(cudaSetDevice(h->device));
-        CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaSetDevice(h->device));
+        QRL_CK(cudaStreamSynchronize(h->stream));
         float *a2 = nullptr, *c2 = nullptr;
         int rc;
         if ((rc = upload_floats(h, &a2, make_arms(t2, h->L2, nt2)))) return rc;
@@ -2591,42 +2438,42 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
     if (n > h->max_items) { set_err(h, "qrl_tx_work: n exceeds max_items given at create"); return QRL_ERANGE; }
     h->n_out_last = 0;
     if (n == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     if (on_device) { int rc = check_device_ptr(h, in, "qrl_tx_work"); if (rc) return rc; }
     if (h->freedv_tx) {
         // `in` = [C][n] int16 modem samples at 8 ksps; every stage is one item per thread (no recurrence), all on the handle's stream
         const short* s = static_cast<const short*>(in);
         long long sstride = stride;
         if (!on_device) {
-            CK(cudaMemcpy2DAsync(h->d_short_in, sizeof(short) * h->max_items, in, sizeof(short) * stride, sizeof(short) * n, h->C,
+            QRL_CK(cudaMemcpy2DAsync(h->d_short_in, sizeof(short) * h->max_items, in, sizeof(short) * stride, sizeof(short) * n, h->C,
                                  cudaMemcpyHostToDevice, h->stream));
             s = h->d_short_in; sstride = h->max_items;
         }
         const long long a0 = h->n_audio, a1 = h->n_audio + n;
         const int TB = 256;
-        cudaEvent_t pe = h->prof_begin(0, h->stream);
+        cudaEvent_t pe = h->prof.begin(0, h->stream);
         short_to_complex_ring_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + TB - 1) / TB, 1024)), h->C), TB, 0, h->stream>>>(
             s, sstride, n, static_cast<float>(1.0 / 32765.0), h->d_rs2, h->rc_mask, h->rc_stride, a0);
         fir_ccc_ring_kernel<<<dim3(static_cast<unsigned>((n + TB - 1) / TB), h->C), TB, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(
             h->d_rs2, h->rc_mask, h->rc_stride, h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, 1.0f, a0, a1, nullptr, 0, 0);
-        h->prof_end(pe);
+        h->prof.end(pe);
         constexpr int AN = 512, ATILE = 3584, ANT = 256;
-        pe = h->prof_begin(1, h->stream);
+        pe = h->prof.begin(1, h->stream);
         ffagc_kernel<AN, ATILE, ANT><<<dim3(static_cast<unsigned>((n + ATILE - 1) / ATILE), h->C), ANT, 0, h->stream>>>(
             h->d_rc, h->rc_mask, h->rc_stride, a0, a1, 1.0f, h->d_if, h->if_mask, h->if_stride);
-        h->prof_end(pe);
+        h->prof.end(pe);
         {   // the HBM-write-bound stage (8 B per output sample): register-tiled, x0.98 and x bb_gain fused (the one shape tx_create accepts)
             constexpr int L = 125, NT = 17, R = 8, G = 4;
             dim3 g(static_cast<unsigned>((n + R * G - 1) / (R * G)), h->C);
-            pe = h->prof_begin(2, h->stream);
+            pe = h->prof.begin(2, h->stream);
             interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, a0, a1, h->d_arms2,
                 h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
-            h->prof_end(pe);
+            h->prof.end(pe);
         }
         h->launches += 4;
         h->n_audio = a1;
         h->n_out_last = static_cast<long>(n * h->L2);
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     if (h->am_tx) {
@@ -2634,7 +2481,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
         const float* au = static_cast<const float*>(in);
         long long astride = stride;
         if (!on_device) {
-            CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
+            QRL_CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
                                  cudaMemcpyHostToDevice, h->stream));
             au = h->d_audio_in; astride = h->max_items;
         }
@@ -2649,7 +2496,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
                                     h->d_out, h->out_stride, o0, 0); if (rc) return rc; }
         h->n_audio = a1;
         h->n_out_last = static_cast<long>(o1 - o0);
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     if (h->kind == QRL_MOD_NBFM || h->kind == QRL_MOD_SSB) {
@@ -2657,7 +2504,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
         const float* au = static_cast<const float*>(in);
         long long astride = stride;
         if (!on_device) {
-            CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
+            QRL_CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
                                  cudaMemcpyHostToDevice, h->stream));
             au = h->d_audio_in; astride = h->max_items;
         }
@@ -2707,13 +2554,13 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
             h->n_mid = s1;
         }
         h->n_audio += n;
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     const unsigned char* b = static_cast<const unsigned char*>(in);
     long long bstride = stride;
     if (!on_device) {
-        CK(cudaMemcpy2DAsync(h->d_in, h->max_items, in, stride, n, h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpy2DAsync(h->d_in, h->max_items, in, stride, n, h->C, cudaMemcpyHostToDevice, h->stream));
         b = h->d_in; bstride = h->max_items;
     }
     const bool cplx = h->kind == QRL_MOD_QPSK || h->kind == QRL_MOD_BPSK;
@@ -2742,7 +2589,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
         h->launches += 4;
         h->n_out_last = static_cast<long>((o1 - o0) * 50);
         h->n_sym += nsym;
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     const long long sym0 = h->n_sym, nsym = (h->m17 ? 4LL : (one_per_bit ? 16LL : 8LL)) * n;
@@ -2761,42 +2608,42 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
     }
     if (pipelined) {
         constexpr int S = qrl_tx::kTxSub;
-        CK(cudaEventRecord(h->ev_start, h->stream));
-        CK(cudaStreamWaitEvent(h->s_bits, h->ev_start, 0));
-        CK(cudaStreamWaitEvent(h->s_bits, h->ev_shape_done, 0));      // previous call: symbol ring consumed
-        CK(cudaStreamWaitEvent(h->s_shape, h->ev_out_done, 0));       // previous call: IF ring consumed
+        QRL_CK(cudaEventRecord(h->ev_start, h->stream));
+        QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_start, 0));
+        QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_shape_done, 0));      // previous call: symbol ring consumed
+        QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_out_done, 0));       // previous call: IF ring consumed
         const long long out_base = sym0 * h->L1 * h->L2;
         for (int j = 0; j < S; j++) {
             const long b0 = n * j / S, b1 = n * (j + 1) / S;
             if (b1 <= b0) continue;
             const long long symA = sym0 + 8LL * b0, nsym_j = 8LL * (b1 - b0);
-            cudaEvent_t pe = h->prof_begin(0, h->s_bits);
+            cudaEvent_t pe = h->prof.begin(0, h->s_bits);
             tx_bits_kernel<TXM_4FSK><<<dim3((h->C + 31) / 32), 32, 0, h->s_bits>>>(h->d_bits, h->C, b + b0, b1 - b0, bstride,
                                                                                  h->d_sym, h->sym_mask, h->sym_stride, symA);
-            h->prof_end(pe);
-            CK(cudaEventRecord(h->ev_bits[j], h->s_bits));
-            CK(cudaStreamWaitEvent(h->s_shape, h->ev_bits[j], 0));
-            pe = h->prof_begin(1, h->s_shape);
+            h->prof.end(pe);
+            QRL_CK(cudaEventRecord(h->ev_bits[j], h->s_bits));
+            QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_bits[j], 0));
+            pe = h->prof.begin(1, h->s_shape);
             tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->s_shape>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, symA, nsym_j,
                 h->L1, h->nt1, h->d_arms1, h->repeat_only, h->pulse_scale, h->fm_sens, h->amplif, h->bb_gain,
                 h->d_if, h->if_mask, h->if_stride);
-            h->prof_end(pe);
-            CK(cudaEventRecord(h->ev_shape[j], h->s_shape));
-            CK(cudaStreamWaitEvent(h->stream, h->ev_shape[j], 0));
+            h->prof.end(pe);
+            QRL_CK(cudaEventRecord(h->ev_shape[j], h->s_shape));
+            QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_shape[j], 0));
             constexpr int L = 20, NT = 35, R = 8, G = 16;
             const long long m0 = symA * h->L1, m1 = (symA + nsym_j) * h->L1;
             dim3 g(static_cast<unsigned>((m1 - m0 + R * G - 1) / (R * G)), h->C);
-            pe = h->prof_begin(2, h->stream);
+            pe = h->prof.begin(2, h->stream);
             interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(
                 h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, out_base);
-            h->prof_end(pe);
+            h->prof.end(pe);
             h->launches += 3;
         }
-        CK(cudaEventRecord(h->ev_shape_done, h->s_shape));
-        CK(cudaEventRecord(h->ev_out_done, h->stream));
+        QRL_CK(cudaEventRecord(h->ev_shape_done, h->s_shape));
+        QRL_CK(cudaEventRecord(h->ev_out_done, h->stream));
         h->n_out_last = static_cast<long>(nsym * h->L1 * h->L2);
         h->n_sym += nsym;
-        CK(cudaGetLastError());
+        QRL_CK(cudaGetLastError());
         return QRL_OK;
     }
     {
@@ -2832,7 +2679,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
             std::vector<long long> ranges;
             h->zi.collect(h->C, m0, m1, 0, ranges);
             if (!ranges.empty()) {
-                CK(h->zi.upload(ranges, h->stream));
+                QRL_CK(h->zi.upload(ranges, h->stream));
                 tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, h->zi.d_ranges);
                 h->launches++;
             }
@@ -2879,7 +2726,7 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
         h->n_out_last = static_cast<long>((m1 - m0) * h->L2);
     }
     h->n_sym += nsym;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int qrl_tx_zero_samples(qrl_tx* h, int channel, long long byte_offset, long n_samples)
@@ -2895,31 +2742,23 @@ int qrl_tx_zero_samples(qrl_tx* h, int channel, long long byte_offset, long n_sa
 int qrl_tx_sync(qrl_tx* h)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 int qrl_tx_profile(qrl_tx* h, int enable)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    h->prof = enable != 0;
-    h->prof_used = 0;
-    for (int i = 0; i < 4; i++) { h->prof_ms[i] = 0; h->prof_n[i] = 0; }
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    h->prof.reset(enable != 0);
     return QRL_OK;
 }
 int qrl_tx_profile_read(qrl_tx* h, int stage, double* ms_total, long* n_launches)
 {
-    if (!h || stage < 0 || stage >= 4) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->s_bits) CK(cudaStreamSynchronize(h->s_bits));
-    if (h->s_shape) CK(cudaStreamSynchronize(h->s_shape));
-    for (size_t i = 0; i < h->prof_used; i++) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, h->prof_recs[i].a, h->prof_recs[i].b) == cudaSuccess) { h->prof_ms[h->prof_recs[i].stage] += ms; h->prof_n[h->prof_recs[i].stage]++; }
-    }
-    h->prof_used = 0;
-    if (ms_total) *ms_total = h->prof_ms[stage];
-    if (n_launches) *n_launches = h->prof_n[stage];
+    if (!h || stage < 0 || stage >= h->prof.stages()) return QRL_EINVAL;
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    if (h->s_bits) QRL_CK(cudaStreamSynchronize(h->s_bits));
+    if (h->s_shape) QRL_CK(cudaStreamSynchronize(h->s_shape));
+    h->prof.read(stage, ms_total, n_launches);
     return QRL_OK;
 }
 int qrl_tx_read(qrl_tx* h, float* dst, long cap, long* n_out, int dst_on_device)
@@ -2928,10 +2767,10 @@ int qrl_tx_read(qrl_tx* h, float* dst, long cap, long* n_out, int dst_on_device)
     *n_out = h->n_out_last;
     if (dst && h->n_out_last > 0) {
         const long w = std::min(cap, h->n_out_last);
-        CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * 8, h->d_out, static_cast<size_t>(h->out_stride) * 8, static_cast<size_t>(w) * 8, h->C,
+        QRL_CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * 8, h->d_out, static_cast<size_t>(h->out_stride) * 8, static_cast<size_t>(w) * 8, h->C,
                              dst_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, h->stream));
     }
-    CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 int qrl_tx_out_device(qrl_tx* h, float** data, long* stride, long* n_out)
@@ -2955,28 +2794,17 @@ struct qrl_frontend : HandleBase {
     std::vector<RotState> rot; RotState* d_rot = nullptr; bool rot_active = false;
 };
 
-int qrl_frontend_destroy(qrl_frontend* h)
-{
-    if (!h) return QRL_OK;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
-}
+int qrl_frontend_destroy(qrl_frontend* h) { return h ? handle_close(h) : QRL_OK; }
 int qrl_frontend_create(int samp_rate, int n_channels, long max_in, int device, qrl_frontend** out)
 {
     if (!out || n_channels <= 0 || max_in <= 0 || samp_rate < 2000000 || samp_rate % 1000000) { set_err(nullptr, "qrl_frontend_create: bad argument (samp_rate must be a multiple of 1e6, >= 2e6)"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_frontend_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_frontend_create", device)) return rc;
     qrl_frontend* h = new qrl_frontend();
-    h->samp_rate = samp_rate; h->D = samp_rate / 1000000; h->C = n_channels; h->max_in = max_in; h->device = device;
-    auto fail = [&](int rc) { std::string e = h->err; qrl_frontend_destroy(h); g_err = e; return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { set_err(h, "cudaSetDevice failed"); return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { set_err(h, "stream create failed"); return fail(QRL_ECUDA); }
-    h->own_stream = true;
-    int rc = upload_tables(h);
+    h->samp_rate = samp_rate; h->D = samp_rate / 1000000; h->C = n_channels; h->max_in = max_in;
+    auto fail = [&](int rc) { return create_failed(h, qrl_frontend_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
     // gr_demod_base.cpp:1329-1333: low_pass(1, samp_rate, 480000, 100000, BLACKMAN_HARRIS) in rational_resampler_ccf(1, samp_rate / 1e6)
     std::vector<float> taps = low_pass(1, samp_rate, 480000, 100000, WIN_BLACKMAN_HARRIS);
@@ -2996,28 +2824,16 @@ int qrl_frontend_create(int samp_rate, int n_channels, long max_in, int device, 
 int qrl_frontend_set_stream(qrl_frontend* h, void* s)
 {
     if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->own_stream && h->stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (s) h->stream = static_cast<cudaStream_t>(s);
-    else { CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
+    return handle_set_stream(h, s);
 }
 int qrl_frontend_set_carrier_offset(qrl_frontend* h, int channel, double offset_hz)
 {
     // gr_demod_base::set_carrier_offset (:1220-1225): rotator phase increment 2 pi (-offset) / samp_rate at the DEVICE rate
     if (!h || channel >= h->C) return QRL_EINVAL;
     const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(-offset_hz / h->samp_rate * 4294967296.0))));
-    for (int c = 0; c < h->C; c++) {
-        if (channel >= 0 && c != channel) continue;
-        RotState& r = h->rot[c];
-        r.base = r.base + r.inc * static_cast<unsigned>(h->n_in - r.n_base);
-        r.n_base = h->n_in;
-        r.inc = inc;
-    }
-    h->rot_active = false;
-    for (auto& r : h->rot) if (r.inc != 0 || r.base != 0) h->rot_active = true;
-    CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
+    h->rot_active = retune(h->rot, channel, inc, h->n_in);
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
     return QRL_OK;
 }
 int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int on_device, long* n_out)
@@ -3027,12 +2843,12 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     h->n_out_last = 0;
     if (n_out) *n_out = 0;
     if (T == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
     if (!on_device) {
         if (!h->d_in) { int rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_in) * h->C, false); if (rc) return rc; }
-        CK(cudaMemcpy2DAsync(h->d_in, sizeof(float2) * h->max_in, iq, sizeof(float2) * stride, sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpy2DAsync(h->d_in, sizeof(float2) * h->max_in, iq, sizeof(float2) * stride, sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
         x = h->d_in; xstride = h->max_in;
     }
     const long long N = h->n_in + T;
@@ -3040,8 +2856,7 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     const RotState* rs = h->rot_active ? h->d_rot : nullptr;
     if (k1 > k0) {
         const size_t smem = sizeof(float) * ((h->ntaps + 1) & ~1) + sizeof(float2) * (127 * h->D + h->ntaps);
-        static bool attr[16] = { false };
-        if (!attr[h->device & 15]) { CK(cudaFuncSetAttribute(frontend_fir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr[h->device & 15] = true; }
+        if (int rc = smem_opt_in(h, frontend_fir_kernel, 160 * 1024)) return rc;
         if (smem > 160 * 1024) { set_err(h, "qrl_frontend_work: device rate too high for this kernel"); return QRL_EINVAL; }
         dim3 g(static_cast<unsigned>((k1 - k0 + 127) / 128), h->C);
         frontend_fir_kernel<<<g, 128, smem, h->stream>>>(rs, x, xstride, T, h->n_in, h->d_hist[h->hist_cur], h->H, h->d_taps, h->ntaps, h->D,
@@ -3055,7 +2870,7 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     h->n_in = N; h->n1 = k1;
     h->n_out_last = static_cast<long>(k1 - k0);
     if (n_out) *n_out = h->n_out_last;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int qrl_frontend_out_device(qrl_frontend* h, float** data, long* stride, long* n_out)
@@ -3070,8 +2885,8 @@ int qrl_frontend_read(qrl_frontend* h, float* dst, long cap)
 {
     if (!h || !dst) return QRL_EINVAL;
     const long w = std::min(cap, h->n_out_last);
-    if (w > 0) CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * 8, h->d_out, static_cast<size_t>(h->out_stride) * 8, static_cast<size_t>(w) * 8, h->C, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    if (w > 0) QRL_CK(cudaMemcpy2DAsync(dst, static_cast<size_t>(cap) * 8, h->d_out, static_cast<size_t>(h->out_stride) * 8, static_cast<size_t>(w) * 8, h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 long qrl_frontend_launch_count(const qrl_frontend* h) { return h ? h->launches : 0; }
@@ -3117,7 +2932,7 @@ int qrl_fir_decim_ccf_device(const float* taps, int ntaps, int D, const float* x
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     float* d_taps = nullptr;
     HandleBase* h = nullptr;
-    CK(cudaMalloc(&d_taps, sizeof(float) * ntaps));
+    QRL_CK(cudaMalloc(&d_taps, sizeof(float) * ntaps));
     cudaError_t e = cudaMemcpyAsync(d_taps, taps, sizeof(float) * ntaps, cudaMemcpyHostToDevice, st);
     int dev = 0, n_sm = 0;
     if (e == cudaSuccess) e = cudaGetDevice(&dev);
@@ -3168,25 +2983,6 @@ struct qrl_mmdvm_tx : HandleBase {
     ZeroIdle zi;                                   // gr_zero_idle_bursts(0): behind the FM modulator (single) / behind the resampler (multi2)
 };
 
-template <class H> static int mmdvm_destroy(H* h)
-{
-    if (!h) return QRL_OK;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
-}
-template <class H> static int mmdvm_set_stream(H* h, void* s)
-{
-    if (!h) return QRL_EINVAL;
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->own_stream && h->stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (s) h->stream = static_cast<cudaStream_t>(s);
-    else { CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
-}
 static int mmdvm_rows(HandleBase* h, int** d_rows, const int* rows, int C, int n_rows)
 {
     std::vector<int> r(C);
@@ -3202,20 +2998,18 @@ static int mmdvm_rows(HandleBase* h, int** d_rows, const int* rows, int C, int n
 
 extern "C" {
 
-int qrl_mmdvm_rx_destroy(qrl_mmdvm_rx* h) { return mmdvm_destroy(h); }
-int qrl_mmdvm_rx_set_stream(qrl_mmdvm_rx* h, void* s) { return mmdvm_set_stream(h, s); }
+int qrl_mmdvm_rx_destroy(qrl_mmdvm_rx* h) { return h ? handle_close(h) : QRL_OK; }
+int qrl_mmdvm_rx_set_stream(qrl_mmdvm_rx* h, void* s) { return h ? handle_set_stream(h, s) : QRL_EINVAL; }
 int qrl_mmdvm_rx_create(int variant, int n_channels, const int* rows, int n_rows, int filter_width, long max_in, int device, qrl_mmdvm_rx** out)
 {
     if (!out || variant < 0 || variant > 1 || n_channels <= 0 || n_rows < n_channels || max_in <= 0 || filter_width <= 0) { set_err(nullptr, "qrl_mmdvm_rx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_mmdvm_rx_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_mmdvm_rx_create", device)) return rc;
     qrl_mmdvm_rx* h = new qrl_mmdvm_rx();
-    h->C = n_channels; h->n_rows = n_rows; h->max_in = max_in; h->device = device;
-    auto fail = [&](int rc) { std::string e = h->err; qrl_mmdvm_rx_destroy(h); g_err = e; return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { set_err(h, "cudaSetDevice failed"); return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { set_err(h, "stream create failed"); return fail(QRL_ECUDA); }
-    h->own_stream = true;
-    int rc = upload_tables(h);
+    h->C = n_channels; h->n_rows = n_rows; h->max_in = max_in;
+    auto fail = [&](int rc) { return create_failed(h, qrl_mmdvm_rx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
     if ((rc = mmdvm_rows(h, &h->d_rows, rows, h->C, n_rows))) return fail(rc);
     // gr_demod_mmdvm_multi2.cpp:58-62,66,71,76 | gr_demod_mmdvm.cpp:43-52
@@ -3250,13 +3044,13 @@ int qrl_mmdvm_rx_work(qrl_mmdvm_rx* h, const float* iq, long n, long stride, int
     h->n_out_last = 0; h->n_rssi_last = 0;
     if (n_out) *n_out = 0;
     if (n == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
     if (on_device) { int rc = check_device_ptr(h, iq, "qrl_mmdvm_rx_work"); if (rc) return rc; }
     else {
         if (!h->d_in) { int rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_in) * h->n_rows, false); if (rc) return rc; }
-        CK(cudaMemcpy2DAsync(h->d_in, sizeof(float2) * h->max_in, iq, sizeof(float2) * stride, sizeof(float2) * n, h->n_rows, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpy2DAsync(h->d_in, sizeof(float2) * h->max_in, iq, sizeof(float2) * stride, sizeof(float2) * n, h->n_rows, cudaMemcpyHostToDevice, h->stream));
         x = h->d_in; xstride = h->max_in;
     }
     const int TB = 256;
@@ -3290,7 +3084,7 @@ int qrl_mmdvm_rx_work(qrl_mmdvm_rx* h, const float* iq, long n, long stride, int
     h->n_in = N; h->n24 = o1;
     h->n_out_last = static_cast<long>(o1 - o0);
     if (n_out) *n_out = h->n_out_last;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int qrl_mmdvm_rx_out_device(qrl_mmdvm_rx* h, short** data, long* stride, long* n_out, float** rssi_db, long* rssi_stride, int* n_rssi, long long* first_rssi_item)
@@ -3308,34 +3102,39 @@ int qrl_mmdvm_rx_out_device(qrl_mmdvm_rx* h, short** data, long* stride, long* n
 int qrl_mmdvm_rx_read(qrl_mmdvm_rx* h, short* dst, long dst_stride, float* rssi_db, long rssi_cap, int* n_rssi, long long* first_rssi_item)
 {
     if (!h || !dst) return QRL_EINVAL;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     if (h->n_out_last > 0)
-        CK(cudaMemcpy2DAsync(dst, sizeof(short) * dst_stride, h->d_out, sizeof(short) * h->out_stride, sizeof(short) * h->n_out_last, h->C, cudaMemcpyDeviceToHost, h->stream));
+        QRL_CK(cudaMemcpy2DAsync(dst, sizeof(short) * dst_stride, h->d_out, sizeof(short) * h->out_stride, sizeof(short) * h->n_out_last, h->C, cudaMemcpyDeviceToHost, h->stream));
     const int nr = static_cast<int>(std::min<long>(h->n_rssi_last, rssi_cap));
     if (rssi_db && nr > 0)
-        CK(cudaMemcpy2DAsync(rssi_db, sizeof(float) * rssi_cap, h->d_rssi, sizeof(float) * h->rssi_stride, sizeof(float) * nr, h->C, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaMemcpy2DAsync(rssi_db, sizeof(float) * rssi_cap, h->d_rssi, sizeof(float) * h->rssi_stride, sizeof(float) * nr, h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     if (n_rssi) *n_rssi = nr;
     if (first_rssi_item) *first_rssi_item = h->rssi_b0_last * 300 + 299;
     return QRL_OK;
 }
 long qrl_mmdvm_rx_launch_count(qrl_mmdvm_rx* h) { return h ? h->launches : 0; }
 
-int qrl_mmdvm_tx_destroy(qrl_mmdvm_tx* h) { if (h) { cudaSetDevice(h->device); if (h->stream) cudaStreamSynchronize(h->stream); h->zi.release(); } return mmdvm_destroy(h); }
-int qrl_mmdvm_tx_set_stream(qrl_mmdvm_tx* h, void* s) { return mmdvm_set_stream(h, s); }
+int qrl_mmdvm_tx_destroy(qrl_mmdvm_tx* h)
+{
+    if (!h) return QRL_OK;
+    cudaSetDevice(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    h->zi.release();
+    return handle_close(h);
+}
+int qrl_mmdvm_tx_set_stream(qrl_mmdvm_tx* h, void* s) { return h ? handle_set_stream(h, s) : QRL_EINVAL; }
 int qrl_mmdvm_tx_create(int variant, int n_channels, const int* rows, int n_rows, int filter_width, long max_in, int device, qrl_mmdvm_tx** out)
 {
     if (!out || variant < 0 || variant > 1 || n_channels <= 0 || n_rows < n_channels || max_in <= 0 || filter_width <= 0) { set_err(nullptr, "qrl_mmdvm_tx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_mmdvm_tx_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_mmdvm_tx_create", device)) return rc;
     qrl_mmdvm_tx* h = new qrl_mmdvm_tx();
-    h->C = n_channels; h->n_rows = n_rows; h->num_channels = n_channels; h->max_in = max_in; h->device = device;
+    h->C = n_channels; h->n_rows = n_rows; h->num_channels = n_channels; h->max_in = max_in;
     h->zi.init(h->C);
-    auto fail = [&](int rc) { std::string e = h->err; qrl_mmdvm_tx_destroy(h); g_err = e; return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { set_err(h, "cudaSetDevice failed"); return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { set_err(h, "stream create failed"); return fail(QRL_ECUDA); }
-    h->own_stream = true;
-    int rc = upload_tables(h);
+    auto fail = [&](int rc) { return create_failed(h, qrl_mmdvm_tx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
     if ((rc = mmdvm_rows(h, &h->d_rows, rows, h->C, n_rows))) return fail(rc);
     // gr_mod_mmdvm_multi2.cpp:47-50,64,72,80 | gr_mod_mmdvm.cpp:36-45
@@ -3379,12 +3178,12 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
     h->n_out_last = 0;
     if (n_out) *n_out = 0;
     if (n == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     const short* s = in; long long sstride = stride;
     if (on_device) { int rc = check_device_ptr(h, in, "qrl_mmdvm_tx_work"); if (rc) return rc; }
     else {
         if (!h->d_in) { int rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_in) * h->C, false); if (rc) return rc; }
-        CK(cudaMemcpy2DAsync(h->d_in, sizeof(short) * h->max_in, in, sizeof(short) * stride, sizeof(short) * n, h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpy2DAsync(h->d_in, sizeof(short) * h->max_in, in, sizeof(short) * stride, sizeof(short) * n, h->C, cudaMemcpyHostToDevice, h->stream));
         s = h->d_in; sstride = h->max_in;
     }
     const int TB = 256;
@@ -3399,7 +3198,7 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
         std::vector<long long> ranges;
         h->zi.collect(h->C, a0, a1, 0, ranges);
         if (!ranges.empty()) {
-            CK(h->zi.upload(ranges, h->stream));
+            QRL_CK(h->zi.upload(ranges, h->stream));
             tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, h->zi.d_ranges);
             h->launches++;
         }
@@ -3419,7 +3218,7 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
             std::vector<long long> ranges;
             h->zi.collect(h->C, o0, o1, o0, ranges);
             if (!ranges.empty()) {
-                CK(h->zi.upload(ranges, h->stream));
+                QRL_CK(h->zi.upload(ranges, h->stream));
                 tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_lin, 0xffffffffu, h->lin_stride, h->zi.d_ranges);
                 h->launches++;
             }
@@ -3431,7 +3230,7 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
     h->n_in = a1; h->n25 = o1;
     h->n_out_last = static_cast<long>(o1 - o0);
     if (n_out) *n_out = h->n_out_last;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int qrl_mmdvm_tx_out_device(qrl_mmdvm_tx* h, float** data, long* stride, long* n_out)
@@ -3445,10 +3244,10 @@ int qrl_mmdvm_tx_out_device(qrl_mmdvm_tx* h, float** data, long* stride, long* n
 int qrl_mmdvm_tx_read(qrl_mmdvm_tx* h, float* dst, long dst_stride)
 {
     if (!h || !dst) return QRL_EINVAL;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     if (h->n_out_last > 0)
-        CK(cudaMemcpy2DAsync(dst, sizeof(float2) * dst_stride, h->d_out, sizeof(float2) * h->out_stride, sizeof(float2) * h->n_out_last, h->n_rows, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaMemcpy2DAsync(dst, sizeof(float2) * dst_stride, h->d_out, sizeof(float2) * h->out_stride, sizeof(float2) * h->n_out_last, h->n_rows, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 // behind the synthesizer (gr_mod_mmdvm_multi2.cpp:94-96,123-125): multiply_const_cc(1 / num_channels) -> multiply_const_cc(bb_gain), in place
@@ -3456,16 +3255,16 @@ int qrl_mmdvm_tx_finish(qrl_mmdvm_tx* h, float* wideband_dev, long n)
 {
     if (!h || !wideband_dev || n < 0) return QRL_EINVAL;
     if (n == 0) return QRL_OK;
-    CK(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     int rc = check_device_ptr(h, wideband_dev, "qrl_mmdvm_tx_finish"); if (rc) return rc;
     scale2_linear_kernel<<<static_cast<unsigned>(std::min<long>((n + 255) / 256, 4096)), 256, 0, h->stream>>>(
         reinterpret_cast<float2*>(wideband_dev), n, 1.0f / static_cast<float>(h->num_channels), h->bb_gain);
     h->launches++;
-    CK(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
-int qrl_mmdvm_rx_sync(qrl_mmdvm_rx* h) { if (!h) return QRL_EINVAL; CK(cudaStreamSynchronize(h->stream)); return QRL_OK; }
-int qrl_mmdvm_tx_sync(qrl_mmdvm_tx* h) { if (!h) return QRL_EINVAL; CK(cudaStreamSynchronize(h->stream)); return QRL_OK; }
+int qrl_mmdvm_rx_sync(qrl_mmdvm_rx* h) { if (!h) return QRL_EINVAL; QRL_CK(cudaStreamSynchronize(h->stream)); return QRL_OK; }
+int qrl_mmdvm_tx_sync(qrl_mmdvm_tx* h) { if (!h) return QRL_EINVAL; QRL_CK(cudaStreamSynchronize(h->stream)); return QRL_OK; }
 long qrl_mmdvm_tx_launch_count(qrl_mmdvm_tx* h) { return h ? h->launches : 0; }
 
 }  // extern "C"

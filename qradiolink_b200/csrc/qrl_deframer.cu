@@ -23,9 +23,6 @@
 #include <string>
 #include <vector>
 
-extern "C" int qrl_device_count(void);
-void qrl_internal_set_err(const std::string& s);
-
 namespace {
 
 enum : uint32_t { FT_VOICE = 0xED89, FT_VOICE1 = 0xB5, FT_TEXT = 0x89EDAA, FT_IP = 0xDE98AA, FT_VIDEO = 0x98DEAA,
@@ -254,27 +251,12 @@ struct qrl_dfbb : QrlHandleBase {
     int *d_counts = nullptr, *d_stage_counts = nullptr;
 };
 
-#define CKD(call)                                                                                    \
-    do {                                                                                             \
-        cudaError_t e__ = (call);                                                                    \
-        if (e__ != cudaSuccess) {                                                                    \
-            h->err = std::string(#call) + ": " + cudaGetErrorString(e__);                            \
-            qrl_internal_set_err(h->err);                                                            \
-            return QRL_ECUDA;                                                                        \
-        }                                                                                            \
-    } while (0)
-
 extern "C" {
 
 int qrl_deframer_destroy(qrl_deframer* h)
 {
     if (!h) return QRL_EINVAL;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 
 int qrl_deframer_create(int sync_class, int bit_buf_len, int rx_frame_length, int n_channels, long max_bits, int max_frames,
@@ -282,34 +264,25 @@ int qrl_deframer_create(int sync_class, int bit_buf_len, int rx_frame_length, in
 {
     if (!out || sync_class < 1 || sync_class > 4 || bit_buf_len < 16 || (bit_buf_len & 7) || rx_frame_length < 1 || n_channels < 1 ||
         max_bits < 1 || max_frames < 1) {
-        qrl_internal_set_err("qrl_deframer_create: bad argument");
+        set_err(nullptr, "qrl_deframer_create: bad argument");
         return QRL_EINVAL;
     }
     *out = nullptr;
-    if (qrl_device_count() <= device) { qrl_internal_set_err("qrl_deframer_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_deframer_create", device)) return rc;
     qrl_deframer* h = new qrl_deframer();
     h->sync_class = sync_class; h->bit_buf_len = bit_buf_len; h->rx_frame_length = rx_frame_length; h->C = n_channels;
-    h->max_bits = max_bits; h->max_frames = max_frames; h->device = device;
+    h->max_bits = max_bits; h->max_frames = max_frames;
     h->rec_bytes = (8 + bit_buf_len / 8 + 7) & ~7;
-    auto fail = [&](int rc, const char* what) { qrl_internal_set_err(what); qrl_deframer_destroy(h); return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) return fail(QRL_ECUDA, "cudaSetDevice failed");
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return fail(QRL_ECUDA, "stream create failed");
-    h->own_stream = true;
-    auto alloc = [&](void** p, size_t bytes) {
-        if (cudaMalloc(p, std::max<size_t>(bytes, 16)) != cudaSuccess) return false;
-        h->allocs.push_back(*p);
-        return cudaMemsetAsync(*p, 0, std::max<size_t>(bytes, 16), h->stream) == cudaSuccess;
-    };
+    auto fail = [&](int rc) { return create_failed(h, qrl_deframer_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (rc) return fail(rc);
     const size_t C = static_cast<size_t>(n_channels);
-    if (!alloc(reinterpret_cast<void**>(&h->d_state), C * sizeof(DeframerState)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_bit_buf), C * bit_buf_len) ||
-        !alloc(reinterpret_cast<void**>(&h->d_records), C * max_frames * h->rec_bytes) ||
-        !alloc(reinterpret_cast<void**>(&h->d_counts), C * sizeof(int)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_stage), C * static_cast<size_t>(max_bits)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_stage_counts), C * sizeof(int)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_dropped), C * sizeof(int)))
-        return fail(QRL_ENOMEM, "qrl_deframer_create: device allocation failed");
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(QRL_ECUDA, "create sync failed");
+    if ((rc = dev_alloc(h, &h->d_state, C)) || (rc = dev_alloc(h, &h->d_bit_buf, C * bit_buf_len)) ||
+        (rc = dev_alloc(h, &h->d_records, C * max_frames * h->rec_bytes)) || (rc = dev_alloc(h, &h->d_counts, C)) ||
+        (rc = dev_alloc(h, &h->d_stage, C * static_cast<size_t>(max_bits))) || (rc = dev_alloc(h, &h->d_stage_counts, C)) ||
+        (rc = dev_alloc(h, &h->d_dropped, C)))
+        return fail(rc);
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
 }
@@ -317,23 +290,19 @@ int qrl_deframer_create(int sync_class, int bit_buf_len, int rx_frame_length, in
 int qrl_deframer_set_stream(qrl_deframer* h, void* cuda_stream)
 {
     if (!h) return QRL_EINVAL;
-    CKD(cudaStreamSynchronize(h->stream));
-    if (h->own_stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (cuda_stream) h->stream = static_cast<cudaStream_t>(cuda_stream);
-    else { CKD(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }     // NULL = back to an own stream
-    return QRL_OK;
+    return handle_set_stream(h, cuda_stream);
 }
 
 int qrl_deframer_work(qrl_deframer* h, const unsigned char* bits, const int* counts, long stride, int on_device)
 {
-    if (!h || !bits || !counts || stride < 0) { qrl_internal_set_err("qrl_deframer_work: bad argument"); return QRL_EINVAL; }
-    CKD(cudaSetDevice(h->device));
+    if (!h || !bits || !counts || stride < 0) { set_err(nullptr, "qrl_deframer_work: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
     const unsigned char* d_bits = bits; const int* d_cnt = counts; long long d_stride = stride;
     if (!on_device) {
-        if (stride > h->max_bits) { qrl_internal_set_err("qrl_deframer_work: stride exceeds max_bits"); return QRL_ERANGE; }
-        for (int c = 0; c < h->C; c++) if (counts[c] < 0 || counts[c] > stride) { qrl_internal_set_err("qrl_deframer_work: bad count"); return QRL_ERANGE; }
-        CKD(cudaMemcpyAsync(h->d_stage, bits, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
-        CKD(cudaMemcpyAsync(h->d_stage_counts, counts, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
+        if (stride > h->max_bits) { set_err(nullptr, "qrl_deframer_work: stride exceeds max_bits"); return QRL_ERANGE; }
+        for (int c = 0; c < h->C; c++) if (counts[c] < 0 || counts[c] > stride) { set_err(nullptr, "qrl_deframer_work: bad count"); return QRL_ERANGE; }
+        QRL_CK(cudaMemcpyAsync(h->d_stage, bits, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage_counts, counts, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
         d_bits = h->d_stage; d_cnt = h->d_stage_counts;
     }
     const int warps_per_block = 4;
@@ -341,29 +310,27 @@ int qrl_deframer_work(qrl_deframer* h, const unsigned char* bits, const int* cou
         h->C, h->sync_class, h->bit_buf_len, h->rx_frame_length, d_bits, d_stride, d_cnt, 0, nullptr, nullptr,
         h->d_state, h->d_bit_buf, h->d_records, h->rec_bytes, h->max_frames, h->d_counts, h->d_dropped);
     h->launches++;
-    CKD(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
 int qrl_deframer_work2(qrl_deframer* h, const unsigned char* bits_a, const int* counts_a, const unsigned char* bits_b, const int* counts_b,
                        long stride, int on_device)
 {
-    if (!h || !bits_a || !counts_a || !bits_b || !counts_b || stride < 0) { qrl_internal_set_err("qrl_deframer_work2: bad argument"); return QRL_EINVAL; }
-    CKD(cudaSetDevice(h->device));
+    if (!h || !bits_a || !counts_a || !bits_b || !counts_b || stride < 0) { set_err(nullptr, "qrl_deframer_work2: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
     const unsigned char *da = bits_a, *db = bits_b; const int *ca = counts_a, *cb = counts_b;
     if (!on_device) {
-        if (stride > h->max_bits) { qrl_internal_set_err("qrl_deframer_work2: stride exceeds max_bits"); return QRL_ERANGE; }
+        if (stride > h->max_bits) { set_err(nullptr, "qrl_deframer_work2: stride exceeds max_bits"); return QRL_ERANGE; }
         if (!h->d_stage2) {
-            void* p = nullptr;
-            if (cudaMalloc(&p, static_cast<size_t>(h->C) * h->max_bits) != cudaSuccess) { qrl_internal_set_err("qrl_deframer_work2: allocation failed"); return QRL_ENOMEM; }
-            h->allocs.push_back(p); h->d_stage2 = static_cast<unsigned char*>(p);
-            if (cudaMalloc(&p, sizeof(int) * h->C) != cudaSuccess) { qrl_internal_set_err("qrl_deframer_work2: allocation failed"); return QRL_ENOMEM; }
-            h->allocs.push_back(p); h->d_stage_counts2 = static_cast<int*>(p);
+            int rc;
+            if ((rc = dev_alloc(h, &h->d_stage2, static_cast<size_t>(h->C) * h->max_bits, false)) ||
+                (rc = dev_alloc(h, &h->d_stage_counts2, h->C, false))) return rc;
         }
-        CKD(cudaMemcpyAsync(h->d_stage, bits_a, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
-        CKD(cudaMemcpyAsync(h->d_stage_counts, counts_a, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
-        CKD(cudaMemcpyAsync(h->d_stage2, bits_b, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
-        CKD(cudaMemcpyAsync(h->d_stage_counts2, counts_b, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage, bits_a, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage_counts, counts_a, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage2, bits_b, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage_counts2, counts_b, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
         da = h->d_stage; ca = h->d_stage_counts; db = h->d_stage2; cb = h->d_stage_counts2;
     }
     const int warps_per_block = 4;
@@ -371,16 +338,16 @@ int qrl_deframer_work2(qrl_deframer* h, const unsigned char* bits_a, const int* 
         h->C, h->sync_class, h->bit_buf_len, h->rx_frame_length, da, stride, ca, 0, db, cb,
         h->d_state, h->d_bit_buf, h->d_records, h->rec_bytes, h->max_frames, h->d_counts, h->d_dropped);
     h->launches++;
-    CKD(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
 int qrl_deframer_dropped(qrl_deframer* h, int* dropped_host)
 {
     if (!h || !dropped_host) return QRL_EINVAL;
-    CKD(cudaSetDevice(h->device));
-    CKD(cudaMemcpyAsync(dropped_host, h->d_dropped, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
-    CKD(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpyAsync(dropped_host, h->d_dropped, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 
@@ -389,16 +356,16 @@ int qrl_deframer_record_bytes(qrl_deframer* h) { return h ? h->rec_bytes : 0; }
 int qrl_deframer_read(qrl_deframer* h, unsigned char* records_host, int* frame_counts_host, int* modem_sync_host)
 {
     if (!h || !frame_counts_host) return QRL_EINVAL;
-    CKD(cudaSetDevice(h->device));
-    CKD(cudaMemcpyAsync(frame_counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpyAsync(frame_counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
     if (records_host)
-        CKD(cudaMemcpyAsync(records_host, h->d_records, static_cast<size_t>(h->C) * h->max_frames * h->rec_bytes, cudaMemcpyDeviceToHost, h->stream));
+        QRL_CK(cudaMemcpyAsync(records_host, h->d_records, static_cast<size_t>(h->C) * h->max_frames * h->rec_bytes, cudaMemcpyDeviceToHost, h->stream));
     std::vector<DeframerState> st;
     if (modem_sync_host) {
         st.resize(h->C);
-        CKD(cudaMemcpyAsync(st.data(), h->d_state, sizeof(DeframerState) * h->C, cudaMemcpyDeviceToHost, h->stream));
+        QRL_CK(cudaMemcpyAsync(st.data(), h->d_state, sizeof(DeframerState) * h->C, cudaMemcpyDeviceToHost, h->stream));
     }
-    CKD(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     if (modem_sync_host) for (int c = 0; c < h->C; c++) modem_sync_host[c] = st[c].modem_sync;
     return QRL_OK;
 }
@@ -414,7 +381,7 @@ int qrl_deframer_out_device(qrl_deframer* h, void** records, int** frame_counts)
 int qrl_deframer_sync(qrl_deframer* h)
 {
     if (!h) return QRL_EINVAL;
-    CKD(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 
@@ -425,10 +392,10 @@ int qrl_frame_build(int n_channels, const unsigned char* payload, long payload_s
                     int one_k_mode, int burst_ip, unsigned char* out, long out_stride, int* out_len, int on_device, int device, void* cuda_stream)
 {
     if (n_channels < 1 || !payload || !payload_len || !frame_type || !out || !out_len || payload_stride < 0 || out_stride < 1) {
-        qrl_internal_set_err("qrl_frame_build: bad argument"); return QRL_EINVAL;
+        set_err(nullptr, "qrl_frame_build: bad argument"); return QRL_EINVAL;
     }
-    if (qrl_device_count() <= device) { qrl_internal_set_err("qrl_frame_build: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
-    auto ck = [](cudaError_t e, const char* what) { if (e != cudaSuccess) { qrl_internal_set_err(std::string(what) + ": " + cudaGetErrorString(e)); return false; } return true; };
+    if (qrl_device_count() <= device) { set_err(nullptr, "qrl_frame_build: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    auto ck = [](cudaError_t e, const char* what) { if (e != cudaSuccess) { set_err(nullptr, std::string(what) + ": " + cudaGetErrorString(e)); return false; } return true; };
     if (!ck(cudaSetDevice(device), "cudaSetDevice")) return QRL_ECUDA;
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     if (on_device) {
@@ -454,40 +421,27 @@ int qrl_frame_build(int n_channels, const unsigned char* payload, long payload_s
 int qrl_dfbb_destroy(qrl_dfbb* h)
 {
     if (!h) return QRL_EINVAL;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 
 int qrl_dfbb_create(int modem_type, int n_channels, long max_bits, int device, qrl_dfbb** out)
 {
-    if (!out || modem_type < 1 || modem_type > 3 || n_channels < 1 || max_bits < 1) { qrl_internal_set_err("qrl_dfbb_create: bad argument"); return QRL_EINVAL; }
+    if (!out || modem_type < 1 || modem_type > 3 || n_channels < 1 || max_bits < 1) { set_err(nullptr, "qrl_dfbb_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
-    if (qrl_device_count() <= device) { qrl_internal_set_err("qrl_dfbb_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_dfbb_create", device)) return rc;
     qrl_dfbb* h = new qrl_dfbb();
     h->type = modem_type; h->len = modem_type == 1 ? 64 : (modem_type == 2 ? 32 : 384);      // gr_deframer_bb.cpp:36-47
-    h->C = n_channels; h->max_bits = max_bits; h->device = device;
+    h->C = n_channels; h->max_bits = max_bits;
     h->out_stride = max_bits + 32;          // a call emits at most its input plus one sync word whose last bit just arrived
-    auto fail = [&](int rc, const char* what) { qrl_internal_set_err(what); qrl_dfbb_destroy(h); return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) return fail(QRL_ECUDA, "cudaSetDevice failed");
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) return fail(QRL_ECUDA, "stream create failed");
-    h->own_stream = true;
-    auto alloc = [&](void** p, size_t bytes) {
-        if (cudaMalloc(p, std::max<size_t>(bytes, 16)) != cudaSuccess) return false;
-        h->allocs.push_back(*p);
-        return cudaMemsetAsync(*p, 0, std::max<size_t>(bytes, 16), h->stream) == cudaSuccess;
-    };
+    auto fail = [&](int rc) { return create_failed(h, qrl_dfbb_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (rc) return fail(rc);
     const size_t C = static_cast<size_t>(n_channels);
-    if (!alloc(reinterpret_cast<void**>(&h->d_state), C * sizeof(DfbbState)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_out), C * static_cast<size_t>(h->out_stride)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_counts), C * sizeof(int)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_stage), C * static_cast<size_t>(max_bits)) ||
-        !alloc(reinterpret_cast<void**>(&h->d_stage_counts), C * sizeof(int)))
-        return fail(QRL_ENOMEM, "qrl_dfbb_create: device allocation failed");
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) return fail(QRL_ECUDA, "create sync failed");
+    if ((rc = dev_alloc(h, &h->d_state, C)) || (rc = dev_alloc(h, &h->d_out, C * static_cast<size_t>(h->out_stride))) ||
+        (rc = dev_alloc(h, &h->d_counts, C)) || (rc = dev_alloc(h, &h->d_stage, C * static_cast<size_t>(max_bits))) ||
+        (rc = dev_alloc(h, &h->d_stage_counts, C)))
+        return fail(rc);
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
 }
@@ -495,30 +449,26 @@ int qrl_dfbb_create(int modem_type, int n_channels, long max_bits, int device, q
 int qrl_dfbb_set_stream(qrl_dfbb* h, void* cuda_stream)
 {
     if (!h) return QRL_EINVAL;
-    CKD(cudaStreamSynchronize(h->stream));
-    if (h->own_stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (cuda_stream) h->stream = static_cast<cudaStream_t>(cuda_stream);
-    else { CKD(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
+    return handle_set_stream(h, cuda_stream);
 }
 
 int qrl_dfbb_work(qrl_dfbb* h, const unsigned char* bits, const int* counts, long stride, int on_device)
 {
-    if (!h || !bits || !counts || stride < 0) { qrl_internal_set_err("qrl_dfbb_work: bad argument"); return QRL_EINVAL; }
-    CKD(cudaSetDevice(h->device));
+    if (!h || !bits || !counts || stride < 0) { set_err(nullptr, "qrl_dfbb_work: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
     const unsigned char* d_bits = bits; const int* d_cnt = counts;
-    if (stride > h->max_bits) { qrl_internal_set_err("qrl_dfbb_work: stride exceeds max_bits"); return QRL_ERANGE; }
+    if (stride > h->max_bits) { set_err(nullptr, "qrl_dfbb_work: stride exceeds max_bits"); return QRL_ERANGE; }
     if (!on_device) {
-        for (int c = 0; c < h->C; c++) if (counts[c] < 0 || counts[c] > stride) { qrl_internal_set_err("qrl_dfbb_work: bad count"); return QRL_ERANGE; }
-        CKD(cudaMemcpyAsync(h->d_stage, bits, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
-        CKD(cudaMemcpyAsync(h->d_stage_counts, counts, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
+        for (int c = 0; c < h->C; c++) if (counts[c] < 0 || counts[c] > stride) { set_err(nullptr, "qrl_dfbb_work: bad count"); return QRL_ERANGE; }
+        QRL_CK(cudaMemcpyAsync(h->d_stage, bits, static_cast<size_t>(h->C) * stride, cudaMemcpyHostToDevice, h->stream));
+        QRL_CK(cudaMemcpyAsync(h->d_stage_counts, counts, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
         d_bits = h->d_stage; d_cnt = h->d_stage_counts;
     }
     const int warps_per_block = 4;
     dfbb_kernel<<<(h->C + warps_per_block - 1) / warps_per_block, 32 * warps_per_block, 0, h->stream>>>(
         h->C, h->type, h->len, d_bits, stride, d_cnt, h->d_state, h->d_out, h->out_stride, h->d_counts);
     h->launches++;
-    CKD(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -534,19 +484,19 @@ int qrl_dfbb_out_device(qrl_dfbb* h, void** bits, long* stride, int** counts)
 int qrl_dfbb_read(qrl_dfbb* h, unsigned char* out_host, long cap, int* counts_host)
 {
     if (!h || !counts_host) return QRL_EINVAL;
-    CKD(cudaSetDevice(h->device));
-    CKD(cudaMemcpyAsync(counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpyAsync(counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
     if (out_host && cap > 0)
-        CKD(cudaMemcpy2DAsync(out_host, static_cast<size_t>(cap), h->d_out, static_cast<size_t>(h->out_stride), static_cast<size_t>(std::min(cap, h->out_stride)), h->C,
+        QRL_CK(cudaMemcpy2DAsync(out_host, static_cast<size_t>(cap), h->d_out, static_cast<size_t>(h->out_stride), static_cast<size_t>(std::min(cap, h->out_stride)), h->C,
                               cudaMemcpyDeviceToHost, h->stream));
-    CKD(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 
 int qrl_dfbb_sync(qrl_dfbb* h)
 {
     if (!h) return QRL_EINVAL;
-    CKD(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 

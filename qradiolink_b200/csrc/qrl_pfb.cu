@@ -25,9 +25,6 @@
 #include <string>
 #include <vector>
 
-extern "C" int qrl_device_count(void);
-void qrl_internal_set_err(const std::string& s);      // qrl_b200.cu: thread-local last error read by qrl_last_error(NULL)
-
 using namespace qrl;
 
 namespace {
@@ -301,16 +298,6 @@ __global__ void pfb_synth_tail_kernel(int M, int hl, const float2* __restrict__ 
     dst[i] = n < 0 ? hist[c * hl + hl + n] : in[c * in_stride + n];
 }
 
-#define CKP(call)                                                                                    \
-    do {                                                                                             \
-        cudaError_t e__ = (call);                                                                    \
-        if (e__ != cudaSuccess) {                                                                    \
-            h->err = std::string(#call) + ": " + cudaGetErrorString(e__);                            \
-            qrl_internal_set_err(h->err);                                                            \
-            return QRL_ECUDA;                                                                        \
-        }                                                                                            \
-    } while (0)
-
 }  // namespace
 
 struct qrl_pfb : QrlHandleBase {        // err / device / stream / launches / allocs: qrl_handle.hpp
@@ -326,16 +313,6 @@ struct qrl_pfb : QrlHandleBase {        // err / device / stream / launches / al
 };
 
 namespace {
-template <class T> int pfb_alloc(qrl_pfb* h, T** p, size_t n, bool zero = true)
-{
-    void* q = nullptr;
-    const size_t bytes = std::max<size_t>(n * sizeof(T), 16);
-    if (cudaMalloc(&q, bytes) != cudaSuccess) { h->err = "cudaMalloc failed"; qrl_internal_set_err(h->err); return QRL_ENOMEM; }
-    if (zero && cudaMemsetAsync(q, 0, bytes, h->stream) != cudaSuccess) { h->err = "cudaMemset failed"; qrl_internal_set_err(h->err); return QRL_ECUDA; }
-    h->allocs.push_back(q);
-    *p = static_cast<T*>(q);
-    return QRL_OK;
-}
 constexpr int kFastM = 10, kFastTpf = 35, kChanR = 9, kChanG = 32, kSynR = 10, kSynG = 32;
 long long chan_hist_len(int tpf, int M, int pend) { return (static_cast<long long>(tpf - 1) * M + pend + 2) & ~1LL; }
 }  // namespace
@@ -345,29 +322,23 @@ extern "C" {
 int qrl_pfb_destroy(qrl_pfb* h)
 {
     if (!h) return QRL_EINVAL;
-    cudaSetDevice(h->device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 
 int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, int device, qrl_pfb** out)
 {
     if (!out || !taps || (kind != QRL_PFB_CHANNELIZER && kind != QRL_PFB_SYNTHESIZER) || M < 1 || M > 64 || ntaps < 1 ||
         max_in < 1 || (ntaps + M - 1) / M > 128) {
-        qrl_internal_set_err("qrl_pfb_create: bad argument");
+        set_err(nullptr, "qrl_pfb_create: bad argument");
         return QRL_EINVAL;
     }
     *out = nullptr;
-    if (qrl_device_count() <= device) { qrl_internal_set_err("qrl_pfb_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_pfb_create", device)) return rc;
     qrl_pfb* h = new qrl_pfb();
-    h->kind = kind; h->M = M; h->tpf = (ntaps + M - 1) / M; h->max_in = max_in; h->device = device;
-    auto fail = [&](int rc) { std::string e = h->err; qrl_pfb_destroy(h); qrl_internal_set_err(e); return rc; };
-    if (cudaSetDevice(device) != cudaSuccess) { h->err = "cudaSetDevice failed"; return fail(QRL_ECUDA); }
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { h->err = "stream create failed"; return fail(QRL_ECUDA); }
-    h->own_stream = true;
+    h->kind = kind; h->M = M; h->tpf = (ntaps + M - 1) / M; h->max_in = max_in;
+    auto fail = [&](int rc) { return create_failed(h, qrl_pfb_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (rc) return fail(rc);
     // branch taps [M][tpf] (polyphase_filterbank::set_taps: filter k holds taps[k + t*M], zero padded) and twiddles
     std::vector<float> bt(static_cast<size_t>(M) * h->tpf, 0.0f), w(static_cast<size_t>(M) * 2);
     for (int j = 0; j < ntaps; j++) bt[static_cast<size_t>(j % M) * h->tpf + j / M] = taps[j];
@@ -375,27 +346,24 @@ int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, i
         const double a = 2.0 * 3.14159265358979323846 * static_cast<double>(q) / static_cast<double>(M);
         w[2 * q] = static_cast<float>(std::cos(a)); w[2 * q + 1] = static_cast<float>(std::sin(a));
     }
-    int rc;
-    if ((rc = pfb_alloc(h, &h->d_bt, bt.size(), false)) || (rc = pfb_alloc(h, &h->d_w, w.size(), false))) return fail(rc);
-    if (cudaMemcpyAsync(h->d_bt, bt.data(), bt.size() * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess ||
-        cudaMemcpyAsync(h->d_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice, h->stream) != cudaSuccess) { h->err = "tap upload failed"; return fail(QRL_ECUDA); }
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->err = "tap upload sync failed"; return fail(QRL_ECUDA); }
+    if ((rc = dev_alloc(h, &h->d_bt, bt.size(), false)) || (rc = dev_alloc(h, &h->d_w, w.size(), false)) ||
+        (rc = upload_state(h, h->d_bt, bt.data(), bt.size() * 4)) || (rc = upload_state(h, h->d_w, w.data(), w.size() * 4))) return fail(rc);
     h->fast = (M == kFastM && h->tpf == kFastTpf);
     if (kind == QRL_PFB_CHANNELIZER) {
         const size_t hcap = static_cast<size_t>(h->tpf) * M + 4;
-        if ((rc = pfb_alloc(h, &h->d_hist[0], hcap)) || (rc = pfb_alloc(h, &h->d_hist[1], hcap))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_hist[0], hcap)) || (rc = dev_alloc(h, &h->d_hist[1], hcap))) return fail(rc);
         h->pend = 0; h->hist_len = chan_hist_len(h->tpf, M, 0);
         h->out_stride = (max_in + M - 1) / M + 2;
-        if ((rc = pfb_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * M))) return fail(rc);
-        if ((rc = pfb_alloc(h, &h->d_stage, static_cast<size_t>(max_in)))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * M))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_stage, static_cast<size_t>(max_in)))) return fail(rc);
     } else {
         const size_t hl = static_cast<size_t>(std::max(1, h->tpf - 1)) * M;
-        if ((rc = pfb_alloc(h, &h->d_hist[0], hl)) || (rc = pfb_alloc(h, &h->d_hist[1], hl))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_hist[0], hl)) || (rc = dev_alloc(h, &h->d_hist[1], hl))) return fail(rc);
         h->out_stride = max_in * M;
-        if ((rc = pfb_alloc(h, &h->d_out, static_cast<size_t>(max_in) * M))) return fail(rc);
-        if ((rc = pfb_alloc(h, &h->d_stage, static_cast<size_t>(max_in) * M))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(max_in) * M))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_stage, static_cast<size_t>(max_in) * M))) return fail(rc);
     }
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { h->err = "create sync failed"; return fail(QRL_ECUDA); }
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
 }
@@ -403,24 +371,21 @@ int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, i
 int qrl_pfb_set_stream(qrl_pfb* h, void* cuda_stream)
 {
     if (!h) return QRL_EINVAL;
-    if (!cuda_stream) return QRL_OK;
-    CKP(cudaStreamSynchronize(h->stream));
-    if (h->own_stream) cudaStreamDestroy(h->stream);
-    h->stream = static_cast<cudaStream_t>(cuda_stream); h->own_stream = false;
-    return QRL_OK;
+    if (!cuda_stream) return QRL_OK;       // unlike the other handle types: NULL keeps the current stream
+    return handle_set_stream(h, cuda_stream);
 }
 
 int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_on_device, long* n_out)
 {
-    if (!h || (!in && n_in > 0) || n_in < 0 || n_in > h->max_in) { qrl_internal_set_err("qrl_pfb_work: bad argument"); return QRL_EINVAL; }
-    CKP(cudaSetDevice(h->device));
+    if (!h || (!in && n_in > 0) || n_in < 0 || n_in > h->max_in) { set_err(nullptr, "qrl_pfb_work: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
     const int M = h->M, tpf = h->tpf;
     const float2* hist = h->d_hist[h->hist_cur];
     float2* hist_next = h->d_hist[h->hist_cur ^ 1];
     if (h->kind == QRL_PFB_CHANNELIZER) {
         const float2* x = static_cast<const float2*>(in);
         if (!in_on_device && n_in > 0) {
-            CKP(cudaMemcpyAsync(h->d_stage, in, sizeof(float2) * n_in, cudaMemcpyHostToDevice, h->stream));
+            QRL_CK(cudaMemcpyAsync(h->d_stage, in, sizeof(float2) * n_in, cudaMemcpyHostToDevice, h->stream));
             x = h->d_stage;
         }
         const long long frames = (static_cast<long long>(h->pend) + n_in) / M;
@@ -429,8 +394,7 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                 constexpr int TM = kChanR * kChanG, SPAN = (TM + kFastTpf - 1) * kFastM, SPANP = (SPAN + 3) & ~1;
                 const size_t smem = sizeof(float2) * (SPANP + kFastM * (TM + 1));
                 auto kern = pfb_chan_kernel<kFastM, kFastTpf, kChanR, kChanG>;
-                static bool attr[16] = { false };    // per device: function attributes belong to the device's context
-                if (!attr[h->device & 15]) { CKP(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); attr[h->device & 15] = true; }
+                if (int rc = smem_opt_in(h, kern, static_cast<int>(smem))) return rc;
                 const int use_tma = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
                 kern<<<static_cast<unsigned>((frames + TM - 1) / TM), kFastM * kChanG, smem, h->stream>>>(
                     h->d_bt, h->d_w, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames,
@@ -456,7 +420,7 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
         const float2* x = static_cast<const float2*>(in);
         long long stride = in_stride;
         if (!in_on_device && n_in > 0) {
-            CKP(cudaMemcpy2DAsync(h->d_stage, sizeof(float2) * n_in, in, sizeof(float2) * in_stride, sizeof(float2) * n_in, M,
+            QRL_CK(cudaMemcpy2DAsync(h->d_stage, sizeof(float2) * n_in, in, sizeof(float2) * in_stride, sizeof(float2) * n_in, M,
                                   cudaMemcpyHostToDevice, h->stream));
             x = h->d_stage; stride = n_in;
         }
@@ -466,8 +430,7 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                 constexpr int TN = kSynR * kSynG, COLS = TN + kFastTpf - 1, VP = COLS | 1;
                 const size_t smem = sizeof(float2) * (kFastM * COLS + kFastM * VP);
                 auto kern = pfb_synth_kernel<kFastM, kFastTpf, kSynR, kSynG>;
-                static bool attr[16] = { false };    // per device: function attributes belong to the device's context
-                if (!attr[h->device & 15]) { CKP(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); attr[h->device & 15] = true; }
+                if (int rc = smem_opt_in(h, kern, static_cast<int>(smem))) return rc;
                 kern<<<static_cast<unsigned>((n_in + TN - 1) / TN), kFastM * kSynG, smem, h->stream>>>(
                     h->d_bt, h->d_w, hist, x, stride, n_in, h->d_out);
             } else {
@@ -485,14 +448,14 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
         h->out_items = static_cast<long long>(n_in) * M;
         if (n_out) *n_out = static_cast<long>(h->out_items);
     }
-    CKP(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
 int qrl_pfb_sync(qrl_pfb* h)
 {
     if (!h) return QRL_EINVAL;
-    CKP(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 
@@ -508,15 +471,15 @@ int qrl_pfb_out_device(qrl_pfb* h, void** data, long* stride, long* items)
 int qrl_pfb_read(qrl_pfb* h, void* host_dst, long dst_stride)
 {
     if (!h || !host_dst) return QRL_EINVAL;
-    CKP(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     if (h->out_items > 0) {
         if (h->kind == QRL_PFB_CHANNELIZER)
-            CKP(cudaMemcpy2DAsync(host_dst, sizeof(float2) * dst_stride, h->d_out, sizeof(float2) * h->out_stride,
+            QRL_CK(cudaMemcpy2DAsync(host_dst, sizeof(float2) * dst_stride, h->d_out, sizeof(float2) * h->out_stride,
                                   sizeof(float2) * h->out_items, h->M, cudaMemcpyDeviceToHost, h->stream));
         else
-            CKP(cudaMemcpyAsync(host_dst, h->d_out, sizeof(float2) * h->out_items, cudaMemcpyDeviceToHost, h->stream));
+            QRL_CK(cudaMemcpyAsync(host_dst, h->d_out, sizeof(float2) * h->out_items, cudaMemcpyDeviceToHost, h->stream));
     }
-    CKP(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     return QRL_OK;
 }
 

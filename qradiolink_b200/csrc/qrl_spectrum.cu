@@ -27,9 +27,6 @@
 #include <string>
 #include <vector>
 
-extern "C" int qrl_device_count(void);
-void qrl_internal_set_err(const std::string& s);
-
 namespace {
 
 constexpr int kCols = 16;       // columns (pass A) / rows (pass B) per CTA
@@ -143,16 +140,6 @@ struct qrl_spectrum : QrlHandleBase {
     float *d_window = nullptr, *d_points = nullptr;
 };
 
-#define CKS(call)                                                                                    \
-    do {                                                                                             \
-        cudaError_t e__ = (call);                                                                    \
-        if (e__ != cudaSuccess) {                                                                    \
-            h->err = std::string(#call) + ": " + cudaGetErrorString(e__);                            \
-            qrl_internal_set_err(h->err);                                                            \
-            return QRL_ECUDA;                                                                        \
-        }                                                                                            \
-    } while (0)
-
 namespace {
 void spectrum_free_buffers(qrl_spectrum* h)
 {
@@ -165,15 +152,15 @@ int spectrum_alloc_buffers(qrl_spectrum* h, int n)
     int lb = 0; while ((1 << lb) < n) lb++;
     h->N = n; h->LB1 = lb / 2; h->LB2 = lb - h->LB1; h->N1 = 1 << h->LB1; h->N2 = 1 << h->LB2;
     const size_t items = static_cast<size_t>(n) * h->S;
-    CKS(cudaMalloc(&h->d_buf, sizeof(float2) * items));
-    CKS(cudaMalloc(&h->d_work, sizeof(float2) * items));
-    CKS(cudaMalloc(&h->d_points, sizeof(float) * items));
-    CKS(cudaMalloc(&h->d_window, sizeof(float) * n));
-    CKS(cudaMemsetAsync(h->d_buf, 0, sizeof(float2) * items, h->stream));
-    CKS(cudaMemsetAsync(h->d_points, 0, sizeof(float) * items, h->stream));
+    QRL_CK(cudaMalloc(&h->d_buf, sizeof(float2) * items));
+    QRL_CK(cudaMalloc(&h->d_work, sizeof(float2) * items));
+    QRL_CK(cudaMalloc(&h->d_points, sizeof(float) * items));
+    QRL_CK(cudaMalloc(&h->d_window, sizeof(float) * n));
+    QRL_CK(cudaMemsetAsync(h->d_buf, 0, sizeof(float2) * items, h->stream));
+    QRL_CK(cudaMemsetAsync(h->d_points, 0, sizeof(float) * items, h->stream));
     const std::vector<float> w = qrl::window_build(h->win, n);          // gr::filter::firdes::window(type, N, 6.76) (rx_fft.cpp:181)
-    CKS(cudaMemcpyAsync(h->d_window, w.data(), sizeof(float) * n, cudaMemcpyHostToDevice, h->stream));
-    CKS(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaMemcpyAsync(h->d_window, w.data(), sizeof(float) * n, cudaMemcpyHostToDevice, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     h->counter = 0; h->data_ready = false;
     return QRL_OK;
 }
@@ -183,26 +170,21 @@ extern "C" {
 
 int qrl_spectrum_create(int fft_size, int window_type, int n_streams, long max_samples, int device, qrl_spectrum** out)
 {
-    if (!out || n_streams <= 0 || max_samples <= 0) { qrl_internal_set_err("qrl_spectrum_create: bad argument"); return QRL_EINVAL; }
+    if (!out || n_streams <= 0 || max_samples <= 0) { set_err(nullptr, "qrl_spectrum_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
     if (fft_size < 256 || fft_size > 65536 || (fft_size & (fft_size - 1))) {
-        qrl_internal_set_err("qrl_spectrum_create: fft_size must be a power of two in [256, 65536]"); return QRL_EINVAL;
+        set_err(nullptr, "qrl_spectrum_create: fft_size must be a power of two in [256, 65536]"); return QRL_EINVAL;
     }
     if (window_type < 0 || window_type > 7) window_type = qrl::WIN_HAMMING;           // rx_fft.cpp:176-179
     if (window_type == qrl::WIN_KAISER || window_type > qrl::WIN_BLACKMAN_HARRIS) {
-        qrl_internal_set_err("qrl_spectrum_create: window type not built (Hamming, Hann, Blackman, rectangular, Blackman-Harris are)"); return QRL_EINVAL;
+        set_err(nullptr, "qrl_spectrum_create: window type not built (Hamming, Hann, Blackman, rectangular, Blackman-Harris are)"); return QRL_EINVAL;
     }
-    if (qrl_device_count() <= device) { qrl_internal_set_err("qrl_spectrum_create: no CUDA device (this library has no CPU fallback)"); return QRL_ENODEV; }
+    if (int rc = check_device("qrl_spectrum_create", device)) return rc;
     qrl_spectrum* h = new qrl_spectrum;
-    h->device = device; h->S = n_streams; h->win = window_type; h->max_samples = max_samples;
-    auto fail = [&](int rc) { std::string e = h->err; spectrum_free_buffers(h); if (h->d_stage) cudaFree(h->d_stage);
-                              if (h->own_stream && h->stream) cudaStreamDestroy(h->stream); delete h; qrl_internal_set_err(e); return rc; };
-    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        h->err = "qrl_spectrum_create: cannot create a stream"; return fail(QRL_ECUDA);
-    }
-    h->own_stream = true;
-    int rc = spectrum_alloc_buffers(h, fft_size);
-    if (rc) return fail(rc);
+    h->S = n_streams; h->win = window_type; h->max_samples = max_samples;
+    int rc = handle_open(h, device);
+    if (!rc) rc = spectrum_alloc_buffers(h, fft_size);
+    if (rc) return create_failed(h, qrl_spectrum_destroy, rc);
     *out = h;
     return QRL_OK;
 }
@@ -213,20 +195,13 @@ int qrl_spectrum_destroy(qrl_spectrum* h)
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     spectrum_free_buffers(h);
-    if (h->d_stage) cudaFree(h->d_stage);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-    return QRL_OK;
+    return handle_close(h);
 }
 
 int qrl_spectrum_set_stream(qrl_spectrum* h, void* s)
 {
     if (!h) return QRL_EINVAL;
-    CKS(cudaStreamSynchronize(h->stream));
-    if (h->own_stream && h->stream) { cudaStreamDestroy(h->stream); h->own_stream = false; }
-    if (s) h->stream = static_cast<cudaStream_t>(s);
-    else { CKS(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    return QRL_OK;
+    return handle_set_stream(h, s);
 }
 
 int qrl_spectrum_set_enabled(qrl_spectrum* h, int enabled)      // rx_fft_c::set_enabled (rx_fft.cpp:103-108)
@@ -241,8 +216,8 @@ int qrl_spectrum_set_fft_size(qrl_spectrum* h, int fft_size)    // rx_fft_c::set
     if (!h) return QRL_EINVAL;
     if (fft_size == h->N) return QRL_OK;
     if (fft_size < 256 || fft_size > 65536 || (fft_size & (fft_size - 1))) { h->err = "qrl_spectrum_set_fft_size: power of two in [256, 65536]"; return QRL_EINVAL; }
-    CKS(cudaSetDevice(h->device));
-    CKS(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     spectrum_free_buffers(h);
     return spectrum_alloc_buffers(h, fft_size);
 }
@@ -252,12 +227,12 @@ int qrl_spectrum_work(qrl_spectrum* h, const float* iq, long T, long stride, int
     if (!h || !iq || T < 0) return QRL_EINVAL;
     if (T > h->max_samples) { h->err = "qrl_spectrum_work: T exceeds max_samples given at create"; return QRL_ERANGE; }
     if (T == 0 || h->push > 0 || !h->enabled) return QRL_OK;         // rx_fft.cpp:80-84: nobody is reading, the whole call is dropped
-    CKS(cudaSetDevice(h->device));
+    QRL_CK(cudaSetDevice(h->device));
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
     if (!on_device) {
-        if (!h->d_stage) CKS(cudaMalloc(&h->d_stage, sizeof(float2) * static_cast<size_t>(h->max_samples) * h->S));
-        CKS(cudaMemcpy2DAsync(h->d_stage, sizeof(float2) * h->max_samples, iq, sizeof(float2) * stride, sizeof(float2) * T, h->S,
+        if (!h->d_stage) { int rc = dev_alloc(h, &h->d_stage, static_cast<size_t>(h->max_samples) * h->S, false); if (rc) return rc; }
+        QRL_CK(cudaMemcpy2DAsync(h->d_stage, sizeof(float2) * h->max_samples, iq, sizeof(float2) * stride, sizeof(float2) * T, h->S,
                               cudaMemcpyHostToDevice, h->stream));
         x = h->d_stage; xstride = h->max_samples;
     }
@@ -288,7 +263,7 @@ int qrl_spectrum_work(qrl_spectrum* h, const float* iq, long T, long stride, int
         fill(i_last, T, 0);
         h->counter = static_cast<unsigned>(T - i_last);
     }
-    CKS(cudaGetLastError());
+    QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
@@ -297,10 +272,10 @@ int qrl_spectrum_get(qrl_spectrum* h, float* dst, long dst_stride, int dst_on_de
     if (!h || !dst || !fft_size) return QRL_EINVAL;
     h->push = 0;                                                        // rx_fft.cpp:115: want more samples
     if (!h->data_ready) { *fft_size = 0; return QRL_OK; }
-    CKS(cudaSetDevice(h->device));
-    CKS(cudaMemcpy2DAsync(dst, sizeof(float) * dst_stride, h->d_points, sizeof(float) * h->N, sizeof(float) * h->N, h->S,
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpy2DAsync(dst, sizeof(float) * dst_stride, h->d_points, sizeof(float) * h->N, sizeof(float) * h->N, h->S,
                           dst_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, h->stream));
-    CKS(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
     *fft_size = static_cast<unsigned>(h->N);
     h->data_ready = false;
     return QRL_OK;

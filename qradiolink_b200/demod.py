@@ -14,40 +14,26 @@ import threading
 
 import numpy as np
 
-from .lib import KIND, PARAM, QrlError, check, load_library
+from .lib import KIND, PARAM, Handle, check, load_library
 
 
-class RxBlock:
+class RxBlock(Handle):
     """n_channels instances of one reference demod hier-block, batched on one GPU."""
+    ABI = "rx"
 
     def __init__(self, kind, sps, samp_rate, carrier_freq, filter_width, flag=0, n_channels=1,
                  max_samples=1 << 20, device=0, low_cutoff=None):
         self._L = load_library()
         self.kind, self.n_channels, self.max_samples = kind, int(n_channels), int(max_samples)
-        self._h = C.c_void_p()
+        # constructor failures surface like the std::runtime_error RadioController::toggleRX catches
         if kind == KIND.DEMOD_FREEDV:
-            rc = self._L.qrl_rx_create_freedv(sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
-                                              self.n_channels, self.max_samples, device, C.byref(self._h))
+            self._create(self._L.qrl_rx_create_freedv, sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
+                         self.n_channels, self.max_samples, device)
         else:
-            rc = self._L.qrl_rx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
-                                       self.n_channels, self.max_samples, device, C.byref(self._h))
-        if rc != 0:
-            # constructor failures surface like the std::runtime_error RadioController::toggleRX catches
-            raise QrlError("qrl_rx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+            self._create(self._L.qrl_rx_create, kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
+                         self.n_channels, self.max_samples, device)
         self.nports = self._L.qrl_rx_num_ports(self._h)
         self._itemsize = [self._L.qrl_rx_port_itemsize(self._h, p) for p in range(self.nports)]
-
-    # -- lifetime
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_rx_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # -- runtime setters (gr_demod_nbfm.h:47-49, gr_demod_base.cpp:1220-1225)
     def set_param(self, key, value, channel=-1):
@@ -76,8 +62,7 @@ class RxBlock:
     def set_carrier_offset(self, hz, channel=-1):
         self.set_param(PARAM.CARRIER_OFFSET_HZ, hz, channel)
 
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_rx_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_rx_set_stream")
+    set_stream = Handle._set_stream
 
     def reset(self):
         check(self._L.qrl_rx_reset(self._h), self._h, "qrl_rx_reset")
@@ -121,8 +106,7 @@ class RxBlock:
         """iq already resident in HBM: dev_ptr = address of [n_channels][stride] complex64."""
         check(self._L.qrl_rx_work(self._h, C.c_void_p(dev_ptr), T, stride, 1), self._h, "qrl_rx_work")
 
-    def sync(self):
-        check(self._L.qrl_rx_sync(self._h), self._h, "qrl_rx_sync")
+    sync = Handle._sync
 
     def set_overlap(self, on=True):
         """Streaming mode: the loop / FEC tail of work() call k runs under the parallel stages of call k+1; read_port(),
@@ -160,9 +144,7 @@ class RxBlock:
         check(self._L.qrl_rx_read_port(self._h, port, None, 0, counts.ctypes.data_as(C.c_void_p), 0), self._h, "read counts")
         return counts
 
-    @property
-    def launches(self):
-        return self._L.qrl_rx_launch_count(self._h)
+    launches = property(Handle._launches)
 
 
 def make_gr_demod_4fsk(sps, samp_rate, carrier_freq, filter_width, fm, n_channels=1, **kw):

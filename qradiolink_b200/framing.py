@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import QrlError, check, load_library
+from .lib import Handle, check, load_library
 
 SYNC_1K, SYNC_NARROW, SYNC_WIDE = 1, 2, 3
 
@@ -46,35 +46,22 @@ def frame(payloads, frame_types, one_k_mode=False, burst_ip=False, device=0):
     return [out[c, :olen[c]].copy() for c in range(Cn)]
 
 
-class Deframer:
+class Deframer(Handle):
+    ABI = "deframer"
+
     def __init__(self, sync_class, bit_buf_len, rx_frame_length, n_channels=1, max_bits=1 << 20, max_frames=None, device=0):
         self._L = load_library()
         self.n_channels, self.max_bits = int(n_channels), int(max_bits)
         self.max_frames = int(max_frames) if max_frames else max(4, self.max_bits // max(8, bit_buf_len - 8) + 2)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_deframer_create(sync_class, bit_buf_len, rx_frame_length, self.n_channels, self.max_bits, self.max_frames,
-                                         device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_deframer_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_deframer_create, sync_class, bit_buf_len, rx_frame_length, self.n_channels, self.max_bits, self.max_frames,
+                     device)
         self.rec_bytes = self._L.qrl_deframer_record_bytes(self._h)
 
     @classmethod
     def for_mode(cls, mode, **kw):
         return cls(*MODE_FRAMING[mode], **kw)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_deframer_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_deframer_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_deframer_set_stream")
+    set_stream = Handle._set_stream
 
     def _collect(self):
         rec = np.zeros((self.n_channels, self.max_frames, self.rec_bytes), np.uint8)
@@ -141,36 +128,20 @@ class Deframer:
         check(self._L.qrl_deframer_dropped(self._h, d.ctypes.data_as(C.c_void_p)), self._h, "qrl_deframer_dropped")
         return d
 
-    @property
-    def launches(self):
-        return self._L.qrl_deframer_launch_count(self._h)
+    launches = property(Handle._launches)
 
 
-class DeframerBB:
+class DeframerBB(Handle):
     """gr_deframer_bb (src/gr/gr_deframer_bb.cpp:83-185) for a batch of channels: modem_type 1 / 2 / 3 as gr_demod_base creates them
     (_deframer1/2, _deframer_700_1/2, _deframer_10k_1/2).  work() returns, per channel, the bit stream get_data() would hand to gr_modem."""
+    ABI = "dfbb"
 
     def __init__(self, modem_type, n_channels=1, max_bits=1 << 20, device=0):
         self._L = load_library()
         self.n_channels, self.max_bits = int(n_channels), int(max_bits)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_dfbb_create(int(modem_type), self.n_channels, self.max_bits, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_dfbb_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_dfbb_create, int(modem_type), self.n_channels, self.max_bits, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_dfbb_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def sync(self):
-        check(self._L.qrl_dfbb_sync(self._h), self._h, "qrl_dfbb_sync")
+    sync = Handle._sync
 
     def out_device(self):
         p, s, c = C.c_void_p(), C.c_long(), C.c_void_p()

@@ -5,31 +5,18 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import QrlError, check, load_library
+from .lib import Handle, check, load_library
 
 
-class Frontend:
+class Frontend(Handle):
+    ABI = "frontend"
+
     def __init__(self, samp_rate, n_channels=1, max_in=1 << 21, device=0):
         self._L = load_library()
         self.n_channels, self.max_in, self.decimation = int(n_channels), int(max_in), int(samp_rate) // 1000000
-        self._h = C.c_void_p()
-        rc = self._L.qrl_frontend_create(int(samp_rate), self.n_channels, self.max_in, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_frontend_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_frontend_create, int(samp_rate), self.n_channels, self.max_in, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_frontend_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_frontend_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_frontend_set_stream")
+    set_stream = Handle._set_stream
 
     def set_carrier_offset(self, hz, channel=-1):
         check(self._L.qrl_frontend_set_carrier_offset(self._h, channel, float(hz)), self._h, "qrl_frontend_set_carrier_offset")

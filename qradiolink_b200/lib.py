@@ -161,3 +161,40 @@ def check(rc, handle=None, what=""):
     if rc != 0:
         msg = load_library().qrl_last_error(handle)
         raise QrlError("%s failed (%d): %s" % (what, rc, (msg or b"").decode()))
+
+
+class Handle:
+    """Owner of one library handle of the ABI family qrl_<ABI>_*: creation, close() (also on garbage collection) and the
+    set_stream / sync / launch-count calls.  A wrapper exposes those of the last three its family has, e.g.
+    `set_stream = Handle._set_stream`, `launches = property(Handle._launches)`."""
+    ABI = None
+
+    def _create(self, create, *args):
+        """create(*args, &handle), e.g. self._L.qrl_rx_create; raises QrlError with the library's last error when it fails."""
+        self._h = C.c_void_p()
+        rc = create(*args, C.byref(self._h))
+        if rc != 0:
+            raise QrlError("qrl_%s_create failed (%d): %s" % (self.ABI, rc, (self._L.qrl_last_error(None) or b"").decode()))
+
+    def _fn(self, what):
+        return getattr(self._L, "qrl_%s_%s" % (self.ABI, what))
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._fn("destroy")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _set_stream(self, cuda_stream_ptr):
+        check(self._fn("set_stream")(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_%s_set_stream" % self.ABI)
+
+    def _sync(self):
+        check(self._fn("sync")(self._h), self._h, "qrl_%s_sync" % self.ABI)
+
+    def _launches(self):
+        return int(self._fn("launch_count")(self._h))

@@ -7,7 +7,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import QrlError, check, load_library
+from .lib import Handle, QrlError, check, load_library
 from .pfb import PfbChannelizer, PfbSynthesizer, mmdvm_port_map
 
 MAX_MMDVM_CHANNELS = 7            # src/bursttimer.h:28
@@ -22,8 +22,9 @@ def _low_pass_2(L, gain, fs, fc, tw, att):
     return buf[:n].copy()
 
 
-class MmdvmChannelsRx:
+class MmdvmChannelsRx(Handle):
     """The per-channel part alone (qrl_mmdvm_rx_*): rows of a [n_rows][stride] gr_complex slab at 25 ksps -> int16 at 24 ksps + RSSI."""
+    ABI = "mmdvm_rx"
 
     def __init__(self, n_channels, rows=None, n_rows=None, filter_width=5000, max_in=1 << 16, device=0, single=False):
         """single=True: make_gr_demod_mmdvm (gr_demod_mmdvm.cpp:30-64) for n_channels independent 250 ksps streams."""
@@ -32,25 +33,10 @@ class MmdvmChannelsRx:
         self.n_rows = int(n_rows if n_rows is not None else n_channels)
         self.max_in = int(max_in)
         r = None if rows is None else np.ascontiguousarray(rows, np.int32)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_mmdvm_rx_create(int(bool(single)), self.n_channels, None if r is None else r.ctypes.data_as(C.c_void_p), self.n_rows, int(filter_width),
-                                         self.max_in, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_mmdvm_rx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_mmdvm_rx_create, int(bool(single)), self.n_channels, None if r is None else r.ctypes.data_as(C.c_void_p), self.n_rows,
+                     int(filter_width), self.max_in, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_mmdvm_rx_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_mmdvm_rx_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_mmdvm_rx_set_stream")
+    set_stream = Handle._set_stream
 
     def calibrate_rssi(self, level):
         check(self._L.qrl_mmdvm_rx_calibrate_rssi(self._h, float(level)), self._h, "qrl_mmdvm_rx_calibrate_rssi")
@@ -78,9 +64,7 @@ class MmdvmChannelsRx:
         check(self._L.qrl_mmdvm_rx_work(self._h, C.c_void_p(dev_ptr), n, stride, 1, C.byref(cnt)), self._h, "qrl_mmdvm_rx_work")
         return cnt.value
 
-    @property
-    def launches(self):
-        return int(self._L.qrl_mmdvm_rx_launch_count(self._h))
+    launches = property(Handle._launches)
 
 
 def mmdvm_tag_item(sample_index, single=False):
@@ -91,8 +75,9 @@ def mmdvm_tag_item(sample_index, single=False):
     return k if single else (2 * k * 25 + 24) // 48
 
 
-class MmdvmChannelsTx:
+class MmdvmChannelsTx(Handle):
     """The per-channel part alone (qrl_mmdvm_tx_*): int16 [n_channels][n] at 24 ksps -> rows of a [n_rows][stride] slab at 25 ksps."""
+    ABI = "mmdvm_tx"
 
     def __init__(self, n_channels, rows=None, n_rows=None, filter_width=5000, max_in=1 << 16, device=0, single=False):
         """single=True: make_gr_mod_mmdvm (gr_mod_mmdvm.cpp:28-70) for n_channels independent streams, 250 ksps out."""
@@ -102,25 +87,10 @@ class MmdvmChannelsTx:
         self.max_in = int(max_in)
         self.single = bool(single)
         r = None if rows is None else np.ascontiguousarray(rows, np.int32)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_mmdvm_tx_create(int(bool(single)), self.n_channels, None if r is None else r.ctypes.data_as(C.c_void_p), self.n_rows, int(filter_width),
-                                         self.max_in, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_mmdvm_tx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_mmdvm_tx_create, int(bool(single)), self.n_channels, None if r is None else r.ctypes.data_as(C.c_void_p), self.n_rows,
+                     int(filter_width), self.max_in, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_mmdvm_tx_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_mmdvm_tx_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_mmdvm_tx_set_stream")
+    set_stream = Handle._set_stream
 
     def set_bb_gain(self, g):
         check(self._L.qrl_mmdvm_tx_set_bb_gain(self._h, float(g)), self._h, "qrl_mmdvm_tx_set_bb_gain")
@@ -147,9 +117,7 @@ class MmdvmChannelsTx:
         check(self._L.qrl_mmdvm_tx_out_device(self._h, C.byref(d), C.byref(s), C.byref(n)), self._h, "qrl_mmdvm_tx_out_device")
         return d.value, s.value, n.value
 
-    @property
-    def launches(self):
-        return int(self._L.qrl_mmdvm_tx_launch_count(self._h))
+    launches = property(Handle._launches)
 
 
 class MmdvmDemod:

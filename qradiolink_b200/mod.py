@@ -5,34 +5,22 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import KIND, PARAM, QrlError, check, load_library
+from .lib import KIND, PARAM, Handle, check, load_library
 
 
-class TxBlock:
+class TxBlock(Handle):
+    ABI = "tx"
+
     def __init__(self, kind, sps, samp_rate, carrier_freq, filter_width, flag=0, n_channels=1,
                  max_items=1 << 12, device=0, low_cutoff=None):
         self._L = load_library()
         self.n_channels, self.max_items = int(n_channels), int(max_items)
-        self._h = C.c_void_p()
         if kind == KIND.MOD_FREEDV:
-            rc = self._L.qrl_tx_create_freedv(sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
-                                              self.n_channels, self.max_items, device, C.byref(self._h))
+            self._create(self._L.qrl_tx_create_freedv, sps, samp_rate, carrier_freq, filter_width, int(low_cutoff), int(flag),
+                         self.n_channels, self.max_items, device)
         else:
-            rc = self._L.qrl_tx_create(kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
-                                       self.n_channels, self.max_items, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_tx_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_tx_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+            self._create(self._L.qrl_tx_create, kind, sps, samp_rate, carrier_freq, filter_width, int(flag),
+                         self.n_channels, self.max_items, device)
 
     def zero_samples(self, byte_offset, n_samples, channel=-1):
         """gr_mod_dmr: the "zero_samples" tag on input byte `byte_offset` of `channel` (-1: all), see qrl_tx_zero_samples."""
@@ -49,8 +37,7 @@ class TxBlock:
     def set_bb_gain(self, value):
         check(self._L.qrl_tx_set_param(self._h, -1, PARAM.BB_GAIN, float(value)), self._h, "set_bb_gain")
 
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_tx_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_tx_set_stream")
+    set_stream = Handle._set_stream
 
     def work(self, data):
         """data: uint8 [n_channels, n] frame bytes -> complex64 [n_channels, n_out] at 1 Msps."""
@@ -97,12 +84,8 @@ class TxBlock:
     def work_device(self, dev_ptr, n, stride):
         check(self._L.qrl_tx_work(self._h, C.c_void_p(dev_ptr), n, stride, 1), self._h, "qrl_tx_work")
 
-    def sync(self):
-        check(self._L.qrl_tx_sync(self._h), self._h, "qrl_tx_sync")
-
-    @property
-    def launches(self):
-        return self._L.qrl_tx_launch_count(self._h)
+    sync = Handle._sync
+    launches = property(Handle._launches)
 
 
 def make_gr_mod_4fsk(sps, samp_rate, carrier_freq, filter_width, fm, n_channels=1, **kw):

@@ -6,7 +6,7 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import QrlError, check, load_library
+from .lib import Handle, check, load_library
 
 PFB_CHANNELIZER, PFB_SYNTHESIZER = 201, 202
 
@@ -23,32 +23,17 @@ def mmdvm_port_map(num_channels):
     return ports
 
 
-class _Pfb:
+class _Pfb(Handle):
+    ABI = "pfb"
+
     def __init__(self, kind, M, taps, max_in, device=0):
         self._L = load_library()
         taps = np.ascontiguousarray(taps, np.float32)
         self.M, self.kind, self.max_in = int(M), kind, int(max_in)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_pfb_create(kind, self.M, taps.ctypes.data_as(C.c_void_p), len(taps), self.max_in, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_pfb_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_pfb_create, kind, self.M, taps.ctypes.data_as(C.c_void_p), len(taps), self.max_in, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_pfb_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_pfb_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_pfb_set_stream")
-
-    def sync(self):
-        check(self._L.qrl_pfb_sync(self._h), self._h, "qrl_pfb_sync")
+    set_stream = Handle._set_stream
+    sync = Handle._sync
 
     def out_device(self):
         """(device pointer, stride in items, valid items) of the last call's output."""
@@ -56,9 +41,7 @@ class _Pfb:
         check(self._L.qrl_pfb_out_device(self._h, C.byref(d), C.byref(s), C.byref(n)), self._h, "qrl_pfb_out_device")
         return d.value, s.value, n.value
 
-    @property
-    def launches(self):
-        return self._L.qrl_pfb_launch_count(self._h)
+    launches = property(Handle._launches)
 
 
 class PfbChannelizer(_Pfb):

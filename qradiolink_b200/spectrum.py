@@ -4,36 +4,22 @@ import ctypes as C
 
 import numpy as np
 
-from .lib import QrlError, check, load_library
+from .lib import Handle, check, load_library
 
 WIN_HAMMING, WIN_HANN, WIN_BLACKMAN, WIN_RECTANGULAR, WIN_KAISER, WIN_BLACKMAN_HARRIS = 0, 1, 2, 3, 4, 5
 
 
-class Spectrum:
+class Spectrum(Handle):
     """make_rx_fft_c(fftsize, wintype) for n_streams streams; work() = one rx_fft_c::work call, get_fft_data() as in the reference
     (None while no spectrum is ready)."""
+    ABI = "spectrum"
 
     def __init__(self, fft_size=32768, window=WIN_BLACKMAN_HARRIS, n_streams=1, max_samples=1 << 20, device=0):
         self._L = load_library()
         self.n_streams, self.fft_size, self.max_samples = int(n_streams), int(fft_size), int(max_samples)
-        self._h = C.c_void_p()
-        rc = self._L.qrl_spectrum_create(self.fft_size, int(window), self.n_streams, self.max_samples, device, C.byref(self._h))
-        if rc != 0:
-            raise QrlError("qrl_spectrum_create failed (%d): %s" % (rc, (self._L.qrl_last_error(None) or b"").decode()))
+        self._create(self._L.qrl_spectrum_create, self.fft_size, int(window), self.n_streams, self.max_samples, device)
 
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self._L.qrl_spectrum_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_stream(self, cuda_stream_ptr):
-        check(self._L.qrl_spectrum_set_stream(self._h, C.c_void_p(cuda_stream_ptr)), self._h, "qrl_spectrum_set_stream")
+    set_stream = Handle._set_stream
 
     def set_enabled(self, on):
         check(self._L.qrl_spectrum_set_enabled(self._h, int(bool(on))), self._h, "qrl_spectrum_set_enabled")
@@ -61,6 +47,4 @@ class Spectrum:
         check(self._L.qrl_spectrum_get(self._h, out.ctypes.data_as(C.c_void_p), self.fft_size, 0, C.byref(n)), self._h, "qrl_spectrum_get")
         return out if n.value else None
 
-    @property
-    def launches(self):
-        return int(self._L.qrl_spectrum_launch_count(self._h))
+    launches = property(Handle._launches)
