@@ -203,6 +203,26 @@ int  qrl_frontend_out_device(qrl_frontend*, float** data, long* stride, long* n_
 int  qrl_frontend_read(qrl_frontend*, float* dst /* [n_channels][cap] gr_complex */, long cap);
 long qrl_frontend_launch_count(const qrl_frontend*);
 
+/* ---- transmit front end: carrier offset and x N to the device rate ------------------------------------------------------------------
+ * gr_mod_base (src/gr/gr_mod_base.cpp:38,211-293,799-805): every modulator's 1 Msps output goes through rotator_cc(2 pi offset / 1e6)
+ * and, when the device runs at samp_rate >= 2 Msps, through rational_resampler_ccf(N, 1, low_pass(N, samp_rate, 480000, 20000,
+ * BLACKMAN_HARRIS)) with N = samp_rate / 1e6 (about 210 taps per arm) in front of the SDR sink; at 1 Msps the rotator feeds the sink
+ * directly.  This object is that pair for a batch of channels: [n_channels][n] gr_complex at 1 Msps in (host memory, or the device
+ * pointer and stride of qrl_tx_out_device on the same device), [n_channels][N n] at samp_rate out.  The rotator divides by 1e6 whatever
+ * samp_rate is, as the reference's set_carrier_offset(offset, sample_rate = 1000000) does.  Streaming (any chunking gives the same
+ * output, n = 0 is valid), phase-continuous retunes from the next input sample on; channel -1 retunes every channel.
+ * qrl_tx_frontend_work returns QRL_ERANGE for n > max_in and QRL_EINVAL for a device pointer of another GPU; the output stays on the
+ * device until the next call (qrl_tx_frontend_out_device) or is copied out with qrl_tx_frontend_read.  destroy(NULL) is QRL_OK. */
+typedef struct qrl_tx_frontend qrl_tx_frontend;
+int  qrl_tx_frontend_create(int samp_rate /* multiple of 1e6, 1e6..32e6 */, int n_channels, long max_in, int device, qrl_tx_frontend** out);
+int  qrl_tx_frontend_destroy(qrl_tx_frontend*);
+int  qrl_tx_frontend_set_stream(qrl_tx_frontend*, void* cuda_stream);
+int  qrl_tx_frontend_set_carrier_offset(qrl_tx_frontend*, int channel /* -1 = all */, double offset_hz);
+int  qrl_tx_frontend_work(qrl_tx_frontend*, const float* iq, long n, long stride, int on_device, long* n_out /* N n */);
+int  qrl_tx_frontend_out_device(qrl_tx_frontend*, float** data, long* stride, long* n_out);
+int  qrl_tx_frontend_read(qrl_tx_frontend*, float* dst /* [n_channels][cap] gr_complex */, long cap);
+long qrl_tx_frontend_launch_count(const qrl_tx_frontend*);
+
 /* ---- design helpers (host only; the gr::filter::firdes calls the reference makes at construction /
  *      in set_filter_width, e.g. gr_demod_nbfm.cpp:82-90).  Return tap count or negative error. ---- */
 int qrl_firdes_low_pass(double gain, double fs, double fc, double tw, int window, float* out, int cap);

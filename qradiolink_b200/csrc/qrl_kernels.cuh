@@ -2864,6 +2864,83 @@ __global__ void frontend_hist_kernel(const RotState* __restrict__ rs, const floa
     new_hist[static_cast<long long>(c) * H + i] = v;
 }
 
+// Transmit front end at device rates >= 2 Msps (gr_mod_base.cpp:38,211-259): rotator_cc at 1 Msps fused into
+// rational_resampler_ccf(L, 1) with L = samp_rate / 1e6 and about 210 taps per arm, y[L m + p] = sum_k arm[p][k] x[m - k].
+// The arms are too long for interp_fir_ccf_rt_kernel's all-taps-in-registers shape, so:
+//   * one CTA = a tile of G R input positions m of one channel, all L phases.  The window is rotated while it is filled into shared
+//     memory (same Q32 phase arithmetic as frontend_fir_kernel); the previous calls' NTP - 1 samples come ALREADY ROTATED from `hist`
+//     (frontend_hist_kernel keeps that tail), so a retune never touches samples already inside the filter;
+//   * the arm table sits in shared memory as [NTP][L] (= the zero-padded tap array), so lanes on consecutive phases read consecutive
+//     words;
+//   * thread (phase p = tid % L, group q = tid / L) accumulates R consecutive outputs of its phase.  It walks the taps from k = NTP - 1
+//     down to 0 in chunks of KC held in registers; within a chunk each window sample is loaded once (a broadcast LDS: the lanes of a
+//     group read one address) and feeds every accumulator that needs it, 2 R KC FFMA per R + KC - 1 window loads and KC tap loads.
+// Each output's sum is one fmaf chain per component over k = NTP - 1 .. 0, oldest sample first: the oracle's order for L > 1.  The
+// rows k >= NT of the table are zero and come first in the chain, so they leave the accumulator at +0 (bit-identical for finite input).
+template <int KC, int R>
+__global__ void __launch_bounds__(512)
+tx_frontend_interp_kernel(const RotState* __restrict__ rs /* nullptr: no rotation */, const float2* __restrict__ in, long long in_stride,
+                          long long T, long long n_abs0 /* absolute index of in[c][0] */, const float2* __restrict__ hist /* [C][H] rotated */,
+                          int H /* NTP - 1 */, const float* __restrict__ arms /* [NTP][L] */, int L, int NTP, int G,
+                          float2* __restrict__ out, long long out_stride /* out[c][L m + p], m relative to in[c][0] */)
+{
+    extern __shared__ __align__(16) float sm_tf[];
+    float* hs = sm_tf;                                                   // NTP * L taps
+    float2* xs = reinterpret_cast<float2*>(sm_tf + ((NTP * L + 3) & ~3)); // G R + NTP - 1 rotated samples
+    const int c = blockIdx.y;
+    const int TM = G * R;
+    const long long m0 = static_cast<long long>(blockIdx.x) * TM;       // first input position of the tile, relative to in[c][0]
+    for (int i = threadIdx.x; i < NTP * L; i += blockDim.x) hs[i] = arms[i];
+    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* hc = hist + static_cast<long long>(c) * H;
+    RotState r{ 0u, 0u, 0 };
+    if (rs) r = rs[c];
+    for (int i = threadIdx.x; i < TM + NTP - 1; i += blockDim.x) {
+        const long long li = m0 - (NTP - 1) + i;                         // index into this call's input
+        float2 v = make_float2(0.0f, 0.0f);
+        if (li >= 0) {
+            if (li < T) {
+                v = x[li];
+                if (rs) {
+                    const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs0 + li - r.n_base);
+                    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
+                    float sn, cs;
+                    qrl_sincosf(ang, sn, cs);
+                    v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
+                }
+            }
+        } else v = hc[H + li];
+        xs[i] = v;
+    }
+    __syncthreads();
+    const int p = threadIdx.x % L, q = threadIdx.x / L;
+    float2 acc[R];
+#pragma unroll
+    for (int j = 0; j < R; j++) acc[j] = make_float2(0.0f, 0.0f);
+    const float2* s = xs + q * R;                                        // s[j] = x[m0 + q R - (NTP - 1) + j]
+    for (int kb = NTP - KC; kb >= 0; kb -= KC) {
+        float h[KC];
+#pragma unroll
+        for (int i = 0; i < KC; i++) h[i] = hs[(kb + i) * L + p];
+        const float2* sb = s + (NTP - KC - kb);                          // output j, tap kb + KC - 1 - i reads sb[j + i]
+#pragma unroll
+        for (int u = 0; u < R + KC - 1; u++) {
+            const float2 v = sb[u];
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                const int i = u - j;
+                if (i >= 0 && i < KC) ffma2(acc[j], h[KC - 1 - i], v);
+            }
+        }
+    }
+    float2* oc = out + static_cast<long long>(c) * out_stride;
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+        const long long m = m0 + q * R + j;
+        if (m < T) oc[m * L + p] = acc[j];                               // the L phases of one m: one contiguous row
+    }
+}
+
 // roll the stage-1 history: new_hist = last H samples of (old_hist ++ iq[0..T))
 __global__ void hist_update_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
                                    const float2* __restrict__ old_hist, float2* __restrict__ new_hist, int H)

@@ -43,3 +43,52 @@ class Frontend(Handle):
         p, s, n = C.c_void_p(), C.c_long(), C.c_long()
         check(self._L.qrl_frontend_out_device(self._h, C.byref(p), C.byref(s), C.byref(n)), self._h, "qrl_frontend_out_device")
         return p.value, s.value, n.value
+
+
+class TxFrontend(Handle):
+    """Transmit side of the same pair, gr_mod_base::set_samp_rate / set_carrier_offset (gr_mod_base.cpp:38,211-293,799-805): rotator
+    at 1 Msps + rational_resampler_ccf(samp_rate / 1e6, 1) behind the modulators, for a batch of channels.  Takes the layout
+    TxBlock.out_device gives; the output at samp_rate stays in HBM until read."""
+    ABI = "tx_frontend"
+
+    def __init__(self, samp_rate, n_channels=1, max_in=1 << 16, device=0):
+        self._L = load_library()
+        self.n_channels, self.max_in, self.interpolation = int(n_channels), int(max_in), int(samp_rate) // 1000000
+        self._create(self._L.qrl_tx_frontend_create, int(samp_rate), self.n_channels, self.max_in, device)
+
+    set_stream = Handle._set_stream
+    launches = property(Handle._launches)
+
+    def set_carrier_offset(self, hz, channel=-1):
+        check(self._L.qrl_tx_frontend_set_carrier_offset(self._h, channel, float(hz)), self._h, "qrl_tx_frontend_set_carrier_offset")
+
+    def work(self, iq):
+        """iq: complex64 [n_channels, n] at 1 Msps (host) -> complex64 [n_channels, N n] at the device rate."""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        if iq.ndim == 1:
+            iq = iq[None, :]
+        n_in = iq.shape[1]
+        n = C.c_long()
+        check(self._L.qrl_tx_frontend_work(self._h, iq.ctypes.data_as(C.c_void_p), n_in, n_in, 0, C.byref(n)), self._h, "qrl_tx_frontend_work")
+        out = np.zeros((self.n_channels, max(1, n.value)), np.complex64)
+        check(self._L.qrl_tx_frontend_read(self._h, out.ctypes.data_as(C.c_void_p), out.shape[1]), self._h, "qrl_tx_frontend_read")
+        return out[:, :n.value]
+
+    def work_device(self, dev_ptr, n, stride):
+        """device input, e.g. TxBlock.out_device()'s pointer and stride; returns the number of output items per channel (N n)."""
+        out = C.c_long()
+        check(self._L.qrl_tx_frontend_work(self._h, C.c_void_p(dev_ptr), n, stride, 1, C.byref(out)), self._h, "qrl_tx_frontend_work")
+        return out.value
+
+    def read(self):
+        """complex64 [n_channels, items] of the last call (waits for the handle's stream)."""
+        n = self.out_device()[2]
+        out = np.zeros((self.n_channels, max(1, n)), np.complex64)
+        check(self._L.qrl_tx_frontend_read(self._h, out.ctypes.data_as(C.c_void_p), out.shape[1]), self._h, "qrl_tx_frontend_read")
+        return out[:, :n]
+
+    def out_device(self):
+        """(device pointer, stride, items) of the last call's output at the device rate, e.g. for Frontend.work_device(ptr, items, stride)."""
+        p, s, n = C.c_void_p(), C.c_long(), C.c_long()
+        check(self._L.qrl_tx_frontend_out_device(self._h, C.byref(p), C.byref(s), C.byref(n)), self._h, "qrl_tx_frontend_out_device")
+        return p.value, s.value, n.value
