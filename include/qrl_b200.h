@@ -192,7 +192,12 @@ int qrl_tx_profile_read(qrl_tx* h, int stage, double* ms_total, long* n_launches
  * reference puts rational_resampler_ccf(1, samp_rate / 1e6, low_pass(1, samp_rate, 480000, 100000, BLACKMAN_HARRIS)) behind the
  * rotator (which then runs at the device rate, :1220-1225,1358) and in front of the demodulators.  This object is that pair for a batch
  * of channels: [n_channels][T] gr_complex at samp_rate in, [n_channels][T / N] at 1 Msps out -- the device-resident input layout of
- * qrl_rx_work.  Streaming (any chunking), phase-continuous retunes. */
+ * qrl_rx_work.  Streaming (any chunking), phase-continuous retunes.
+ * qrl_frontend_work's stride: >= T, channel c reads iq[c * stride .. c * stride + T).  stride == 0: ONE wideband stream iq[0 .. T) feeds
+ * every channel (one SDR, n_channels receivers at their own carrier offsets, gr_demod_mmdvm_multi.cpp:68-123); channel c's output is
+ * what [n_channels][T] with n_channels identical rows would give, bit for bit.  Host input is copied to the device once (T samples),
+ * device input is read in place.  A handle may alternate between shared and per-channel calls: each channel's stream continues.
+ * T > max_in returns QRL_ERANGE; T == 0 returns QRL_OK with no output. */
 typedef struct qrl_frontend qrl_frontend;
 int  qrl_frontend_create(int samp_rate /* multiple of 1e6, >= 2e6 */, int n_channels, long max_in, int device, qrl_frontend** out);
 int  qrl_frontend_destroy(qrl_frontend*);

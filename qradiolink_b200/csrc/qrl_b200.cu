@@ -2784,6 +2784,18 @@ int qrl_tx_out_device(qrl_tx* h, float** data, long* stride, long* n_out)
 long qrl_tx_launch_count(const qrl_tx* h) { return h ? h->launches : 0; }
 
 // ---------------------------------------------------------------------------------------------- front end (device rate >= 2 Msps)
+namespace {
+// frontend_shared_kernel: outputs per work item (odd: conflict-free window loads), taps per register chunk, threads per CTA; it
+// serves D <= FESH_DMAX, where THE FIR order's slots are single branches.  Above, a shared stream runs frontend_fir_kernel with
+// in_stride = 0.  The shared-memory budget keeps two CTAs on an SM.
+constexpr int FESH_K = 9, FESH_KC = 8, FESH_NT = 256, FESH_DMAX = 32, FESH_SMEM = 113 * 1024;
+size_t fesh_smem(int D, int QP, int Qmax, int NB)
+{
+    const int NOUT = NB * FESH_K, MW = NOUT + Qmax - 1;
+    return sizeof(float) * D * QP + sizeof(float2) * D * (MW + (MW | 1) + NOUT);
+}
+}  // namespace
+
 struct qrl_frontend : HandleBase {
     int samp_rate = 0, D = 1, C = 0, ntaps = 0, H = 0, hist_cur = 0;
     long max_in = 0;
@@ -2792,6 +2804,9 @@ struct qrl_frontend : HandleBase {
     float2* d_in = nullptr; float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_in = 0, n1 = 0;
     std::vector<RotState> rot; RotState* d_rot = nullptr; bool rot_active = false;
+    // shared stream (stride 0): [max_in] host staging, and frontend_shared_kernel's chain-order taps [D][QP] and strip shape
+    float2* d_in1 = nullptr;
+    float* d_ht = nullptr; int QP = 0, Qmax = 0, NB = 0, n_sm = 0; size_t fs_smem = 0;
 };
 
 int qrl_frontend_destroy(qrl_frontend* h) { return h ? handle_close(h) : QRL_OK; }
@@ -2817,6 +2832,26 @@ int qrl_frontend_create(int samp_rate, int n_channels, long max_in, int device, 
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
     if ((rc = dev_alloc(h, &h->d_rot, h->C))) return fail(rc);
     h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
+    if (h->D <= FESH_DMAX) {
+        h->Qmax = (h->ntaps - 1) / h->D + 1;
+        h->QP = (h->Qmax + 3) & ~3;
+        std::vector<float> ht(static_cast<size_t>(h->D) * h->QP, 0.0f);
+        for (int r = 0; r < h->D; r++) {
+            const int Qr = (h->ntaps - 1 - r) / h->D + 1;
+            for (int s = 0; s < Qr; s++) ht[static_cast<size_t>(r) * h->QP + s] = taps[static_cast<size_t>(h->D) * (Qr - 1 - s) + r];
+        }
+        if ((rc = upload_floats(h, &h->d_ht, ht))) return fail(rc);
+        // strip of NB K outputs: the most useful work per CTA, i.e. the share of busy item slots (D NB items over whole rounds of
+        // FESH_NT threads) times the share of the window that is not overlap with the next strip (NOUT / (NOUT + Qmax - 1))
+        double best = -1.0;
+        for (int nb = 1; fesh_smem(h->D, h->QP, h->Qmax, nb) <= FESH_SMEM; nb++) {
+            const int items = h->D * nb, nout = nb * FESH_K;
+            const double score = items / (static_cast<double>(FESH_NT) * ((items + FESH_NT - 1) / FESH_NT)) * nout / (nout + h->Qmax - 1.0);
+            if (score > best + 1e-9) { best = score; h->NB = nb; }
+        }
+        h->fs_smem = fesh_smem(h->D, h->QP, h->Qmax, h->NB);
+        if (cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess) { set_err(h, "SM count query failed"); return fail(QRL_ECUDA); }
+    }
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
@@ -2846,7 +2881,12 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     QRL_CK(cudaSetDevice(h->device));
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
-    if (!on_device) {
+    const bool shared = stride == 0;                                     // one stream for every channel
+    if (!on_device && shared) {
+        if (!h->d_in1) { int rc = dev_alloc(h, &h->d_in1, static_cast<size_t>(h->max_in), false); if (rc) return rc; }
+        QRL_CK(cudaMemcpyAsync(h->d_in1, iq, sizeof(float2) * T, cudaMemcpyHostToDevice, h->stream));
+        x = h->d_in1;
+    } else if (!on_device) {
         if (!h->d_in) { int rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_in) * h->C, false); if (rc) return rc; }
         QRL_CK(cudaMemcpy2DAsync(h->d_in, sizeof(float2) * h->max_in, iq, sizeof(float2) * stride, sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
         x = h->d_in; xstride = h->max_in;
@@ -2854,7 +2894,18 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     const long long N = h->n_in + T;
     const long long k0 = h->n1, k1 = (N + h->D - 1) / h->D;              // outputs k with D k <= N - 1
     const RotState* rs = h->rot_active ? h->d_rot : nullptr;
-    if (k1 > k0) {
+    if (k1 > k0 && shared && h->D <= FESH_DMAX) {
+        auto kern = frontend_shared_kernel<FESH_K, FESH_KC>;
+        if (int rc = smem_opt_in(h, kern, FESH_SMEM)) return rc;
+        // channel groups: enough CTAs for two per SM (a short call splits the channels), else one group, one raw load per strip
+        const long long strips = (k1 - k0 + h->NB * FESH_K - 1) / (h->NB * FESH_K);
+        const long long groups = std::min<long long>(h->C, (2LL * h->n_sm + strips - 1) / strips);
+        const int CG = static_cast<int>((h->C + groups - 1) / groups);
+        dim3 g(static_cast<unsigned>(strips), static_cast<unsigned>((h->C + CG - 1) / CG));
+        kern<<<g, FESH_NT, h->fs_smem, h->stream>>>(rs, x, T, h->n_in, h->d_hist[h->hist_cur], h->H, h->d_ht, h->QP, h->ntaps, h->D, h->Qmax,
+                                                    h->NB, h->C, CG, h->d_out, h->out_stride, k0, k1);
+        h->launches++;
+    } else if (k1 > k0) {
         const size_t smem = sizeof(float) * ((h->ntaps + 1) & ~1) + sizeof(float2) * (127 * h->D + h->ntaps);
         if (int rc = smem_opt_in(h, frontend_fir_kernel, 160 * 1024)) return rc;
         if (smem > 160 * 1024) { set_err(h, "qrl_frontend_work: device rate too high for this kernel"); return QRL_EINVAL; }

@@ -2864,6 +2864,123 @@ __global__ void frontend_hist_kernel(const RotState* __restrict__ rs, const floa
     new_hist[static_cast<long long>(c) * H + i] = v;
 }
 
+// Front end for C channels at C carrier offsets inside ONE wideband stream (qrl_frontend_work with stride 0), D = N <= 32:
+// gr_demod_mmdvm_multi.cpp:68-123's wiring, one rotator + /D resampler per channel behind one source.  The outputs are those of
+// frontend_fir_kernel for each channel fed the shared stream, bit for bit; what changes is how the work is laid out:
+//   * one CTA = NB K consecutive outputs (a strip) of a group of CG channels.  The raw window of the strip is loaded from HBM into
+//     shared memory ONCE (coalesced 8-byte loads, any sample alignment), then for each channel of the group it is rotated (the
+//     same Q32 phase arithmetic as frontend_fir_kernel) into a polyphase-split copy xr[r][m] = x[D (kb - Qmax + 1 + m) - r].  The
+//     first strip of a call takes its older samples from the channel's own already-rotated tail (frontend_hist_kernel);
+//   * phase 1: work item (branch r, block b) = K consecutive outputs of branch r.  With D <= 32 branch r is THE FIR order's slot r,
+//     accumulated oldest sample first: the taps sit in shared memory in chain order ht[r][s] = h[D (Q_r - 1 - s) + r], each chunk of
+//     KC taps is held in registers and every window sample loaded once feeds all K accumulators that need it (2 K KC FFMA per
+//     K + KC - 1 window loads).  Lanes are consecutive blocks of one branch, so the tap loads are broadcasts and the window loads
+//     K (odd) samples apart hit distinct banks.  No lane idles at small D: the items are D NB, spread over every thread;
+//   * phase 2: thread per output, the xor butterfly 16, 8, 4, 2, 1 over the D slot sums, in place in shared memory.  A slot past D
+//     is +0.  At level 16 every slot l < min(D, 16) is added its partner (s[l + 16], or +0 where l + 16 >= D), as the butterfly does;
+//     at the lower levels the adds of +0 are skipped: such a slot l received +0 at level 16 and no real add since (l + off >= D
+//     implies l + 2 off >= D), and (x + 0) + 0 == x + 0 for every x, so the skipped adds change no bit.
+template <int K, int KC>
+__global__ void __launch_bounds__(256, 2)
+frontend_shared_kernel(const RotState* __restrict__ rs /* nullptr: no rotation */, const float2* __restrict__ in /* the shared stream */,
+                       long long T, long long n_abs0 /* absolute index of in[0] */, const float2* __restrict__ hist /* [C][H] rotated */,
+                       int H, const float* __restrict__ ht /* [D][QP] chain order */, int QP, int ntaps, int D, int Qmax, int NB,
+                       int C, int CG, float2* __restrict__ out, long long out_stride, long long k0, long long k1)
+{
+    static_assert(K % 2 == 1 && KC % 4 == 0, "K odd (bank-conflict free window loads), KC a multiple of 4 (float4 tap loads)");
+    extern __shared__ __align__(16) float sm_fs[];
+    const int NOUT = NB * K, MW = NOUT + Qmax - 1, MWp = MW | 1, WN = D * MW;
+    float* hs = sm_fs;                                                   // D QP taps (QP a multiple of 4)
+    float2* rw = reinterpret_cast<float2*>(sm_fs + D * QP);             // WN raw samples
+    float2* xr = rw + WN;                                                // [D][MWp] rotated, polyphase split
+    float2* ps = xr + D * MWp;                                           // [D][NOUT] slot sums
+    const long long kb = k0 + static_cast<long long>(blockIdx.x) * NOUT;
+    const int nout = (k1 - kb) < NOUT ? static_cast<int>(k1 - kb) : NOUT;
+    const long long a_lo = D * (kb - Qmax + 1) - (D - 1);              // absolute index of the oldest sample of the window
+    const float invD = 1.0f / static_cast<float>(D);
+    for (int i = threadIdx.x; i < D * QP; i += blockDim.x) hs[i] = ht[i];
+    for (int i = threadIdx.x; i < WN; i += blockDim.x) {                // each thread rotates below exactly the samples it loads here
+        const long long li = a_lo + i - n_abs0;
+        rw[i] = (li >= 0 && li < T) ? __ldg(in + li) : make_float2(0.0f, 0.0f);
+    }
+    const int c_end = (blockIdx.y + 1) * CG < C ? (blockIdx.y + 1) * CG : C;
+    for (int c = blockIdx.y * CG; c < c_end; c++) {
+        RotState r{ 0u, 0u, 0 };
+        if (rs) r = rs[c];
+        const float2* hc = hist + static_cast<long long>(c) * H;
+        for (int i = threadIdx.x; i < WN; i += blockDim.x) {
+            const long long a = a_lo + i, li = a - n_abs0;
+            float2 v = make_float2(0.0f, 0.0f);
+            if (li >= 0) {
+                if (li < T) {
+                    v = rw[i];
+                    if (rs) {
+                        const unsigned ph = r.base + r.inc * static_cast<unsigned>(a - r.n_base);
+                        const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
+                        float sn, cs;
+                        qrl_sincosf(ang, sn, cs);
+                        v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
+                    }
+                }
+            } else if (H + li >= 0) v = hc[H + li];
+            const int m = static_cast<int>((static_cast<float>(i) + 0.5f) * invD);   // i / D (exact: i < 2^16, D <= 32)
+            xr[(D - 1 - (i - m * D)) * MWp + m] = v;
+        }
+        __syncthreads();
+        for (int it = threadIdx.x; it < D * NB; it += blockDim.x) {
+            const int br = it / NB, b = it - br * NB;
+            const int Qr = (ntaps - 1 - br) / D + 1;
+            const float2* xp = xr + br * MWp + b * K + (Qmax - Qr);     // xp[s + i]: the sample of output b K + i at chain step s
+            const float* hp = hs + br * QP;
+            float2 acc[K];
+#pragma unroll
+            for (int i = 0; i < K; i++) acc[i] = make_float2(0.0f, 0.0f);
+            int s0 = 0;
+            for (; s0 + KC <= Qr; s0 += KC) {
+                float h[KC];
+#pragma unroll
+                for (int i = 0; i < KC; i += 4) {
+                    const float4 t = *reinterpret_cast<const float4*>(hp + s0 + i);
+                    h[i] = t.x; h[i + 1] = t.y; h[i + 2] = t.z; h[i + 3] = t.w;
+                }
+#pragma unroll
+                for (int u = 0; u < K + KC - 1; u++) {
+                    const float2 v = xp[s0 + u];
+#pragma unroll
+                    for (int i = 0; i < K; i++) {
+                        const int j = u - i;
+                        if (j >= 0 && j < KC) ffma2(acc[i], h[j], v);
+                    }
+                }
+            }
+            for (; s0 < Qr; s0++) {
+                const float hv = hp[s0];
+#pragma unroll
+                for (int i = 0; i < K; i++) ffma2(acc[i], hv, xp[s0 + i]);
+            }
+            float2* pp = ps + br * NOUT + b * K;
+#pragma unroll
+            for (int i = 0; i < K; i++) pp[i] = acc[i];
+        }
+        __syncthreads();
+        float2* oc = out + static_cast<long long>(c) * out_stride + (kb - k0);
+        for (int u = threadIdx.x; u < nout; u += blockDim.x) {
+            float2* p = ps + u;
+            for (int l = 0; l < D && l < 16; l++) {
+                const float2 a = p[l * NOUT];
+                const float2 b = l + 16 < D ? p[(l + 16) * NOUT] : make_float2(0.0f, 0.0f);
+                p[l * NOUT] = make_float2(a.x + b.x, a.y + b.y);
+            }
+            for (int off = 8; off >= 1; off >>= 1)
+                for (int l = 0; l < off && l + off < D; l++) {
+                    const float2 a = p[l * NOUT], b = p[(l + off) * NOUT];
+                    p[l * NOUT] = make_float2(a.x + b.x, a.y + b.y);
+                }
+            oc[u] = p[0];
+        }
+    }
+}
+
 // Transmit front end at device rates >= 2 Msps (gr_mod_base.cpp:38,211-259): rotator_cc at 1 Msps fused into
 // rational_resampler_ccf(L, 1) with L = samp_rate / 1e6 and about 210 taps per arm, y[L m + p] = sum_k arm[p][k] x[m - k].
 // The arms are too long for interp_fir_ccf_rt_kernel's all-taps-in-registers shape, so:

@@ -22,18 +22,23 @@ class Frontend(Handle):
         check(self._L.qrl_frontend_set_carrier_offset(self._h, channel, float(hz)), self._h, "qrl_frontend_set_carrier_offset")
 
     def work(self, iq):
-        """iq: complex64 [n_channels, T] at the device rate (host) -> complex64 [n_channels, n_out] at 1 Msps."""
+        """iq at the device rate (host), complex64: [n_channels, T], one stream per channel, or [T], one wideband stream that every
+        channel reads at its own carrier offset -> complex64 [n_channels, n_out] at 1 Msps."""
         iq = np.ascontiguousarray(iq, np.complex64)
         if iq.ndim == 1:
-            iq = iq[None, :]
-        T = iq.shape[1]
+            T, stride = iq.shape[0], 0
+        elif iq.ndim == 2 and iq.shape[0] == self.n_channels:
+            T = stride = iq.shape[1]
+        else:
+            raise ValueError("Frontend.work: iq must be [T] (one shared stream) or [%d, T], got shape %s" % (self.n_channels, iq.shape))
         n = C.c_long()
-        check(self._L.qrl_frontend_work(self._h, iq.ctypes.data_as(C.c_void_p), T, T, 0, C.byref(n)), self._h, "qrl_frontend_work")
+        check(self._L.qrl_frontend_work(self._h, iq.ctypes.data_as(C.c_void_p), T, stride, 0, C.byref(n)), self._h, "qrl_frontend_work")
         out = np.zeros((self.n_channels, max(1, n.value)), np.complex64)
         check(self._L.qrl_frontend_read(self._h, out.ctypes.data_as(C.c_void_p), out.shape[1]), self._h, "qrl_frontend_read")
         return out[:, :n.value]
 
     def work_device(self, dev_ptr, T, stride):
+        """device input: channel c reads dev_ptr[c * stride ..][:T]; stride 0 = one stream for every channel."""
         n = C.c_long()
         check(self._L.qrl_frontend_work(self._h, C.c_void_p(dev_ptr), T, stride, 1, C.byref(n)), self._h, "qrl_frontend_work")
         return n.value
