@@ -197,9 +197,11 @@ int qrl_tx_profile_read(qrl_tx* h, int stage, double* ms_total, long* n_launches
  * every channel (one SDR, n_channels receivers at their own carrier offsets, gr_demod_mmdvm_multi.cpp:68-123); channel c's output is
  * what [n_channels][T] with n_channels identical rows would give, bit for bit.  Host input is copied to the device once (T samples),
  * device input is read in place.  A handle may alternate between shared and per-channel calls: each channel's stream continues.
- * T > max_in returns QRL_ERANGE; T == 0 returns QRL_OK with no output. */
+ * T > max_in returns QRL_ERANGE; T == 0 returns QRL_OK with no output.
+ * samp_rate: a multiple of 1 MHz from 2 to 107 Msps.  Above 107 Msps the /N filter (4517 taps at 108 Msps) and its window no longer fit
+ * the decimating kernel's 160 KiB of shared memory, and create returns QRL_EINVAL. */
 typedef struct qrl_frontend qrl_frontend;
-int  qrl_frontend_create(int samp_rate /* multiple of 1e6, >= 2e6 */, int n_channels, long max_in, int device, qrl_frontend** out);
+int  qrl_frontend_create(int samp_rate /* multiple of 1e6, 2e6 .. 107e6 */, int n_channels, long max_in, int device, qrl_frontend** out);
 int  qrl_frontend_destroy(qrl_frontend*);
 int  qrl_frontend_set_stream(qrl_frontend*, void* cuda_stream);
 int  qrl_frontend_set_carrier_offset(qrl_frontend*, int channel /* -1 = all */, double offset_hz);
@@ -256,7 +258,9 @@ int qrl_design_deemph(int fs, double tau, double* a2, double* b2);
  * channel-rate sample), which the symbol-timing loops downstream absorb. */
 enum { QRL_PFB_CHANNELIZER = 201, QRL_PFB_SYNTHESIZER = 202 };
 typedef struct qrl_pfb qrl_pfb;
-/* max_in: channelizer = wideband samples per call; synthesizer = columns (samples per channel) per call */
+/* max_in: channelizer = wideband samples per call; synthesizer = columns (samples per channel) per call.
+ * Accepted shapes: 1 <= M <= 64 and ceil(ntaps / M) <= 128 taps per branch; anything else returns QRL_EINVAL.  M = 10 with 35 taps
+ * per branch (the reference's 341-tap prototype) runs register-tiled kernels, every other accepted shape generic ones. */
 int  qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, int device, qrl_pfb** out);
 int  qrl_pfb_destroy(qrl_pfb*);
 int  qrl_pfb_set_stream(qrl_pfb*, void* cuda_stream);

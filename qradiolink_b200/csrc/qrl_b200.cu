@@ -2794,6 +2794,10 @@ size_t fesh_smem(int D, int QP, int Qmax, int NB)
     const int NOUT = NB * FESH_K, MW = NOUT + Qmax - 1;
     return sizeof(float) * D * QP + sizeof(float2) * D * (MW + (MW | 1) + NOUT);
 }
+// frontend_fir_kernel (per-channel calls, and shared calls above FESH_DMAX): the taps (rounded up to even) and the window of 128
+// outputs.  Both grow with the rate, and FEFIR_SMEM_MAX caps it: 107 Msps needs 162 416 B (4475 taps), 108 Msps 163 936 B.
+constexpr size_t FEFIR_SMEM_MAX = 160 * 1024;
+size_t fefir_smem(int D, int ntaps) { return sizeof(float) * ((ntaps + 1) & ~1) + sizeof(float2) * (127 * static_cast<size_t>(D) + ntaps); }
 }  // namespace
 
 struct qrl_frontend : HandleBase {
@@ -2807,6 +2811,7 @@ struct qrl_frontend : HandleBase {
     // shared stream (stride 0): [max_in] host staging, and frontend_shared_kernel's chain-order taps [D][QP] and strip shape
     float2* d_in1 = nullptr;
     float* d_ht = nullptr; int QP = 0, Qmax = 0, NB = 0, n_sm = 0; size_t fs_smem = 0;
+    size_t fir_smem = 0;                // frontend_fir_kernel's dynamic shared memory
 };
 
 int qrl_frontend_destroy(qrl_frontend* h) { return h ? handle_close(h) : QRL_OK; }
@@ -2814,15 +2819,21 @@ int qrl_frontend_create(int samp_rate, int n_channels, long max_in, int device, 
 {
     if (!out || n_channels <= 0 || max_in <= 0 || samp_rate < 2000000 || samp_rate % 1000000) { set_err(nullptr, "qrl_frontend_create: bad argument (samp_rate must be a multiple of 1e6, >= 2e6)"); return QRL_EINVAL; }
     *out = nullptr;
+    // gr_demod_base.cpp:1329-1333: low_pass(1, samp_rate, 480000, 100000, BLACKMAN_HARRIS) in rational_resampler_ccf(1, samp_rate / 1e6)
+    std::vector<float> taps = low_pass(1, samp_rate, 480000, 100000, WIN_BLACKMAN_HARRIS);
+    const size_t fir_smem = fefir_smem(samp_rate / 1000000, static_cast<int>(taps.size()));
+    if (fir_smem > FEFIR_SMEM_MAX) {
+        set_err(nullptr, "qrl_frontend_create: samp_rate above 107 Msps (the decimating FIR's " + std::to_string(taps.size()) +
+                             " taps and window need " + std::to_string(fir_smem) + " B of shared memory, the limit is 160 KiB)");
+        return QRL_EINVAL;
+    }
     if (int rc = check_device("qrl_frontend_create", device)) return rc;
     qrl_frontend* h = new qrl_frontend();
-    h->samp_rate = samp_rate; h->D = samp_rate / 1000000; h->C = n_channels; h->max_in = max_in;
+    h->samp_rate = samp_rate; h->D = samp_rate / 1000000; h->C = n_channels; h->max_in = max_in; h->fir_smem = fir_smem;
     auto fail = [&](int rc) { return create_failed(h, qrl_frontend_destroy, rc); };
     int rc = handle_open(h, device);
     if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
-    // gr_demod_base.cpp:1329-1333: low_pass(1, samp_rate, 480000, 100000, BLACKMAN_HARRIS) in rational_resampler_ccf(1, samp_rate / 1e6)
-    std::vector<float> taps = low_pass(1, samp_rate, 480000, 100000, WIN_BLACKMAN_HARRIS);
     h->ntaps = static_cast<int>(taps.size());
     h->H = h->ntaps + h->D;
     if ((rc = upload_floats(h, &h->d_taps, taps))) return fail(rc);
@@ -2906,12 +2917,10 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
                                                     h->NB, h->C, CG, h->d_out, h->out_stride, k0, k1);
         h->launches++;
     } else if (k1 > k0) {
-        const size_t smem = sizeof(float) * ((h->ntaps + 1) & ~1) + sizeof(float2) * (127 * h->D + h->ntaps);
-        if (int rc = smem_opt_in(h, frontend_fir_kernel, 160 * 1024)) return rc;
-        if (smem > 160 * 1024) { set_err(h, "qrl_frontend_work: device rate too high for this kernel"); return QRL_EINVAL; }
+        if (int rc = smem_opt_in(h, frontend_fir_kernel, static_cast<int>(FEFIR_SMEM_MAX))) return rc;       // create checked fir_smem
         dim3 g(static_cast<unsigned>((k1 - k0 + 127) / 128), h->C);
-        frontend_fir_kernel<<<g, 128, smem, h->stream>>>(rs, x, xstride, T, h->n_in, h->d_hist[h->hist_cur], h->H, h->d_taps, h->ntaps, h->D,
-                                                          h->d_out, h->out_stride, k0, k1);
+        frontend_fir_kernel<<<g, 128, h->fir_smem, h->stream>>>(rs, x, xstride, T, h->n_in, h->d_hist[h->hist_cur], h->H, h->d_taps,
+                                                                h->ntaps, h->D, h->d_out, h->out_stride, k0, k1);
         h->launches++;
     }
     dim3 gh((h->H + 127) / 128, h->C);

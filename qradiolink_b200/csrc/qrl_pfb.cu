@@ -314,6 +314,10 @@ struct qrl_pfb : QrlHandleBase {        // err / device / stream / launches / al
 
 namespace {
 constexpr int kFastM = 10, kFastTpf = 35, kChanR = 9, kChanG = 32, kSynR = 10, kSynG = 32;
+constexpr int kMaxM = 64, kMaxTpf = 128, kGenericItems = 2048;
+// pfb_synth_generic_kernel's window [M][tn + tpf - 1] with tn = max(1, 2048 / M): M tn <= 2048, so at most 2048 + 64 * 127 items
+// (81 408 B at M = 64, tpf = 128), above the 48 KiB a launch gets without opting in
+constexpr int kSynGenericSmemMax = static_cast<int>(sizeof(float2)) * (kGenericItems + kMaxM * (kMaxTpf - 1));
 long long chan_hist_len(int tpf, int M, int pend) { return (static_cast<long long>(tpf - 1) * M + pend + 2) & ~1LL; }
 }  // namespace
 
@@ -327,8 +331,8 @@ int qrl_pfb_destroy(qrl_pfb* h)
 
 int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, int device, qrl_pfb** out)
 {
-    if (!out || !taps || (kind != QRL_PFB_CHANNELIZER && kind != QRL_PFB_SYNTHESIZER) || M < 1 || M > 64 || ntaps < 1 ||
-        max_in < 1 || (ntaps + M - 1) / M > 128) {
+    if (!out || !taps || (kind != QRL_PFB_CHANNELIZER && kind != QRL_PFB_SYNTHESIZER) || M < 1 || M > kMaxM || ntaps < 1 ||
+        max_in < 1 || (ntaps + M - 1) / M > kMaxTpf) {
         set_err(nullptr, "qrl_pfb_create: bad argument");
         return QRL_EINVAL;
     }
@@ -400,7 +404,7 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                     h->d_bt, h->d_w, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames,
                     h->d_out, h->out_stride, use_tma);
             } else {
-                const int tm = std::max(1, 2048 / M);
+                const int tm = std::max(1, kGenericItems / M);
                 pfb_chan_generic_kernel<<<static_cast<unsigned>((frames + tm - 1) / tm), 256, sizeof(float2) * tm * M, h->stream>>>(
                     M, tpf, h->d_bt, h->d_w, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames,
                     h->d_out, h->out_stride, tm);
@@ -434,7 +438,8 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                 kern<<<static_cast<unsigned>((n_in + TN - 1) / TN), kFastM * kSynG, smem, h->stream>>>(
                     h->d_bt, h->d_w, hist, x, stride, n_in, h->d_out);
             } else {
-                const int tn = std::max(1, 2048 / M);
+                const int tn = std::max(1, kGenericItems / M);
+                if (int rc = smem_opt_in(h, pfb_synth_generic_kernel, kSynGenericSmemMax)) return rc;
                 pfb_synth_generic_kernel<<<static_cast<unsigned>((n_in + tn - 1) / tn), 256, sizeof(float2) * M * (tn + tpf - 1), h->stream>>>(
                     M, tpf, h->d_bt, h->d_w, hist, x, stride, n_in, h->d_out, tn);
             }

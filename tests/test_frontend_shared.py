@@ -1,6 +1,6 @@
 """CPU tier: the receive front end fed one wideband stream (qrl_frontend_work with stride 0), through the library's own sources run on
 host threads (tools/emu/build_emulated_lib.py): every channel equal to the oracle front end fed the same stream and to a twin handle
-fed identical rows; host, device and per-channel calls on one handle; Frontend.work's shape rules."""
+fed identical rows; host, device and per-channel calls on one handle; the top rate create accepts; Frontend.work's shape rules."""
 import os
 import sys
 
@@ -47,6 +47,14 @@ def test_host_device_and_per_channel_calls_on_one_handle(emu_frontend, oracle):
     from tests import test_gpu_frontend_shared as TG
     TG.parity(emu_frontend, oracle, 2000000, 3, [2500, 777, 3100, 5, 2000], RETUNES, kinds=("host", "dev", "rows"),
               dev_input=_host_as_device)
+
+
+def test_top_rate_is_checked_at_create(emu_frontend):
+    """107 Msps is the highest rate whose decimating FIR fits its kernel's shared memory: 108 Msps fails at create with the limit named"""
+    emu_frontend.Frontend(107000000, n_channels=2, max_in=4096).close()
+    for rate in (108000000, 250000000):
+        with pytest.raises(emu_frontend.QrlError, match="qrl_frontend_create: samp_rate above 107 Msps"):
+            emu_frontend.Frontend(rate, n_channels=2, max_in=4096)
 
 
 def test_shapes(emu_frontend):

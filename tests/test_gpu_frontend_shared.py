@@ -11,8 +11,9 @@ from tests import siggen
 
 pytestmark = pytest.mark.gpu
 
-SIZES = [20000, 0, 1, 3, 50, 7777, 2501, 60000]
+SIZES = [20000, 0, 1, 3, 50, 7777, 2501, 60000]  # at 107 Msps the last chunk alone is 560 outputs: five 128-output CTAs per channel
 TOP_TILED = 32                                  # frontend_shared_kernel serves N <= 32; above, frontend_fir_kernel reads the one stream
+TOP_RATE = 107000000                            # the highest rate qrl_frontend_create accepts (frontend_fir_kernel's shared memory)
 
 
 def _same(a, b):
@@ -98,10 +99,10 @@ def _offsets(samp_rate, Cn):
 RETUNES_ALL = {3: [(-1, 137500.0)], 5: [(1, -250000.0)]}
 
 
-@pytest.mark.parametrize("samp_rate", [2000000, 5000000, 10000000, 20000000, TOP_TILED * 1000000, (TOP_TILED + 1) * 1000000])
+@pytest.mark.parametrize("samp_rate", [2000000, 5000000, 10000000, 20000000, TOP_TILED * 1000000, (TOP_TILED + 1) * 1000000, TOP_RATE])
 def test_shared_stream_matches_twin_and_oracle(qrl, oracle, samp_rate):
     """3 channels at their own offsets (channel 0 at zero until all retune), then a retune of all and of one; host and device input
-    at an odd sample offset, and per-channel calls, on one handle"""
+    at an odd sample offset, and per-channel calls, on one handle; up to the top rate (4475 taps, 162 416 B of shared memory)"""
     r = _offsets(samp_rate, 3)
     r.update(RETUNES_ALL)
     parity(qrl, oracle, samp_rate, 3, SIZES, r, kinds=("host", "dev", "rows", "host", "dev"), dev_input=torch_device_input)
@@ -173,4 +174,14 @@ def test_shared_stream_error_codes(qrl):
     assert L.qrl_frontend_work(fe._h, x.ctypes.data_as(C.c_void_p), 17, 0, 0, C.byref(n)) == -34       # QRL_ERANGE
     assert L.qrl_frontend_work(fe._h, x.ctypes.data_as(C.c_void_p), 0, 0, 0, C.byref(n)) == 0 and n.value == 0
     assert fe.out_device()[2] == 0
+    fe.close()
+    # above the top rate the decimating FIR does not fit its kernel's shared memory: refused at create, not at every work call
+    h = C.c_void_p()
+    assert L.qrl_frontend_create(TOP_RATE + 1000000, 3, 4096, 0, C.byref(h)) == -22 and not h.value        # QRL_EINVAL
+    msg = L.qrl_last_error(None).decode()
+    assert msg.startswith("qrl_frontend_create: ") and "107 Msps" in msg, msg
+    with pytest.raises(qrl.QrlError, match="107 Msps"):
+        qrl.Frontend(108000000, n_channels=3, max_in=4096)
+    fe = qrl.Frontend(TOP_RATE, n_channels=3, max_in=4096)
+    assert fe.work(np.zeros(4096, np.complex64)).shape == (3, 39)
     fe.close()

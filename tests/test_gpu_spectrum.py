@@ -26,14 +26,15 @@ def check(got, want, where):
     assert np.sqrt(np.mean((ag - aw) ** 2)) < 1e-5 * np.sqrt(np.mean(aw ** 2)), where
 
 
-@pytest.mark.parametrize("n_fft", [256, 2048, 32768, 65536])
-def test_spectrum_matches_the_oracle(qrl, oracle, n_fft):
-    S = 3
-    rng = np.random.default_rng(8100 + n_fft)
+def ragged_parity(qrl, oracle, n_fft, window, S, seed, oracle_window=None):
+    """S streams through one handle and through S oracle blocks in the same ragged calls (the first while disabled); every other call
+    fetches the spectra: the same ready / not-ready sequence, each stream within check() and its strongest line on the right bin.
+    Returns the fetched spectra."""
+    rng = np.random.default_rng(seed)
     n = 7 * n_fft + 1234
     X = signal(rng, S, n)
-    g = qrl.Spectrum(n_fft, 5, n_streams=S, max_samples=3 * n_fft + 64)
-    os_ = [oracle.Spectrum(n_fft, oracle.WIN_BLACKMAN_HARRIS) for _ in range(S)]
+    g = qrl.Spectrum(n_fft, window, n_streams=S, max_samples=3 * n_fft + 64)
+    os_ = [oracle.Spectrum(n_fft, window if oracle_window is None else oracle_window) for _ in range(S)]
     sizes = [n_fft // 3, 17, n_fft, n_fft // 2 + 5, 2 * n_fft + 9, 100, n_fft - 1, 3 * n_fft]
     g.work(X[:, :50])                                   # disabled: dropped on both sides
     for o, x in zip(os_, X):
@@ -41,7 +42,7 @@ def test_spectrum_matches_the_oracle(qrl, oracle, n_fft):
     g.set_enabled(True)
     for o in os_:
         o.set_enabled(True)
-    lo, ready = 0, 0
+    lo, spectra = 0, []
     for step, m in enumerate(sizes):
         m = min(m, n - lo)
         g.work(X[:, lo:lo + m])
@@ -53,11 +54,46 @@ def test_spectrum_matches_the_oracle(qrl, oracle, n_fft):
             want = [o.get() for o in os_]
             assert (got is None) == (want[0] is None), step
             if got is not None:
-                ready += 1
+                spectra.append(got)
                 for s in range(S):
                     check(got[s], want[s], (step, s))
-                    assert abs(int(np.argmax(got[s])) - (n_fft // 2 + round((0.05 + 0.11 * s) * n_fft))) <= 1
-    assert ready >= 3
+                    f = (0.05 + 0.11 * s + 0.5) % 1.0 - 0.5                    # stream s's strong line, aliased into [-fs/2, fs/2)
+                    assert abs(int(np.argmax(got[s])) - (n_fft // 2 + round(f * n_fft))) <= 1, (step, s)
+    assert len(spectra) >= 3
+    g.close()
+    return spectra
+
+
+@pytest.mark.parametrize("n_fft", [256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536])
+def test_spectrum_matches_the_oracle(qrl, oracle, n_fft):
+    """every size the handle accepts: each is its own (N1, N2) split of the four-step FFT"""
+    ragged_parity(qrl, oracle, n_fft, oracle.WIN_BLACKMAN_HARRIS, 3, 8100 + n_fft)
+
+
+@pytest.mark.parametrize("window", [0, 1, 2, 3, 5])
+def test_spectrum_windows(qrl, oracle, window):
+    """Hamming, Hann, Blackman, rectangular and Blackman-Harris against the oracle's window of the same type"""
+    ragged_parity(qrl, oracle, 4096, window, 3, 8300 + window)
+
+
+def test_spectrum_out_of_range_window_is_hamming(qrl, oracle):
+    """a window type outside 0..7 is Hamming (rx_fft.cpp:176-179): bit for bit what type 0 gives, and the oracle's Hamming"""
+    ham = ragged_parity(qrl, oracle, 4096, 0, 3, 8400)
+    for window in (-1, 8, 9):
+        got = ragged_parity(qrl, oracle, 4096, window, 3, 8400, oracle_window=oracle.WIN_HAMMING)
+        assert len(got) == len(ham) and all(np.array_equal(a.view(np.uint32), b.view(np.uint32)) for a, b in zip(got, ham)), window
+
+
+@pytest.mark.parametrize("window", [4, 6, 7])
+def test_spectrum_refuses_the_windows_it_does_not_build(qrl, window):
+    """Kaiser, Bartlett and flat-top are valid types that this handle does not build: create fails instead of using another window"""
+    with pytest.raises(qrl.QrlError, match="window type not built"):
+        qrl.Spectrum(4096, window)
+
+
+def test_spectrum_many_streams(qrl, oracle):
+    """37 streams from host input (a stream per channel of a batch): every stream against its own oracle block"""
+    ragged_parity(qrl, oracle, 1024, oracle.WIN_BLACKMAN_HARRIS, 37, 8500)
 
 
 def test_spectrum_set_fft_size_and_device_input(qrl, oracle):
