@@ -230,6 +230,35 @@ int  qrl_tx_frontend_out_device(qrl_tx_frontend*, float** data, long* stride, lo
 int  qrl_tx_frontend_read(qrl_tx_frontend*, float* dst /* [n_channels][cap] gr_complex */, long cap);
 long qrl_tx_frontend_launch_count(const qrl_tx_frontend*);
 
+/* ---- transmit combiner: N modulators -> one SDR sink ------------------------------------------------------------------------------------
+ * gr_mod_mmdvm_multi (src/gr/gr_mod_mmdvm_multi.cpp:53-125) wired for a batch of channels at SDR rates: per channel c, gr_mod_base's
+ * interpolator rational_resampler_ccf(N, 1, low_pass(N, samp_rate, 480000, 20000, BLACKMAN_HARRIS)) with N = samp_rate / 1e6 (none at
+ * 1 Msps), then rotator_cc(2 pi offset_c / samp_rate) AT THE DEVICE RATE, so a channel can sit anywhere in +-samp_rate / 2; then add_cc
+ * over the channels, multiply_const_cc(1 / n_channels) and multiply_const_cc(bb_gain) (default 1).  Out: ONE stream of N n gr_complex.
+ *   - rows: a host array of n_channels pointers to n gr_complex each at 1 Msps, 8-byte aligned; all in host memory (on_device = 0,
+ *     staged into a [n_channels][max_in] buffer) or all on the handle's device (on_device = 1, read in place: e.g. qrl_tx_out_device's
+ *     pointer + c stride, or rows of several modulator handles).  Device rows are read on the combiner's stream: the caller orders
+ *     their producers before the call (one shared stream through *_set_stream, or a synchronisation).
+ *   - Channels are added in blocks of 8, left to right from each block's first channel, then the block sums left to right: the order
+ *     does not depend on chunking or launch shape (with n_channels <= 8 it is add_cc's order).
+ *   - Streaming: any chunking gives the same output, n = 0 is valid and gives none.  A carrier-offset change (channel -1 = all) is
+ *     phase-continuous from the next output sample; a channel whose rotator never turned (offset 0 since create) is passed unrotated.
+ *     A gain change applies from the next call.
+ *   - Errors: QRL_EINVAL for a bad samp_rate, channel, a NULL or misaligned row, |offset| > samp_rate / 2, or a device row of another
+ *     GPU; QRL_ERANGE for n > max_in.  The output stays on the device until the next work (qrl_tx_combiner_out_device) or is copied out
+ *     with qrl_tx_combiner_read.  destroy(NULL) is QRL_OK. */
+typedef struct qrl_tx_combiner qrl_tx_combiner;
+int  qrl_tx_combiner_create(int samp_rate /* multiple of 1e6, 1e6..32e6 */, int n_channels, long max_in, int device, qrl_tx_combiner** out);
+int  qrl_tx_combiner_destroy(qrl_tx_combiner*);
+int  qrl_tx_combiner_set_stream(qrl_tx_combiner*, void* cuda_stream);
+int  qrl_tx_combiner_set_carrier_offset(qrl_tx_combiner*, int channel /* -1 = all */, double offset_hz /* |f| <= samp_rate / 2 */);
+int  qrl_tx_combiner_set_gain(qrl_tx_combiner*, float bb_gain);
+int  qrl_tx_combiner_work(qrl_tx_combiner*, const float* const* rows /* host array of n_channels row pointers */, long n, int on_device,
+                          long* n_out /* N n */);
+int  qrl_tx_combiner_out_device(qrl_tx_combiner*, float** data, long* n_out);   /* one stream, valid until the next work */
+int  qrl_tx_combiner_read(qrl_tx_combiner*, float* dst /* cap gr_complex */, long cap);
+long qrl_tx_combiner_launch_count(const qrl_tx_combiner*);
+
 /* ---- design helpers (host only; the gr::filter::firdes calls the reference makes at construction /
  *      in set_filter_width, e.g. gr_demod_nbfm.cpp:82-90).  Return tap count or negative error. ---- */
 int qrl_firdes_low_pass(double gain, double fs, double fc, double tw, int window, float* out, int cap);

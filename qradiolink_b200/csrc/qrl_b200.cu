@@ -2958,6 +2958,28 @@ namespace {
 // N = 2 against 0.56 with R = 18 (64 channels, H100 SXM at 700 W; R = 14 / 16 / 17 / 18 measured at N = 2 ... 32, 18 the best or
 // within 2 % at every N)
 constexpr int TXFE_KC = 10, TXFE_R = 18;
+
+// gr_mod_base.cpp:211-259: rational_resampler_ccf(N, 1, low_pass(N, samp_rate, 480000, 20000, BLACKMAN_HARRIS)) as the arm table of
+// the interpolating kernels ([NTP][N], the taps zero-padded to NTP N, NTP a multiple of kc), and G, the groups of N threads of a CTA
+struct TxInterp { std::vector<float> arms; int ntaps = 0, NTP = 0, G = 0; };
+TxInterp tx_interp_design(int samp_rate, int kc)
+{
+    const int N = samp_rate / 1000000;
+    TxInterp d;
+    d.arms = low_pass(N, samp_rate, 480000, 20000, WIN_BLACKMAN_HARRIS);
+    d.ntaps = static_cast<int>(d.arms.size());
+    const int nt = (d.ntaps + N - 1) / N;
+    d.NTP = (nt + kc - 1) / kc * kc;
+    d.arms.resize(static_cast<size_t>(d.NTP) * N, 0.0f);
+    // threads per CTA = N G: whole warps where possible, near 256
+    double best = -1.0;
+    for (int g = (128 + N - 1) / N; g * N <= 512; g++) {
+        const int t = g * N;
+        const double eff = t / (32.0 * ((t + 31) / 32)) - std::abs(t - 256) * 1e-6;
+        if (eff > best) { best = eff; d.G = g; }
+    }
+    return d;
+}
 }  // namespace
 
 struct qrl_tx_frontend : HandleBase {
@@ -2986,21 +3008,10 @@ int qrl_tx_frontend_create(int samp_rate, int n_channels, long max_in, int devic
     if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
     if (h->N >= 2) {
-        // gr_mod_base.cpp:211-259: rational_resampler_ccf(N, 1, low_pass(N, samp_rate, 480000, 20000, BLACKMAN_HARRIS))
-        std::vector<float> taps = low_pass(h->N, samp_rate, 480000, 20000, WIN_BLACKMAN_HARRIS);
-        h->ntaps = static_cast<int>(taps.size());
-        const int nt = (h->ntaps + h->N - 1) / h->N;
-        h->NTP = (nt + TXFE_KC - 1) / TXFE_KC * TXFE_KC;
+        const TxInterp d = tx_interp_design(samp_rate, TXFE_KC);
+        h->ntaps = d.ntaps; h->NTP = d.NTP; h->G = d.G;
         h->H = h->NTP - 1;
-        taps.resize(static_cast<size_t>(h->NTP) * h->N, 0.0f);
-        // threads per CTA = N G: whole warps where possible, near 256
-        double best = -1.0;
-        for (int g = (128 + h->N - 1) / h->N; g * h->N <= 512; g++) {
-            const int t = g * h->N;
-            const double eff = t / (32.0 * ((t + 31) / 32)) - std::abs(t - 256) * 1e-6;
-            if (eff > best) { best = eff; h->G = g; }
-        }
-        if ((rc = upload_floats(h, &h->d_arms, taps))) return fail(rc);
+        if ((rc = upload_floats(h, &h->d_arms, d.arms))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_hist[0], static_cast<size_t>(h->H) * h->C))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C))) return fail(rc);
     }
@@ -3097,6 +3108,171 @@ int qrl_tx_frontend_read(qrl_tx_frontend* h, float* dst, long cap)
     return QRL_OK;
 }
 long qrl_tx_frontend_launch_count(const qrl_tx_frontend* h) { return h ? h->launches : 0; }
+
+// ---------------------------------------------------------------------------------------------- transmit combiner (N modulators -> one SDR stream)
+namespace {
+// tx_combiner_kernel: taps per register chunk, outputs per thread (tx_frontend_interp_kernel's bank argument: R = 18 keeps the groups
+// of an N = 2 warp on different banks)
+constexpr int TXC_KC = 10, TXC_R = 18;
+// bound on the block partial sums: a call is cut into input ranges whose partials fit in this many bytes
+constexpr long long TXC_SCRATCH_BYTES = 64ll << 20;
+}  // namespace
+
+struct qrl_tx_combiner : HandleBase {
+    int samp_rate = 0, N = 1, C = 0, nblk = 1, NTP = 0, G = 0, H = 0, hist_cur = 0;
+    long max_in = 0;
+    long long range = 0;                        // input positions per launch range
+    float gain = 1.0f;
+    float* d_arms = nullptr;                    // [NTP][N]
+    float2* d_hist[2] = { nullptr, nullptr };   // [C][H]: the raw inputs' tail
+    float2* d_in = nullptr;                     // [C][max_in]: host rows staged
+    float2* d_y = nullptr; long n_out_last = 0; // [max_in N]: the summed stream
+    float2* d_part = nullptr;                   // [nblk][range N]: block partial sums (nblk > 1)
+    const float2** d_rows = nullptr; std::vector<const float2*> rows;
+    long long n_out = 0;                        // absolute device-rate index of the next output
+    std::vector<RotState> rot; RotState* d_rot = nullptr;
+};
+
+int qrl_tx_combiner_destroy(qrl_tx_combiner* h) { return h ? handle_close(h) : QRL_OK; }
+int qrl_tx_combiner_create(int samp_rate, int n_channels, long max_in, int device, qrl_tx_combiner** out)
+{
+    if (!out || n_channels <= 0 || max_in <= 0 || samp_rate < 1000000 || samp_rate > 32000000 || samp_rate % 1000000) {
+        set_err(nullptr, "qrl_tx_combiner_create: bad argument (samp_rate must be a multiple of 1e6 in [1e6, 32e6])");
+        return QRL_EINVAL;
+    }
+    *out = nullptr;
+    if (int rc = check_device("qrl_tx_combiner_create", device)) return rc;
+    qrl_tx_combiner* h = new qrl_tx_combiner();
+    h->samp_rate = samp_rate; h->N = samp_rate / 1000000; h->C = n_channels; h->max_in = max_in;
+    h->nblk = (n_channels + TXC_BLOCK - 1) / TXC_BLOCK;
+    auto fail = [&](int rc) { return create_failed(h, qrl_tx_combiner_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
+    if (rc) return fail(rc);
+    long long tile = 256;
+    if (h->N >= 2) {
+        const TxInterp d = tx_interp_design(samp_rate, TXC_KC);
+        h->NTP = d.NTP; h->G = d.G; h->H = h->NTP - 1;
+        tile = static_cast<long long>(h->G) * TXC_R;
+        if ((rc = upload_floats(h, &h->d_arms, d.arms))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_hist[0], static_cast<size_t>(h->H) * h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C))) return fail(rc);
+    }
+    h->range = max_in;
+    if (h->nblk > 1) {
+        const long long fit = TXC_SCRATCH_BYTES / (static_cast<long long>(h->nblk) * h->N * 8) / tile * tile;
+        h->range = std::min<long long>(max_in, std::max(fit, tile));
+        if ((rc = dev_alloc(h, &h->d_part, static_cast<size_t>(h->nblk) * h->range * h->N, false))) return fail(rc);
+    }
+    if ((rc = dev_alloc(h, &h->d_y, static_cast<size_t>(max_in) * h->N, false))) return fail(rc);
+    if ((rc = dev_alloc(h, &h->d_rows, h->C))) return fail(rc);
+    if ((rc = dev_alloc(h, &h->d_rot, h->C))) return fail(rc);
+    h->rows.assign(h->C, nullptr);
+    h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
+    *out = h;
+    return QRL_OK;
+}
+int qrl_tx_combiner_set_stream(qrl_tx_combiner* h, void* s)
+{
+    if (!h) return QRL_EINVAL;
+    return handle_set_stream(h, s);
+}
+int qrl_tx_combiner_set_carrier_offset(qrl_tx_combiner* h, int channel, double offset_hz)
+{
+    // gr_mod_mmdvm_multi.cpp:53-125: rotator_cc(2 pi offset / samp_rate) behind each channel's resampler, at the device rate
+    if (!h || channel < -1 || channel >= h->C || !(std::abs(offset_hz) <= 0.5 * h->samp_rate)) {
+        set_err(h, "qrl_tx_combiner_set_carrier_offset: bad channel or |offset| > samp_rate / 2");
+        return QRL_EINVAL;
+    }
+    const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(offset_hz / h->samp_rate * 4294967296.0))));
+    retune(h->rot, channel, inc, h->n_out);
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
+    return QRL_OK;
+}
+int qrl_tx_combiner_set_gain(qrl_tx_combiner* h, float bb_gain)
+{
+    if (!h) return QRL_EINVAL;
+    h->gain = bb_gain;
+    return QRL_OK;
+}
+int qrl_tx_combiner_work(qrl_tx_combiner* h, const float* const* rows, long n, int on_device, long* n_out)
+{
+    if (!h || !rows || n < 0) return QRL_EINVAL;
+    for (int c = 0; c < h->C; c++) {
+        if (!rows[c] || (reinterpret_cast<uintptr_t>(rows[c]) & 7)) {
+            set_err(h, "qrl_tx_combiner_work: row " + std::to_string(c) + " is NULL or not 8-byte aligned");
+            return QRL_EINVAL;
+        }
+    }
+    if (n > h->max_in) { set_err(h, "qrl_tx_combiner_work: n exceeds max_in given at create"); return QRL_ERANGE; }
+    if (on_device)
+        for (int c = 0; c < h->C; c++) { int rc = check_device_ptr(h, rows[c], "qrl_tx_combiner_work"); if (rc) return rc; }
+    h->n_out_last = 0;
+    if (n_out) *n_out = 0;
+    if (n == 0) return QRL_OK;
+    QRL_CK(cudaSetDevice(h->device));
+    if (!on_device && !h->d_in) { int rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_in) * h->C, false); if (rc) return rc; }
+    for (int c = 0; c < h->C; c++) {
+        if (on_device) { h->rows[c] = reinterpret_cast<const float2*>(rows[c]); continue; }
+        h->rows[c] = h->d_in + static_cast<long long>(c) * h->max_in;
+        QRL_CK(cudaMemcpyAsync(h->d_in + static_cast<long long>(c) * h->max_in, rows[c], sizeof(float2) * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    QRL_CK(cudaMemcpyAsync(h->d_rows, h->rows.data(), sizeof(float2*) * h->C, cudaMemcpyHostToDevice, h->stream));
+    const float g1 = 1.0f / static_cast<float>(h->C), g2 = h->gain;
+    const int final = h->nblk == 1;
+    const size_t smem = h->N >= 2 ? sizeof(float) * ((h->NTP * h->N + 3) & ~3) + sizeof(float2) * 2 * ((h->G * TXC_R + h->NTP + 1) & ~1) : 0;
+    auto kern = tx_combiner_kernel<TXC_KC, TXC_R>;
+    if (h->N >= 2) {
+        if (int rc = smem_opt_in(h, kern, 96 * 1024)) return rc;
+        if (smem > 96 * 1024) { set_err(h, "qrl_tx_combiner_work: arm table too large for this kernel"); return QRL_EINVAL; }
+    }
+    for (long long lo = 0; lo < n; lo += h->range) {
+        const long long hi = std::min<long long>(n, lo + h->range);
+        float2* dst = final ? h->d_y + lo * h->N : h->d_part;
+        const long long pstride = h->range * h->N;
+        if (h->N == 1) {
+            dim3 g(static_cast<unsigned>(std::min<long long>((hi - lo + 255) / 256, 4096)), h->nblk);
+            tx_combiner_direct_kernel<<<g, 256, 0, h->stream>>>(h->d_rows, h->C, h->d_rot, lo, hi, h->n_out, dst, pstride, final, g1, g2);
+        } else {
+            const long long TM = static_cast<long long>(h->G) * TXC_R;
+            dim3 g(static_cast<unsigned>((hi - lo + TM - 1) / TM), h->nblk);
+            kern<<<g, h->G * h->N, smem, h->stream>>>(h->d_rows, h->C, h->d_rot, n, lo, hi, h->n_out, h->d_hist[h->hist_cur],
+                                                      hi == n ? h->d_hist[h->hist_cur ^ 1] : nullptr, h->H, h->d_arms, h->N, h->NTP, h->G,
+                                                      dst, pstride, final, g1, g2);
+        }
+        h->launches++;
+        if (!final) {
+            const long long m = (hi - lo) * h->N;
+            tx_combiner_sum_kernel<<<static_cast<unsigned>(std::min<long long>((m + 255) / 256, 4096)), 256, 0, h->stream>>>(
+                h->d_part, pstride, h->nblk, m, h->d_y + lo * h->N, g1, g2);
+            h->launches++;
+        }
+    }
+    if (h->N >= 2) h->hist_cur ^= 1;
+    h->n_out += static_cast<long long>(n) * h->N;
+    h->n_out_last = n * h->N;
+    if (n_out) *n_out = h->n_out_last;
+    QRL_CK(cudaGetLastError());
+    return QRL_OK;
+}
+int qrl_tx_combiner_out_device(qrl_tx_combiner* h, float** data, long* n_out)
+{
+    if (!h) return QRL_EINVAL;
+    if (data) *data = reinterpret_cast<float*>(h->d_y);
+    if (n_out) *n_out = h->n_out_last;
+    return QRL_OK;
+}
+int qrl_tx_combiner_read(qrl_tx_combiner* h, float* dst, long cap)
+{
+    if (!h || !dst) return QRL_EINVAL;
+    const long w = std::min(cap, h->n_out_last);
+    if (w > 0) QRL_CK(cudaMemcpyAsync(dst, h->d_y, static_cast<size_t>(w) * 8, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+long qrl_tx_combiner_launch_count(const qrl_tx_combiner* h) { return h ? h->launches : 0; }
 
 // ---------------------------------------------------------------------------------------------- design helpers
 static int copy_out(const std::vector<float>& v, float* out, int cap, int per_item = 1)

@@ -3058,6 +3058,164 @@ tx_frontend_interp_kernel(const RotState* __restrict__ rs /* nullptr: no rotatio
     }
 }
 
+// ---- transmit combiner (gr_mod_mmdvm_multi.cpp:53-125 wiring, gr_mod_base's interpolator): per channel x L interpolation, then a
+// rotator at the DEVICE rate, then add_cc over the channels, x 1 / C, x bb_gain.  Channels are summed in blocks of TXC_BLOCK: within
+// a block left to right from its first channel, then the block sums left to right (tx_combiner_sum_kernel), so the order does not
+// depend on the launch shape or on how a stream is chunked.
+constexpr int TXC_BLOCK = 8;
+
+// the device-rate NCO of one channel at absolute output index n_abs: the Q32 phase and qrl_sincosf of frontend_hist_kernel, applied
+// after the interpolator; a channel with inc == base == 0 is not rotated (bit-exact pass-through)
+__device__ __forceinline__ float2 tx_combiner_rotate(const RotState& r, long long n_abs, float2 v)
+{
+    if (r.inc == 0u && r.base == 0u) return v;
+    const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs - r.n_base);
+    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
+    float sn, cs;
+    qrl_sincosf(ang, sn, cs);
+    return make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
+}
+
+// y = (S * g1) * g2 per component (scale2_linear_kernel's arithmetic: multiply_const_cc(1 / C) then multiply_const_cc(bb_gain))
+__device__ __forceinline__ float2 tx_combiner_scale(float2 v, float g1, float g2)
+{
+    v.x = v.x * g1; v.y = v.y * g1; v.x = v.x * g2; v.y = v.y * g2;
+    return v;
+}
+
+// L >= 2.  tx_frontend_interp_kernel's layout (a tile of G R input positions x all L phases, the arm table [NTP][L] in shared memory,
+// thread (phase p, group q) accumulating R outputs over KC-tap register chunks fed by broadcast window loads) with the channel loop
+// inside: CTA (tile, channel block) loads the arm table once and walks the block's channels in order.  Per channel the raw window
+// (the previous calls' tail from `hist` + this call's input) is fetched while the previous channel computes: two window buffers, the
+// 16-byte aligned body by cp.async.bulk on an mbarrier, the ragged ends (history, one odd sample, past T) by plain loads.  The FIR
+// result of every output is rotated by its own NCO value and added into tot[R].  final != 0 (one channel block): out = y, scaled;
+// else out = this block's partial sums [blockIdx.y][out_stride].  Outputs are those of input positions [m_base, m_end), stored at
+// (m - m_base) L + p.  new_hist != nullptr: the call's last tile also stores the raw tail, new_hist = last H samples of
+// (hist ++ x[0..T)), which its window always holds (T - H >= m0 - (NTP - 1)).
+template <int KC, int R>
+__global__ void __launch_bounds__(512)
+tx_combiner_kernel(const float2* const* __restrict__ rows /* [C] */, int C, const RotState* __restrict__ rs /* [C] device-rate NCOs */,
+                   long long T, long long m_base, long long m_end, long long nout_abs0 /* absolute output index of input 0 x L */,
+                   const float2* __restrict__ hist /* [C][H] raw */, float2* __restrict__ new_hist, int H /* NTP - 1 */,
+                   const float* __restrict__ arms /* [NTP][L] */, int L, int NTP, int G,
+                   float2* __restrict__ out, long long out_stride, int final, float g1, float g2)
+{
+    extern __shared__ __align__(16) float sm_txc[];
+    __shared__ __align__(8) uint64_t bar[2];
+    const int TM = G * R, W = TM + NTP - 1, WB = (W + 2) & ~1;
+    float* hs = sm_txc;                                                  // NTP * L taps
+    float2* win0 = reinterpret_cast<float2*>(sm_txc + ((NTP * L + 3) & ~3));   // two buffers of WB samples, 16-byte aligned
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    const int c0 = blockIdx.y * TXC_BLOCK, nc = min(TXC_BLOCK, C - c0);
+    const long long m0 = m_base + static_cast<long long>(blockIdx.x) * TM; // first input position of the tile
+    const long long E0 = m0 - (NTP - 1);                                 // window[i] = input sample E0 + i (E0 >= -H)
+    const bool tail = new_hist && blockIdx.x == gridDim.x - 1;
+    for (int i = tid; i < NTP * L; i += nthr) hs[i] = arms[i];
+    if (tid == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); mbar_fence_init(); }
+    __syncthreads();
+    // window of channel c0 + k into buffer b; returns where sample E0 sits (0 or 1: the body copy must start 16-byte aligned)
+    auto fill = [&](int k, int b) {
+        const int c = c0 + k;
+        const float2* x = rows[c];
+        const float2* hc = hist + static_cast<long long>(c) * H;
+        const int sh = static_cast<int>(((reinterpret_cast<unsigned long long>(x) >> 3) + static_cast<unsigned long long>(E0)) & 1ull);
+        float2* w = win0 + b * WB + sh;
+        long long a = E0 < 0 ? 0 : E0;
+        if ((a - E0 + sh) & 1) a++;
+        const long long e1 = min(E0 + W, T);
+        const long long e2 = e1 > a ? a + ((e1 - a) & ~1ll) : a;        // bulk body [a, e2): even length, both ends 16-byte aligned
+        if (tid == 0) {
+            fence_proxy_async();                                         // the generic proxy's reads of this buffer came before
+            mbar_expect_tx(&bar[b], static_cast<uint32_t>((e2 - a) * 8));
+            if (e2 > a) bulk_g2s(w + (a - E0), x + a, static_cast<uint32_t>((e2 - a) * 8), &bar[b]);
+        }
+        for (int i = tid; i < W; i += nthr) {
+            const long long e = E0 + i;
+            if (e >= a && e < e2) continue;
+            w[i] = e < 0 ? hc[H + e] : (e < T ? x[e] : make_float2(0.0f, 0.0f));
+        }
+        return sh;
+    };
+    const int p = tid % L, q = tid / L;
+    float2 tot[R];
+    int sh_next = fill(0, 0);
+    for (int k = 0; k < nc; k++) {
+        const int b = k & 1, sh = sh_next;
+        __syncthreads();                                                 // channel k's plain loads are in; buffer b ^ 1 is free
+        if (k + 1 < nc) sh_next = fill(k + 1, b ^ 1);
+        mbar_wait(&bar[b], (k >> 1) & 1);
+        const float2* w = win0 + b * WB + sh;
+        const int c = c0 + k;
+        if (tail)
+            for (int i = tid; i < H; i += nthr) new_hist[static_cast<long long>(c) * H + i] = w[T - H + i - E0];
+        float2 acc[R];
+#pragma unroll
+        for (int j = 0; j < R; j++) acc[j] = make_float2(0.0f, 0.0f);
+        const float2* s = w + q * R;                                     // s[j] = x[m0 + q R - (NTP - 1) + j]
+        for (int kb = NTP - KC; kb >= 0; kb -= KC) {
+            float h[KC];
+#pragma unroll
+            for (int i = 0; i < KC; i++) h[i] = hs[(kb + i) * L + p];
+            const float2* sb = s + (NTP - KC - kb);                      // output j, tap kb + KC - 1 - i reads sb[j + i]
+#pragma unroll
+            for (int u = 0; u < R + KC - 1; u++) {
+                const float2 v = sb[u];
+#pragma unroll
+                for (int j = 0; j < R; j++) {
+                    const int i = u - j;
+                    if (i >= 0 && i < KC) ffma2(acc[j], h[KC - 1 - i], v);
+                }
+            }
+        }
+        const RotState r = rs[c];
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            const float2 v = tx_combiner_rotate(r, nout_abs0 + (m0 + q * R + j) * L + p, acc[j]);
+            if (k == 0) tot[j] = v;
+            else { tot[j].x = tot[j].x + v.x; tot[j].y = tot[j].y + v.y; }
+        }
+    }
+    float2* o = out + (final ? 0ll : static_cast<long long>(blockIdx.y) * out_stride);
+#pragma unroll
+    for (int j = 0; j < R; j++) {
+        const long long m = m0 + q * R + j;
+        if (m < m_end) o[(m - m_base) * L + p] = final ? tx_combiner_scale(tot[j], g1, g2) : tot[j];
+    }
+}
+
+// L = 1 (no resampler in the reference's graph): rotate and add the block's channels sample by sample; same outputs and layout as
+// tx_combiner_kernel for input positions [m_base, m_end)
+__global__ void tx_combiner_direct_kernel(const float2* const* __restrict__ rows, int C, const RotState* __restrict__ rs, long long m_base,
+                                          long long m_end, long long nout_abs0, float2* __restrict__ out, long long out_stride, int final,
+                                          float g1, float g2)
+{
+    const int c0 = blockIdx.y * TXC_BLOCK, nc = min(TXC_BLOCK, C - c0);
+    float2* o = out + (final ? 0ll : static_cast<long long>(blockIdx.y) * out_stride);
+    for (long long m = m_base + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; m < m_end;
+         m += static_cast<long long>(gridDim.x) * blockDim.x) {
+        float2 t = tx_combiner_rotate(rs[c0], nout_abs0 + m, rows[c0][m]);
+        for (int k = 1; k < nc; k++) {
+            const float2 v = tx_combiner_rotate(rs[c0 + k], nout_abs0 + m, rows[c0 + k][m]);
+            t.x = t.x + v.x; t.y = t.y + v.y;
+        }
+        o[m - m_base] = final ? tx_combiner_scale(t, g1, g2) : t;
+    }
+}
+
+// y[i] = scale(((part[0][i] + part[1][i]) + ...) + part[nblk - 1][i]): the block sums in ascending block order
+__global__ void tx_combiner_sum_kernel(const float2* __restrict__ part, long long part_stride, int nblk, long long n, float2* __restrict__ y,
+                                       float g1, float g2)
+{
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        float2 t = part[i];
+        for (int b = 1; b < nblk; b++) {
+            const float2 v = part[b * part_stride + i];
+            t.x = t.x + v.x; t.y = t.y + v.y;
+        }
+        y[i] = tx_combiner_scale(t, g1, g2);
+    }
+}
+
 // roll the stage-1 history: new_hist = last H samples of (old_hist ++ iq[0..T))
 __global__ void hist_update_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
                                    const float2* __restrict__ old_hist, float2* __restrict__ new_hist, int H)

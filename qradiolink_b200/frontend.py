@@ -97,3 +97,58 @@ class TxFrontend(Handle):
         p, s, n = C.c_void_p(), C.c_long(), C.c_long()
         check(self._L.qrl_tx_frontend_out_device(self._h, C.byref(p), C.byref(s), C.byref(n)), self._h, "qrl_tx_frontend_out_device")
         return p.value, s.value, n.value
+
+
+class TxCombiner(Handle):
+    """N modulators -> one SDR sink, gr_mod_mmdvm_multi's wiring (gr_mod_mmdvm_multi.cpp:53-125) with gr_mod_base's interpolator: per
+    channel x samp_rate / 1e6, a rotator at the device rate (any offset within +-samp_rate / 2), add_cc, x 1 / C, x bb_gain.  The one
+    summed stream stays in HBM until read."""
+    ABI = "tx_combiner"
+
+    def __init__(self, samp_rate, n_channels=1, max_in=1 << 16, device=0):
+        self._L = load_library()
+        self.n_channels, self.max_in, self.interpolation = int(n_channels), int(max_in), int(samp_rate) // 1000000
+        self._create(self._L.qrl_tx_combiner_create, int(samp_rate), self.n_channels, self.max_in, device)
+
+    set_stream = Handle._set_stream
+    launches = property(Handle._launches)
+
+    def set_carrier_offset(self, hz, channel=-1):
+        check(self._L.qrl_tx_combiner_set_carrier_offset(self._h, channel, float(hz)), self._h, "qrl_tx_combiner_set_carrier_offset")
+
+    def set_gain(self, g):
+        check(self._L.qrl_tx_combiner_set_gain(self._h, float(g)), self._h, "qrl_tx_combiner_set_gain")
+
+    def _work(self, rows, n, on_device):
+        ptrs = (C.c_void_p * self.n_channels)(*rows)
+        out = C.c_long()
+        check(self._L.qrl_tx_combiner_work(self._h, ptrs, n, on_device, C.byref(out)), self._h, "qrl_tx_combiner_work")
+        return out.value
+
+    def work(self, iq):
+        """iq: complex64 [n_channels, n] at 1 Msps (host) -> complex64 [N n] at the device rate."""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        if iq.ndim != 2 or iq.shape[0] != self.n_channels:
+            raise ValueError("TxCombiner.work: iq must be [n_channels, n]")
+        self._work([iq.ctypes.data + c * iq.strides[0] for c in range(self.n_channels)], iq.shape[1], 0)
+        return self.read()
+
+    def work_device(self, rows, n):
+        """rows: n_channels device addresses of n gr_complex each (e.g. TxBlock.out_device()'s pointer + c stride, or rows of several
+        modulators on the combiner's stream); returns the number of output items (N n)."""
+        if len(rows) != self.n_channels:
+            raise ValueError("TxCombiner.work_device: need one row per channel")
+        return self._work([int(r) for r in rows], n, 1)
+
+    def read(self):
+        """complex64 [items] of the last call (waits for the handle's stream)."""
+        n = self.out_device()[1]
+        out = np.zeros(max(1, n), np.complex64)
+        check(self._L.qrl_tx_combiner_read(self._h, out.ctypes.data_as(C.c_void_p), n), self._h, "qrl_tx_combiner_read")
+        return out[:n]
+
+    def out_device(self):
+        """(device pointer, items) of the last call's summed stream, e.g. for Frontend.work_device(ptr, items, 0)."""
+        p, n = C.c_void_p(), C.c_long()
+        check(self._L.qrl_tx_combiner_out_device(self._h, C.byref(p), C.byref(n)), self._h, "qrl_tx_combiner_out_device")
+        return p.value, n.value

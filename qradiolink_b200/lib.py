@@ -105,6 +105,15 @@ SYMBOLS = {
     "qrl_tx_frontend_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_l), C.POINTER(_l)]),
     "qrl_tx_frontend_read": (_i, [_vp, _vp, _l]),
     "qrl_tx_frontend_launch_count": (_l, [_vp]),
+    "qrl_tx_combiner_create": (_i, [_i, _i, _l, _i, C.POINTER(_vp)]),
+    "qrl_tx_combiner_destroy": (_i, [_vp]),
+    "qrl_tx_combiner_set_stream": (_i, [_vp, _vp]),
+    "qrl_tx_combiner_set_carrier_offset": (_i, [_vp, _i, _d]),
+    "qrl_tx_combiner_set_gain": (_i, [_vp, C.c_float]),
+    "qrl_tx_combiner_work": (_i, [_vp, _vp, _l, _i, C.POINTER(_l)]),
+    "qrl_tx_combiner_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_l)]),
+    "qrl_tx_combiner_read": (_i, [_vp, _vp, _l]),
+    "qrl_tx_combiner_launch_count": (_l, [_vp]),
     "qrl_firdes_low_pass": (_i, [_d] * 4 + [_i, _vp, _i]),
     "qrl_firdes_low_pass_2": (_i, [_d] * 5 + [_i, _vp, _i]),
     "qrl_firdes_band_pass": (_i, [_d] * 5 + [_i, _vp, _i]),
