@@ -116,7 +116,13 @@ int qrl_rx_set_param(qrl_rx* h, int channel /* -1 = all */, int key, double valu
 int qrl_rx_reset(qrl_rx* h);
 /* iq: [n_channels][T] interleaved float (re,im) = gr_complex; channel stride = `stride` complex samples.
  * on_device != 0: iq is a device pointer (already in HBM). Otherwise host memory (pinned or pageable);
- * the copy to the device is part of the call.  Asynchronous on the handle's stream. */
+ * the copy to the device is part of the call.  Asynchronous on the handle's stream.
+ * stride == 0 means ONE stream iq[0 .. T) at the handle's 1 Msps feeds every channel (one SDR, several receivers:
+ * gr_demod_mmdvm_multi.cpp:68-123's wiring).  Each channel applies its own QRL_PARAM_CARRIER_OFFSET_HZ rotator.  Channel c's outputs
+ * are, bit for bit, what the same handle gives for [n_channels][T] with n_channels identical rows: every port, the port counts and
+ * qrl_rx_rssi.  Host input is copied to the device once (T samples), device input is read in place; the same holds for
+ * qrl_rx_work_sc16 / _sc8, whose one int pair stream is converted once.  A handle may alternate between shared and per-row calls:
+ * each channel's stream continues across the switch. */
 int qrl_rx_work(qrl_rx* h, const float* iq, long T, long stride, int on_device);
 /* The same call fed with the SDR's wire format: interleaved int16 I/Q (UHD / SoapySDR "sc16": 4 bytes per sample, half the PCIe
  * traffic of gr_complex).  Each component becomes float(v) * scale on the device -- one rounding, the arithmetic of the host-side

@@ -182,6 +182,8 @@ public:
         if (qrl_rx_work(_h, reinterpret_cast<const float*>(iq), T, stride, 0) != QRL_OK) return WORK_DONE;
         return T;
     }
+    // one chunk of ONE stream feeding every channel (one SDR source behind n_channels instances, each at its own carrier offset)
+    int work_shared(const gr_complex* iq, int T) { return work(iq, T, 0); }
     // items the last work() produced on `port` for `channel`: pointer into an internal host buffer + count
     template <class T>
     const T* port(int port, int channel, int* n_items)

@@ -78,6 +78,8 @@ struct qrl_rx : HandleBase {
     float2* d_hist[2] = { nullptr, nullptr };
     float2* d_in_staging = nullptr;
     short2* d_in_sc16 = nullptr;        // qrl_rx_work_sc16 with a host buffer: the int16 slab as it arrived over PCIe
+    float2* d_in1 = nullptr;            // stride 0 (one stream for every channel): [Tmax] staging of host or converted input
+    short2* d_in1_sc16 = nullptr;       // stride 0, sc16 / sc8 from a host buffer: [Tmax] pairs as they arrived over PCIe
     long long n_in = 0, n1 = 0;       // stage-1 progress (absolute input samples consumed / outputs produced)
     long long n_in_s = 0, n1_s = 0;   // progress of the per-slice stages behind it (equal to the above between calls)
     bool fir_group_forced = false;     // QRL_FIR_GROUP given: keep it in overlap mode too
@@ -1245,9 +1247,18 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     if (on_device) { int rc = check_device_ptr(h, iq, "qrl_rx_work"); if (rc) return rc; }
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
+    // stride 0: one stream feeds every channel; it is copied and converted once (one row of T samples), and only the rotation and
+    // what follows it run per channel.  The staging is rewritten on the handle's stream, which every call ends waiting for stage 1.
+    // Stage 1 is the per-row kernel with in_stride 0: its channels read the one stream mostly from L2.  A kernel that fetches each
+    // strip once for a group of channels and rotates it into a second window per channel was slower at every register-tiled shape
+    // (stage 1 of 64 ch x 2^22 on an H100: 1.20 against 1.04 ms at /50, 1.95 against 1.25 ms at /125): two windows per CTA halve
+    // the occupancy, and the per-channel rotation, not the HBM read, is the cost.
+    const bool shared = stride == 0;
+    const int rows = shared ? 1 : h->C;
+    float2*& staging = shared ? h->d_in1 : h->d_in_staging;
     if (!on_device || sc16) {
-        if (!h->d_in_staging) {
-            int rc = dev_alloc(h, &h->d_in_staging, static_cast<size_t>(h->Tmax) * h->C, false);
+        if (!staging) {
+            int rc = dev_alloc(h, &staging, static_cast<size_t>(h->Tmax) * rows, false);
             if (rc) return rc;
         }
     }
@@ -1258,24 +1269,27 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         long long sstride = stride;
         const size_t isz = sc16 == 2 ? sizeof(short2) : sizeof(char2);
         if (!on_device) {
-            if (!h->d_in_sc16) {
-                int rc = dev_alloc(h, &h->d_in_sc16, static_cast<size_t>(h->Tmax) * h->C, false);
+            short2*& wire = shared ? h->d_in1_sc16 : h->d_in_sc16;
+            if (!wire) {
+                int rc = dev_alloc(h, &wire, static_cast<size_t>(h->Tmax) * rows, false);
                 if (rc) return rc;
             }
-            QRL_CK(cudaMemcpy2DAsync(h->d_in_sc16, isz * h->Tmax, iq_any, isz * stride, isz * T, h->C, cudaMemcpyHostToDevice, h->stream));
-            s = h->d_in_sc16; sstride = h->Tmax;
+            if (shared) QRL_CK(cudaMemcpyAsync(wire, iq_any, isz * T, cudaMemcpyHostToDevice, h->stream));
+            else QRL_CK(cudaMemcpy2DAsync(wire, isz * h->Tmax, iq_any, isz * stride, isz * T, h->C, cudaMemcpyHostToDevice, h->stream));
+            s = wire; sstride = h->Tmax;
         }
-        dim3 g(static_cast<unsigned>(std::min<long long>((T + 1023) / 1024, 65535)), h->C);
-        if (sc16 == 2) sc16_to_fc32_kernel<<<g, 256, 0, h->stream>>>(s, sstride, h->d_in_staging, h->Tmax, T, sc16_scale);
-        else sc8_to_fc32_kernel<<<g, 256, 0, h->stream>>>(reinterpret_cast<const char2*>(s), sstride, h->d_in_staging, h->Tmax, T, sc16_scale);
+        dim3 g(static_cast<unsigned>(std::min<long long>((T + 1023) / 1024, 65535)), rows);
+        if (sc16 == 2) sc16_to_fc32_kernel<<<g, 256, 0, h->stream>>>(s, sstride, staging, h->Tmax, T, sc16_scale);
+        else sc8_to_fc32_kernel<<<g, 256, 0, h->stream>>>(reinterpret_cast<const char2*>(s), sstride, staging, h->Tmax, T, sc16_scale);
         h->launches++;
-        x = h->d_in_staging;
-        xstride = h->Tmax;
+        x = staging;
+        xstride = shared ? 0 : h->Tmax;
     } else if (!on_device) {
-        QRL_CK(cudaMemcpy2DAsync(h->d_in_staging, sizeof(float2) * h->Tmax, iq, sizeof(float2) * stride,
-                             sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
-        x = h->d_in_staging;
-        xstride = h->Tmax;
+        if (shared) QRL_CK(cudaMemcpyAsync(staging, iq, sizeof(float2) * T, cudaMemcpyHostToDevice, h->stream));
+        else QRL_CK(cudaMemcpy2DAsync(staging, sizeof(float2) * h->Tmax, iq, sizeof(float2) * stride,
+                                      sizeof(float2) * T, h->C, cudaMemcpyHostToDevice, h->stream));
+        x = staging;
+        xstride = shared ? 0 : h->Tmax;
     }
     // carrier offset: the register-tiled /50, /100, /25, /125 stage-1 instances rotate their window in shared memory (no extra pass over
     // HBM); the other stage-1 shapes take the rotator as a separate pass

@@ -99,11 +99,36 @@ class RxBlock(Handle):
         T = iq8.shape[1]
         check(self._L.qrl_rx_work_sc8(self._h, iq8.ctypes.data_as(C.c_void_p), T, T, float(scale), 0), self._h, "qrl_rx_work_sc8")
 
+    # -- one SDR stream for every channel (stride 0): each channel applies its own carrier offset to the same capture
+    def work_shared(self, iq):
+        """iq: complex64 array [T] in host memory, one stream feeding every channel (copied to the device once)."""
+        iq = np.ascontiguousarray(iq, np.complex64)
+        if iq.ndim != 1:
+            raise ValueError("expected one stream [T], got shape %s" % (iq.shape,))
+        check(self._L.qrl_rx_work(self._h, iq.ctypes.data_as(C.c_void_p), iq.shape[0], 0, 0), self._h, "qrl_rx_work")
+
+    def work_shared_sc16(self, iq16, scale=1.0 / 32767.0):
+        """iq16: int16 array [T, 2] in host memory, one stream feeding every channel (copied and converted once)."""
+        iq16 = np.ascontiguousarray(iq16, np.int16)
+        if iq16.ndim != 2 or iq16.shape[1] != 2:
+            raise ValueError("expected one stream [T][2] int16, got shape %s" % (iq16.shape,))
+        check(self._L.qrl_rx_work_sc16(self._h, iq16.ctypes.data_as(C.c_void_p), iq16.shape[0], 0, float(scale), 0), self._h,
+              "qrl_rx_work_sc16")
+
+    def work_shared_sc8(self, iq8, scale=1.0 / 128.0):
+        """iq8: int8 array [T, 2] in host memory, one stream feeding every channel (copied and converted once)."""
+        iq8 = np.ascontiguousarray(iq8, np.int8)
+        if iq8.ndim != 2 or iq8.shape[1] != 2:
+            raise ValueError("expected one stream [T][2] int8, got shape %s" % (iq8.shape,))
+        check(self._L.qrl_rx_work_sc8(self._h, iq8.ctypes.data_as(C.c_void_p), iq8.shape[0], 0, float(scale), 0), self._h,
+              "qrl_rx_work_sc8")
+
     def work_sc16_device(self, dev_ptr, T, stride, scale=1.0 / 32767.0):
         check(self._L.qrl_rx_work_sc16(self._h, C.c_void_p(dev_ptr), T, stride, float(scale), 1), self._h, "qrl_rx_work_sc16")
 
     def work_device(self, dev_ptr, T, stride):
-        """iq already resident in HBM: dev_ptr = address of [n_channels][stride] complex64."""
+        """iq already resident in HBM: dev_ptr = address of [n_channels][stride] complex64; stride 0 = one stream [T] for every
+        channel, read in place."""
         check(self._L.qrl_rx_work(self._h, C.c_void_p(dev_ptr), T, stride, 1), self._h, "qrl_rx_work")
 
     sync = Handle._sync
