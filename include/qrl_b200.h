@@ -294,8 +294,12 @@ int qrl_design_deemph(int fs, double tau, double* a2, double* b2);
 enum { QRL_PFB_CHANNELIZER = 201, QRL_PFB_SYNTHESIZER = 202 };
 typedef struct qrl_pfb qrl_pfb;
 /* max_in: channelizer = wideband samples per call; synthesizer = columns (samples per channel) per call.
- * Accepted shapes: 1 <= M <= 64 and ceil(ntaps / M) <= 128 taps per branch; anything else returns QRL_EINVAL.  M = 10 with 35 taps
- * per branch (the reference's 341-tap prototype) runs register-tiled kernels, every other accepted shape generic ones. */
+ * Accepted shapes: 1 <= M <= 4096 (4096 channels of 25 kHz = 102.4 Msps) and ceil(ntaps / M) <= 128 taps per branch; M > 4096
+ * returns QRL_EINVAL with the limit in qrl_last_error, as does any other bad argument.  M = 10 with 35 taps per branch (the
+ * reference's 341-tap prototype) runs register-tiled kernels; every other accepted shape runs a branch-FIR kernel and an
+ * exact-order DFT kernel with the intermediate in device memory (about 8 B per wideband sample more of it per handle).
+ * Every shape is bit-identical to the oracle's definition: branch FIRs oldest sample first, the DFT as the direct sum over k
+ * ascending, both in fmaf. */
 int  qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, int device, qrl_pfb** out);
 int  qrl_pfb_destroy(qrl_pfb*);
 int  qrl_pfb_set_stream(qrl_pfb*, void* cuda_stream);

@@ -132,41 +132,160 @@ pfb_chan_kernel(const float* __restrict__ bt /*[M][TPF]*/, const float* __restri
     }
 }
 
-// generic channelizer (any M, tpf): one thread per (m, k) for the branch FIR, then per (m, c) for the DFT
-__global__ void __launch_bounds__(256)
-pfb_chan_generic_kernel(int M, int tpf, const float* __restrict__ bt, const float* __restrict__ w,
-                        const float2* __restrict__ hist, long long hist_len, const float2* __restrict__ x, long long n_x,
-                        long long frame0_e, long long frames, float2* __restrict__ out, long long out_stride, int tm)
+// --------------------------------------------------------------------------------------------------------------
+// Every other shape (1 <= M <= 4096, up to 128 taps per branch): two kernels with the intermediate in HBM.
+//   channelizer: pfb_fir_kernel<false> -> u [frames][M] (branch FIRs), pfb_dft_kernel<.., false> -> out [M][out_stride]
+//   synthesizer: pfb_dft_kernel<.., true> -> v [hl + n][M] (hl = tpf-1 history columns recomputed from the input
+//                history rows), pfb_fir_kernel<true> -> y [n][M]
+// The round trip of u / v costs 16 B per wideband sample against 4 M FFMA of the DFT.
+// --------------------------------------------------------------------------------------------------------------
+constexpr int kFirThreads = 256, kFirR = 9;
+
+// Branch FIR.  CTA = kb consecutive branches (kb = min(32, pow2 >= M)) x TB = (256 / kb) * R output times.  For a block of
+// consecutive branches each time step reads one contiguous run of kb samples (channelizer: stream positions M-1-k; synthesizer:
+// one row of v), so the shared window is [TB + tpf - 1][kb] at any M.  Thread (kk = tid % kb, g = tid / kb) computes the R
+// consecutive times g R .. g R + R - 1 of branch k0 + kk: taps outer, newest-first index t = tpf-1 .. 0 (the oracle's oldest
+// sample first), R window values held in registers and slid by one row per tap, so one tap load and one window load feed
+// 2 R FFMA.  R = 9 keeps the window loads of a half warp on distinct banks for every kb < 16 (9 kb g mod 16 distinct).
+template <bool SYN>
+__global__ void __launch_bounds__(kFirThreads)
+pfb_fir_kernel(int M, int tpf, int kb, const float* __restrict__ bt /*[M][tpf]*/, const float2* __restrict__ hist,
+               long long hist_len, const float2* __restrict__ x, long long n_x, long long frame0_e, long long n_t,
+               float2* __restrict__ out /*[n_t][M]*/)
 {
-    extern __shared__ __align__(16) unsigned char smraw[];
-    float2* ub = reinterpret_cast<float2*>(smraw);                  // [tm][M]
-    const long long m0 = static_cast<long long>(blockIdx.x) * tm;
-    for (int i = threadIdx.x; i < tm * M; i += blockDim.x) {
-        const int k = i % M; const long long m = m0 + i / M;
-        float re = 0.0f, im = 0.0f;
-        if (m < frames) {
-            for (int t = tpf - 1; t >= 0; t--) {
-                const long long e = frame0_e + (m - t) * M + (M - 1 - k);
-                const float2 v = e < 0 ? (e >= -hist_len ? hist[hist_len + e] : make_float2(0.0f, 0.0f)) : x[e];
-                const float h = bt[k * tpf + t];
-                re = fmaf(h, v.x, re); im = fmaf(h, v.y, im);
+    const int G = kFirThreads / kb, TB = G * kFirR, rows = TB + tpf - 1;
+    extern __shared__ __align__(128) unsigned char smraw[];
+    float2* win = reinterpret_cast<float2*>(smraw);                 // [rows][kb]
+    float* hs = reinterpret_cast<float*>(win + rows * kb);          // [tpf][kb]
+    const int tid = threadIdx.x;
+    const long long m0 = static_cast<long long>(blockIdx.x) * TB;
+    const int k0 = blockIdx.y * kb;
+    for (int i = tid; i < tpf * kb; i += kFirThreads) {
+        const int t = i / kb, k = k0 + i % kb;
+        hs[i] = k < M ? bt[k * tpf + t] : 0.0f;
+    }
+    for (int i = tid; i < rows * kb; i += kFirThreads) {
+        const int j = i / kb, k = k0 + i % kb;
+        float2 v = make_float2(0.0f, 0.0f);
+        if (k < M) {
+            if (SYN) {                                              // x = v [n_t + tpf - 1][M]; window row j = v row m0 + j
+                const long long r = m0 + j;
+                if (r < n_t + tpf - 1) v = x[r * M + k];
+            } else {                                                // stream sample (time m0 - (tpf-1) + j, position M-1-k)
+                const long long e = frame0_e + (m0 - (tpf - 1) + j) * M + (M - 1 - k);
+                if (e < 0) { if (e >= -hist_len) v = hist[hist_len + e]; }
+                else if (e < n_x) v = x[e];
             }
         }
-        ub[i] = make_float2(re, im);
+        win[i] = v;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < tm * M; i += blockDim.x) {
-        const int ml = i % tm, c = i / tm;
-        if (m0 + ml >= frames) continue;
-        float re = 0.0f, im = 0.0f;
-        for (int k = 0; k < M; k++) {
-            const int qd = static_cast<int>((static_cast<long long>(k) * c) % M);
-            const float wr = w[2 * qd], wi = w[2 * qd + 1];
-            const float2 u = ub[ml * M + k];
-            re = fmaf(u.x, wr, re); re = fmaf(-u.y, wi, re);
-            im = fmaf(u.x, wi, im); im = fmaf(u.y, wr, im);
+    const int kk = tid % kb, g = tid / kb;
+    if (k0 + kk >= M) return;
+    const float2* s = win + (g * kFirR) * kb + kk;                  // s[j kb] = sample of output time g R at tap tpf-1-j
+    float2 acc[kFirR], v[kFirR];
+#pragma unroll
+    for (int r = 0; r < kFirR; r++) { acc[r] = make_float2(0.0f, 0.0f); v[r] = s[r * kb]; }
+    for (int t = tpf - 1;; t--) {
+        const float h = hs[t * kb + kk];
+#pragma unroll
+        for (int r = 0; r < kFirR; r++) ffma2(acc[r], h, v[r]);    // v[r] = sample of output time g R + r at tap t
+        if (t == 0) break;
+#pragma unroll
+        for (int r = 0; r < kFirR - 1; r++) v[r] = v[r + 1];
+        v[kFirR - 1] = s[(kFirR + tpf - 1 - t) * kb];
+    }
+#pragma unroll
+    for (int r = 0; r < kFirR; r++) {
+        const long long m = m0 + g * kFirR + r;
+        if (m < n_t) out[m * M + k0 + kk] = acc[r];
+    }
+}
+
+// Exact-order DFT as a register-tiled complex "GEMM": out_p[t] = sum_k W[(k p) mod M] A[t][k], k ascending in one thread.
+//   channelizer: A[t][k] = u[t M + k], out [p][out_stride] (p = channel c), stores coalesced along t
+//   synthesizer: A[t][k] = input column t - hl of channel k (hist rows for t < hl), out [t][out_stride] (p = branch i),
+//                stores coalesced along p
+// CTA tile P = 4 PT outputs x T = 4 TT times (PT x TT = 256 threads); thread (pi, ti) owns p = pi + PT jp, t = ti + TT jt
+// (jp, jt < 4): 16 complex accumulators.  k runs in chunks of KC: A staged as [KC][T + 1], the twiddle tile [KC][P] gathered
+// once per chunk from the [M] table in shared memory, then 64 FFMA per 4 + 4 LDS.64 per k.
+// A chunk past M is padded with zeros: fmaf(0, w, acc) returns acc bit for bit, because acc is never -0 (it starts at +0,
+// and an fma only rounds to -0 from a -0 addend), so the padded terms leave every sum exactly the oracle's.
+constexpr int kDftThreads = 256, kDftKc = 16;
+template <int PT> constexpr int dft_smem(int M)
+{
+    return static_cast<int>(sizeof(float2)) * (M + kDftKc * (4 * (kDftThreads / PT) + 1) + kDftKc * 4 * PT);
+}
+
+template <int PT, bool SYN>
+__global__ void __launch_bounds__(kDftThreads)
+pfb_dft_kernel(int M, const float* __restrict__ wtab /*[M][2]*/, const float2* __restrict__ a, long long a_stride,
+               const float2* __restrict__ hist /*SYN: [M][hl]*/, int hl, long long n_t, float2* __restrict__ out,
+               long long out_stride)
+{
+    constexpr int TT = kDftThreads / PT, P = 4 * PT, T = 4 * TT, KC = kDftKc, TP = T + 1;
+    extern __shared__ __align__(128) unsigned char smraw[];
+    float2* wsm = reinterpret_cast<float2*>(smraw);                 // [M]
+    float2* as = wsm + M;                                           // [KC][TP]
+    float2* ws = as + KC * TP;                                      // [KC][P]
+    const int tid = threadIdx.x;
+    const long long t0 = static_cast<long long>(blockIdx.x) * T;
+    const int p0 = blockIdx.y * P;
+    const int pi = SYN ? tid % PT : tid / TT, ti = SYN ? tid / PT : tid % TT;
+    for (int i = tid; i < M; i += kDftThreads) wsm[i] = make_float2(wtab[2 * i], wtab[2 * i + 1]);
+    float2 acc[4][4];
+#pragma unroll
+    for (int jp = 0; jp < 4; jp++)
+#pragma unroll
+        for (int jt = 0; jt < 4; jt++) acc[jp][jt] = make_float2(0.0f, 0.0f);
+    for (int k0 = 0; k0 < M; k0 += KC) {
+        __syncthreads();                                            // the previous chunk is consumed (first: wsm is written)
+        for (int i = tid; i < KC * T; i += kDftThreads) {
+            const int kc = SYN ? i / T : i % KC, t = SYN ? i % T : i / KC;     // global reads contiguous along k / along t
+            const int k = k0 + kc;
+            const long long tt = t0 + t;
+            float2 v = make_float2(0.0f, 0.0f);
+            if (k < M && tt < n_t) {
+                if (SYN) {
+                    const long long n = tt - hl;
+                    v = n < 0 ? hist[static_cast<long long>(k) * hl + hl + n] : a[k * a_stride + n];
+                } else {
+                    v = a[tt * a_stride + k];
+                }
+            }
+            as[kc * TP + t] = v;
         }
-        out[c * out_stride + m0 + ml] = make_float2(re, im);
+        for (int i = tid; i < KC * P; i += kDftThreads) {
+            const int k = k0 + i / P, p = p0 + i % P;
+            ws[i] = (k < M && p < M) ? wsm[(k * p) % M] : make_float2(0.0f, 0.0f);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kc = 0; kc < KC; kc++) {
+            float2 av[4], wv[4];
+#pragma unroll
+            for (int j = 0; j < 4; j++) { av[j] = as[kc * TP + ti + TT * j]; wv[j] = ws[kc * P + pi + PT * j]; }
+#pragma unroll
+            for (int jp = 0; jp < 4; jp++)
+#pragma unroll
+                for (int jt = 0; jt < 4; jt++) {
+                    // re = fmaf(ur, wr, re); re = fmaf(-ui, wi, re); im = fmaf(ur, wi, im); im = fmaf(ui, wr, im)
+                    ffma2_sp(acc[jp][jt], av[jt].x, wv[jp].x, wv[jp].y);
+                    ffma2_sp(acc[jp][jt], av[jt].y, -wv[jp].y, wv[jp].x);
+                }
+        }
+    }
+#pragma unroll
+    for (int jp = 0; jp < 4; jp++) {
+        const int p = p0 + pi + PT * jp;
+        if (p >= M) continue;
+#pragma unroll
+        for (int jt = 0; jt < 4; jt++) {
+            const long long t = t0 + ti + TT * jt;
+            if (t >= n_t) continue;
+            if (SYN) out[t * out_stride + p] = acc[jp][jt];
+            else out[p * out_stride + t] = acc[jp][jt];
+        }
     }
 }
 
@@ -250,43 +369,6 @@ pfb_synth_kernel(const float* __restrict__ bt, const float* __restrict__ w,
     }
 }
 
-__global__ void __launch_bounds__(256)
-pfb_synth_generic_kernel(int M, int tpf, const float* __restrict__ bt, const float* __restrict__ w,
-                         const float2* __restrict__ hist, const float2* __restrict__ in, long long in_stride,
-                         long long n_cols, float2* __restrict__ out, int tn)
-{
-    extern __shared__ __align__(16) unsigned char smraw[];
-    float2* vb = reinterpret_cast<float2*>(smraw);                  // [M][tn + tpf - 1]
-    const int cols = tn + tpf - 1;
-    const long long n0 = static_cast<long long>(blockIdx.x) * tn;
-    for (int i = threadIdx.x; i < M * cols; i += blockDim.x) {
-        const int br = i / cols, col = i % cols;
-        const long long n = n0 - (tpf - 1) + col;
-        float re = 0.0f, im = 0.0f;
-        for (int c = 0; c < M; c++) {
-            const float2 u = n < 0 ? hist[c * (tpf - 1) + (tpf - 1) + n] : (n < n_cols ? in[c * in_stride + n] : make_float2(0.0f, 0.0f));
-            const int qd = static_cast<int>((static_cast<long long>(br) * c) % M);
-            const float wr = w[2 * qd], wi = w[2 * qd + 1];
-            re = fmaf(u.x, wr, re); re = fmaf(-u.y, wi, re);
-            im = fmaf(u.x, wi, im); im = fmaf(u.y, wr, im);
-        }
-        vb[i] = make_float2(re, im);
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < tn * M; i += blockDim.x) {
-        const int br = i % M, nl = i / M;
-        const long long n = n0 + nl;
-        if (n >= n_cols) continue;
-        float re = 0.0f, im = 0.0f;
-        for (int t = tpf - 1; t >= 0; t--) {
-            const float2 v = vb[br * cols + nl + (tpf - 1) - t];
-            const float h = bt[br * tpf + t];
-            re = fmaf(h, v.x, re); im = fmaf(h, v.y, im);
-        }
-        out[n * M + br] = make_float2(re, im);
-    }
-}
-
 // new per-channel history rows: the last tpf-1 input columns of (hist ++ in)
 __global__ void pfb_synth_tail_kernel(int M, int hl, const float2* __restrict__ hist, const float2* __restrict__ in,
                                       long long in_stride, long long n_cols, float2* __restrict__ dst)
@@ -309,15 +391,48 @@ struct qrl_pfb : QrlHandleBase {        // err / device / stream / launches / al
     float2* d_hist[2] = { nullptr, nullptr }; int hist_cur = 0; long long hist_len = 0; int pend = 0;
     float2* d_stage = nullptr;          // staging for host input
     float2* d_out = nullptr; long long out_stride = 0; long long out_items = 0;
+    float2* d_mid = nullptr;            // two-kernel shapes: channelizer u [frames][M], synthesizer v [tpf-1 + n][M]
     bool fast = false;
 };
 
 namespace {
 constexpr int kFastM = 10, kFastTpf = 35, kChanR = 9, kChanG = 32, kSynR = 10, kSynG = 32;
-constexpr int kMaxM = 64, kMaxTpf = 128, kGenericItems = 2048;
-// pfb_synth_generic_kernel's window [M][tn + tpf - 1] with tn = max(1, 2048 / M): M tn <= 2048, so at most 2048 + 64 * 127 items
-// (81 408 B at M = 64, tpf = 128), above the 48 KiB a launch gets without opting in
-constexpr int kSynGenericSmemMax = static_cast<int>(sizeof(float2)) * (kGenericItems + kMaxM * (kMaxTpf - 1));
+// 4096 channels of 25 kHz = 102.4 Msps, the top of the receive front end's range
+constexpr int kMaxM = 4096, kMaxTpf = 128;
+// pfb_fir_kernel's window and taps: (256 / kb * R + tpf - 1) kb float2 + tpf kb float, at most 67 328 B (kb = 32, tpf = 128)
+constexpr int kFirSmemMax = static_cast<int>(sizeof(float2)) * (kFirThreads * kFirR + (kMaxTpf - 1) * 32) + 4 * kMaxTpf * 32;
+// pfb_dft_kernel: PT = 4 (16 outputs x 256 times per CTA) up to M = 16, PT = 16 (64 x 64) above
+constexpr int kDftSmallM = 16;
+int fir_kb(int M) { int kb = 1; while (kb < M && kb < 32) kb *= 2; return kb; }
+int fir_smem(int tpf, int kb) { return static_cast<int>(sizeof(float2)) * ((kFirThreads / kb * kFirR + tpf - 1) * kb) + 4 * tpf * kb; }
+template <bool SYN>
+int launch_fir(qrl_pfb* h, const float2* hist, long long hist_len, const float2* x, long long n_x, long long frame0_e, long long n_t,
+               float2* out)
+{
+    const int kb = fir_kb(h->M), tb = kFirThreads / kb * kFirR;
+    if (int rc = smem_opt_in(h, pfb_fir_kernel<SYN>, kFirSmemMax)) return rc;
+    pfb_fir_kernel<SYN><<<dim3(static_cast<unsigned>((n_t + tb - 1) / tb), static_cast<unsigned>((h->M + kb - 1) / kb)), kFirThreads,
+                          fir_smem(h->tpf, kb), h->stream>>>(h->M, h->tpf, kb, h->d_bt, hist, hist_len, x, n_x, frame0_e, n_t, out);
+    h->launches++;
+    return QRL_OK;
+}
+template <int PT, bool SYN>
+int launch_dft_pt(qrl_pfb* h, const float2* a, long long a_stride, const float2* hist, int hl, long long n_t, float2* out,
+                  long long out_stride)
+{
+    constexpr int P = 4 * PT, T = 4 * (kDftThreads / PT);
+    if (int rc = smem_opt_in(h, pfb_dft_kernel<PT, SYN>, dft_smem<PT>(PT == 4 ? kDftSmallM : kMaxM))) return rc;
+    pfb_dft_kernel<PT, SYN><<<dim3(static_cast<unsigned>((n_t + T - 1) / T), static_cast<unsigned>((h->M + P - 1) / P)), kDftThreads,
+                              dft_smem<PT>(h->M), h->stream>>>(h->M, h->d_w, a, a_stride, hist, hl, n_t, out, out_stride);
+    h->launches++;
+    return QRL_OK;
+}
+template <bool SYN>
+int launch_dft(qrl_pfb* h, const float2* a, long long a_stride, const float2* hist, int hl, long long n_t, float2* out, long long out_stride)
+{
+    return h->M <= kDftSmallM ? launch_dft_pt<4, SYN>(h, a, a_stride, hist, hl, n_t, out, out_stride)
+                              : launch_dft_pt<16, SYN>(h, a, a_stride, hist, hl, n_t, out, out_stride);
+}
 long long chan_hist_len(int tpf, int M, int pend) { return (static_cast<long long>(tpf - 1) * M + pend + 2) & ~1LL; }
 }  // namespace
 
@@ -331,7 +446,11 @@ int qrl_pfb_destroy(qrl_pfb* h)
 
 int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, int device, qrl_pfb** out)
 {
-    if (!out || !taps || (kind != QRL_PFB_CHANNELIZER && kind != QRL_PFB_SYNTHESIZER) || M < 1 || M > kMaxM || ntaps < 1 ||
+    if (M > kMaxM) {
+        set_err(nullptr, "qrl_pfb_create: M above 4096 channels");
+        return QRL_EINVAL;
+    }
+    if (!out || !taps || (kind != QRL_PFB_CHANNELIZER && kind != QRL_PFB_SYNTHESIZER) || M < 1 || ntaps < 1 ||
         max_in < 1 || (ntaps + M - 1) / M > kMaxTpf) {
         set_err(nullptr, "qrl_pfb_create: bad argument");
         return QRL_EINVAL;
@@ -360,12 +479,14 @@ int qrl_pfb_create(int kind, int M, const float* taps, int ntaps, long max_in, i
         h->out_stride = (max_in + M - 1) / M + 2;
         if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * M))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_stage, static_cast<size_t>(max_in)))) return fail(rc);
+        if (!h->fast && (rc = dev_alloc(h, &h->d_mid, static_cast<size_t>(h->out_stride) * M))) return fail(rc);
     } else {
         const size_t hl = static_cast<size_t>(std::max(1, h->tpf - 1)) * M;
         if ((rc = dev_alloc(h, &h->d_hist[0], hl)) || (rc = dev_alloc(h, &h->d_hist[1], hl))) return fail(rc);
         h->out_stride = max_in * M;
         if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(max_in) * M))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_stage, static_cast<size_t>(max_in) * M))) return fail(rc);
+        if (!h->fast && (rc = dev_alloc(h, &h->d_mid, static_cast<size_t>(max_in + h->tpf - 1) * M))) return fail(rc);
     }
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
@@ -403,13 +524,11 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                 kern<<<static_cast<unsigned>((frames + TM - 1) / TM), kFastM * kChanG, smem, h->stream>>>(
                     h->d_bt, h->d_w, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames,
                     h->d_out, h->out_stride, use_tma);
+                h->launches++;
             } else {
-                const int tm = std::max(1, kGenericItems / M);
-                pfb_chan_generic_kernel<<<static_cast<unsigned>((frames + tm - 1) / tm), 256, sizeof(float2) * tm * M, h->stream>>>(
-                    M, tpf, h->d_bt, h->d_w, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames,
-                    h->d_out, h->out_stride, tm);
+                if (int rc = launch_fir<false>(h, hist, h->hist_len, x, n_in, -static_cast<long long>(h->pend), frames, h->d_mid)) return rc;
+                if (int rc = launch_dft<false>(h, h->d_mid, M, nullptr, 0, frames, h->d_out, h->out_stride)) return rc;
             }
-            h->launches++;
         }
         const int new_pend = static_cast<int>((static_cast<long long>(h->pend) + n_in) % M);
         const long long new_len = chan_hist_len(tpf, M, new_pend);
@@ -437,13 +556,11 @@ int qrl_pfb_work(qrl_pfb* h, const void* in, long n_in, long in_stride, int in_o
                 if (int rc = smem_opt_in(h, kern, static_cast<int>(smem))) return rc;
                 kern<<<static_cast<unsigned>((n_in + TN - 1) / TN), kFastM * kSynG, smem, h->stream>>>(
                     h->d_bt, h->d_w, hist, x, stride, n_in, h->d_out);
+                h->launches++;
             } else {
-                const int tn = std::max(1, kGenericItems / M);
-                if (int rc = smem_opt_in(h, pfb_synth_generic_kernel, kSynGenericSmemMax)) return rc;
-                pfb_synth_generic_kernel<<<static_cast<unsigned>((n_in + tn - 1) / tn), 256, sizeof(float2) * M * (tn + tpf - 1), h->stream>>>(
-                    M, tpf, h->d_bt, h->d_w, hist, x, stride, n_in, h->d_out, tn);
+                if (int rc = launch_dft<true>(h, x, stride, hist, hl, hl + n_in, h->d_mid, M)) return rc;
+                if (int rc = launch_fir<true>(h, nullptr, 0, h->d_mid, 0, 0, n_in, h->d_out)) return rc;
             }
-            h->launches++;
             if (hl > 0) {
                 pfb_synth_tail_kernel<<<(M * hl + 255) / 256, 256, 0, h->stream>>>(M, hl, hist, x, stride, n_in, hist_next);
                 h->launches++;
