@@ -231,6 +231,25 @@ int launch_fir_resamp_2_25(qrl_rx* h, const float2* iq, long long stride, long l
     return QRL_OK;
 }
 
+using Stage1Launch = int (*)(qrl_rx*, const float2*, long long, long long, long long, long long);
+
+// The register-tiled instance of the decimating stage 1 for the handle's (D, Q) shape, nullptr where none is built.  Only these
+// instances rotate their window in shared memory (the carrier offset without an extra pass over HBM), so this one list decides both
+// which kernel stage 1 runs and whether rx_work_impl needs the rotator pass.
+Stage1Launch stage1_tiled(const qrl_rx* h)
+{
+    if (h->L1 != 1) return nullptr;
+    if (h->D1 == 50 && h->Q1 == 9) return launch_fir_poly<50, 9, 8, 128, 8>;
+    if (h->D1 == 100 && h->Q1 == 9) return launch_fir_poly<100, 9, 8, 64, 8>;      // 837 taps (4FSK-1k, QPSK-2k shape)
+    if (h->D1 == 25 && h->Q1 == 9) return launch_fir_poly<25, 9, 8, 256, 8>;       // 209 taps (2FSK-2k)
+    if (h->D1 == 125 && h->Q1 == 9) return launch_fir_poly<125, 9, 8, 48, 6>;      // 1045 taps (SSB)
+    if (h->D1 == 25 && h->Q1 == 28) return launch_fir_poly<25, 28, 8, 192, 8>;     // 681 taps (QPSK-20k)
+    if (h->D1 == 100 && h->Q1 == 28) return launch_fir_poly<100, 28, 8, 32, 4>;    // 2727 taps (QPSK-2k)
+    return nullptr;
+}
+
+bool stage1_fuses_rotator(const qrl_rx* h) { return stage1_tiled(h) != nullptr; }
+
 int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long k0, long long k1)
 {
     if (k1 <= k0) return QRL_OK;
@@ -245,12 +264,7 @@ int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long
         return QRL_OK;
     }
     if (h->L1 != 1) { set_err(h, "stage-1 resampler shape not built"); return QRL_EINVAL; }
-    if (h->D1 == 50 && h->Q1 == 9) return launch_fir_poly<50, 9, 8, 128, 8>(h, iq, stride, T, k0, k1);
-    if (h->D1 == 100 && h->Q1 == 9) return launch_fir_poly<100, 9, 8, 64, 8>(h, iq, stride, T, k0, k1);     // 837 taps (4FSK-1k, QPSK-2k shape)
-    if (h->D1 == 25 && h->Q1 == 9) return launch_fir_poly<25, 9, 8, 256, 8>(h, iq, stride, T, k0, k1);      // 209 taps (2FSK-2k)
-    if (h->D1 == 125 && h->Q1 == 9) return launch_fir_poly<125, 9, 8, 48, 6>(h, iq, stride, T, k0, k1);     // 1045 taps (SSB)
-    if (h->D1 == 25 && h->Q1 == 28) return launch_fir_poly<25, 28, 8, 192, 8>(h, iq, stride, T, k0, k1);    // 681 taps (QPSK-20k)
-    if (h->D1 == 100 && h->Q1 == 28) return launch_fir_poly<100, 28, 8, 32, 4>(h, iq, stride, T, k0, k1);   // 2727 taps (QPSK-2k)
+    if (Stage1Launch tiled = stage1_tiled(h)) return tiled(h, iq, stride, T, k0, k1);
     if (h->D1 == 2 && h->ntaps1 <= 56) return launch_fir_d2<56, 8, 128>(h, iq, stride, T, k0, k1);
     if (h->L1 == 1) {      // no register-tiled instance for this shape: one thread per output, same order, same history
         const long long nout = k1 - k0;
@@ -369,16 +383,8 @@ int make_ring(qrl_rx* h, Ring* r, size_t isz, long long min_items, bool interlea
 
 // low-rate stream filters: register-tiled instances for real calls, the one-thread-per-output kernels for slivers
 int launch_fir_ccf_c(HandleBase* h, int C, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
-                     const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved);
-int launch_fir_ccf(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
-                   const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
-{
-    return launch_fir_ccf_c(h, h->C, st, in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
-}
-int launch_fir_ccf_c(HandleBase* h, int C_, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
                      const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
 {
-    struct CShim { int C; } hc{ C_ }; CShim* hC = &hc;
     const long long n = a1 - a0;
     if (n <= 0) return QRL_OK;
     constexpr int K = 8, NT = 128, TILE = K * NT;
@@ -388,15 +394,20 @@ int launch_fir_ccf_c(HandleBase* h, int C_, cudaStream_t st, const float2* in, u
         if (int rc = smem_opt_in(h, fir_ccf_ring_tiled_kernel<K, NT>, 100 * 1024)) return rc;
     }
     if (n >= 256 && smem <= 100 * 1024 && ntaps >= K) {      // (the tiled kernel's head / tail phases assume at least K taps)
-        dim3 g(static_cast<unsigned>((n + TILE - 1) / TILE), hC->C);
+        dim3 g(static_cast<unsigned>((n + TILE - 1) / TILE), C);
         fir_ccf_ring_tiled_kernel<K, NT><<<g, NT, smem, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
     } else {
-        dim3 g(static_cast<unsigned>((n + 255) / 256), hC->C);
+        dim3 g(static_cast<unsigned>((n + 255) / 256), C);
         fir_ccf_ring_kernel<<<g, 256, sizeof(float) * ntaps, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
     }
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
+}
+int launch_fir_ccf(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
+                   const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
+{
+    return launch_fir_ccf_c(h, h->C, st, in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
 }
 int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float* out, unsigned out_mask, long long out_stride,
                       const float* taps, int ntaps, float gain, long long a0, long long a1)
@@ -415,6 +426,407 @@ int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_
     }
     h->launches++;
     QRL_CK(cudaGetLastError());
+    return QRL_OK;
+}
+
+// symbols one CH-row symbol-sync window can hold (the shortest symbol period is min_period - |alpha|)
+int symsync_maxs(const SymSyncParams& p, int CH)
+{
+    return static_cast<int>((CH + 1) / (p.min_period - fabsf(p.alpha)) + 3);
+}
+
+// dynamic shared memory of the 4FSK-FM symbol sync with the external epilogue: NST input stages of CH rows x 32 channels, the tap
+// table, two symbol windows and the header; rep adds the replicated (conflict-free) interpolator bank.  rx_create chooses ss_ch and
+// sizes the epilogue scratch with it, and the launch uses it, so the two always agree.
+size_t symsync_ext_smem(const SymSyncParams& p, int CH, int NST, bool rep)
+{
+    return sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * (symsync_maxs(p, CH) + 2) * 32) + sizeof(int) * 64 + (rep ? 129 * 512 : 0);
+}
+
+// ---- the receive chains behind stage 1.  rx_work_impl cuts each call into slices, runs stage 1 and hands every slice to the
+// slice function of the handle's chain, which queues the rest of that slice on the parallel, loop and FEC streams.
+
+constexpr int kTileThreads = 256;       // CTA size of the per-output stream filters (Slice::gtile)
+
+// slice i of a call: the stage-1 outputs [k0, k1) are new
+struct Slice {
+    int i;
+    long long k0, k1, n_new;
+    long long k_call0;          // stage-1 index of the call's first output (port 0 of the call starts there)
+    long long* nsoft_i;         // [C] soft-bit write index snapshots of this slice
+    cudaStream_t sp;            // stream of the parallel stages
+    dim3 gtile;                 // kTileThreads-thread CTAs over the new outputs, one row per channel
+    int groups;                 // CTAs of 32 channels (the loop kernels)
+};
+
+// `to` runs on behind everything queued on `from` so far
+int hand_off(qrl_rx* h, cudaEvent_t ev, cudaStream_t from, cudaStream_t to)
+{
+    QRL_CK(cudaEventRecord(ev, from));
+    QRL_CK(cudaStreamWaitEvent(to, ev, 0));
+    return QRL_OK;
+}
+
+// fll_band_edge_cc (sequential, per sample) on the loop stream: r1 -> rf
+void launch_fll(qrl_rx* h, const Slice& s)
+{
+    fll_kernel<32><<<s.groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
+        static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, s.k1,
+        static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
+    h->launches++;
+}
+
+// the channel / shaping filter of a slice on `st`: `in` -> r2 (channel-interleaved when `interleaved`) and port 0
+int launch_channel_filter(qrl_rx* h, const Slice& s, cudaStream_t st, const Ring& in, int interleaved)
+{
+    return launch_fir_ccf(h, st, static_cast<const float2*>(in.d), in.mask, in.stride, static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                          h->d_taps2, h->ntaps2, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0, interleaved);
+}
+
+// one symbol-sync launch on `st` over the input ring `in` up to k1 (opting the instance in to `smem_max` bytes first); only the
+// 4FSK-FM symbol sync with the external epilogue passes the epilogue's scratch, chunk bound, chunk capacity and header
+template <class K>
+int launch_symsync(qrl_rx* h, K* kern, int smem_max, int grid, int threads, size_t smem, cudaStream_t st, const Ring& in, long long k1,
+                   int maxs, long long* nsoft_i, float* scratch = nullptr, int chunk_bound = 0, int chunk_cap = 0, int* hdr = nullptr)
+{
+    if (int rc = smem_opt_in(h, kern, smem_max)) return rc;
+    kern<<<grid, threads, smem, st>>>(
+        h->ssp, h->d_ss, h->C, static_cast<const float*>(in.d), in.mask, in.stride, k1,
+        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
+        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, scratch, chunk_bound, chunk_cap, hdr);
+    h->launches++;
+    return QRL_OK;
+}
+
+// stage 5 on the FEC stream: Viterbi + descrambler over the slice's soft bits -> port 2; dual: a second decoder on the same soft
+// stream behind delay(1) -> port 3
+void launch_viterbi(qrl_rx* h, long long* nsoft_i, bool dual)
+{
+    constexpr int CPB = 4;    // 4 channels (8 warps) per CTA
+    cudaEvent_t pe = h->prof.begin(4, h->s_fec);
+    viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
+        static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+        h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
+    if (dual)
+        viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs2, nsoft_i, h->C,
+            static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+            h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
+    h->launches += dual ? 2 : 1;
+    h->prof.end(pe);
+}
+
+// gr_demod_dsss: the whole chain in one kernel on the loop stream, then the two decoders
+int slice_dsss(qrl_rx* h, const Slice& s)
+{
+    if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+    cudaEvent_t pe = h->prof.begin(3, h->s_loop);
+    dsss_chain_kernel<<<h->C, 256, 0, h->s_loop>>>(h->dsp, h->d_ds, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, s.k1,
+        h->d_ds_arms, h->d_taps2, h->d_ds_taps,
+        static_cast<float2*>(h->ds_a.d), static_cast<float2*>(h->ds_c.d), h->ds_a.mask, h->ds_a.stride,
+        static_cast<float2*>(h->ds_d.d), h->ds_d.mask, h->ds_d.stride,
+        h->d_port0, h->port0_cap, h->ds_o_call0,
+        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
+        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, s.nsoft_i);
+    h->launches++;
+    h->prof.end(pe);
+    if (int rc = hand_off(h, h->ev_b[s.i], h->s_loop, h->s_fec)) return rc;
+    launch_viterbi(h, s.nsoft_i, true);
+    return QRL_OK;
+}
+
+// SSB, FreeDV, AM, NBFM, WBFM: channel / side-band filter on the parallel stream (-> port 0), then the audio chain on the loop stream
+// (NBFM: its de-emphasis on the second loop stream)
+int slice_analog(qrl_rx* h, const Slice& s)
+{
+    cudaEvent_t pe;
+    if (s.n_new > 0) {
+        pe = h->prof.begin(1, s.sp);
+        if (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_WBFM) {
+            if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
+        } else {
+            fir_ccc_ring_kernel<<<s.gtile, kTileThreads, sizeof(float) * 2 * h->ntaps2, s.sp>>>(
+                static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
+                static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                h->d_taps2, h->ntaps2, 1.0f, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0);
+            h->launches++;
+        }
+        h->prof.end(pe);
+    }
+    if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+    pe = h->prof.begin(3, h->s_loop);
+    const size_t fat = h->nbfm_split ? 120 * 1024 : 0;       // one CTA per SM, and never next to a de-emphasis CTA
+    switch (h->kind) {
+    case QRL_DEMOD_SSB:
+        ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb,
+            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
+            static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
+            static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
+            h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
+        break;
+    case QRL_DEMOD_FREEDV:
+        freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
+            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
+            static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
+            reinterpret_cast<short*>(h->d_port1), 4 * h->port1_cap, h->d_port1_cnt, static_cast<int>(4 * h->port1_cap));
+        break;
+    default:    // AM, NBFM, WBFM (the de-emphasis ring and the CTCSS squelch ring only exist for NBFM; empty otherwise)
+        if (h->nbfm_split) {
+            int rc;
+            if ((rc = smem_opt_in(h, nbfm_audio_kernel, 120 * 1024)) || (rc = smem_opt_in(h, nbfm_deemph_kernel, 120 * 1024))) return rc;
+        }
+        nbfm_audio_kernel<<<h->C, 128, fat, h->s_loop>>>(h->nbp, h->d_nb,
+            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1, h->d_env,
+            static_cast<float2*>(h->rg.d), h->rg.mask, h->rg.stride,
+            static_cast<float*>(h->rd.d), h->rd.mask, h->rd.stride,
+            static_cast<float*>(h->rr.d), h->rr.mask, h->rr.stride,
+            h->d_arm_taps, h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap),
+            h->nbfm_split ? static_cast<float*>(h->raud.d) : nullptr, h->raud.mask, h->raud.stride, h->nbfm_split ? s.nsoft_i : nullptr,
+            static_cast<float*>(h->rq.d), h->rq.mask, h->rq.stride, h->ctc, h->d_cenv);
+    }
+    h->launches++;
+    h->prof.end(pe);
+    if (h->nbfm_split) {
+        if (int rc = hand_off(h, h->ev_b[s.i], h->s_loop, h->s_loop2)) return rc;
+        pe = h->prof.begin(5, h->s_loop2);
+        nbfm_deemph_kernel<<<h->C, 128, fat, h->s_loop2>>>(h->nbp.b0, h->nbp.b1, h->nbp.a1, h->nbp.out_gain, h->d_nb2,
+            static_cast<const float*>(h->raud.d), h->raud.mask, h->raud.stride, s.nsoft_i,
+            h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
+        h->launches++;
+        h->prof.end(pe);
+    }
+    return QRL_OK;
+}
+
+// BPSK, 2FSK, GMSK: FLL (not GMSK), channel filter / RRC and detector, agc2 (BPSK), symbol sync, all on the loop stream; then the
+// two decoders
+int slice_fll_bpsk_2fsk(qrl_rx* h, const Slice& s)
+{
+    const bool bpsk = h->kind == QRL_DEMOD_BPSK;
+    if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+    cudaEvent_t pe = h->prof.begin(1, h->s_loop);
+    if (!h->gmsk) launch_fll(h, s);
+    h->prof.end(pe);
+    if (s.n_new > 0) {
+        // ---- channel filter / RRC on the FLL output -> port 0 (+ ring: channel-major for 2FSK, interleaved for BPSK)
+        pe = h->prof.begin(2, h->s_loop);
+        if (int rc = launch_channel_filter(h, s, h->s_loop, h->gmsk ? h->r1 : h->rf, bpsk ? 1 : 0)) return rc;     // GMSK: no FLL
+        if (!bpsk && h->flag) {
+            if (int rc = launch_qdemod_fir(h, h->s_loop, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                                           static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
+                                           h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
+        } else if (!bpsk) {
+            fsk_bank_kernel<2><<<s.gtile, kTileThreads, sizeof(float) * 4 * h->nt_bank, h->s_loop>>>(
+                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, s.k0, s.k1,
+                static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
+            fir_fff_ring_kernel<<<s.gtile, kTileThreads, sizeof(float) * h->nt_symf, h->s_loop>>>(
+                static_cast<const float*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
+                static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, h->d_symf_taps, h->nt_symf, s.k0, s.k1);
+            h->launches += 2;
+        }
+        h->prof.end(pe);
+    }
+    pe = h->prof.begin(3, h->s_loop);
+    if (bpsk) {
+        {   // agc2_cc (Costas bypassed): r2 -> r3
+            constexpr int CH = 128, NST = 2;
+            const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
+            auto kern = agc_costas_kernel<CH, NST, 0, 0>;
+            if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
+            kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
+                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
+                static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
+            h->launches++;
+        }
+        // clock_recovery_mm_cc: its window bound is (CH + 1) / min_period symbols
+        constexpr int CH = 128, NST = 3, NEPI = 1;
+        const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period) + 3);
+        const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
+        if (int rc = launch_symsync(h, symsync_kernel<2, SL_BPSK, EPI_BPSK, CH, NST, NEPI, LOOP_CRMM>, 200 * 1024, s.groups, 64 + 32 * NEPI,
+                                    smem, h->s_loop, h->r3, s.k1, maxs, s.nsoft_i)) return rc;
+    } else {
+        constexpr int CH = 256, NST = 3, NEPI = 2;
+        const int maxs = symsync_maxs(h->ssp, CH);
+        const size_t smem = sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * maxs * 32) + sizeof(int) * 64;
+        if (int rc = launch_symsync(h, symsync_kernel<1, SL_BPSK, EPI_REAL1, CH, NST, NEPI>, 200 * 1024, s.groups, 64 + 32 * NEPI,
+                                    smem, h->s_loop, h->r4, s.k1, maxs, s.nsoft_i)) return rc;
+    }
+    h->prof.end(pe);
+    if (int rc = hand_off(h, h->ev_b[s.i], h->s_loop, h->s_fec)) return rc;
+    launch_viterbi(h, s.nsoft_i, true);
+    return QRL_OK;
+}
+
+// 4FSK-FM symbol sync with CH-row windows and NST input stages: lean recurrence on the loop stream + external epilogue (symbols leave
+// the SM by TMA bulk store; the phase modulator / soft-bit stores run on the wide partition behind it, on s_epi when there is one)
+template <int CH, int NST>
+int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
+{
+    cudaEvent_t pe = h->prof.begin(3, h->s_loop);
+    const int maxs = symsync_maxs(h->ssp, CH);
+    const bool rep = symsync_ext_smem(h->ssp, CH, NST, true) <= 220 * 1024 && !h->dmr;
+    // gr_demod_dmr: TED_MUELLER_AND_MULLER instead of the modified detector -> generic recurrence, variant 3
+    auto kern = h->dmr ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>
+              : rep ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 2>
+                    : symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 1>;
+    // overlapped calls: the previous call's Viterbi of slice i still reads d_nsoft[i], its epilogue scratch region i
+    if (h->overlap) QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_v[s.i], 0));
+    // every slice of a call gets its own scratch region and header (the epilogue of slice i overlaps symsync i+1)
+    if (s.i == 0) h->ss_chunk_off = 0;
+    const int chunk_bound = static_cast<int>(std::min<long long>(h->ss_chunk_cap - h->ss_chunk_off, s.n_new / symsync_stride(CH, h->ssp.lookahead) + 3));
+    float* scratch_i = h->d_ss_scratch + static_cast<size_t>(h->ss_chunk_off) * (maxs + 2) * 32;
+    int* hdr_i = h->d_ss_hdr + static_cast<size_t>(s.i) * s.groups * 128;
+    h->ss_chunk_off += chunk_bound;
+    if (int rc = launch_symsync(h, kern, 224 * 1024, s.groups, 96, symsync_ext_smem(h->ssp, CH, NST, rep), h->s_loop, h->r4, s.k1, maxs,
+                                s.nsoft_i, scratch_i, chunk_bound, static_cast<int>(h->ss_chunk_cap), hdr_i)) return rc;
+    h->prof.end(pe);
+    cudaStream_t se = h->s_epi ? h->s_epi : h->s_loop;
+    if (se != h->s_loop || h->overlap) QRL_CK(cudaEventRecord(h->ev_c[s.i], h->s_loop));
+    if (se != h->s_loop) QRL_CK(cudaStreamWaitEvent(se, h->ev_c[s.i], 0));
+    pe = h->prof.begin(5, se);
+    auto epi = h->dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
+    if (chunk_bound > 0)        // (counted in h->launches with the symbol sync it finishes)
+        epi<<<dim3(chunk_bound, s.groups), dim3(32, 8), 0, se>>>(
+            h->ssp, h->C, scratch_i, static_cast<int>(h->ss_chunk_cap), maxs, hdr_i,
+            h->d_port1, h->port1_cap, static_cast<int>(h->port1_cap),
+            static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+            h->m17 ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
+    h->prof.end(pe);
+    QRL_CK(cudaEventRecord(h->ev_b[s.i], se));
+    return QRL_OK;
+}
+
+// 4FSK (FM discriminator or band-pass bank), M17, DMR: channel filter and detector on the parallel stream, symbol sync on the loop
+// stream, then the decoder (M17: none)
+int slice_4fsk(qrl_rx* h, const Slice& s)
+{
+    cudaEvent_t pe;
+    if (s.n_new > 0) {
+        // ---- stage 2: channel filter -> ring + port 0
+        pe = h->prof.begin(1, s.sp);
+        if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
+        h->prof.end(pe);
+        // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
+        // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
+        if (h->overlap && h->prev_nsub > 0) {
+            // the slots [k0, k1) overwrite the samples cap older; the previous call's symbol sync of slice q has
+            // consumed everything up to prev_k1[q] - lookahead
+            const long long must = s.k1 - (static_cast<long long>(h->r4.mask) + 1) + 64;
+            int q = -1;
+            for (int j = 0; j < h->prev_nsub; j++) if (h->prev_k1[j] - 64 < must) q = j;      // not yet safe after slice j alone
+            if (q >= 0) QRL_CK(cudaStreamWaitEvent(s.sp, h->ev_c[std::min(q + 1, h->prev_nsub - 1)], 0));
+        }
+        pe = h->prof.begin(2, s.sp);
+        if (h->flag) {
+            if (int rc = launch_qdemod_fir(h, s.sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                                           static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
+                                           h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
+            if (h->dmr) {      // gr_demod_dmr.cpp:103: the symbol filter output is port 3
+                ring_to_port_f32_kernel<<<dim3(static_cast<unsigned>((s.k1 - s.k0 + 31) / 32), s.groups), dim3(32, 8), 0, s.sp>>>(
+                    static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, h->C, s.k0, s.k1,
+                    h->d_port3f, h->port0_cap, s.k0 - s.k_call0);
+                h->launches++;
+            }
+        } else {
+            fsk_bank_kernel<4><<<s.gtile, kTileThreads, sizeof(float) * 8 * h->nt_bank, s.sp>>>(
+                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, s.k0, s.k1,
+                static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
+            h->launches++;
+            if (int rc = launch_fir_ccf(h, s.sp, static_cast<const float2*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
+                                        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride,
+                                        h->d_symf_taps, h->nt_symf, s.k0, s.k1, nullptr, 0, 0, 1)) return rc;
+        }
+        h->prof.end(pe);
+    }
+    // ---- stage 4: symbol sync (+ phase mod + soft bits) on the loop stream
+    if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+    if (h->flag) {
+        const int rc = h->ss_ch == 512 ? symsync_4fsk_ext<512, 2>(h, s) : symsync_4fsk_ext<256, 3>(h, s);
+        if (rc) return rc;
+    } else {
+        pe = h->prof.begin(3, h->s_loop);
+        constexpr int CH = 128, NST = 3, NEPI = 2;
+        const int maxs = symsync_maxs(h->ssp, CH);
+        const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
+        if (int rc = launch_symsync(h, symsync_kernel<2, SL_RECT4, EPI_CPLX, CH, NST, NEPI>, 200 * 1024, s.groups, 64 + 32 * NEPI,
+                                    smem, h->s_loop, h->r3, s.k1, maxs, s.nsoft_i)) return rc;
+        h->prof.end(pe);
+        QRL_CK(cudaEventRecord(h->ev_b[s.i], h->s_loop));
+    }
+    // ---- stage 5: Viterbi + descrambler on the FEC stream
+    QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[s.i], 0));
+    // gr_demod_m17 has no FEC: the epilogue wrote the hard bits of port 2 (s_fec joins it at the end)
+    if (!h->m17) launch_viterbi(h, s.nsoft_i, false);
+    if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[s.i], h->s_fec));
+    return QRL_OK;
+}
+
+// QPSK agc2 + Costas "PLL" on the loop stream (r2 -> r3): CH-row windows, 2 input stages + the hand-off blocks (164 KB at CH = 128)
+template <int CH>
+int qpsk_agc_costas(qrl_rx* h, const Slice& s)
+{
+    constexpr int NST = 2;
+    const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
+    auto kern = (h->acp.order == 4 && h->acp.use_snr) ? agc_costas_kernel<CH, NST, 4, 1> : agc_costas_kernel<CH, NST>;
+    int rc;                                 // both instantiations, whichever this call takes
+    if ((rc = smem_opt_in(h, agc_costas_kernel<CH, NST, 4, 1>, 200 * 1024)) || (rc = smem_opt_in(h, agc_costas_kernel<CH, NST>, 200 * 1024))) return rc;
+    kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
+        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
+        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
+    h->launches++;
+    return QRL_OK;
+}
+
+// QPSK symbol sync + second Costas + diff phasor + soft bits on the second loop stream.  LEAN: the prefetching complex recurrence
+// (symbol-sync variant 2, replicated tap bank) with the epilogue split into a Costas warp and a feed-forward warp over a 3-deep symbol
+// ring (NEPI = 2); else the generic recurrence, one epilogue warp
+template <int CH, int NST, bool LEAN>
+int qpsk_symsync(qrl_rx* h, const Slice& s)
+{
+    constexpr int NEPI = LEAN ? 2 : 1, NB = LEAN ? 3 : 2;
+    const int maxs = symsync_maxs(h->ssp, CH);
+    const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + NB * maxs * 64) + sizeof(int) * 32 * (NB == 2 ? 2 : 4) +
+                        (LEAN ? 129 * 512 : 0);
+    if (smem > 224 * 1024) { set_err(h, "QPSK symbol sync: window does not fit shared memory"); return QRL_EINVAL; }
+    return launch_symsync(h, symsync_kernel<2, SL_DQPSK, EPI_QPSK, CH, NST, NEPI, LOOP_SYMSYNC, LEAN ? 2 : 0>, 224 * 1024, s.groups,
+                          64 + 32 * NEPI, smem, h->s_loop2, h->r3, s.k1, maxs, s.nsoft_i);
+}
+
+// QPSK: FLL (sps > 4) on the loop stream, RRC shaping filter on the parallel stream, agc2 + Costas on the loop stream, symbol sync on
+// the second loop stream, then the decoder
+int slice_qpsk(qrl_rx* h, const Slice& s)
+{
+    if (h->d_fll) {     // sps > 4: fll_band_edge_cc between resampler and shaping filter (sequential, on the loop stream)
+        if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+        launch_fll(h, s);
+        if (int rc = hand_off(h, h->ev_c[s.i], h->s_loop, s.sp)) return rc;
+    }
+    cudaEvent_t pe;
+    if (s.n_new > 0) {
+        // ---- stage 2: RRC shaping filter -> interleaved ring + port 0
+        pe = h->prof.begin(1, s.sp);
+        if (int rc = launch_channel_filter(h, s, s.sp, h->d_fll ? h->rf : h->r1, 1)) return rc;
+        h->prof.end(pe);
+    }
+    // ---- stage 3: agc2 + costas "PLL" per sample on the loop stream
+    if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
+    pe = h->prof.begin(2, h->s_loop);
+    // many channels: 32-row windows (41 KB of shared memory, five CTAs per SM) instead of 128-row ones (164 KB)
+    if (int rc = h->many ? qpsk_agc_costas<32>(h, s) : qpsk_agc_costas<128>(h, s)) return rc;
+    h->prof.end(pe);
+    // ---- stage 4: symbol sync on the second loop stream
+    if (int rc = hand_off(h, h->ev_c[s.i], h->s_loop, h->s_loop2)) return rc;
+    pe = h->prof.begin(3, h->s_loop2);
+    // many channels: 64-row windows, two stages (~55 KB, four CTAs per SM) instead of 128-row ones
+    const bool small_win = h->many && symsync_stride(64, h->ssp.lookahead) >= 32;
+    static const bool lean_env = [] { const char* e = getenv("QRL_QPSK_LEAN_SS"); return !(e && e[0] == '0'); }();
+    // the lean recurrence needs the in-lock window proof (kernel: lean_ok && window_sure) -- true for every QPSK instance of
+    // gr_demod_base.cpp; the kernel itself falls back to the generic loop when it does not hold
+    const int rc = small_win ? qpsk_symsync<64, 2, false>(h, s) : lean_env ? qpsk_symsync<128, 2, true>(h, s) : qpsk_symsync<128, 3, false>(h, s);
+    if (rc) return rc;
+    h->prof.end(pe);
+    // ---- stage 5: Viterbi + descrambler on the FEC stream
+    if (int rc2 = hand_off(h, h->ev_b[s.i], h->s_loop2, h->s_fec)) return rc2;
+    launch_viterbi(h, s.nsoft_i, false);
     return QRL_OK;
 }
 
@@ -871,13 +1283,9 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         if (flag && kind == QRL_DEMOD_4FSK) {
             // scratch of the external symbol-sync epilogue: [groups][chunks][maxs + 2][32] floats + a 128-int header per group
             // window size: 512 rows x 2 stages when the replicated interpolator bank still fits next to it, else 256 x 3
-            {
-                const int maxs512 = static_cast<int>((512 + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
-                const size_t need512 = sizeof(float) * (2 * 512 * 32 + SYMSYNC_TAB_FLOATS + 2 * (maxs512 + 2) * 32) + sizeof(int) * 64 + 129 * 512;
-                h->ss_ch = need512 <= 220 * 1024 ? 512 : 256;
-            }
+            h->ss_ch = symsync_ext_smem(h->ssp, 512, 2, true) <= 220 * 1024 ? 512 : 256;
             if (const char* e = getenv("QRL_SS_CH")) { const int v = atoi(e); if (v == 512 || v == 256) h->ss_ch = v; }
-            const int maxs = static_cast<int>((h->ss_ch + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
+            const int maxs = symsync_maxs(h->ssp, h->ss_ch);
             h->ss_chunk_cap = h->n1max / symsync_stride(h->ss_ch, h->ssp.lookahead) + 4 + 3 * qrl_rx::kMaxSub;
             const size_t groups = (h->C + 31) / 32;
             if ((rc = dev_alloc(h, &h->d_ss_scratch, groups * h->ss_chunk_cap * (maxs + 2) * 32))) return fail(rc);
@@ -1291,11 +1699,8 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         x = staging;
         xstride = shared ? 0 : h->Tmax;
     }
-    // carrier offset: the register-tiled /50, /100, /25, /125 stage-1 instances rotate their window in shared memory (no extra pass over
-    // HBM); the other stage-1 shapes take the rotator as a separate pass
-    const bool poly_shape = h->L1 == 1 && ((h->D1 == 50 && h->Q1 == 9) || (h->D1 == 100 && (h->Q1 == 9 || h->Q1 == 28)) ||
-                                           (h->D1 == 25 && (h->Q1 == 9 || h->Q1 == 28)) || (h->D1 == 125 && h->Q1 == 9));
-    h->rot_fused = h->rot_active && poly_shape && !getenv("QRL_ROTATOR_PASS");
+    // carrier offset: inside the stage-1 kernel where it can rotate its window, else a separate pass
+    h->rot_fused = h->rot_active && stage1_fuses_rotator(h) && !getenv("QRL_ROTATOR_PASS");
     if (h->rot_active && !h->rot_fused) {
         if (!h->d_rot_buf) { int rc = dev_alloc(h, &h->d_rot_buf, static_cast<size_t>(h->Tmax) * h->C, false); if (rc) return rc; }
         dim3 g(static_cast<unsigned>(std::min<long long>((T + 255) / 256, 4096)), h->C);
@@ -1402,430 +1807,17 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         h->cur_k1[i] = k1;
         const long long n_new = k1 - k0;
         h->port0_n += static_cast<long>(n_new);
-        long long* nsoft_i = h->d_nsoft + static_cast<size_t>(i) * h->C;
-        const int TB = 256;
-        dim3 gtile(static_cast<unsigned>((std::max<long long>(n_new, 1) + TB - 1) / TB), h->C);
-        const int groups = (h->C + 31) / 32;
-        if (h->kind == QRL_DEMOD_DSSS) {
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(3, h->s_loop);
-            dsss_chain_kernel<<<h->C, 256, 0, h->s_loop>>>(h->dsp, h->d_ds, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
-                h->d_ds_arms, h->d_taps2, h->d_ds_taps,
-                static_cast<float2*>(h->ds_a.d), static_cast<float2*>(h->ds_c.d), h->ds_a.mask, h->ds_a.stride,
-                static_cast<float2*>(h->ds_d.d), h->ds_d.mask, h->ds_d.stride,
-                h->d_port0, h->port0_cap, h->ds_o_call0,
-                h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, nsoft_i);
-            h->launches++;
-            h->prof.end(pe);
-            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-            QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
-            pe = h->prof.begin(4, h->s_fec);
-            constexpr int CPB2 = 4;
-            viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
-                static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-                h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
-            viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs2, nsoft_i, h->C,
-                static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-                h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
-            h->launches += 2;
-            h->prof.end(pe);
-            continue;
+        const Slice s{ i, k0, k1, n_new, k_call0, h->d_nsoft + static_cast<size_t>(i) * h->C, sp,
+                       dim3(static_cast<unsigned>((std::max<long long>(n_new, 1) + kTileThreads - 1) / kTileThreads), h->C), (h->C + 31) / 32 };
+        int rc;
+        switch (h->kind) {
+        case QRL_DEMOD_DSSS: rc = slice_dsss(h, s); break;
+        case QRL_DEMOD_SSB: case QRL_DEMOD_FREEDV: case QRL_DEMOD_AM: case QRL_DEMOD_NBFM: case QRL_DEMOD_WBFM: rc = slice_analog(h, s); break;
+        case QRL_DEMOD_BPSK: case QRL_DEMOD_2FSK: rc = slice_fll_bpsk_2fsk(h, s); break;      // (GMSK runs as 2FSK)
+        case QRL_DEMOD_4FSK: rc = slice_4fsk(h, s); break;                                    // (M17 and DMR run as 4FSK)
+        default: rc = slice_qpsk(h, s); break;
         }
-        if (h->kind == QRL_DEMOD_SSB) {
-            if (n_new > 0) {
-                pe = h->prof.begin(1, sp);
-                fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
-                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                    static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                    h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
-                h->launches++;
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(3, h->s_loop);
-            ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb,
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
-                static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
-                static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
-                h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
-            h->launches++;
-            h->prof.end(pe);
-            continue;
-        }
-        if (h->kind == QRL_DEMOD_FREEDV) {
-            if (n_new > 0) {
-                pe = h->prof.begin(1, sp);
-                fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
-                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                    static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                    h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
-                h->launches++;
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(3, h->s_loop);
-            freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
-                static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
-                reinterpret_cast<short*>(h->d_port1), 4 * h->port1_cap, h->d_port1_cnt, static_cast<int>(4 * h->port1_cap));
-            h->launches++;
-            h->prof.end(pe);
-            continue;
-        }
-        if (h->kind == QRL_DEMOD_AM) {
-            if (n_new > 0) {
-                pe = h->prof.begin(1, sp);
-                fir_ccc_ring_kernel<<<gtile, TB, sizeof(float) * 2 * h->ntaps2, sp>>>(
-                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                    static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                    h->d_taps2, h->ntaps2, 1.0f, k0, k1, h->d_port0, h->port0_cap, k_call0);
-                h->launches++;
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(3, h->s_loop);
-            nbfm_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->nbp, h->d_nb,
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1, h->d_env,
-                static_cast<float2*>(h->rg.d), h->rg.mask, h->rg.stride,
-                static_cast<float*>(h->rd.d), h->rd.mask, h->rd.stride,
-                static_cast<float*>(h->rr.d), h->rr.mask, h->rr.stride,
-                h->d_arm_taps, h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
-            h->launches++;
-            h->prof.end(pe);
-            continue;
-        }
-        if (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_WBFM) {
-            if (n_new > 0) {
-                pe = h->prof.begin(1, sp);
-                { int rc = launch_fir_ccf(h, sp, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                                          static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                          h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 0); if (rc) return rc; }
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(3, h->s_loop);
-            const size_t fat = h->nbfm_split ? 120 * 1024 : 0;       // one CTA per SM, and never next to a de-emphasis CTA
-            if (h->nbfm_split) {
-                int rc;
-                if ((rc = smem_opt_in(h, nbfm_audio_kernel, 120 * 1024)) || (rc = smem_opt_in(h, nbfm_deemph_kernel, 120 * 1024))) return rc;
-            }
-            nbfm_audio_kernel<<<h->C, 128, fat, h->s_loop>>>(h->nbp, h->d_nb,
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1, h->d_env,
-                static_cast<float2*>(h->rg.d), h->rg.mask, h->rg.stride,
-                static_cast<float*>(h->rd.d), h->rd.mask, h->rd.stride,
-                static_cast<float*>(h->rr.d), h->rr.mask, h->rr.stride,
-                h->d_arm_taps, h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap),
-                h->nbfm_split ? static_cast<float*>(h->raud.d) : nullptr, h->raud.mask, h->raud.stride, h->nbfm_split ? nsoft_i : nullptr,
-                static_cast<float*>(h->rq.d), h->rq.mask, h->rq.stride, h->ctc, h->d_cenv);
-            h->launches++;
-            h->prof.end(pe);
-            if (h->nbfm_split) {
-                QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-                QRL_CK(cudaStreamWaitEvent(h->s_loop2, h->ev_b[i], 0));
-                pe = h->prof.begin(5, h->s_loop2);
-                nbfm_deemph_kernel<<<h->C, 128, fat, h->s_loop2>>>(h->nbp.b0, h->nbp.b1, h->nbp.a1, h->nbp.out_gain, h->d_nb2,
-                    static_cast<const float*>(h->raud.d), h->raud.mask, h->raud.stride, nsoft_i,
-                    h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
-                h->launches++;
-                h->prof.end(pe);
-            }
-            continue;
-        }
-        if (h->kind == QRL_DEMOD_2FSK || h->kind == QRL_DEMOD_BPSK) {
-            const bool bpsk = h->kind == QRL_DEMOD_BPSK;
-            // ---- FLL (sequential, per sample) on the loop stream: r1 -> rf
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            pe = h->prof.begin(1, h->s_loop);
-            if (!h->gmsk) {
-                fll_kernel<32><<<groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
-                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
-                    static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
-                h->launches++;
-            }
-            h->prof.end(pe);
-            const Ring& fin = h->gmsk ? h->r1 : h->rf;             // GMSK: no FLL in front of the channel filter
-            if (n_new > 0) {
-                // ---- channel filter / RRC on the FLL output -> port 0 (+ ring: channel-major for 2FSK, interleaved for BPSK)
-                pe = h->prof.begin(2, h->s_loop);
-                { int rc = launch_fir_ccf(h, h->s_loop, static_cast<const float2*>(fin.d), fin.mask, fin.stride,
-                                          static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                          h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, bpsk ? 1 : 0); if (rc) return rc; }
-                if (!bpsk && h->flag) {
-                    { int rc = launch_qdemod_fir(h, h->s_loop, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                                 static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
-                                                 h->d_taps3, h->ntaps3, h->qd_gain, k0, k1); if (rc) return rc; }
-                } else if (!bpsk) {
-                    fsk_bank_kernel<2><<<gtile, TB, sizeof(float) * 4 * h->nt_bank, h->s_loop>>>(
-                        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, k0, k1,
-                        static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
-                    fir_fff_ring_kernel<<<gtile, TB, sizeof(float) * h->nt_symf, h->s_loop>>>(
-                        static_cast<const float*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
-                        static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, h->d_symf_taps, h->nt_symf, k0, k1);
-                    h->launches += 2;
-                }
-                h->prof.end(pe);
-            }
-            pe = h->prof.begin(3, h->s_loop);
-            if (bpsk) {
-                {   // agc2_cc (Costas bypassed): r2 -> r3
-                    constexpr int CH = 128, NST = 2;
-                    const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
-                    auto kern = agc_costas_kernel<CH, NST, 0, 0>;
-                    if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
-                    kern<<<groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
-                        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
-                        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
-                    h->launches++;
-                }
-                constexpr int CH = 128, NST = 3, NEPI = 1;
-                const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period) + 3);
-                const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
-                auto kern = symsync_kernel<2, SL_BPSK, EPI_BPSK, CH, NST, NEPI, LOOP_CRMM>;
-                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
-                kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
-                    h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
-                    h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                    static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
-                h->launches++;
-            } else {
-                constexpr int CH = 256, NST = 3, NEPI = 2;
-                const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
-                const size_t smem = sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * maxs * 32) + sizeof(int) * 64;
-                auto kern = symsync_kernel<1, SL_BPSK, EPI_REAL1, CH, NST, NEPI>;
-                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
-                kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
-                    h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, k1,
-                    h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                    static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
-                h->launches++;
-            }
-            h->prof.end(pe);
-            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-            // ---- two decoders on the same soft stream, the second behind delay(1)
-            QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
-            pe = h->prof.begin(4, h->s_fec);
-            constexpr int CPB2 = 4;
-            viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
-                static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-                h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
-            viterbi_k7_kernel<CPB2><<<(h->C + CPB2 - 1) / CPB2, 64 * CPB2, 0, h->s_fec>>>(h->d_vs2, nsoft_i, h->C,
-                static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-                h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
-            h->launches += 2;
-            h->prof.end(pe);
-            continue;
-        }
-        if (h->kind == QRL_DEMOD_4FSK) {
-            if (n_new > 0) {
-                // ---- stage 2: channel filter -> ring + port 0
-                pe = h->prof.begin(1, sp);
-                { int rc = launch_fir_ccf(h, sp, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                                          static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                          h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 0); if (rc) return rc; }
-                h->prof.end(pe);
-                // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
-                // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
-                if (h->overlap && h->prev_nsub > 0) {
-                    // the slots [k0, k1) overwrite the samples cap older; the previous call's symbol sync of slice q has
-                    // consumed everything up to prev_k1[q] - lookahead
-                    const long long must = k1 - (static_cast<long long>(h->r4.mask) + 1) + 64;
-                    int q = -1;
-                    for (int j = 0; j < h->prev_nsub; j++) if (h->prev_k1[j] - 64 < must) q = j;      // not yet safe after slice j alone
-                    if (q >= 0) QRL_CK(cudaStreamWaitEvent(sp, h->ev_c[std::min(q + 1, h->prev_nsub - 1)], 0));
-                }
-                pe = h->prof.begin(2, sp);
-                if (h->flag) {
-                    { int rc = launch_qdemod_fir(h, sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                                 static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
-                                                 h->d_taps3, h->ntaps3, h->qd_gain, k0, k1); if (rc) return rc; }
-                    if (h->dmr) {      // gr_demod_dmr.cpp:103: the symbol filter output is port 3
-                        ring_to_port_f32_kernel<<<dim3(static_cast<unsigned>((k1 - k0 + 31) / 32), groups), dim3(32, 8), 0, sp>>>(
-                            static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, h->C, k0, k1,
-                            h->d_port3f, h->port0_cap, k0 - k_call0);
-                        h->launches++;
-                    }
-                } else {
-                    fsk_bank_kernel<4><<<gtile, TB, sizeof(float) * 8 * h->nt_bank, sp>>>(
-                        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, k0, k1,
-                        static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
-                    h->launches++;
-                    { int rc = launch_fir_ccf(h, sp, static_cast<const float2*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
-                                              static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride,
-                                              h->d_symf_taps, h->nt_symf, k0, k1, nullptr, 0, 0, 1); if (rc) return rc; }
-                }
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            // ---- stage 4: symbol sync (+ phase mod + soft bits) on the loop stream
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            bool ext_recorded = false;
-            if (!h->flag) {
-                pe = h->prof.begin(3, h->s_loop);
-                constexpr int CH = 128, NST = 3, NEPI = 2;
-                const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
-                const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + 2 * maxs * 64) + sizeof(int) * 64;
-                auto kern = symsync_kernel<2, SL_RECT4, EPI_CPLX, CH, NST, NEPI>;
-                if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
-                kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop>>>(
-                    h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
-                    h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                    static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
-                h->launches++;
-                h->prof.end(pe);
-            } else {
-                pe = h->prof.begin(3, h->s_loop);
-                // real symbols: lean recurrence + external epilogue (symbols leave the SM by TMA bulk store; the phase
-                // modulator / soft-bit stores run on the wide partition behind it, same stream)
-                auto run_ext = [&](auto ch_tag, auto nst_tag) -> int {
-                constexpr int CH = decltype(ch_tag)::value, NST = decltype(nst_tag)::value;
-                const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
-                const size_t smem_base = sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * (maxs + 2) * 32) + sizeof(int) * 64;
-                const size_t smem_rep = smem_base + 129 * 512;          // + replicated (conflict-free) interpolator bank
-                const bool rep = smem_rep <= 220 * 1024 && !h->dmr;
-                const size_t smem = rep ? smem_rep : smem_base;
-                // gr_demod_dmr: TED_MUELLER_AND_MULLER instead of the modified detector -> generic recurrence, variant 3
-                auto kern = h->dmr ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>
-                          : rep ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 2>
-                                : symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 1>;
-                if (int rc = smem_opt_in(h, kern, 224 * 1024)) return rc;
-                // overlapped calls: the previous call's Viterbi of slice i still reads d_nsoft[i], its epilogue scratch region i
-                if (h->overlap) QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_v[i], 0));
-                // every slice of a call gets its own scratch region and header (the epilogue of slice i overlaps symsync i+1)
-                if (i == 0) h->ss_chunk_off = 0;
-                const int chunk_bound = static_cast<int>(std::min<long long>(h->ss_chunk_cap - h->ss_chunk_off, n_new / symsync_stride(CH, h->ssp.lookahead) + 3));
-                float* scratch_i = h->d_ss_scratch + static_cast<size_t>(h->ss_chunk_off) * (maxs + 2) * 32;
-                int* hdr_i = h->d_ss_hdr + static_cast<size_t>(i) * groups * 128;
-                h->ss_chunk_off += chunk_bound;
-                kern<<<groups, 96, smem, h->s_loop>>>(
-                    h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, k1,
-                    h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                    static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i,
-                    scratch_i, chunk_bound, static_cast<int>(h->ss_chunk_cap), hdr_i);
-                h->prof.end(pe);
-                cudaStream_t se = h->s_epi ? h->s_epi : h->s_loop;
-                if (se != h->s_loop || h->overlap) QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
-                if (se != h->s_loop) QRL_CK(cudaStreamWaitEvent(se, h->ev_c[i], 0));
-                pe = h->prof.begin(5, se);
-                auto epi = h->dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
-                if (chunk_bound > 0)
-                    epi<<<dim3(chunk_bound, groups), dim3(32, 8), 0, se>>>(
-                        h->ssp, h->C, scratch_i, static_cast<int>(h->ss_chunk_cap), maxs, hdr_i,
-                        h->d_port1, h->port1_cap, static_cast<int>(h->port1_cap),
-                        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-                        h->m17 ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
-                h->launches++;
-                h->prof.end(pe);
-                QRL_CK(cudaEventRecord(h->ev_b[i], se));
-                return QRL_OK;
-                };
-                const int rc_ext = h->ss_ch == 512 ? run_ext(std::integral_constant<int, 512>{}, std::integral_constant<int, 2>{})
-                                                   : run_ext(std::integral_constant<int, 256>{}, std::integral_constant<int, 3>{});
-                if (rc_ext) return rc_ext;
-                ext_recorded = true;
-            }
-            if (!ext_recorded) QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop));
-        } else {   // QRL_DEMOD_QPSK
-            const float2* shaping_in = static_cast<const float2*>(h->r1.d);
-            unsigned shaping_mask = h->r1.mask; long long shaping_stride = h->r1.stride;
-            if (h->d_fll) {     // sps > 4: fll_band_edge_cc between resampler and shaping filter (sequential, on the loop stream)
-                QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-                QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-                fll_kernel<32><<<groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
-                    static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, k1,
-                    static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
-                h->launches++;
-                QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
-                QRL_CK(cudaStreamWaitEvent(sp, h->ev_c[i], 0));
-                shaping_in = static_cast<const float2*>(h->rf.d); shaping_mask = h->rf.mask; shaping_stride = h->rf.stride;
-            }
-            if (n_new > 0) {
-                // ---- stage 2: RRC shaping filter -> interleaved ring + port 0
-                pe = h->prof.begin(1, sp);
-                { int rc = launch_fir_ccf(h, sp, shaping_in, shaping_mask, shaping_stride,
-                                          static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                          h->d_taps2, h->ntaps2, k0, k1, h->d_port0, h->port0_cap, k_call0, 1); if (rc) return rc; }
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_a[i], sp));
-            // ---- stage 3: agc2 + costas "PLL" per sample on the loop stream
-            QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_a[i], 0));
-            {
-                pe = h->prof.begin(2, h->s_loop);
-                auto run_ac = [&](auto ch_tag) -> int {
-                    constexpr int CH = decltype(ch_tag)::value, NST = 2;      // input stages (2) + hand-off blocks (3): 164 KB at CH = 128
-                    const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
-                    auto kern = (h->acp.order == 4 && h->acp.use_snr) ? agc_costas_kernel<CH, NST, 4, 1> : agc_costas_kernel<CH, NST>;
-                    int rc;                                 // both instantiations, whichever this call takes
-                    if ((rc = smem_opt_in(h, agc_costas_kernel<CH, NST, 4, 1>, 200 * 1024)) || (rc = smem_opt_in(h, agc_costas_kernel<CH, NST>, 200 * 1024))) return rc;
-                    kern<<<groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
-                        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, k1,
-                        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
-                    return QRL_OK;
-                };
-                // many channels: 32-row windows (41 KB of shared memory, five CTAs per SM) instead of 128-row ones (164 KB)
-                const int rc_ac = h->many ? run_ac(std::integral_constant<int, 32>{}) : run_ac(std::integral_constant<int, 128>{});
-                if (rc_ac) return rc_ac;
-                h->launches++;
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_c[i], h->s_loop));
-            // ---- stage 4: symbol sync + second Costas + diff phasor + soft bits on the second loop stream
-            QRL_CK(cudaStreamWaitEvent(h->s_loop2, h->ev_c[i], 0));
-            {
-                pe = h->prof.begin(3, h->s_loop2);
-                // lean: the prefetching complex recurrence (symbol-sync variant 2, replicated tap bank) with the epilogue split into a
-                // Costas warp and a feed-forward warp over a 3-deep symbol ring (NEPI = 2); else the generic recurrence, one epilogue warp
-                auto run_sq = [&](auto ch_tag, auto nst_tag, auto lean_tag) -> int {
-                    constexpr int CH = decltype(ch_tag)::value, NST = decltype(nst_tag)::value;
-                    constexpr bool LEAN = decltype(lean_tag)::value;
-                    constexpr int NEPI = LEAN ? 2 : 1, NB = LEAN ? 3 : 2;
-                    const int maxs = static_cast<int>((CH + 1) / (h->ssp.min_period - fabsf(h->ssp.alpha)) + 3);
-                    const size_t smem = sizeof(float) * (NST * CH * 64 + SYMSYNC_TAB_FLOATS + NB * maxs * 64) + sizeof(int) * 32 * (NB == 2 ? 2 : 4) +
-                                        (LEAN ? 129 * 512 : 0);
-                    auto kern = symsync_kernel<2, SL_DQPSK, EPI_QPSK, CH, NST, NEPI, LOOP_SYMSYNC, LEAN ? 2 : 0>;
-                    if (int rc = smem_opt_in(h, kern, 224 * 1024)) return rc;
-                    if (smem > 224 * 1024) { set_err(h, "QPSK symbol sync: window does not fit shared memory"); return QRL_EINVAL; }
-                    kern<<<groups, 64 + 32 * NEPI, smem, h->s_loop2>>>(
-                        h->ssp, h->d_ss, h->C, static_cast<const float*>(h->r3.d), h->r3.mask, h->r3.stride, k1,
-                        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-                        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, nullptr, 0, 0, nullptr);
-                    return QRL_OK;
-                };
-                // many channels: 64-row windows, two stages (~55 KB, four CTAs per SM) instead of 128-row ones
-                const bool small_win = h->many && symsync_stride(64, h->ssp.lookahead) >= 32;
-                static const bool lean_env = [] { const char* e = getenv("QRL_QPSK_LEAN_SS"); return !(e && e[0] == '0'); }();
-                // the lean recurrence needs the in-lock window proof (kernel: lean_ok && window_sure) -- true for every QPSK instance of
-                // gr_demod_base.cpp; the kernel itself falls back to the generic loop when it does not hold
-                const int rc_sq = small_win ? run_sq(std::integral_constant<int, 64>{}, std::integral_constant<int, 2>{}, std::false_type{})
-                                : lean_env  ? run_sq(std::integral_constant<int, 128>{}, std::integral_constant<int, 2>{}, std::true_type{})
-                                            : run_sq(std::integral_constant<int, 128>{}, std::integral_constant<int, 3>{}, std::false_type{});
-                if (rc_sq) return rc_sq;
-                h->launches++;
-                h->prof.end(pe);
-            }
-            QRL_CK(cudaEventRecord(h->ev_b[i], h->s_loop2));
-        }
-        // ---- stage 5: Viterbi + descrambler on the FEC stream
-        QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[i], 0));
-        if (h->m17) {                    // gr_demod_m17 has no FEC: the epilogue wrote the hard bits of port 2 (s_fec joins it at the end)
-            if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[i], h->s_fec));
-            continue;
-        }
-        pe = h->prof.begin(4, h->s_fec);
-        constexpr int CPB = 4;    // 4 channels (8 warps) per CTA
-        viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
-            static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-            h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
-        h->launches++;
-        h->prof.end(pe);
-        if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[i], h->s_fec));
+        if (rc) return rc;
     }
     if (!began) { int rc = begin_call(); if (rc) return rc; }     // every slice was empty
     if (h->kind == QRL_DEMOD_DSSS) {          // port 0 holds 5200 sps items (13 / 50 of the stage-1 items counted in the loop)
