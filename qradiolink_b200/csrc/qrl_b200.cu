@@ -36,6 +36,15 @@ unsigned pow2_at_least(long long n)
     return static_cast<unsigned>(c);
 }
 
+// a polyphase interpolator's taps as L arms of nt taps each (arm p holds taps p, p + L, ...; zero past the end)
+std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
+{
+    std::vector<float> a(static_cast<size_t>(L) * nt, 0.0f);
+    for (int p = 0; p < L; p++)
+        for (int k = 0; k < nt; k++) { const size_t j = p + static_cast<size_t>(k) * L; if (j < taps.size()) a[p * nt + k] = taps[j]; }
+    return a;
+}
+
 using HandleBase = QrlHandleBase;       // qrl_handle.hpp: shared by every handle type of the library
 
 // a device pointer handed to a *_work call must live on the handle's device (a pointer from another GPU would fault inside a kernel
@@ -1060,9 +1069,7 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         if (sps < 1 || d.nt_arm > 8 || d.nt2 > 64 || d.ntaps > 640 || d.N + d.ntaps - 1 > kDsssChunk) {
             set_err(h, "make_gr_demod_dsss: sps / filter_width outside what the chain kernel holds in shared memory"); return fail(QRL_EINVAL);
         }
-        std::vector<float> arms(static_cast<size_t>(13) * d.nt_arm, 0.0f);
-        for (int p = 0; p < 13; p++) for (int k = 0; k < d.nt_arm; k++) { const size_t j = p + static_cast<size_t>(k) * 13; if (j < tif.size()) arms[p * d.nt_arm + k] = tif[j]; }
-        if ((rc = upload_floats(h, &h->d_ds_arms, arms))) return fail(rc);
+        if ((rc = upload_floats(h, &h->d_ds_arms, make_arms(tif, 13, d.nt_arm)))) return fail(rc);
         {   // dsss_decoder_cc_impl.cc:60-96: reversed Barker-13, `sps` items per chip, shaped by RRC(1, sps, 1, 0.35f, 11 sps); the block's
             // fir_filter_ccc keeps the taps reversed (what is uploaded)
             static const int barker_13[13] = { 1, 1, 1, 1, 1, 0, 0, 1, 1, 0, 1, 0, 1 };
@@ -2016,35 +2023,32 @@ struct ZeroIdle {
     void release() { if (d_ranges) cudaFree(d_ranges); d_ranges = nullptr; }
 };
 
+// the transmit chains (DESIGN.md section 5): tx_create picks one and designs its taps and rings, qrl_tx_work runs its work function
+enum class TxChain { Fsk, Psk, M17, Dmr, Dsss, Nbfm, Ssb, Am, Freedv };
 struct qrl_tx : HandleBase {
-    int kind = 0, sps = 0, samp_rate = 0, filter_width = 0, flag = 0, C = 0;
+    TxChain chain = TxChain::Fsk;
+    int txm = 0, sym_per_item = 0;  // the byte-fed chains: tx_bits_kernel mode (TXM_*), symbols (DSSS: chips) per input byte
+    int samp_rate = 0, flag = 0, C = 0;
     long max_items = 0;
     int L1 = 1, nt1 = 0;            // first interpolation (RRC): L1 arms of nt1 taps
-    int L2 = 1, nt2 = 0;            // second interpolation (x20 low-pass), 4FSK only
+    int L2 = 1, nt2 = 0;            // final interpolation (4FSK: the x20 low-pass): L2 arms of nt2 taps
     float* d_arms1 = nullptr; float* d_arms2 = nullptr;
     float fm_sens = 0, amplif = 0, bb_gain = 1.0f, pulse_scale = 0.66666666f;
     int repeat_only = 0;
-    bool m17 = false; int M2 = 1;  // gr_mod_m17: 4 symbols per byte, IF low-pass at 24 ksps, x L2 / M2 rational interpolator
-    // gr_mod_dsss: chips (complex ring d_sym) -> x25 (ring d_if) -> x50 / 13 (ring d_rc, arms in d_cfilt) -> x50 (d_out)
-    bool dsss_tx = false;
-    // gr_mod_am: audio ring d_ra -> 8 ksps complex ring d_if -> x sps (ring d_rc at the output rate) -> output filter (taps d_cfilt) -> d_out
-    bool am_tx = false; float am_dc = 0.0f;
-    // gr_mod_freedv: int16 in (d_short_in) -> complex ring d_rs2 -> side-band filter (taps d_cfilt) -> ring d_rc -> feedforward AGC -> ring d_if
-    // (same geometry) -> x sps (arms d_arms2) -> d_out
-    bool freedv_tx = false; short* d_short_in = nullptr;
+    int M2 = 1;                     // gr_mod_m17 / gr_mod_dmr: 4 symbols per byte, IF stage at 24 ksps, x L2 / M2 rational interpolator
+    float am_dc = 0.0f;             // gr_mod_am: the carrier added to the audio
     // gr_mod_nbfm::set_ctcss: multiply_const_ff gain and the CTCSS tone source (fxpt_nco phase / increment, advanced per sample with the tone on)
     float audio_gain = 0.99f; bool tone_on = false; unsigned tone_phase = 0, tone_inc = 0;
     // gr_mod_dmr: the m17 path with gr_zero_idle_bursts in place of the IF low-pass (a delay of history - 1 items + "zero_samples" tags)
-    bool dmr_tx = false; long long zi_delay_items = 0; unsigned zi_tag_delay = 0;
+    long long zi_delay_items = 0; unsigned zi_tag_delay = 0;
     ZeroIdle zi;                                                      // gr_mod_dmr: gr_zero_idle_bursts(62)
     TxBitState* d_bits = nullptr;
-    unsigned char* d_in = nullptr;
+    unsigned char* d_in = nullptr; size_t in_isz = 1;   // [C][max_items] staging of host input: bytes, float audio (NBFM / SSB / AM) or int16 (FreeDV)
     float* d_sym = nullptr; unsigned sym_mask = 0; long long sym_stride = 0;    // float (4FSK) / float2 (QPSK)
     float2* d_if = nullptr; unsigned if_mask = 0; long long if_stride = 0;
     float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_sym = 0;           // symbols produced so far (absolute)
-    // analog modulators (NBFM / SSB)
-    TxAnalogState* d_an = nullptr;
+    TxAnalogState* d_an = nullptr;                                                 // analog modulators (NBFM / SSB / AM)
     float* d_ra = nullptr; unsigned ra_mask = 0; long long ra_stride = 0;          // audio ring
     float* d_rb = nullptr;                                                         // filtered audio ring (same geometry)
     float2* d_rc = nullptr; unsigned rc_mask = 0; long long rc_stride = 0;         // SSB clip ring / NBFM IF-filter ring
@@ -2052,7 +2056,6 @@ struct qrl_tx : HandleBase {
     float* d_lpf = nullptr; int nt_lpf = 0; float* d_cfilt = nullptr; int nt_cfilt = 0;
     double pe_b0 = 0, pe_b1 = 0, pe_a1 = 0;
     long long n_audio = 0, n_mid = 0;        // audio samples consumed / mid-rate items produced (host mirror of the device counters)
-    float* d_audio_in = nullptr;
     // 4FSK: the three stages (bit chain, pulse shaping + FM scan, x20 interpolator) run slice by slice on three streams
     static constexpr int kTxSub = 8;
     cudaStream_t s_bits = nullptr, s_shape = nullptr;
@@ -2060,157 +2063,42 @@ struct qrl_tx : HandleBase {
     // optional per-stage device timing (qrl_tx_profile): 0 = bit chain, 1 = pulse shaping / FM scan, 2 = final interpolator
     StageProfiler prof{ 4 };
 };
-
-static std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
+namespace {
+// the interpolator and resampler kernels stage a whole arm table (L arms of nt taps) in shared memory
+bool arms_fit(int L, int nt) { return static_cast<size_t>(L) * nt * sizeof(float) <= 40 * 1024; }
+int arms_nt(const std::vector<float>& taps, int L) { return (static_cast<int>(taps.size()) + L - 1) / L; }
+// register-tiled interpolator shapes.  tx_create pads a shorter arm table to the instance's taps per arm, so the same predicate
+// picks the instance in qrl_tx_work: interp_fir_ccf_rt_kernel<20, 35, 8, 16> (4FSK's final x20), interp_fir_ccf_kernel<4, 16, 8, 64> (QPSK)
+constexpr int kFskRtL = 20, kFskRtNT = 35, kQpskRtL = 4, kQpskRtNT = 16;
+bool fsk_rt(int L2, int nt2) { return L2 == kFskRtL && nt2 <= kFskRtNT; }
+bool qpsk_rt(int L1, int nt1) { return L1 == kQpskRtL && nt1 <= kQpskRtNT; }
+// what a chain's create function designs; tx_create uploads the tables and allocates the rings
+struct TxDesign {
+    std::vector<float> t1, t2, lpf, cfilt;     // prototypes of d_arms1 (L1 arms of nt1) and d_arms2 (L2 arms of nt2); d_lpf, d_cfilt as given
+    long long sym = 0, if_ = 0, rc = 0, ra = 0, out = 0;      // items each ring must hold (0: the chain has no such ring); out_stride
+    int sym_floats = 1;                                       // 2: complex symbols
+    bool rb = false, rs2 = false;                             // d_rb in d_ra's geometry, d_rs2 in d_rc's
+};
+// a [C][capacity] ring of at least min_items items, each `per_item` Ts
+extern "C++" template <class T> int tx_ring(qrl_tx* h, T** d, unsigned* mask, long long* stride, long long min_items, int per_item = 1)
 {
-    std::vector<float> a(static_cast<size_t>(L) * nt, 0.0f);
-    for (int p = 0; p < L; p++)
-        for (int k = 0; k < nt; k++) { const size_t j = p + static_cast<size_t>(k) * L; if (j < taps.size()) a[p * nt + k] = taps[j]; }
-    return a;
+    const unsigned cap = pow2_at_least(min_items); *mask = cap - 1; *stride = cap;
+    return dev_alloc(h, d, static_cast<size_t>(cap) * h->C * per_item);
 }
-
-static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
-                     int n_channels, long max_items, int device, qrl_tx** out);
-
-int qrl_tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
-                  int n_channels, long max_items, int device, qrl_tx** out)
+void create_fsk(qrl_tx* h, TxDesign& d, int kind, int sps, int samp_rate, int fw)
 {
-    if (kind == QRL_MOD_FREEDV) { set_err(nullptr, "qrl_tx_create: QRL_MOD_FREEDV takes a low cutoff: use qrl_tx_create_freedv"); return QRL_EINVAL; }
-    return tx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, 0, n_channels, max_items, device, out);
-}
-
-int qrl_tx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
-                         int n_channels, long max_items, int device, qrl_tx** out)
-{
-    int rc = check_freedv_args("qrl_tx_create_freedv", sps, samp_rate, filter_width, low_cutoff);
-    if (rc) return rc;
-    return tx_create(QRL_MOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_items, device, out);
-}
-
-static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
-                     int n_channels, long max_items, int device, qrl_tx** out)
-{
-    (void)carrier_freq;
-    if (!out || n_channels <= 0 || max_items <= 0) { set_err(nullptr, "qrl_tx_create: bad argument"); return QRL_EINVAL; }
-    *out = nullptr;
-    if (int rc = check_device("qrl_tx_create", device)) return rc;
-    qrl_tx* h = new qrl_tx();
-    h->kind = kind; h->sps = sps; h->samp_rate = samp_rate; h->filter_width = filter_width; h->flag = flag;
-    h->C = n_channels; h->max_items = max_items;
-    auto fail = [&](int rc) { return create_failed(h, qrl_tx_destroy, rc); };
-    int rc = handle_open(h, device);
-    if (!rc) rc = upload_tables(h);
-    if (rc) return fail(rc);
-    std::vector<float> t1, t2;
     if (kind == QRL_MOD_4FSK) {
         // gr_mod_4fsk.cpp:55-92
         int sym_sps = sps, nfilts = sym_sps * 10, second_interp = 20;
         if (sps == 2) { sym_sps = 5; second_interp = 2; nfilts = 256; }
         int spacing = 2; h->amplif = 0.8f;
-        if (flag) { h->amplif = 0.9f; spacing = 1; }
-        h->repeat_only = flag ? 0 : 1;
-        t1 = root_raised_cosine(sym_sps, sym_sps, 1, 0.2, nfilts);
-        h->L1 = sym_sps; h->nt1 = (static_cast<int>(t1.size()) + sym_sps - 1) / sym_sps;
+        if (h->flag) { h->amplif = 0.9f; spacing = 1; }
+        h->repeat_only = h->flag ? 0 : 1;
+        h->txm = TXM_4FSK; h->sym_per_item = 8;
+        d.t1 = root_raised_cosine(sym_sps, sym_sps, 1, 0.2, nfilts);
+        h->L1 = sym_sps;
         h->fm_sens = static_cast<float>((spacing * kPi) / sym_sps);
-        t2 = low_pass(second_interp, samp_rate, filter_width, filter_width, WIN_HAMMING);
-        h->L2 = second_interp; h->nt2 = (static_cast<int>(t2.size()) + second_interp - 1) / second_interp;
-        if (h->L2 == 20 && h->nt2 <= 35) h->nt2 = 35;      // register-tiled instance <20, 35>
-    } else if (kind == QRL_MOD_QPSK) {
-        // gr_mod_qpsk.cpp:58-75
-        int nfilts = sps > 120 ? 11 : (sps > 10 ? 13 : 15);
-        t1 = root_raised_cosine(sps, sps, 1, 0.35, nfilts * sps);
-        h->L1 = sps; h->nt1 = (static_cast<int>(t1.size()) + sps - 1) / sps;
-        if (h->L1 == 4 && h->nt1 <= 16) h->nt1 = 16;      // register-tiled instance <4, 16>
-        h->amplif = 0.6f;
-    } else if (kind == QRL_MOD_NBFM) {
-        // gr_mod_nbfm.cpp:35-63 (sps = final interpolation, 20)
-        double a[2], b[2];
-        preemph_taps(8000, 50e-6, -1.0, a, b);
-        h->pe_b0 = b[0]; h->pe_b1 = b[1]; h->pe_a1 = a[1];
-        std::vector<float> lp = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
-        h->nt_lpf = static_cast<int>(lp.size());
-        if ((rc = upload_floats(h, &h->d_lpf, lp))) return fail(rc);
-        t1 = low_pass_2(25, 50000 * 4, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS);          // 25/4 resampler arms
-        h->L1 = 25; h->nt1 = (static_cast<int>(t1.size()) + 24) / 25;
-        h->fm_sens = static_cast<float>(4 * kPi * filter_width / 50000.0f);
-        std::vector<float> ifl = low_pass_2(1, 50000, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS);
-        h->nt_cfilt = static_cast<int>(ifl.size());
-        if ((rc = upload_floats(h, &h->d_cfilt, ifl))) return fail(rc);
-        t2 = low_pass_2(sps, samp_rate, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS);
-        h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        h->amplif = 0.8f;
-    } else if (kind == QRL_MOD_SSB) {
-        // gr_mod_ssb.cpp:40-58 (sps = final interpolation, 125; flag = sb)
-        std::vector<float> bp = band_pass_2(1, 8000, 300, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        h->nt_lpf = static_cast<int>(bp.size());
-        if ((rc = upload_floats(h, &h->d_lpf, bp))) return fail(rc);
-        std::vector<float> sb = flag ? complex_band_pass_2(1, 8000, -filter_width, -200, 200, 90, WIN_BLACKMAN_HARRIS)
-                                     : complex_band_pass_2(1, 8000, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        h->nt_cfilt = static_cast<int>(sb.size() / 2);
-        if ((rc = upload_floats(h, &h->d_cfilt, sb))) return fail(rc);
-        t2 = low_pass_2(sps, samp_rate, filter_width, filter_width, 90, WIN_BLACKMAN_HARRIS);
-        h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        h->L1 = 1; h->nt1 = 1; t1 = { 1.0f };
-        h->amplif = 0.9f;
-    } else if (kind == QRL_MOD_FREEDV) {
-        // gr_mod_freedv.cpp:34-85 (sps = final interpolation, 125; flag = sb): side-band filter complex_band_pass_2(1, 8000, lo, fw, 250, 90, BH)
-        // (LSB: (-fw, -lo)), feedforward_agc_cc(512, 1), rational_resampler_ccf(sps, 1, low_pass(sps, fs, fw, 1200)) (Hamming), x0.98, x bb gain
-        h->freedv_tx = true; h->amplif = 0.98f;
-        std::vector<float> sb = flag ? complex_band_pass_2(1, 8000, -filter_width, -low_cutoff, 250, 90, WIN_BLACKMAN_HARRIS)
-                                     : complex_band_pass_2(1, 8000, low_cutoff, filter_width, 250, 90, WIN_BLACKMAN_HARRIS);
-        h->nt_cfilt = static_cast<int>(sb.size() / 2);
-        if ((rc = upload_floats(h, &h->d_cfilt, sb))) return fail(rc);
-        t2 = low_pass(sps, samp_rate, filter_width, 1200, WIN_HAMMING);
-        h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        t1 = { 1.0f }; h->L1 = 1; h->nt1 = 1;
-        if (h->L2 != 125 || h->nt2 != 17) {     // the register-tiled x125 instance (2007 taps, 17 per arm) is the one built
-            set_err(h, "make_gr_mod_freedv: interpolator shape not built (sps " + std::to_string(sps) + ", " + std::to_string(t2.size()) + " taps)");
-            return fail(QRL_EINVAL);
-        }
-    } else if (kind == QRL_MOD_BPSK) {
-        // gr_mod_bpsk.cpp:44-56
-        t1 = root_raised_cosine(sps, sps, 1, 0.35, 11 * sps);
-        h->L1 = sps; h->nt1 = (static_cast<int>(t1.size()) + sps - 1) / sps;
-        h->amplif = 0.6f;
-    } else if (kind == QRL_MOD_AM) {
-        // gr_mod_am.cpp:25-72: agc2_ff -> rail -> x0.95 -> band_pass_2(1, 8000, 300, 3000, 200, 60, Hamming) -> + 0.5 cos(0) -> float_to_complex ->
-        // rational_resampler_ccf(sps, 1, low_pass(sps, fs, fw, fw)) -> x0.5 -> bb gain -> fft_filter_ccc(complex_band_pass_2(1, fs, -fw, fw, 1200,
-        // 120, BH)).  The band is symmetric, so the complex taps are the low-pass prototype times e^{j0}: imaginary parts exactly 0 and the
-        // filter is the real-tap ring FIR (same accumulation, see oracle fircc_work with hi = 0).
-        h->am_tx = true; h->amplif = 0.5f;
-        const std::vector<float> bp = band_pass_2(1, 8000, 300, 3000, 200, 60, WIN_HAMMING);
-        h->nt_lpf = static_cast<int>(bp.size());
-        if ((rc = upload_floats(h, &h->d_lpf, bp))) return fail(rc);
-        t1 = { 1.0f }; h->L1 = 1; h->nt1 = 1;
-        t2 = low_pass(sps, samp_rate, filter_width, filter_width, WIN_HAMMING);
-        h->L2 = sps; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        const std::vector<float> cb = complex_band_pass_2(1, samp_rate, -filter_width, filter_width, 1200, 120, WIN_BLACKMAN_HARRIS);
-        std::vector<float> of(cb.size() / 2);
-        for (size_t i = 0; i < of.size(); i++) {
-            if (cb[2 * i + 1] != 0.0f) { set_err(h, "make_gr_mod_am: output filter taps are not real"); return fail(QRL_EINVAL); }
-            of[i] = cb[2 * i];
-        }
-        h->nt_cfilt = static_cast<int>(of.size());
-        if ((rc = upload_floats(h, &h->d_cfilt, of))) return fail(rc);
-        if (static_cast<size_t>(h->L2) * h->nt2 * sizeof(float) > 40 * 1024 || h->nt_cfilt > 8192) { set_err(h, "make_gr_mod_am: unsupported sps / filter_width"); return fail(QRL_EINVAL); }
-        { const std::vector<float> st_ = fxpt_sine_table(); const unsigned uc = 0x40000000u; const int ci = uc >> 22;
-          const float c0 = st_[2 * ci] * static_cast<float>(uc >> 1) + st_[2 * ci + 1];
-          h->am_dc = static_cast<float>(static_cast<double>(c0) * 0.5); }
-    } else if (kind == QRL_MOD_DSSS) {
-        // gr_mod_dsss.cpp:27-93: scrambler -> cc_encoder -> Barker-13 spreading -> {-1, +1} -> rational_resampler_ccf(sps, 1, RRC(sps, sps, 1,
-        // 0.35, 11 sps)) -> x0.65 -> bb gain -> rational_resampler_ccf(50, 13, low_pass(50, 5200 * 50, fw, 5 fw)) ->
-        // rational_resampler_ccf(50, 1, low_pass(50, fs, fw, 5 fw)); one input byte = 208 chips = 10^6 output samples (sps = 25)
-        h->dsss_tx = true; h->amplif = 0.65f;
-        t1 = root_raised_cosine(sps, sps, 1, 0.35, 11 * sps);
-        h->L1 = sps; h->nt1 = (static_cast<int>(t1.size()) + sps - 1) / sps;
-        const std::vector<float> tif = low_pass(50.0, 5200.0 * 50, filter_width, filter_width * 5, WIN_HAMMING);
-        h->nt_cfilt = (static_cast<int>(tif.size()) + 49) / 50;
-        if ((rc = upload_floats(h, &h->d_cfilt, make_arms(tif, 50, h->nt_cfilt)))) return fail(rc);
-        t2 = low_pass(50, samp_rate, filter_width, filter_width * 5, WIN_HAMMING);
-        h->L2 = 50; h->nt2 = (static_cast<int>(t2.size()) + 49) / 50;
-        if (static_cast<size_t>(50) * std::max(h->nt2, h->nt_cfilt) * sizeof(float) > 40 * 1024 || static_cast<size_t>(h->L1) * h->nt1 * sizeof(float) > 40 * 1024) {
-            set_err(h, "make_gr_mod_dsss: filter_width too small for the shared-memory arm tables"); return fail(QRL_EINVAL);
-        }
+        h->L2 = second_interp;
     } else if (kind == QRL_MOD_GMSK) {
         // gr_mod_gmsk.cpp:30-100: the 2FSK (fm) modulator path with a Gaussian pulse (BT 0.3), sensitivity (pi/2)/sps and a
         // x5 (x1 for the 10k mode) final interpolation; instances gr_mod_base.cpp:160-162
@@ -2219,125 +2107,251 @@ static int tx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         if (sps == 50) nfilts = 55;
         if (sps == 100) nfilts = 35;
         if ((nfilts % 2) == 0) nfilts += 1;
-        kind = QRL_MOD_2FSK; h->kind = QRL_MOD_2FSK; h->sps = sps; flag = 1; h->flag = 1;
+        h->flag = 1;
         h->amplif = 0.9f; h->repeat_only = 0; h->pulse_scale = 1.0f;
-        t1 = gaussian(sps, sps, 0.3, nfilts);
-        h->L1 = sps; h->nt1 = (static_cast<int>(t1.size()) + sps - 1) / sps;
+        h->txm = TXM_2FSK; h->sym_per_item = 16;
+        d.t1 = gaussian(sps, sps, 0.3, nfilts);
+        h->L1 = sps;
         h->fm_sens = static_cast<float>((kPi / 2) / sps);
-        t2 = low_pass(second_interp, samp_rate, filter_width, filter_width, WIN_HAMMING);
-        h->L2 = second_interp; h->nt2 = (static_cast<int>(t2.size()) + second_interp - 1) / second_interp;
-    } else if (kind == QRL_MOD_M17) {
+        h->L2 = second_interp;
+    } else {
+        // gr_mod_2fsk.cpp:43-76
+        int nfilts = 25 * sps, spacing = 2; h->amplif = 0.8f;
+        if (h->flag) { spacing = 1; h->amplif = 0.9f; }
+        if (sps == 5) nfilts = nfilts * 5;
+        if ((nfilts % 2) == 0) nfilts += 1;
+        h->repeat_only = h->flag ? 0 : 1;
+        h->pulse_scale = 1.0f;
+        h->txm = TXM_2FSK; h->sym_per_item = 16;
+        d.t1 = root_raised_cosine(sps, sps, 1, 0.2, nfilts);
+        h->L1 = sps;
+        h->fm_sens = static_cast<float>((spacing * kPi / 2) / sps);
+        h->L2 = 10;
+    }
+    d.t2 = low_pass(h->L2, samp_rate, fw, fw, WIN_HAMMING);
+    h->nt1 = arms_nt(d.t1, h->L1); h->nt2 = arms_nt(d.t2, h->L2);
+    if (fsk_rt(h->L2, h->nt2)) h->nt2 = kFskRtNT;
+    const long long max_sym = static_cast<long long>(h->sym_per_item) * h->max_items;
+    d.sym = max_sym + 64; d.if_ = max_sym * h->L1 + 128; d.out = max_sym * h->L1 * h->L2;
+}
+void create_psk(qrl_tx* h, TxDesign& d, int kind, int sps)
+{
+    if (kind == QRL_MOD_QPSK) {
+        // gr_mod_qpsk.cpp:58-75
+        const int nfilts = sps > 120 ? 11 : (sps > 10 ? 13 : 15);
+        d.t1 = root_raised_cosine(sps, sps, 1, 0.35, nfilts * sps);
+        h->txm = TXM_QPSK; h->sym_per_item = 8;
+    } else {
+        // gr_mod_bpsk.cpp:44-56
+        d.t1 = root_raised_cosine(sps, sps, 1, 0.35, 11 * sps);
+        h->txm = TXM_BPSK; h->sym_per_item = 16;
+    }
+    h->L1 = sps; h->nt1 = arms_nt(d.t1, sps);
+    if (h->txm == TXM_QPSK && qpsk_rt(h->L1, h->nt1)) h->nt1 = kQpskRtNT;
+    h->amplif = 0.6f;
+    const long long max_sym = static_cast<long long>(h->sym_per_item) * h->max_items;
+    d.sym = max_sym + 64; d.sym_floats = 2; d.out = max_sym * h->L1;
+}
+int create_m17_dmr(qrl_tx* h, TxDesign& d, bool dmr, int sps, int samp_rate, int fw)
+{
+    h->amplif = 0.9f; h->repeat_only = 0;
+    h->txm = TXM_M17; h->sym_per_item = 4;
+    if (!dmr) {
         // gr_mod_m17.cpp:30-95: pulse shaping x5 (RRC 0.5, 250 + 1 taps) -> x0.66666666 -> frequency modulator (pi / 5) -> low-pass at
         // 24 ksps -> x0.9 -> bb gain -> rational_resampler_ccf(sps = 125, 3)
-        h->m17 = true; h->amplif = 0.9f; h->repeat_only = 0;
-        t1 = root_raised_cosine(5, 5, 1, 0.5, 250);
-        h->L1 = 5; h->nt1 = (static_cast<int>(t1.size()) + 4) / 5;
+        d.t1 = root_raised_cosine(5, 5, 1, 0.5, 250);
         h->fm_sens = static_cast<float>(kPi / 5);
-        std::vector<float> ifl = low_pass(1, 24000, filter_width, filter_width, WIN_BLACKMAN_HARRIS);
-        h->nt_cfilt = static_cast<int>(ifl.size());
-        if ((rc = upload_floats(h, &h->d_cfilt, ifl))) return fail(rc);
-        t2 = low_pass(sps, 3.0 * samp_rate, 12000, 12000, WIN_BLACKMAN_HARRIS);
-        h->L2 = sps; h->M2 = 3; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        if (sps <= 3 || static_cast<size_t>(h->L2) * h->nt2 * sizeof(float) > 40 * 1024) { set_err(h, "make_gr_mod_m17: unsupported sps"); return fail(QRL_EINVAL); }
-    } else if (kind == QRL_MOD_DMR) {
+        d.cfilt = low_pass(1, 24000, fw, fw, WIN_BLACKMAN_HARRIS);
+        h->nt_cfilt = static_cast<int>(d.cfilt.size());
+        d.t2 = low_pass(sps, 3.0 * samp_rate, 12000, 12000, WIN_BLACKMAN_HARRIS);
+    } else {
         // gr_mod_dmr.cpp:27-93: pulse shaping x5 (RRC(5, 24000, 4800, 0.2, 125 taps)) -> x0.66666666 -> frequency modulator
         // (pi * 4800 * 0.85 / 24000) -> gr_zero_idle_bursts(62) -> x0.9 -> bb gain -> rational_resampler_ccf(sps, 3, low_pass_2(sps, 3 fs,
         // fw, 2000, 60, BH)); the fft_filter_ccf of :72-73 is never connected
-        h->m17 = true; h->dmr_tx = true; h->amplif = 0.9f; h->repeat_only = 0;
         const float if_samp_rate = 24000, symbol_rate = if_samp_rate / 5.0f;
-        t1 = root_raised_cosine(5, if_samp_rate, symbol_rate, 0.2, 25 * 5);
-        h->L1 = 5; h->nt1 = (static_cast<int>(t1.size()) + 4) / 5;
-        h->zi_tag_delay = static_cast<unsigned>((t1.size() - 1) / 2);                        // gr_mod_dmr.cpp:58
+        d.t1 = root_raised_cosine(5, if_samp_rate, symbol_rate, 0.2, 25 * 5);
+        h->zi_tag_delay = static_cast<unsigned>((d.t1.size() - 1) / 2);                      // gr_mod_dmr.cpp:58
         h->zi_delay_items = h->zi_tag_delay > 0 ? 2 * 720 - 1 : 0;                             // gr_zero_idle_bursts.cpp:35-38, bursttimer.h:30
         h->fm_sens = static_cast<float>((kPi * symbol_rate * 0.85) / if_samp_rate);
-        t2 = low_pass_2(sps, 3.0 * samp_rate, filter_width, 2000, 60, WIN_BLACKMAN_HARRIS);
-        h->L2 = sps; h->M2 = 3; h->nt2 = (static_cast<int>(t2.size()) + sps - 1) / sps;
-        if (sps <= 3 || static_cast<size_t>(h->L2) * h->nt2 * sizeof(float) > 40 * 1024) { set_err(h, "make_gr_mod_dmr: unsupported sps"); return fail(QRL_EINVAL); }
-        h->zi.init(h->C);
-    } else if (kind == QRL_MOD_2FSK) {
-        // gr_mod_2fsk.cpp:43-76
-        int nfilts = 25 * sps, spacing = 2; h->amplif = 0.8f;
-        if (flag) { spacing = 1; h->amplif = 0.9f; }
-        if (sps == 5) nfilts = nfilts * 5;
-        if ((nfilts % 2) == 0) nfilts += 1;
-        h->repeat_only = flag ? 0 : 1;
-        h->pulse_scale = 1.0f;
-        t1 = root_raised_cosine(sps, sps, 1, 0.2, nfilts);
-        h->L1 = sps; h->nt1 = (static_cast<int>(t1.size()) + sps - 1) / sps;
-        h->fm_sens = static_cast<float>((spacing * kPi / 2) / sps);
-        t2 = low_pass(10, samp_rate, filter_width, filter_width, WIN_HAMMING);
-        h->L2 = 10; h->nt2 = (static_cast<int>(t2.size()) + 9) / 10;
-    } else { set_err(h, "qrl_tx_create: mod kind " + std::to_string(kind) + " not built"); return fail(QRL_EINVAL); }
-    if ((rc = upload_floats(h, &h->d_arms1, make_arms(t1, h->L1, h->nt1)))) return fail(rc);
-    if (!t2.empty() && (rc = upload_floats(h, &h->d_arms2, make_arms(t2, h->L2, h->nt2)))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_bits, h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_in, static_cast<size_t>(h->max_items) * h->C))) return fail(rc);
-    const bool one_per_bit = kind == QRL_MOD_BPSK || kind == QRL_MOD_2FSK;
-    const bool analog = kind == QRL_MOD_NBFM || kind == QRL_MOD_SSB;
-    long long max_sym = (one_per_bit ? 16LL : 8LL) * max_items;
-    if (kind == QRL_MOD_NBFM) max_sym = max_items * 25 / 4 + 8;        // 50 ksps items per call
-    if (kind == QRL_MOD_SSB) max_sym = max_items + 8;                  // 8 ksps complex items per call
-    if (h->am_tx) {
-        unsigned cap = pow2_at_least(max_items + h->nt_lpf + 64); h->ra_mask = cap - 1; h->ra_stride = cap;
-        if ((rc = dev_alloc(h, &h->d_ra, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        unsigned cap2 = pow2_at_least(static_cast<long long>(max_items) * h->L2 + h->nt_cfilt + 64); h->rc_mask = cap2 - 1; h->rc_stride = cap2;
-        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_an, h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_audio_in, static_cast<size_t>(max_items) * h->C))) return fail(rc);
+        d.t2 = low_pass_2(sps, 3.0 * samp_rate, fw, 2000, 60, WIN_BLACKMAN_HARRIS);
+    }
+    h->L1 = 5; h->nt1 = arms_nt(d.t1, 5);
+    h->L2 = sps; h->M2 = 3; h->nt2 = arms_nt(d.t2, sps);
+    if (sps <= 3 || !arms_fit(h->L2, h->nt2)) { set_err(h, dmr ? "make_gr_mod_dmr: unsupported sps" : "make_gr_mod_m17: unsupported sps"); return QRL_EINVAL; }
+    if (dmr) h->zi.init(h->C);
+    const long long max_sym = 8LL * h->max_items;      // the symbol and IF rings have room for 8 symbols per byte
+    d.sym = max_sym + 64; d.if_ = max_sym * h->L1 + 128 + h->zi_delay_items;
+    d.rc = max_sym * h->L1 + 512 + h->nt2;             // behind the IF low-pass / delay
+    d.out = (static_cast<long long>(h->sym_per_item) * h->max_items * h->L1 * h->L2 + h->M2 - 1) / h->M2 + 8;
+    return QRL_OK;
+}
+// gr_mod_dsss.cpp:27-93: scrambler -> cc_encoder -> Barker-13 spreading -> {-1, +1} -> rational_resampler_ccf(sps, 1, RRC(sps, sps, 1,
+// 0.35, 11 sps)) -> x0.65 -> bb gain -> rational_resampler_ccf(50, 13, low_pass(50, 5200 * 50, fw, 5 fw)) ->
+// rational_resampler_ccf(50, 1, low_pass(50, fs, fw, 5 fw)); one input byte = 208 chips = 10^6 output samples (sps = 25)
+int create_dsss(qrl_tx* h, TxDesign& d, int sps, int samp_rate, int fw)
+{
+    h->amplif = 0.65f;
+    h->txm = TXM_DSSS; h->sym_per_item = 16 * 13;
+    d.t1 = root_raised_cosine(sps, sps, 1, 0.35, 11 * sps);
+    h->L1 = sps; h->nt1 = arms_nt(d.t1, sps);
+    const std::vector<float> tif = low_pass(50.0, 5200.0 * 50, fw, fw * 5, WIN_HAMMING);
+    h->nt_cfilt = arms_nt(tif, 50);
+    d.t2 = low_pass(50, samp_rate, fw, fw * 5, WIN_HAMMING);
+    h->L2 = 50; h->nt2 = arms_nt(d.t2, 50);
+    if (!arms_fit(50, std::max(h->nt2, h->nt_cfilt)) || !arms_fit(h->L1, h->nt1)) {
+        set_err(h, "make_gr_mod_dsss: filter_width too small for the shared-memory arm tables"); return QRL_EINVAL;
+    }
+    d.cfilt = make_arms(tif, 50, h->nt_cfilt);
+    const long long max_sym = static_cast<long long>(h->sym_per_item) * h->max_items;         // chips per call
+    const long long n20 = (max_sym * h->L1 * 50 + 12) / 13;                                    // 20 ksps items per call
+    d.sym = max_sym + 64; d.sym_floats = 2;                                                    // complex chips
+    d.if_ = max_sym * h->L1 + h->nt_cfilt + 128; d.rc = n20 + 8 + h->nt2 + 512; d.out = (n20 + 1) * 50;
+    return QRL_OK;
+}
+// gr_mod_nbfm.cpp:35-63 (sps = final interpolation, 20)
+void create_nbfm(qrl_tx* h, TxDesign& d, int sps, int samp_rate, int fw)
+{
+    double a[2], b[2];
+    preemph_taps(8000, 50e-6, -1.0, a, b);
+    h->pe_b0 = b[0]; h->pe_b1 = b[1]; h->pe_a1 = a[1];
+    d.lpf = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
+    d.t1 = low_pass_2(25, 50000 * 4, fw, 3500, 60, WIN_BLACKMAN_HARRIS);          // 25/4 resampler arms
+    h->L1 = 25; h->nt1 = arms_nt(d.t1, 25);
+    h->fm_sens = static_cast<float>(4 * kPi * fw / 50000.0f);
+    d.cfilt = low_pass_2(1, 50000, fw, 3500, 60, WIN_BLACKMAN_HARRIS);
+    h->nt_cfilt = static_cast<int>(d.cfilt.size());
+    d.t2 = low_pass_2(sps, samp_rate, fw, 3500, 60, WIN_BLACKMAN_HARRIS);
+    h->L2 = sps; h->nt2 = arms_nt(d.t2, sps);
+    h->amplif = 0.8f;
+    const long long max_mid = h->max_items * 25 / 4 + 8;                                       // 50 ksps items per call
+    d.ra = h->max_items + 512; d.rb = true;
+    d.rc = max_mid + 512; d.sym = max_mid + 64; d.if_ = max_mid + 128; d.out = max_mid * h->L2;
+}
+// gr_mod_ssb.cpp:40-58 (sps = final interpolation, 125; flag = sb)
+void create_ssb(qrl_tx* h, TxDesign& d, int sps, int samp_rate, int fw)
+{
+    d.lpf = band_pass_2(1, 8000, 300, fw, 200, 90, WIN_BLACKMAN_HARRIS);
+    d.cfilt = h->flag ? complex_band_pass_2(1, 8000, -fw, -200, 200, 90, WIN_BLACKMAN_HARRIS)
+                      : complex_band_pass_2(1, 8000, 200, fw, 200, 90, WIN_BLACKMAN_HARRIS);
+    h->nt_cfilt = static_cast<int>(d.cfilt.size() / 2);
+    d.t2 = low_pass_2(sps, samp_rate, fw, fw, 90, WIN_BLACKMAN_HARRIS);
+    h->L2 = sps; h->nt2 = arms_nt(d.t2, sps);
+    h->amplif = 0.9f;
+    const long long max_mid = h->max_items + 8;                                                // 8 ksps complex items per call
+    d.ra = h->max_items + 512; d.rc = max_mid + 512; d.rs2 = true; d.if_ = max_mid + 128; d.out = max_mid * h->L2;
+}
+// gr_mod_am.cpp:25-72: agc2_ff -> rail -> x0.95 -> band_pass_2(1, 8000, 300, 3000, 200, 60, Hamming) -> + 0.5 cos(0) -> float_to_complex ->
+// rational_resampler_ccf(sps, 1, low_pass(sps, fs, fw, fw)) -> x0.5 -> bb gain -> fft_filter_ccc(complex_band_pass_2(1, fs, -fw, fw, 1200,
+// 120, BH)).  The band is symmetric, so the complex taps are the low-pass prototype times e^{j0}: imaginary parts exactly 0 and the
+// filter is the real-tap ring FIR (same accumulation, see oracle fircc_work with hi = 0).
+int create_am(qrl_tx* h, TxDesign& d, int sps, int samp_rate, int fw)
+{
+    h->amplif = 0.5f;
+    d.lpf = band_pass_2(1, 8000, 300, 3000, 200, 60, WIN_HAMMING);
+    d.t2 = low_pass(sps, samp_rate, fw, fw, WIN_HAMMING);
+    h->L2 = sps; h->nt2 = arms_nt(d.t2, sps);
+    const std::vector<float> cb = complex_band_pass_2(1, samp_rate, -fw, fw, 1200, 120, WIN_BLACKMAN_HARRIS);
+    d.cfilt.resize(cb.size() / 2);
+    for (size_t i = 0; i < d.cfilt.size(); i++) {
+        if (cb[2 * i + 1] != 0.0f) { set_err(h, "make_gr_mod_am: output filter taps are not real"); return QRL_EINVAL; }
+        d.cfilt[i] = cb[2 * i];
+    }
+    h->nt_cfilt = static_cast<int>(d.cfilt.size());
+    if (!arms_fit(h->L2, h->nt2) || h->nt_cfilt > 8192) { set_err(h, "make_gr_mod_am: unsupported sps / filter_width"); return QRL_EINVAL; }
+    { const std::vector<float> st_ = fxpt_sine_table(); const unsigned uc = 0x40000000u; const int ci = uc >> 22;
+      const float c0 = st_[2 * ci] * static_cast<float>(uc >> 1) + st_[2 * ci + 1];
+      h->am_dc = static_cast<float>(static_cast<double>(c0) * 0.5); }
+    d.ra = h->max_items + static_cast<long long>(d.lpf.size()) + 64;
+    d.rc = static_cast<long long>(h->max_items) * h->L2 + h->nt_cfilt + 64; d.rs2 = true;
+    d.if_ = 8LL * h->max_items + 128;                                                          // 8 ksps, room for 8 items per input sample
+    d.out = static_cast<long long>(h->max_items) * h->L2;
+    return QRL_OK;
+}
+// gr_mod_freedv.cpp:34-85 (sps = final interpolation, 125; flag = sb): side-band filter complex_band_pass_2(1, 8000, lo, fw, 250, 90, BH)
+// (LSB: (-fw, -lo)), feedforward_agc_cc(512, 1), rational_resampler_ccf(sps, 1, low_pass(sps, fs, fw, 1200)) (Hamming), x0.98, x bb gain
+int create_freedv(qrl_tx* h, TxDesign& d, int sps, int samp_rate, int fw, int low_cutoff)
+{
+    h->amplif = 0.98f;
+    d.cfilt = h->flag ? complex_band_pass_2(1, 8000, -fw, -low_cutoff, 250, 90, WIN_BLACKMAN_HARRIS)
+                      : complex_band_pass_2(1, 8000, low_cutoff, fw, 250, 90, WIN_BLACKMAN_HARRIS);
+    h->nt_cfilt = static_cast<int>(d.cfilt.size() / 2);
+    d.t2 = low_pass(sps, samp_rate, fw, 1200, WIN_HAMMING);
+    h->L2 = sps; h->nt2 = arms_nt(d.t2, sps);
+    if (h->L2 != 125 || h->nt2 != 17) {     // the register-tiled x125 instance (2007 taps, 17 per arm) is the one built
+        set_err(h, "make_gr_mod_freedv: interpolator shape not built (sps " + std::to_string(sps) + ", " + std::to_string(d.t2.size()) + " taps)"); return QRL_EINVAL;
+    }
+    // three 8 ksps complex rings of one geometry: the 512-item AGC window and the filters' history stay behind the newest call
+    d.rc = d.if_ = h->max_items + 1024; d.rs2 = true; d.out = static_cast<long long>(h->max_items) * h->L2;
+    return QRL_OK;
+}
+int tx_create(int kind, int sps, int samp_rate, int fw, int flag, int low_cutoff, int n_channels, long max_items, int device, qrl_tx** out)
+{
+    if (!out || n_channels <= 0 || max_items <= 0) { set_err(nullptr, "qrl_tx_create: bad argument"); return QRL_EINVAL; }
+    *out = nullptr;
+    if (int rc = check_device("qrl_tx_create", device)) return rc;
+    qrl_tx* h = new qrl_tx();
+    h->samp_rate = samp_rate; h->flag = flag;
+    h->C = n_channels; h->max_items = max_items;
+    auto fail = [&](int rc) { return create_failed(h, qrl_tx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (!rc) rc = upload_tables(h);
+    if (!rc) rc = dev_alloc(h, &h->d_bits, h->C);
+    if (rc) return fail(rc);
+    TxDesign d;
+    switch (kind) {
+    case QRL_MOD_4FSK: case QRL_MOD_2FSK: case QRL_MOD_GMSK: h->chain = TxChain::Fsk; create_fsk(h, d, kind, sps, samp_rate, fw); break;
+    case QRL_MOD_QPSK: case QRL_MOD_BPSK: h->chain = TxChain::Psk; create_psk(h, d, kind, sps); break;
+    case QRL_MOD_M17: case QRL_MOD_DMR:
+        h->chain = kind == QRL_MOD_DMR ? TxChain::Dmr : TxChain::M17; rc = create_m17_dmr(h, d, kind == QRL_MOD_DMR, sps, samp_rate, fw); break;
+    case QRL_MOD_DSSS: h->chain = TxChain::Dsss; rc = create_dsss(h, d, sps, samp_rate, fw); break;
+    case QRL_MOD_NBFM: h->chain = TxChain::Nbfm; create_nbfm(h, d, sps, samp_rate, fw); break;
+    case QRL_MOD_SSB: h->chain = TxChain::Ssb; create_ssb(h, d, sps, samp_rate, fw); break;
+    case QRL_MOD_AM: h->chain = TxChain::Am; rc = create_am(h, d, sps, samp_rate, fw); break;
+    case QRL_MOD_FREEDV: h->chain = TxChain::Freedv; rc = create_freedv(h, d, sps, samp_rate, fw, low_cutoff); break;
+    default: set_err(h, "qrl_tx_create: mod kind " + std::to_string(kind) + " not built"); rc = QRL_EINVAL;
+    }
+    h->nt_lpf = static_cast<int>(d.lpf.size());
+    h->in_isz = h->chain == TxChain::Freedv ? sizeof(short) : d.ra ? sizeof(float) : 1;      // int16 modem samples, float audio, bytes
+    if (!rc && !d.t1.empty()) rc = upload_floats(h, &h->d_arms1, make_arms(d.t1, h->L1, h->nt1));
+    if (!rc && !d.t2.empty()) rc = upload_floats(h, &h->d_arms2, make_arms(d.t2, h->L2, h->nt2));
+    if (!rc && !d.lpf.empty()) rc = upload_floats(h, &h->d_lpf, d.lpf);
+    if (!rc && !d.cfilt.empty()) rc = upload_floats(h, &h->d_cfilt, d.cfilt);
+    if (!rc) rc = dev_alloc(h, &h->d_in, h->in_isz * h->max_items * h->C);
+    if (!rc && d.sym) rc = tx_ring(h, &h->d_sym, &h->sym_mask, &h->sym_stride, d.sym, d.sym_floats);
+    if (!rc && d.if_) rc = tx_ring(h, &h->d_if, &h->if_mask, &h->if_stride, d.if_);
+    if (!rc && d.rc) rc = tx_ring(h, &h->d_rc, &h->rc_mask, &h->rc_stride, d.rc);
+    if (!rc && d.rs2) rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(h->rc_stride) * h->C);
+    if (!rc && d.ra) {      // the audio chains: audio ring and [C] states (AM: agc2_ff::make(1e-2, 1e-4, 1, 1), initial gain 1)
         std::vector<TxAnalogState> an(h->C);
-        for (auto& a : an) { std::memset(&a, 0, sizeof a); a.agc = 1.0f; }               // agc2_ff::make(1e-2, 1e-4, 1, 1): initial gain 1
-        if ((rc = upload_state(h, h->d_an, an.data(), sizeof(TxAnalogState) * h->C))) return fail(rc);
+        for (auto& a : an) { std::memset(&a, 0, sizeof a); a.agc = h->chain == TxChain::Am ? 1.0f : 0.0f; }
+        rc = tx_ring(h, &h->d_ra, &h->ra_mask, &h->ra_stride, d.ra);
+        if (!rc && d.rb) rc = dev_alloc(h, &h->d_rb, static_cast<size_t>(h->ra_stride) * h->C);
+        if (!rc) rc = dev_alloc(h, &h->d_an, h->C);
+        if (!rc) rc = upload_state(h, h->d_an, an.data(), sizeof(TxAnalogState) * h->C);
     }
-    if (h->freedv_tx) {
-        // three 8 ksps complex rings of one geometry: the 512-item AGC window and the filters' history stay behind the newest call
-        max_sym = max_items;
-        unsigned cap = pow2_at_least(max_items + 1024); h->rc_mask = cap - 1; h->rc_stride = cap; h->if_mask = cap - 1; h->if_stride = cap;
-        if ((rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_short_in, static_cast<size_t>(max_items) * h->C))) return fail(rc);
-    }
-    if (h->dsss_tx) {
-        max_sym = 16LL * 13 * max_items;                               // chips per call
-        unsigned cap1 = pow2_at_least(max_sym * h->L1 + h->nt_cfilt + 128); h->if_mask = cap1 - 1; h->if_stride = cap1;
-        if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap1) * h->C))) return fail(rc);
-        const long long n20 = (max_sym * h->L1 * 50 + 12) / 13 + 8;
-        unsigned cap2 = pow2_at_least(n20 + h->nt2 + 512); h->rc_mask = cap2 - 1; h->rc_stride = cap2;
-        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-    }
-    if (h->m17) {                                                      // IF ring behind the 24 ksps low-pass: 20 samples per byte
-        unsigned cap2 = pow2_at_least(max_sym * h->L1 + 512 + h->nt2); h->rc_mask = cap2 - 1; h->rc_stride = cap2;
-        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-    }
-    if (analog) {
-        unsigned cap = pow2_at_least(max_items + 512); h->ra_mask = cap - 1; h->ra_stride = cap;
-        if ((rc = dev_alloc(h, &h->d_ra, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_rb, static_cast<size_t>(cap) * h->C))) return fail(rc);
-        unsigned cap2 = pow2_at_least(max_sym + 512); h->rc_mask = cap2 - 1; h->rc_stride = cap2;
-        if ((rc = dev_alloc(h, &h->d_rc, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(cap2) * h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_an, h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_audio_in, static_cast<size_t>(max_items) * h->C))) return fail(rc);
-    }
-    const bool qpsk = kind == QRL_MOD_QPSK || kind == QRL_MOD_BPSK || h->dsss_tx;      // complex symbols (QPSK / BPSK: single interpolation stage)
-    { unsigned cap = pow2_at_least(max_sym + 64); h->sym_mask = cap - 1; h->sym_stride = cap;
-      if ((rc = dev_alloc(h, &h->d_sym, static_cast<size_t>(cap) * h->C * (qpsk ? 2 : 1)))) return fail(rc); }
-    if (!qpsk && !h->freedv_tx) {
-        unsigned cap = pow2_at_least(max_sym * (analog ? 1 : h->L1) + 128 + h->zi_delay_items); h->if_mask = cap - 1; h->if_stride = cap;
-        if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap) * h->C))) return fail(rc);
-    }
-    h->out_stride = analog ? max_sym * h->L2 : max_sym * h->L1 * (qpsk ? 1 : h->L2);
-    if (h->m17) h->out_stride = (4LL * max_items * h->L1 * h->L2 + h->M2 - 1) / h->M2 + 8;
-    if (h->dsss_tx) h->out_stride = ((max_sym * h->L1 * 50 + 12) / 13 + 1) * 50;
-    if (h->am_tx || h->freedv_tx) h->out_stride = static_cast<long long>(max_items) * h->L2;
-    if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
+    h->out_stride = d.out;
+    if (!rc) rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false);
     std::vector<TxBitState> st(h->C);
     for (auto& x : st) { x.scr_reg = 0x7F; x.enc_state = 0; x.diff_prev = 0; x.phase_q = 0; }
-    if ((rc = upload_state(h, h->d_bits, st.data(), sizeof(TxBitState) * h->C))) return fail(rc);
+    if (!rc) rc = upload_state(h, h->d_bits, st.data(), sizeof(TxBitState) * h->C);
+    if (rc) return fail(rc);
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
+}
+}  // namespace
+int qrl_tx_create(int kind, int sps, int samp_rate, int /*carrier_freq*/, int filter_width, int flag,
+                  int n_channels, long max_items, int device, qrl_tx** out)
+{
+    if (kind == QRL_MOD_FREEDV) { set_err(nullptr, "qrl_tx_create: QRL_MOD_FREEDV takes a low cutoff: use qrl_tx_create_freedv"); return QRL_EINVAL; }
+    return tx_create(kind, sps, samp_rate, filter_width, flag, 0, n_channels, max_items, device, out);
+}
+int qrl_tx_create_freedv(int sps, int samp_rate, int /*carrier_freq*/, int filter_width, int low_cutoff, int sb,
+                         int n_channels, long max_items, int device, qrl_tx** out)
+{
+    int rc = check_freedv_args("qrl_tx_create_freedv", sps, samp_rate, filter_width, low_cutoff);
+    if (rc) return rc;
+    return tx_create(QRL_MOD_FREEDV, sps, samp_rate, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_items, device, out);
 }
 int qrl_tx_destroy(qrl_tx* h)
 {
@@ -2356,85 +2370,334 @@ int qrl_tx_set_stream(qrl_tx* h, void* s)
     if (!h) return QRL_EINVAL;
     return handle_set_stream(h, s);
 }
+namespace {
+// set_param: the handle's stream drains, then the new tables replace the old ones once every upload succeeded
+int swap_tables(qrl_tx* h, std::initializer_list<std::pair<float**, std::vector<float>>> tables)
+{
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    std::vector<float*> d;
+    for (const auto& t : tables) { d.push_back(nullptr); if (int rc = upload_floats(h, &d.back(), t.second)) return rc; }
+    for (size_t i = 0; i < d.size(); i++) *tables.begin()[i].first = d[i];
+    return QRL_OK;
+}
+// gr_mod_nbfm::set_filter_width (gr_mod_nbfm.cpp:78-93): new taps for the 25/4 resampler, the 50 ksps filter and the final
+// interpolator, new sensitivity.  The rings keep the stream's true history, which the longer filters read from their next output on.
+int nbfm_set_filter_width(qrl_tx* h, int fw)
+{
+    if (fw <= 0) { set_err(h, "qrl_tx_set_param: filter width must be positive"); return QRL_EINVAL; }
+    const float if_samp_rate = 50000;
+    const std::vector<float> t1 = low_pass_2(25, if_samp_rate * 4, fw, fw, 60, WIN_BLACKMAN_HARRIS);
+    const std::vector<float> tc = low_pass_2(1, if_samp_rate, fw, 1200, 60, WIN_BLACKMAN_HARRIS);
+    const std::vector<float> t2 = low_pass_2(h->L2, h->samp_rate, fw, fw, 60, WIN_BLACKMAN_HARRIS);
+    const int nt1 = arms_nt(t1, 25), nt2 = arms_nt(t2, h->L2);
+    if (nt1 > 256 || static_cast<int>(tc.size()) > 400 || nt2 > 400 || !arms_fit(h->L2, nt2)) {
+        set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
+    }
+    if (int rc = swap_tables(h, { { &h->d_arms1, make_arms(t1, 25, nt1) }, { &h->d_cfilt, tc }, { &h->d_arms2, make_arms(t2, h->L2, nt2) } })) return rc;
+    h->nt1 = nt1; h->nt_cfilt = static_cast<int>(tc.size()); h->nt2 = nt2;
+    h->fm_sens = static_cast<float>(4 * kPi * fw / if_samp_rate);
+    return QRL_OK;
+}
+// gr_mod_nbfm::set_ctcss (gr_mod_nbfm.cpp:101-139)
+int nbfm_set_ctcss(qrl_tx* h, double value)
+{
+    std::vector<float> lp;
+    if (value == 0) { h->audio_gain = 0.98f; h->tone_on = false; lp = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS); }
+    else {
+        h->audio_gain = 0.85f; h->tone_on = true;
+        lp = band_pass_2(1, 8000, 300, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
+        float x = static_cast<float>(2 * kPi * static_cast<double>(static_cast<float>(value)) / 8000.0);      // fxpt::float_to_fixed
+        const int d = static_cast<int>(std::floor(x / static_cast<float>(2.0 * kPi) + 0.5));
+        x -= d * static_cast<float>(2.0 * kPi);
+        h->tone_inc = static_cast<unsigned>(static_cast<int>(static_cast<float>(x) * 2147483648.0f / static_cast<float>(kPi)));
+    }
+    if (static_cast<int>(lp.size()) > 400) { set_err(h, "qrl_tx_set_param: audio filter too long"); return QRL_EINVAL; }
+    if (int rc = swap_tables(h, { { &h->d_lpf, lp } })) return rc;
+    h->nt_lpf = static_cast<int>(lp.size());
+    return QRL_OK;
+}
+// gr_mod_ssb::set_filter_width (gr_mod_ssb.cpp:85-100) / gr_mod_am::set_filter_width (gr_mod_am.cpp:75-85)
+int ssb_am_set_filter_width(qrl_tx* h, int fw)
+{
+    if (fw <= 0) { set_err(h, "qrl_tx_set_param: filter width must be positive"); return QRL_EINVAL; }
+    const bool am = h->chain == TxChain::Am;
+    std::vector<float> t2, cf;
+    if (am) {
+        t2 = low_pass(h->L2, h->samp_rate, fw, fw, WIN_HAMMING);
+        const std::vector<float> cb = complex_band_pass_2(1, h->samp_rate, -fw, fw, 1200, 120, WIN_BLACKMAN_HARRIS);
+        cf.resize(cb.size() / 2);
+        for (size_t i = 0; i < cf.size(); i++) cf[i] = cb[2 * i];
+    } else {
+        t2 = low_pass_2(h->L2, h->samp_rate, fw, fw, 90, WIN_BLACKMAN_HARRIS);
+        cf = h->flag ? complex_band_pass_2(1, 8000, -fw, -300, 250, 90, WIN_BLACKMAN_HARRIS) : complex_band_pass_2(1, 8000, 300, fw, 250, 90, WIN_BLACKMAN_HARRIS);
+    }
+    const int nt2 = arms_nt(t2, h->L2), ntc = static_cast<int>(am ? cf.size() : cf.size() / 2);
+    if (nt2 > 60 || !arms_fit(h->L2, nt2) || ntc > (am ? 8192 : 500)) {
+        set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
+    }
+    if (int rc = swap_tables(h, { { &h->d_arms2, make_arms(t2, h->L2, nt2) }, { &h->d_cfilt, cf } })) return rc;
+    h->nt2 = nt2; h->nt_cfilt = ntc;
+    return QRL_OK;
+}
+// launch helpers of the transmit chains: each writes one kernel's grid / shared-memory formula; the callers count the launches
+dim3 grid256(const qrl_tx* h, long long n) { return dim3(static_cast<unsigned>((n + 255) / 256), h->C); }
+void launch_tx_bits(qrl_tx* h, cudaStream_t st, const unsigned char* b, long n, long long stride, long long sym0)
+{
+    const dim3 g((h->C + 31) / 32);
+    switch (h->txm) {
+    case TXM_4FSK: tx_bits_kernel<TXM_4FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_QPSK: tx_bits_kernel<TXM_QPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_BPSK: tx_bits_kernel<TXM_BPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_2FSK: tx_bits_kernel<TXM_2FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_M17: tx_bits_kernel<TXM_M17><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_DSSS: tx_bits_kernel<TXM_DSSS><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    }
+}
+// pulse shaping + FM scan: symbol ring -> IF ring
+void launch_shape_fm(qrl_tx* h, cudaStream_t st, long long sym0, long long nsym, int L, int nt, int repeat_only, float pulse_scale, float g1, float g2)
+{
+    tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, st>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, sym0, nsym,
+        L, nt, h->d_arms1, repeat_only, pulse_scale, h->fm_sens, g1, g2, h->d_if, h->if_mask, h->if_stride);
+}
+// xL interpolator, ring items [m0, m1) -> d_out from output m0 L on
+void launch_interp_generic(qrl_tx* h, const float2* in, unsigned mask, long long stride, long long m0, long long m1, const float* arms,
+                           int L, int NT, float g1, float g2, int apply)
+{
+    const int MT = std::max(1, 4096 / L);
+    const size_t smem = sizeof(float) * ((L * NT + 1) & ~1) + sizeof(float2) * (MT + NT);
+    interp_fir_ccf_generic_kernel<<<dim3(static_cast<unsigned>((m1 - m0 + MT - 1) / MT), h->C), 256, smem, h->stream>>>(
+        in, mask, stride, m0, m1, arms, L, NT, MT, g1, g2, apply, h->d_out, h->out_stride, m0 * L);
+}
+// the FSK chains' final interpolator, IF items [m0, m1) -> d_out from output m0 L2 - out_base on
+void launch_fsk_interp(qrl_tx* h, long long m0, long long m1, long long out_base)
+{
+    if (!fsk_rt(h->L2, h->nt2)) return launch_interp_generic(h, h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    constexpr int L = kFskRtL, NT = kFskRtNT, R = 8, G = 16;
+    interp_fir_ccf_rt_kernel<L, NT, R, G><<<dim3(static_cast<unsigned>((m1 - m0 + R * G - 1) / (R * G)), h->C), L * G, 0, h->stream>>>(
+        h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, out_base);
+}
+// rational resampler xL / M, ring to ring: outputs [o0, o1)
+void launch_resamp(qrl_tx* h, const float2* in, unsigned in_mask, long long in_stride, const float* arms, int L, int M, int nt,
+                   long long o0, long long o1, float g1, float g2, int apply, float2* out, unsigned out_mask, long long out_stride)
+{
+    resamp_ring_to_ring_ccf_kernel<<<grid256(h, o1 - o0), 256, sizeof(float) * L * nt, h->stream>>>(
+        in, in_mask, in_stride, arms, L, M, nt, o0, o1, g1, g2, apply, out, out_mask, out_stride);
+}
+// real-tap filter d_cfilt, IF ring -> ring d_rc (NBFM's 50 ksps filter, M17's IF low-pass)
+void launch_if_filter(qrl_tx* h, long long a0, long long a1)
+{
+    fir_ccf_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * h->nt_cfilt, h->stream>>>(h->d_if, h->if_mask, h->if_stride,
+        h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, a0, a1, nullptr, 0, 0, 0);
+}
+// complex side-band filter d_cfilt, ring d_rs2 -> `out` (SSB, FreeDV)
+void launch_sideband_filter(qrl_tx* h, float2* out, unsigned mask, long long stride, long long a0, long long a1)
+{
+    fir_ccc_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(h->d_rs2, h->rc_mask, h->rc_stride,
+        out, mask, stride, h->d_cfilt, h->nt_cfilt, 1.0f, a0, a1, nullptr, 0, 0);
+}
+void launch_gains(qrl_tx* h, float2* ring, unsigned mask, long long stride, long long a0, long long a1)
+{
+    scale2_ring_kernel<<<grid256(h, a1 - a0), 256, 0, h->stream>>>(ring, mask, stride, a0, a1, h->amplif, h->bb_gain);
+}
+// 4FSK: bit chain / pulse shaping + FM scan / x20 interpolator are pipelined slice by slice on three streams (the first two are
+// one-CTA-per-channel recurrences that leave most SMs idle; the interpolator fills them)
+int tx_work_4fsk_pipelined(qrl_tx* h, const unsigned char* b, long n, long long stride)
+{
+    if (!h->s_bits) {
+        int lo = 0, hi = 0;
+        cudaDeviceGetStreamPriorityRange(&lo, &hi);
+        bool ok = cudaStreamCreateWithPriority(&h->s_bits, cudaStreamNonBlocking, hi) == cudaSuccess &&
+                  cudaStreamCreateWithPriority(&h->s_shape, cudaStreamNonBlocking, hi) == cudaSuccess;
+        auto mk = [&](cudaEvent_t* e) { ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess; };
+        mk(&h->ev_start); mk(&h->ev_shape_done); mk(&h->ev_out_done);
+        for (int i = 0; i < qrl_tx::kTxSub; i++) { mk(&h->ev_bits[i]); mk(&h->ev_shape[i]); }
+        if (!ok) { set_err(h, "qrl_tx_work: stream/event creation failed"); return QRL_ECUDA; }
+    }
+    constexpr int S = qrl_tx::kTxSub;
+    const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n, out_base = sym0 * h->L1 * h->L2;
+    QRL_CK(cudaEventRecord(h->ev_start, h->stream));
+    QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_start, 0));
+    QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_shape_done, 0));      // previous call: symbol ring consumed
+    QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_out_done, 0));       // previous call: IF ring consumed
+    for (int j = 0; j < S; j++) {
+        const long b0 = n * j / S, b1 = n * (j + 1) / S;
+        if (b1 <= b0) continue;
+        const long long symA = sym0 + h->sym_per_item * b0, nsym_j = h->sym_per_item * (b1 - b0);
+        cudaEvent_t pe = h->prof.begin(0, h->s_bits);
+        launch_tx_bits(h, h->s_bits, b + b0, b1 - b0, stride, symA);
+        h->prof.end(pe);
+        QRL_CK(cudaEventRecord(h->ev_bits[j], h->s_bits));
+        QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_bits[j], 0));
+        pe = h->prof.begin(1, h->s_shape);
+        launch_shape_fm(h, h->s_shape, symA, nsym_j, h->L1, h->nt1, h->repeat_only, h->pulse_scale, h->amplif, h->bb_gain);
+        h->prof.end(pe);
+        QRL_CK(cudaEventRecord(h->ev_shape[j], h->s_shape));
+        QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_shape[j], 0));
+        pe = h->prof.begin(2, h->stream);
+        launch_fsk_interp(h, symA * h->L1, (symA + nsym_j) * h->L1, out_base);
+        h->prof.end(pe);
+        h->launches += 3;
+    }
+    QRL_CK(cudaEventRecord(h->ev_shape_done, h->s_shape));
+    QRL_CK(cudaEventRecord(h->ev_out_done, h->stream));
+    h->n_out_last = static_cast<long>(nsym * h->L1 * h->L2);
+    return QRL_OK;
+}
+// 4FSK (pipelined from 8 bytes per slice on when the final interpolator is the register-tiled x20), 2FSK, GMSK
+int tx_work_fsk(qrl_tx* h, const unsigned char* b, long n, long long stride)
+{
+    if (h->txm == TXM_4FSK && fsk_rt(h->L2, h->nt2) && n >= 8 * qrl_tx::kTxSub) return tx_work_4fsk_pipelined(h, b, n, stride);
+    const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n, m0 = sym0 * h->L1, m1 = (sym0 + nsym) * h->L1;
+    launch_tx_bits(h, h->stream, b, n, stride, sym0);
+    launch_shape_fm(h, h->stream, sym0, nsym, h->L1, h->nt1, h->repeat_only, h->pulse_scale, h->amplif, h->bb_gain);
+    launch_fsk_interp(h, m0, m1, m0 * h->L2);
+    h->launches += 3;
+    h->n_out_last = static_cast<long>((m1 - m0) * h->L2);
+    return QRL_OK;
+}
+// QPSK, BPSK: complex symbols -> xL1 RRC interpolator (x amplif x bb gain) -> d_out
+void tx_work_psk(qrl_tx* h, const unsigned char* b, long n, long long stride)
+{
+    const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n;
+    launch_tx_bits(h, h->stream, b, n, stride, sym0);
+    const float2* sym = reinterpret_cast<const float2*>(h->d_sym);
+    if (h->txm == TXM_QPSK && qpsk_rt(h->L1, h->nt1)) {
+        constexpr int L = kQpskRtL, NT = kQpskRtNT, MB = 8, MLEN = 64;
+        interp_fir_ccf_kernel<L, NT, MB, MLEN><<<dim3(static_cast<unsigned>((nsym + MB * MLEN - 1) / (MB * MLEN)), h->C), L * MB, 0, h->stream>>>(
+            sym, h->sym_mask, h->sym_stride, sym0, sym0 + nsym, h->d_arms1, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, sym0 * L);
+    } else {
+        launch_interp_generic(h, sym, h->sym_mask, h->sym_stride, sym0, sym0 + nsym, h->d_arms1, h->L1, h->nt1, h->amplif, h->bb_gain, 1);
+    }
+    h->launches += 2;
+    h->n_out_last = static_cast<long>(nsym * h->L1);
+}
+// M17, DMR: pulse shaping + FM scan (gains of 1: x0.9 and the bb gain sit behind the IF filter here), IF low-pass (DMR: the
+// zero-idle delay), gains, x125 / 3
+int tx_work_m17_dmr(qrl_tx* h, const unsigned char* b, long n, long long stride)
+{
+    const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n, m0 = sym0 * h->L1, m1 = (sym0 + nsym) * h->L1;
+    launch_tx_bits(h, h->stream, b, n, stride, sym0);
+    h->launches++;
+    launch_shape_fm(h, h->stream, sym0, nsym, h->L1, h->nt1, 0, h->pulse_scale, 1.0f, 1.0f);
+    if (h->chain == TxChain::Dmr) {
+        tx_delay_ring_kernel<<<grid256(h, m1 - m0), 256, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, h->d_rc, h->rc_mask, h->rc_stride,
+                                                                          m0, m1, h->zi_delay_items);
+        // the "zero_samples" counters of this call as item ranges (gr_zero_idle_bursts.cpp:61-79: a tag loads the counter, a later
+        // one overrides what is left of it, one output is cleared per count)
+        std::vector<long long> ranges;
+        h->zi.collect(h->C, m0, m1, 0, ranges);
+        if (!ranges.empty()) {
+            QRL_CK(h->zi.upload(ranges, h->stream));
+            tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, h->zi.d_ranges);
+            h->launches++;
+        }
+    } else {
+        launch_if_filter(h, m0, m1);
+    }
+    launch_gains(h, h->d_rc, h->rc_mask, h->rc_stride, m0, m1);
+    const long long o0 = (m0 * h->L2 + h->M2 - 1) / h->M2, o1 = (m1 * h->L2 + h->M2 - 1) / h->M2;   // outputs i with floor(i M / L) < m1
+    if (o1 - o0 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
+    resamp_ring_ccf_generic_kernel<<<grid256(h, o1 - o0), 256, sizeof(float) * h->L2 * h->nt2, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride,
+        h->d_arms2, h->L2, h->M2, h->nt2, o0, o1, h->d_out, h->out_stride);
+    h->launches += 4;
+    h->n_out_last = static_cast<long>(o1 - o0);
+    return QRL_OK;
+}
+// DSSS: chips -> x sps pulse shaping + the two gains (5200 sps ring) -> x50 / 13 (20 ksps ring: outputs i with floor(13 i / 50) < a1) -> x50
+int tx_work_dsss(qrl_tx* h, const unsigned char* b, long n, long long stride)
+{
+    const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n, a0 = sym0 * h->L1, a1 = (sym0 + nsym) * h->L1;
+    const long long o0 = (a0 * 50 + 12) / 13, o1 = (a1 * 50 + 12) / 13;
+    launch_tx_bits(h, h->stream, b, n, stride, sym0);
+    launch_resamp(h, reinterpret_cast<const float2*>(h->d_sym), h->sym_mask, h->sym_stride, h->d_arms1, h->L1, 1, h->nt1, a0, a1,
+                  h->amplif, h->bb_gain, 1, h->d_if, h->if_mask, h->if_stride);
+    launch_resamp(h, h->d_if, h->if_mask, h->if_stride, h->d_cfilt, 50, 13, h->nt_cfilt, o0, o1, 1.0f, 1.0f, 0, h->d_rc, h->rc_mask, h->rc_stride);
+    if ((o1 - o0) * 50 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
+    launch_interp_generic(h, h->d_rc, h->rc_mask, h->rc_stride, o0, o1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    h->launches += 4;
+    h->n_out_last = static_cast<long>((o1 - o0) * 50);
+    return QRL_OK;
+}
+void tx_work_nbfm(qrl_tx* h, const float* au, long n, long long stride)
+{
+    tx_nbfm_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->d_ra, h->ra_mask, h->ra_stride,
+        h->d_rb, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->pe_b0, h->pe_b1, h->pe_a1, h->d_arms1, h->nt1,
+        h->d_sym, h->sym_mask, h->sym_stride, h->audio_gain, h->tone_on ? 1 : 0, h->tone_phase, h->tone_inc);
+    if (h->tone_on) h->tone_phase += h->tone_inc * static_cast<unsigned>(n);
+    const long long r0 = h->n_mid, r1 = ((h->n_audio + n) * 25 + 3) / 4;
+    // frequency modulator (Q32 scan) on the 50 ksps stream: "RRC" stage degenerated to a pass-through arm {1}
+    launch_shape_fm(h, h->stream, r0, r1 - r0, 1, 1, 1, 1.0f, 1.0f, 1.0f);
+    if (r1 > r0) {
+        launch_if_filter(h, r0, r1);
+        launch_gains(h, h->d_rc, h->rc_mask, h->rc_stride, r0, r1);
+        launch_interp_generic(h, h->d_rc, h->rc_mask, h->rc_stride, r0, r1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    }
+    h->launches += 5;
+    h->n_out_last = static_cast<long>((r1 - r0) * h->L2);
+    h->n_mid = r1;
+}
+void tx_work_ssb(qrl_tx* h, const float* au, long n, long long stride)
+{
+    tx_ssb_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->d_ra, h->ra_mask, h->ra_stride,
+        h->d_rc, h->rc_mask, h->rc_stride, h->d_lpf, h->nt_lpf, 0.95f, static_cast<float>(1 / (std::sqrt(0.5) / 2)),
+        h->d_rs2, h->rc_mask, h->rc_stride);
+    const long long s0 = h->n_mid, s1 = std::max<long long>(s0, h->n_audio + n - 2);
+    if (s1 > s0) {
+        launch_sideband_filter(h, h->d_if, h->if_mask, h->if_stride, s0, s1);
+        launch_gains(h, h->d_if, h->if_mask, h->if_stride, s0, s1);
+        launch_interp_generic(h, h->d_if, h->if_mask, h->if_stride, s0, s1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    }
+    h->launches += 4;
+    h->n_out_last = static_cast<long>((s1 - s0) * h->L2);
+    h->n_mid = s1;
+}
+// AM: audio ring d_ra -> 8 ksps complex ring d_if -> x sps (ring d_rc at the output rate) -> output filter (taps d_cfilt) -> d_out
+int tx_work_am(qrl_tx* h, const float* au, long n, long long stride)
+{
+    const long long o0 = h->n_audio * h->L2, o1 = (h->n_audio + n) * h->L2;
+    tx_am_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, 1e-2f, 1e-4f, 1.0f, 1.0f,
+        h->d_ra, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->am_dc, h->d_if, h->if_mask, h->if_stride);
+    launch_resamp(h, h->d_if, h->if_mask, h->if_stride, h->d_arms2, h->L2, 1, h->nt2, o0, o1, h->amplif, h->bb_gain, 1,
+                  h->d_rc, h->rc_mask, h->rc_stride);
+    h->launches += 2;
+    if (int rc = launch_fir_ccf_c(h, h->C, h->stream, h->d_rc, h->rc_mask, h->rc_stride, h->d_rs2, h->rc_mask, h->rc_stride,
+                                  h->d_cfilt, h->nt_cfilt, o0, o1, h->d_out, h->out_stride, o0, 0)) return rc;
+    h->n_out_last = static_cast<long>(o1 - o0);
+    return QRL_OK;
+}
+// FreeDV: int16 modem samples at 8 ksps -> ring d_rs2 -> side-band filter -> ring d_rc -> feedforward AGC -> ring d_if -> x sps -> d_out;
+// every stage is one item per thread (no recurrence), all on the handle's stream
+void tx_work_freedv(qrl_tx* h, const short* s, long n, long long stride)
+{
+    const long long a0 = h->n_audio, a1 = h->n_audio + n;
+    cudaEvent_t pe = h->prof.begin(0, h->stream);
+    short_to_complex_ring_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + 255) / 256, 1024)), h->C), 256, 0, h->stream>>>(
+        s, stride, n, static_cast<float>(1.0 / 32765.0), h->d_rs2, h->rc_mask, h->rc_stride, a0);
+    launch_sideband_filter(h, h->d_rc, h->rc_mask, h->rc_stride, a0, a1);
+    h->prof.end(pe);
+    constexpr int AN = 512, ATILE = 3584, ANT = 256;
+    pe = h->prof.begin(1, h->stream);
+    ffagc_kernel<AN, ATILE, ANT><<<dim3(static_cast<unsigned>((n + ATILE - 1) / ATILE), h->C), ANT, 0, h->stream>>>(
+        h->d_rc, h->rc_mask, h->rc_stride, a0, a1, 1.0f, h->d_if, h->if_mask, h->if_stride);
+    h->prof.end(pe);
+    // the HBM-write-bound stage (8 B per output sample): register-tiled, x0.98 and x bb_gain fused (the one shape tx_create accepts)
+    constexpr int L = 125, NT = 17, R = 8, G = 4;
+    pe = h->prof.begin(2, h->stream);
+    interp_fir_ccf_rt_kernel<L, NT, R, G><<<dim3(static_cast<unsigned>((n + R * G - 1) / (R * G)), h->C), L * G, 0, h->stream>>>(
+        h->d_if, h->if_mask, h->if_stride, a0, a1, h->d_arms2, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
+    h->prof.end(pe);
+    h->launches += 4;
+    h->n_out_last = static_cast<long>(n * h->L2);
+}
+}  // namespace
 int qrl_tx_set_param(qrl_tx* h, int, int key, double value)
 {
     if (!h) return QRL_EINVAL;
     if (key == QRL_PARAM_BB_GAIN) { h->bb_gain = static_cast<float>(value); return QRL_OK; }   // gr_mod_4fsk::set_bb_gain
-    if (key == QRL_PARAM_FILTER_WIDTH && h->kind == QRL_MOD_NBFM) {
-        // gr_mod_nbfm::set_filter_width (gr_mod_nbfm.cpp:78-93): new taps for the 25/4 resampler, the 50 ksps filter and the final
-        // interpolator, new sensitivity.  The rings keep the stream's true history, which the longer filters read from their next output on.
-        const int fw = static_cast<int>(value);
-        if (fw <= 0) { set_err(h, "qrl_tx_set_param: filter width must be positive"); return QRL_EINVAL; }
-        const float if_samp_rate = 50000;
-        const std::vector<float> t1 = low_pass_2(25, if_samp_rate * 4, fw, fw, 60, WIN_BLACKMAN_HARRIS);
-        const std::vector<float> tc = low_pass_2(1, if_samp_rate, fw, 1200, 60, WIN_BLACKMAN_HARRIS);
-        const std::vector<float> t2 = low_pass_2(h->L2, h->samp_rate, fw, fw, 60, WIN_BLACKMAN_HARRIS);
-        const int nt1 = (static_cast<int>(t1.size()) + 24) / 25, nt2 = (static_cast<int>(t2.size()) + h->L2 - 1) / h->L2;
-        if (nt1 > 256 || static_cast<int>(tc.size()) > 400 || nt2 > 400 || static_cast<size_t>(h->L2) * nt2 * sizeof(float) > 40 * 1024) {
-            set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
-        }
-        QRL_CK(cudaSetDevice(h->device));
-        QRL_CK(cudaStreamSynchronize(h->stream));
-        float *a1 = nullptr, *cf = nullptr, *a2 = nullptr;
-        int rc;
-        if ((rc = upload_floats(h, &a1, make_arms(t1, 25, nt1)))) return rc;
-        if ((rc = upload_floats(h, &cf, tc))) return rc;
-        if ((rc = upload_floats(h, &a2, make_arms(t2, h->L2, nt2)))) return rc;
-        h->d_arms1 = a1; h->nt1 = nt1; h->d_cfilt = cf; h->nt_cfilt = static_cast<int>(tc.size()); h->d_arms2 = a2; h->nt2 = nt2;
-        h->fm_sens = static_cast<float>(4 * kPi * fw / if_samp_rate);
-        h->filter_width = fw;
-        return QRL_OK;
-    }
-    if (key == QRL_PARAM_CTCSS && h->kind == QRL_MOD_NBFM) {
-        // gr_mod_nbfm::set_ctcss (gr_mod_nbfm.cpp:101-139)
-        std::vector<float> lp;
-        if (value == 0) { h->audio_gain = 0.98f; h->tone_on = false; lp = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS); }
-        else {
-            h->audio_gain = 0.85f; h->tone_on = true;
-            lp = band_pass_2(1, 8000, 300, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
-            float x = static_cast<float>(2 * kPi * static_cast<double>(static_cast<float>(value)) / 8000.0);      // fxpt::float_to_fixed
-            const int d = static_cast<int>(std::floor(x / static_cast<float>(2.0 * kPi) + 0.5));
-            x -= d * static_cast<float>(2.0 * kPi);
-            h->tone_inc = static_cast<unsigned>(static_cast<int>(static_cast<float>(x) * 2147483648.0f / static_cast<float>(kPi)));
-        }
-        if (static_cast<int>(lp.size()) > 400) { set_err(h, "qrl_tx_set_param: audio filter too long"); return QRL_EINVAL; }
-        QRL_CK(cudaSetDevice(h->device));
-        QRL_CK(cudaStreamSynchronize(h->stream));
-        float* p = nullptr;
-        int rc = upload_floats(h, &p, lp);
-        if (rc) return rc;
-        h->d_lpf = p; h->nt_lpf = static_cast<int>(lp.size());
-        return QRL_OK;
-    }
-    if (key == QRL_PARAM_FILTER_WIDTH && (h->kind == QRL_MOD_SSB || h->am_tx)) {
-        // gr_mod_ssb::set_filter_width (gr_mod_ssb.cpp:85-100) / gr_mod_am::set_filter_width (gr_mod_am.cpp:75-85)
-        const int fw = static_cast<int>(value);
-        if (fw <= 0) { set_err(h, "qrl_tx_set_param: filter width must be positive"); return QRL_EINVAL; }
-        std::vector<float> t2, cf;
-        if (h->am_tx) {
-            t2 = low_pass(h->L2, h->samp_rate, fw, fw, WIN_HAMMING);
-            const std::vector<float> cb = complex_band_pass_2(1, h->samp_rate, -fw, fw, 1200, 120, WIN_BLACKMAN_HARRIS);
-            cf.resize(cb.size() / 2);
-            for (size_t i = 0; i < cf.size(); i++) cf[i] = cb[2 * i];
-        } else {
-            t2 = low_pass_2(h->L2, h->samp_rate, fw, fw, 90, WIN_BLACKMAN_HARRIS);
-            cf = h->flag ? complex_band_pass_2(1, 8000, -fw, -300, 250, 90, WIN_BLACKMAN_HARRIS) : complex_band_pass_2(1, 8000, 300, fw, 250, 90, WIN_BLACKMAN_HARRIS);
-        }
-        const int nt2 = (static_cast<int>(t2.size()) + h->L2 - 1) / h->L2;
-        const int ntc = static_cast<int>(h->am_tx ? cf.size() : cf.size() / 2);
-        if (nt2 > 60 || static_cast<size_t>(h->L2) * nt2 * sizeof(float) > 40 * 1024 || ntc > (h->am_tx ? 8192 : 500)) {
-            set_err(h, "qrl_tx_set_param: filter width too small for the rings' history"); return QRL_EINVAL;
-        }
-        QRL_CK(cudaSetDevice(h->device));
-        QRL_CK(cudaStreamSynchronize(h->stream));
-        float *a2 = nullptr, *c2 = nullptr;
-        int rc;
-        if ((rc = upload_floats(h, &a2, make_arms(t2, h->L2, nt2)))) return rc;
-        if ((rc = upload_floats(h, &c2, cf))) return rc;
-        h->d_arms2 = a2; h->nt2 = nt2; h->d_cfilt = c2; h->nt_cfilt = ntc;
-        h->filter_width = fw;
-        return QRL_OK;
-    }
+    if (key == QRL_PARAM_FILTER_WIDTH && h->chain == TxChain::Nbfm) return nbfm_set_filter_width(h, static_cast<int>(value));
+    if (key == QRL_PARAM_CTCSS && h->chain == TxChain::Nbfm) return nbfm_set_ctcss(h, value);
+    if (key == QRL_PARAM_FILTER_WIDTH && (h->chain == TxChain::Ssb || h->chain == TxChain::Am)) return ssb_am_set_filter_width(h, static_cast<int>(value));
     set_err(h, "qrl_tx_set_param: unsupported key");
     return QRL_EINVAL;
 }
@@ -2445,300 +2708,36 @@ int qrl_tx_work(qrl_tx* h, const void* in, long n, long stride, int on_device)
     h->n_out_last = 0;
     if (n == 0) return QRL_OK;
     QRL_CK(cudaSetDevice(h->device));
-    if (on_device) { int rc = check_device_ptr(h, in, "qrl_tx_work"); if (rc) return rc; }
-    if (h->freedv_tx) {
-        // `in` = [C][n] int16 modem samples at 8 ksps; every stage is one item per thread (no recurrence), all on the handle's stream
-        const short* s = static_cast<const short*>(in);
-        long long sstride = stride;
-        if (!on_device) {
-            QRL_CK(cudaMemcpy2DAsync(h->d_short_in, sizeof(short) * h->max_items, in, sizeof(short) * stride, sizeof(short) * n, h->C,
-                                 cudaMemcpyHostToDevice, h->stream));
-            s = h->d_short_in; sstride = h->max_items;
-        }
-        const long long a0 = h->n_audio, a1 = h->n_audio + n;
-        const int TB = 256;
-        cudaEvent_t pe = h->prof.begin(0, h->stream);
-        short_to_complex_ring_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + TB - 1) / TB, 1024)), h->C), TB, 0, h->stream>>>(
-            s, sstride, n, static_cast<float>(1.0 / 32765.0), h->d_rs2, h->rc_mask, h->rc_stride, a0);
-        fir_ccc_ring_kernel<<<dim3(static_cast<unsigned>((n + TB - 1) / TB), h->C), TB, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(
-            h->d_rs2, h->rc_mask, h->rc_stride, h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, 1.0f, a0, a1, nullptr, 0, 0);
-        h->prof.end(pe);
-        constexpr int AN = 512, ATILE = 3584, ANT = 256;
-        pe = h->prof.begin(1, h->stream);
-        ffagc_kernel<AN, ATILE, ANT><<<dim3(static_cast<unsigned>((n + ATILE - 1) / ATILE), h->C), ANT, 0, h->stream>>>(
-            h->d_rc, h->rc_mask, h->rc_stride, a0, a1, 1.0f, h->d_if, h->if_mask, h->if_stride);
-        h->prof.end(pe);
-        {   // the HBM-write-bound stage (8 B per output sample): register-tiled, x0.98 and x bb_gain fused (the one shape tx_create accepts)
-            constexpr int L = 125, NT = 17, R = 8, G = 4;
-            dim3 g(static_cast<unsigned>((n + R * G - 1) / (R * G)), h->C);
-            pe = h->prof.begin(2, h->stream);
-            interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, a0, a1, h->d_arms2,
-                h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
-            h->prof.end(pe);
-        }
-        h->launches += 4;
-        h->n_audio = a1;
-        h->n_out_last = static_cast<long>(n * h->L2);
-        QRL_CK(cudaGetLastError());
-        return QRL_OK;
-    }
-    if (h->am_tx) {
-        // `in` = [C][n] float audio at 8 ksps
-        const float* au = static_cast<const float*>(in);
-        long long astride = stride;
-        if (!on_device) {
-            QRL_CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
-                                 cudaMemcpyHostToDevice, h->stream));
-            au = h->d_audio_in; astride = h->max_items;
-        }
-        const long long a0 = h->n_audio, a1 = h->n_audio + n;
-        tx_am_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, astride, 1e-2f, 1e-4f, 1.0f, 1.0f,
-            h->d_ra, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->am_dc, h->d_if, h->if_mask, h->if_stride);
-        const long long o0 = a0 * h->L2, o1 = a1 * h->L2;
-        resamp_ring_to_ring_ccf_kernel<<<dim3(static_cast<unsigned>((o1 - o0 + 255) / 256), h->C), 256, sizeof(float) * h->L2 * h->nt2, h->stream>>>(
-            h->d_if, h->if_mask, h->if_stride, h->d_arms2, h->L2, 1, h->nt2, o0, o1, h->amplif, h->bb_gain, 1, h->d_rc, h->rc_mask, h->rc_stride);
-        h->launches += 2;
-        { int rc = launch_fir_ccf_c(h, h->C, h->stream, h->d_rc, h->rc_mask, h->rc_stride, h->d_rs2, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, o0, o1,
-                                    h->d_out, h->out_stride, o0, 0); if (rc) return rc; }
-        h->n_audio = a1;
-        h->n_out_last = static_cast<long>(o1 - o0);
-        QRL_CK(cudaGetLastError());
-        return QRL_OK;
-    }
-    if (h->kind == QRL_MOD_NBFM || h->kind == QRL_MOD_SSB) {
-        // `in` = [C][n] float audio at 8 ksps
-        const float* au = static_cast<const float*>(in);
-        long long astride = stride;
-        if (!on_device) {
-            QRL_CK(cudaMemcpy2DAsync(h->d_audio_in, sizeof(float) * h->max_items, in, sizeof(float) * stride, sizeof(float) * n, h->C,
-                                 cudaMemcpyHostToDevice, h->stream));
-            au = h->d_audio_in; astride = h->max_items;
-        }
-        const int TB = 256;
-        if (h->kind == QRL_MOD_NBFM) {
-            tx_nbfm_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, astride, h->d_ra, h->ra_mask, h->ra_stride,
-                h->d_rb, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->pe_b0, h->pe_b1, h->pe_a1, h->d_arms1, h->nt1,
-                h->d_sym, h->sym_mask, h->sym_stride, h->audio_gain, h->tone_on ? 1 : 0, h->tone_phase, h->tone_inc);
-            if (h->tone_on) h->tone_phase += h->tone_inc * static_cast<unsigned>(n);
-            const long long r0 = h->n_mid, r1 = ((h->n_audio + n) * 25 + 3) / 4;
-            static const float one = 1.0f; (void)one;
-            // frequency modulator (Q32 scan) on the 50 ksps stream: "RRC" stage degenerated to a pass-through arm {1}
-            tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->stream>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, r0, r1 - r0,
-                1, 1, h->d_arms1, 1, 1.0f, h->fm_sens, 1.0f, 1.0f, h->d_if, h->if_mask, h->if_stride);
-            dim3 g(static_cast<unsigned>((r1 - r0 + TB - 1) / TB), h->C);
-            if (r1 > r0) {
-                fir_ccf_ring_kernel<<<g, TB, sizeof(float) * h->nt_cfilt, h->stream>>>(h->d_if, h->if_mask, h->if_stride,
-                    h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, r0, r1, nullptr, 0, 0, 0);
-                scale2_ring_kernel<<<g, TB, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, r0, r1, h->amplif, h->bb_gain);
-                int MT = std::max(1, 4096 / h->L2);
-                const size_t smem = sizeof(float) * ((h->L2 * h->nt2 + 1) & ~1) + sizeof(float2) * (MT + h->nt2);
-                dim3 gi(static_cast<unsigned>((r1 - r0 + MT - 1) / MT), h->C);
-                interp_fir_ccf_generic_kernel<<<gi, 256, smem, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, r0, r1, h->d_arms2, h->L2, h->nt2, MT,
-                                                                            1.0f, 1.0f, 0, h->d_out, h->out_stride, r0 * h->L2);
-            }
-            h->launches += 5;
-            h->n_out_last = static_cast<long>((r1 - r0) * h->L2);
-            h->n_mid = r1;
-        } else {
-            tx_ssb_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, astride, h->d_ra, h->ra_mask, h->ra_stride,
-                h->d_rc, h->rc_mask, h->rc_stride, h->d_lpf, h->nt_lpf, 0.95f, static_cast<float>(1 / (std::sqrt(0.5) / 2)),
-                h->d_rs2, h->rc_mask, h->rc_stride);
-            const long long s0 = h->n_mid, s1 = std::max<long long>(s0, h->n_audio + n - 2);
-            if (s1 > s0) {
-                dim3 g(static_cast<unsigned>((s1 - s0 + TB - 1) / TB), h->C);
-                fir_ccc_ring_kernel<<<g, TB, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(h->d_rs2, h->rc_mask, h->rc_stride,
-                    h->d_if, h->if_mask, h->if_stride, h->d_cfilt, h->nt_cfilt, 1.0f, s0, s1, nullptr, 0, 0);
-                scale2_ring_kernel<<<g, TB, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, s0, s1, h->amplif, h->bb_gain);
-                int MT = std::max(1, 4096 / h->L2);
-                const size_t smem = sizeof(float) * ((h->L2 * h->nt2 + 1) & ~1) + sizeof(float2) * (MT + h->nt2);
-                dim3 gi(static_cast<unsigned>((s1 - s0 + MT - 1) / MT), h->C);
-                interp_fir_ccf_generic_kernel<<<gi, 256, smem, h->stream>>>(h->d_if, h->if_mask, h->if_stride, s0, s1, h->d_arms2, h->L2, h->nt2, MT,
-                                                                            1.0f, 1.0f, 0, h->d_out, h->out_stride, s0 * h->L2);
-            }
-            h->launches += 4;
-            h->n_out_last = static_cast<long>((s1 - s0) * h->L2);
-            h->n_mid = s1;
-        }
-        h->n_audio += n;
-        QRL_CK(cudaGetLastError());
-        return QRL_OK;
+    long long s = stride;
+    if (on_device) { if (int rc = check_device_ptr(h, in, "qrl_tx_work")) return rc; }
+    else {                  // [C][n] items of in_isz bytes at row stride `stride` -> the [C][max_items] staging buffer
+        const size_t isz = h->in_isz;
+        QRL_CK(cudaMemcpy2DAsync(h->d_in, isz * h->max_items, in, isz * stride, isz * n, h->C, cudaMemcpyHostToDevice, h->stream));
+        in = h->d_in; s = h->max_items;
     }
     const unsigned char* b = static_cast<const unsigned char*>(in);
-    long long bstride = stride;
-    if (!on_device) {
-        QRL_CK(cudaMemcpy2DAsync(h->d_in, h->max_items, in, stride, n, h->C, cudaMemcpyHostToDevice, h->stream));
-        b = h->d_in; bstride = h->max_items;
+    const float* au = static_cast<const float*>(in);
+    int rc = QRL_OK;
+    switch (h->chain) {
+    case TxChain::Fsk: rc = tx_work_fsk(h, b, n, s); break;
+    case TxChain::Psk: tx_work_psk(h, b, n, s); break;
+    case TxChain::M17: case TxChain::Dmr: rc = tx_work_m17_dmr(h, b, n, s); break;
+    case TxChain::Dsss: rc = tx_work_dsss(h, b, n, s); break;
+    case TxChain::Nbfm: tx_work_nbfm(h, au, n, s); break;
+    case TxChain::Ssb: tx_work_ssb(h, au, n, s); break;
+    case TxChain::Am: rc = tx_work_am(h, au, n, s); break;
+    case TxChain::Freedv: tx_work_freedv(h, static_cast<const short*>(in), n, s); break;
     }
-    const bool cplx = h->kind == QRL_MOD_QPSK || h->kind == QRL_MOD_BPSK;
-    const bool one_per_bit = h->kind == QRL_MOD_BPSK || h->kind == QRL_MOD_2FSK;
-    if (h->dsss_tx) {
-        const long long sym0 = h->n_sym, nsym = 16LL * 13 * n;                         // chips
-        tx_bits_kernel<TXM_DSSS><<<dim3((h->C + 31) / 32), 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        // x sps pulse shaping + the two gains -> 5200 sps ring
-        const long long a0 = sym0 * h->L1, a1 = (sym0 + nsym) * h->L1;
-        resamp_ring_to_ring_ccf_kernel<<<dim3(static_cast<unsigned>((a1 - a0 + 255) / 256), h->C), 256, sizeof(float) * h->L1 * h->nt1, h->stream>>>(
-            reinterpret_cast<const float2*>(h->d_sym), h->sym_mask, h->sym_stride, h->d_arms1, h->L1, 1, h->nt1, a0, a1,
-            h->amplif, h->bb_gain, 1, h->d_if, h->if_mask, h->if_stride);
-        // x50 / 13 -> 20 ksps ring: outputs i with floor(13 i / 50) < a1
-        const long long o0 = (a0 * 50 + 12) / 13, o1 = (a1 * 50 + 12) / 13;
-        resamp_ring_to_ring_ccf_kernel<<<dim3(static_cast<unsigned>((o1 - o0 + 255) / 256), h->C), 256, sizeof(float) * 50 * h->nt_cfilt, h->stream>>>(
-            h->d_if, h->if_mask, h->if_stride, h->d_cfilt, 50, 13, h->nt_cfilt, o0, o1, 1.0f, 1.0f, 0, h->d_rc, h->rc_mask, h->rc_stride);
-        // x50 -> output
-        if ((o1 - o0) * 50 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
-        {
-            const int L = 50, NT = h->nt2, MT = std::max(1, 4096 / L);
-            const size_t smem = sizeof(float) * ((L * NT + 1) & ~1) + sizeof(float2) * (MT + NT);
-            dim3 g(static_cast<unsigned>((o1 - o0 + MT - 1) / MT), h->C);
-            interp_fir_ccf_generic_kernel<<<g, 256, smem, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, o0, o1, h->d_arms2, L, NT, MT, 1.0f, 1.0f, 0,
-                                                                       h->d_out, h->out_stride, o0 * L);
-        }
-        h->launches += 4;
-        h->n_out_last = static_cast<long>((o1 - o0) * 50);
-        h->n_sym += nsym;
-        QRL_CK(cudaGetLastError());
-        return QRL_OK;
-    }
-    const long long sym0 = h->n_sym, nsym = (h->m17 ? 4LL : (one_per_bit ? 16LL : 8LL)) * n;
-    // 4FSK: bit chain / pulse shaping + FM scan / x20 interpolator are pipelined slice by slice on three streams (the
-    // first two are one-CTA-per-channel recurrences that leave most SMs idle; the interpolator fills them)
-    bool pipelined = h->kind == QRL_MOD_4FSK && h->L2 == 20 && h->nt2 == 35 && n >= 8 * qrl_tx::kTxSub;
-    if (pipelined && !h->s_bits) {
-        int lo = 0, hi = 0;
-        cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        bool ok = cudaStreamCreateWithPriority(&h->s_bits, cudaStreamNonBlocking, hi) == cudaSuccess &&
-                  cudaStreamCreateWithPriority(&h->s_shape, cudaStreamNonBlocking, hi) == cudaSuccess;
-        auto mk = [&](cudaEvent_t* e) { ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess; };
-        mk(&h->ev_start); mk(&h->ev_shape_done); mk(&h->ev_out_done);
-        for (int i = 0; i < qrl_tx::kTxSub; i++) { mk(&h->ev_bits[i]); mk(&h->ev_shape[i]); }
-        if (!ok) { set_err(h, "qrl_tx_work: stream/event creation failed"); return QRL_ECUDA; }
-    }
-    if (pipelined) {
-        constexpr int S = qrl_tx::kTxSub;
-        QRL_CK(cudaEventRecord(h->ev_start, h->stream));
-        QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_start, 0));
-        QRL_CK(cudaStreamWaitEvent(h->s_bits, h->ev_shape_done, 0));      // previous call: symbol ring consumed
-        QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_out_done, 0));       // previous call: IF ring consumed
-        const long long out_base = sym0 * h->L1 * h->L2;
-        for (int j = 0; j < S; j++) {
-            const long b0 = n * j / S, b1 = n * (j + 1) / S;
-            if (b1 <= b0) continue;
-            const long long symA = sym0 + 8LL * b0, nsym_j = 8LL * (b1 - b0);
-            cudaEvent_t pe = h->prof.begin(0, h->s_bits);
-            tx_bits_kernel<TXM_4FSK><<<dim3((h->C + 31) / 32), 32, 0, h->s_bits>>>(h->d_bits, h->C, b + b0, b1 - b0, bstride,
-                                                                                 h->d_sym, h->sym_mask, h->sym_stride, symA);
-            h->prof.end(pe);
-            QRL_CK(cudaEventRecord(h->ev_bits[j], h->s_bits));
-            QRL_CK(cudaStreamWaitEvent(h->s_shape, h->ev_bits[j], 0));
-            pe = h->prof.begin(1, h->s_shape);
-            tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->s_shape>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, symA, nsym_j,
-                h->L1, h->nt1, h->d_arms1, h->repeat_only, h->pulse_scale, h->fm_sens, h->amplif, h->bb_gain,
-                h->d_if, h->if_mask, h->if_stride);
-            h->prof.end(pe);
-            QRL_CK(cudaEventRecord(h->ev_shape[j], h->s_shape));
-            QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_shape[j], 0));
-            constexpr int L = 20, NT = 35, R = 8, G = 16;
-            const long long m0 = symA * h->L1, m1 = (symA + nsym_j) * h->L1;
-            dim3 g(static_cast<unsigned>((m1 - m0 + R * G - 1) / (R * G)), h->C);
-            pe = h->prof.begin(2, h->stream);
-            interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(
-                h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, out_base);
-            h->prof.end(pe);
-            h->launches += 3;
-        }
-        QRL_CK(cudaEventRecord(h->ev_shape_done, h->s_shape));
-        QRL_CK(cudaEventRecord(h->ev_out_done, h->stream));
-        h->n_out_last = static_cast<long>(nsym * h->L1 * h->L2);
-        h->n_sym += nsym;
-        QRL_CK(cudaGetLastError());
-        return QRL_OK;
-    }
-    {
-        dim3 g((h->C + 31) / 32);
-        if (h->m17) tx_bits_kernel<TXM_M17><<<g, 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        else if (h->kind == QRL_MOD_QPSK) tx_bits_kernel<TXM_QPSK><<<g, 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        else if (h->kind == QRL_MOD_BPSK) tx_bits_kernel<TXM_BPSK><<<g, 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        else if (h->kind == QRL_MOD_2FSK) tx_bits_kernel<TXM_2FSK><<<g, 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        else tx_bits_kernel<TXM_4FSK><<<g, 32, 0, h->stream>>>(h->d_bits, h->C, b, n, bstride, h->d_sym, h->sym_mask, h->sym_stride, sym0);
-        h->launches++;
-    }
-    auto generic_interp = [&](const float2* in, unsigned mask, long long stride_, long long m0, long long m1, const float* arms, int L, int NT,
-                              float g1, float g2, int apply) {
-        int MT = std::max(1, 4096 / L);
-        const size_t smem = sizeof(float) * ((L * NT + 1) & ~1) + sizeof(float2) * (MT + NT);
-        dim3 g(static_cast<unsigned>((m1 - m0 + MT - 1) / MT), h->C);
-        interp_fir_ccf_generic_kernel<<<g, 256, smem, h->stream>>>(in, mask, stride_, m0, m1, arms, L, NT, MT, g1, g2, apply,
-                                                                   h->d_out, h->out_stride, m0 * L);
-        h->launches++;
-    };
-    if (h->m17) {
-        // pulse shaping + FM scan (gains of 1: x0.9 and the bb gain sit behind the IF filter here), IF low-pass, gains, x125 / 3
-        tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->stream>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, sym0, nsym,
-            h->L1, h->nt1, h->d_arms1, 0, h->pulse_scale, h->fm_sens, 1.0f, 1.0f, h->d_if, h->if_mask, h->if_stride);
-        const long long m0 = sym0 * h->L1, m1 = (sym0 + nsym) * h->L1;
-        const int TB = 256;
-        dim3 g(static_cast<unsigned>((m1 - m0 + TB - 1) / TB), h->C);
-        if (h->dmr_tx) {
-            tx_delay_ring_kernel<<<g, TB, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, h->d_rc, h->rc_mask, h->rc_stride, m0, m1,
-                                                          h->zi_delay_items);
-            // the "zero_samples" counters of this call as item ranges (gr_zero_idle_bursts.cpp:61-79: a tag loads the counter, a later
-            // one overrides what is left of it, one output is cleared per count)
-            std::vector<long long> ranges;
-            h->zi.collect(h->C, m0, m1, 0, ranges);
-            if (!ranges.empty()) {
-                QRL_CK(h->zi.upload(ranges, h->stream));
-                tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, h->zi.d_ranges);
-                h->launches++;
-            }
-        } else {
-        fir_ccf_ring_kernel<<<g, TB, sizeof(float) * h->nt_cfilt, h->stream>>>(h->d_if, h->if_mask, h->if_stride,
-            h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, m0, m1, nullptr, 0, 0, 0);
-        }
-        scale2_ring_kernel<<<g, TB, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, m0, m1, h->amplif, h->bb_gain);
-        const long long o0 = (m0 * h->L2 + h->M2 - 1) / h->M2, o1 = (m1 * h->L2 + h->M2 - 1) / h->M2;   // outputs i with floor(i M / L) < m1
-        if (o1 - o0 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
-        dim3 go(static_cast<unsigned>((o1 - o0 + 255) / 256), h->C);
-        resamp_ring_ccf_generic_kernel<<<go, 256, sizeof(float) * h->L2 * h->nt2, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride,
-            h->d_arms2, h->L2, h->M2, h->nt2, o0, o1, h->d_out, h->out_stride);
-        h->launches += 4;
-        h->n_out_last = static_cast<long>(o1 - o0);
-    } else if (cplx) {
-        if (h->L1 == 4 && h->nt1 == 16) {
-            constexpr int L = 4, NT = 16, MB = 8, MLEN = 64;
-            dim3 g(static_cast<unsigned>((nsym + MB * MLEN - 1) / (MB * MLEN)), h->C);
-            interp_fir_ccf_kernel<L, NT, MB, MLEN><<<g, L * MB, 0, h->stream>>>(
-                reinterpret_cast<const float2*>(h->d_sym), h->sym_mask, h->sym_stride, sym0, sym0 + nsym,
-                h->d_arms1, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, sym0 * L);
-            h->launches++;
-        } else {
-            generic_interp(reinterpret_cast<const float2*>(h->d_sym), h->sym_mask, h->sym_stride, sym0, sym0 + nsym,
-                           h->d_arms1, h->L1, h->nt1, h->amplif, h->bb_gain, 1);
-        }
-        h->n_out_last = static_cast<long>(nsym * h->L1);
-    } else {
-        tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->stream>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, sym0, nsym,
-            h->L1, h->nt1, h->d_arms1, h->repeat_only, h->pulse_scale, h->fm_sens, h->amplif, h->bb_gain,
-            h->d_if, h->if_mask, h->if_stride);
-        h->launches++;
-        const long long m0 = sym0 * h->L1, m1 = (sym0 + nsym) * h->L1;
-        if (h->L2 == 20 && h->nt2 == 35) {
-            constexpr int L = 20, NT = 35, R = 8, G = 16;
-            dim3 g(static_cast<unsigned>((m1 - m0 + R * G - 1) / (R * G)), h->C);
-            interp_fir_ccf_rt_kernel<L, NT, R, G><<<g, L * G, 0, h->stream>>>(
-                h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, m0 * L);
-            h->launches++;
-        } else {
-            generic_interp(h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
-        }
-        h->n_out_last = static_cast<long>((m1 - m0) * h->L2);
-    }
-    h->n_sym += nsym;
+    if (rc) return rc;
+    if (h->sym_per_item) h->n_sym += static_cast<long long>(h->sym_per_item) * n;     // symbols, or audio / modem samples consumed
+    else h->n_audio += n;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 int qrl_tx_zero_samples(qrl_tx* h, int channel, long long byte_offset, long n_samples)
 {
     if (!h || channel < -1 || channel >= h->C || byte_offset < 0 || n_samples < 0) return QRL_EINVAL;
-    if (!h->dmr_tx) { set_err(h, "qrl_tx_zero_samples: only gr_mod_dmr has a zero-idle stage"); return QRL_EINVAL; }
+    if (h->chain != TxChain::Dmr) { set_err(h, "qrl_tx_zero_samples: only gr_mod_dmr has a zero-idle stage"); return QRL_EINVAL; }
     // the tag rides through packed_to_unpacked (x8), pack_k_bits(2) (/2) and the x5 pulse shaper: item 20 * byte_offset at the block
     const long long item = byte_offset * 4 * h->L1;
     if (item < static_cast<long long>(h->zi_tag_delay)) return QRL_OK;          // gr_zero_idle_bursts.cpp:63 can never match

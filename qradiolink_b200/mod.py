@@ -39,47 +39,31 @@ class TxBlock(Handle):
 
     set_stream = Handle._set_stream
 
-    def work(self, data):
-        """data: uint8 [n_channels, n] frame bytes -> complex64 [n_channels, n_out] at 1 Msps."""
-        data = np.ascontiguousarray(data, np.uint8)
+    def _work(self, data, dtype):
+        """[n_channels, n] items of `dtype` from a host array -> complex64 [n_channels, n_out]."""
+        data = np.ascontiguousarray(data, dtype)
         if data.ndim == 1:
             data = data[None, :]
         n = data.shape[1]
         check(self._L.qrl_tx_work(self._h, data.ctypes.data_as(C.c_void_p), n, n, 0), self._h, "qrl_tx_work")
-        dptr, stride, nout = C.c_void_p(), C.c_long(), C.c_long()
-        check(self._L.qrl_tx_out_device(self._h, C.byref(dptr), C.byref(stride), C.byref(nout)), self._h, "tx_out_device")
-        out = np.zeros((self.n_channels, nout.value), np.complex64)
-        n2 = C.c_long()
-        check(self._L.qrl_tx_read(self._h, out.ctypes.data_as(C.c_void_p), nout.value, C.byref(n2), 0), self._h, "qrl_tx_read")
-        return out[:, :n2.value]
-
-    def work_audio(self, audio):
-        """analog modulators (NBFM / SSB): float32 [n_channels, n] audio at 8 ksps -> complex64 [n_channels, n_out]."""
-        audio = np.ascontiguousarray(audio, np.float32)
-        if audio.ndim == 1:
-            audio = audio[None, :]
-        n = audio.shape[1]
-        check(self._L.qrl_tx_work(self._h, audio.ctypes.data_as(C.c_void_p), n, n, 0), self._h, "qrl_tx_work")
-        dptr, stride, nout = C.c_void_p(), C.c_long(), C.c_long()
-        check(self._L.qrl_tx_out_device(self._h, C.byref(dptr), C.byref(stride), C.byref(nout)), self._h, "tx_out_device")
-        out = np.zeros((self.n_channels, max(1, nout.value)), np.complex64)
-        n2 = C.c_long()
-        check(self._L.qrl_tx_read(self._h, out.ctypes.data_as(C.c_void_p), max(1, nout.value), C.byref(n2), 0), self._h, "qrl_tx_read")
-        return out[:, :n2.value]
-
-    def work_modem(self, samples):
-        """FreeDV: int16 [n_channels, n] modem samples at 8 ksps (what freedv_tx_ss produces) -> complex64 [n_channels, n x sps]."""
-        samples = np.ascontiguousarray(samples, np.int16)
-        if samples.ndim == 1:
-            samples = samples[None, :]
-        n = samples.shape[1]
-        check(self._L.qrl_tx_work(self._h, samples.ctypes.data_as(C.c_void_p), n, n, 0), self._h, "qrl_tx_work")
         nout = C.c_long()
         check(self._L.qrl_tx_out_device(self._h, None, None, C.byref(nout)), self._h, "tx_out_device")
         out = np.zeros((self.n_channels, max(1, nout.value)), np.complex64)
         n2 = C.c_long()
         check(self._L.qrl_tx_read(self._h, out.ctypes.data_as(C.c_void_p), max(1, nout.value), C.byref(n2), 0), self._h, "qrl_tx_read")
         return out[:, :n2.value]
+
+    def work(self, data):
+        """data: uint8 [n_channels, n] frame bytes -> complex64 [n_channels, n_out] at 1 Msps."""
+        return self._work(data, np.uint8)
+
+    def work_audio(self, audio):
+        """analog modulators (NBFM / SSB): float32 [n_channels, n] audio at 8 ksps -> complex64 [n_channels, n_out]."""
+        return self._work(audio, np.float32)
+
+    def work_modem(self, samples):
+        """FreeDV: int16 [n_channels, n] modem samples at 8 ksps (what freedv_tx_ss produces) -> complex64 [n_channels, n x sps]."""
+        return self._work(samples, np.int16)
 
     def work_device(self, dev_ptr, n, stride):
         check(self._L.qrl_tx_work(self._h, C.c_void_p(dev_ptr), n, stride, 1), self._h, "qrl_tx_work")

@@ -8,6 +8,7 @@ loader for this module only and removed again; the package has no switch for it 
 races on real hardware or the memory model -- that is the GPU tier's job; what it does catch is wrong indexing, wrong buffer sizes,
 wrong launch geometry, state that does not carry across calls, and barrier mistakes (it found a missing __syncthreads in the SSB
 audio kernel that the GPU's scheduling had been hiding)."""
+import ctypes
 import os
 import sys
 
@@ -15,6 +16,7 @@ import numpy as np
 import pytest
 
 from tests.golden import cases
+from tests.test_gpu_dispatch import TX, tx_bases
 
 pytestmark = pytest.mark.timeout(900)      # pytest-timeout: a scheduling bug in the emulator must fail, not hang the tier
 
@@ -49,6 +51,42 @@ def test_golden_rx_through_the_emulated_library(emu_qrl, oracle, name):
 def test_golden_tx_through_the_emulated_library(emu_qrl, name):
     from tests import test_golden as TG
     TG.test_golden_tx_cuda(emu_qrl, name)
+
+
+# every row of the GPU tier's TX channel-count table, plus 4FSK-FM at 64 bytes per call (the three-stream pipelined path)
+@pytest.mark.parametrize("name,n", [(k, TX[k][3]) for k in TX] + [("4fsk2kfm", 64)])
+def test_tx_chain_through_the_emulated_library(emu_qrl, oracle, name, n):
+    """2 channels, two calls (state carried across them), every output bit-identical to the oracle.  4FSK-FM runs its bit chain in
+    8 slices per call (qrl_tx_profile stage 0) from 64 bytes per call on, in one launch per call below."""
+    factory, ofactory, kind, _ = TX[name]
+    D = tx_bases(kind, 2 * n)[:2]
+    lib = emu_qrl.load_library()
+    tx = factory(emu_qrl, 2, n)
+    try:
+        lib.qrl_tx_profile(tx._h, 1)
+        work = {"bytes": tx.work, "audio": tx.work_audio, "modem": tx.work_modem}[kind]
+        calls = [work(D[:, :n]), work(D[:, n:])]
+        ms, cnt = ctypes.c_double(), ctypes.c_long()
+        assert lib.qrl_tx_profile_read(tx._h, 0, ctypes.byref(ms), ctypes.byref(cnt)) == 0
+    finally:
+        tx.close()
+    if name == "4fsk2kfm":
+        assert cnt.value == (2 * 8 if n >= 64 else 0), (n, cnt.value)
+    for c in range(2):
+        o = ofactory(oracle)
+        for k, got in enumerate(calls):
+            want = o.work(D[c, k * n:(k + 1) * n])
+            assert len(want) == got.shape[1] and np.array_equal(got[c], want), (name, c, k)
+
+
+def test_tx_set_filter_width_and_ctcss_through_the_emulated_library(emu_qrl, oracle):
+    """gr_mod_nbfm / gr_mod_ssb / gr_mod_am::set_filter_width and gr_mod_nbfm::set_ctcss between calls (tests/test_gpu_tx.py): new taps
+    meet the rings' history, the tone source keeps its phase."""
+    from tests import test_gpu_tx as TT
+    TT.test_tx_nbfm_set_filter_width_mid_stream(emu_qrl, oracle)
+    for kind in ("usb", "am"):
+        TT.test_tx_ssb_am_set_filter_width_mid_stream(emu_qrl, oracle, kind)
+    TT.nbfm_ctcss_case(emu_qrl, oracle)
 
 
 def test_dmr_chain_through_the_emulated_library(emu_qrl, oracle):

@@ -230,9 +230,9 @@ def test_tx_ssb_am_set_filter_width_mid_stream(qrl, oracle, kind):
         assert got.shape[1] == len(w) and np.array_equal(got[c], w), c
 
 
-def test_tx_nbfm_set_ctcss(qrl, oracle):
+def nbfm_ctcss_case(qrl, oracle):
     """gr_mod_nbfm::set_ctcss (gr_mod_nbfm.cpp:101-139) mid-stream: tone on (88.5 Hz, then 123 Hz: the tone source keeps its phase), tone
-    off (gain 0.98, not the constructor's 0.99), against the oracle; the tone is in the demodulated audio of the CUDA receiver."""
+    off (gain 0.98, not the constructor's 0.99), IQ bit-identical to the oracle; returns the IQ."""
     C, n = 2, 6000
     t = np.arange(n)
     audio = np.stack([(0.4 * np.sin(2 * np.pi * (900 + 250 * c) * t / 8000)).astype(np.float32) for c in range(C)])
@@ -251,6 +251,12 @@ def test_tx_nbfm_set_ctcss(qrl, oracle):
     for c in range(C):
         w = np.concatenate(want[c])
         assert got.shape[1] == len(w) and np.array_equal(got[c], w), c
+    return got
+
+
+def test_tx_nbfm_set_ctcss(qrl, oracle):
+    """nbfm_ctcss_case against the oracle; the tone is in the demodulated audio of the CUDA receiver."""
+    got = nbfm_ctcss_case(qrl, oracle)
     rx = qrl.make_gr_demod_nbfm(125, 1000000, 1700, 2500, n_channels=1, max_samples=got.shape[1])
     rx.work(got[:1])
     a = rx.read_port(1)[0]
