@@ -445,6 +445,49 @@ int  qrl_dfbb_read(qrl_dfbb*, unsigned char* out_host /* [n_channels][cap] */, l
 int  qrl_dfbb_sync(qrl_dfbb*);
 long qrl_dfbb_launch_count(qrl_dfbb*);
 
+/* ---- M17 frame codec on the device (qradiolink_b200/csrc/qrl_m17.cu) --------------------------------------------------------------
+ * Receive: M17FrameDecoder (/root/reference/src/M17/M17/M17FrameDecoder.cpp) and the lines of gr_modem::processReceivedData that drive
+ * it (/root/reference/src/gr_modem.cpp:1370-1440) for a batch of channels.  Input: the records of the layer-1 deframer (sync class 4),
+ * [n_channels][max_frames][record_bytes] of { uint32 frame_type, uint32 nbytes, 46 payload bytes } with per-channel frame_counts --
+ * exactly qrl_deframer_out_device(), record_bytes = qrl_deframer_record_bytes() -- or host arrays of the same layout (on_device = 0).
+ * max_frames (of the input layout) may not exceed the handle's.  Output, per input record in order, one 56-byte record
+ * { uint32 frame_type, lsf[30] (getLsf()), lsf_valid (lsf.valid()), 0, stream_frame[18] (getStreamFrame(): frame number, 16-byte
+ * codec2 payload), 0, 0 } as it stands after the record: LSF records (0x55F7) overwrite the LSF whatever its CRC; stream records
+ * (0xFF5D) add their LICH segment (a reassembled LSF replaces the current one only if its CRC holds) and decode the stream frame; an
+ * EOT record (0x555D555D) reports the current LSF, then resets the channel's decoder if that LSF is valid; other types change nothing.
+ * State (LSF, partial LSF, segment map, stream frame) carries across calls.  Records are valid until the next work call. */
+typedef struct qrl_m17_rx qrl_m17_rx;
+int  qrl_m17_rx_create(int n_channels, int max_frames, int device, qrl_m17_rx** out);
+int  qrl_m17_rx_destroy(qrl_m17_rx*);
+int  qrl_m17_rx_set_stream(qrl_m17_rx*, void* cuda_stream);
+int  qrl_m17_rx_work(qrl_m17_rx*, const unsigned char* records, const int* frame_counts, int record_bytes, int max_frames, int on_device);
+/* M17FrameDecoder::reset for one channel */
+int  qrl_m17_rx_reset(qrl_m17_rx*, int channel);
+/* records_host [n_channels][max_frames][56] (may be NULL), counts_host [n_channels]; synchronises */
+int  qrl_m17_rx_read(qrl_m17_rx*, unsigned char* records_host, int* counts_host);
+int  qrl_m17_rx_out_device(qrl_m17_rx*, void** records, int** counts);
+int  qrl_m17_rx_sync(qrl_m17_rx*);
+long qrl_m17_rx_launch_count(qrl_m17_rx*);
+/* Transmit: M17Transmitter::start / send (/root/reference/src/M17/M17/M17Transmitter.cpp) and gr_modem::endTransmission's M17 tail
+ * (gr_modem.cpp:680-735, 719-728, 868-882) for a batch of channels.  set_lsf: the 28 LSF bytes before the CRC (dst, src, type, meta; a
+ * C++ caller fills them with M17LinkSetupFrame); the handle adds the CRC and the six Golay-coded LICH segments.  work: ops [n_channels][K]
+ * and payloads [n_channels][K][16], K <= max_steps; op 0 = none, 1 = start (counters reset; 48 x 0x77 preamble, then the LSF frame:
+ * 96 bytes), 2 = stream frame (48 bytes), 3 = last stream frame, then 8 x 0x55 0x5D (64 bytes); other values count as none.  Output:
+ * [n_channels][stride = max_steps * 96] bytes with per-channel counts, valid until the next work call -- with the same ops on every
+ * channel, the input of qrl_tx_work(QRL_MOD_M17, ..., on_device = 1) as it is.  Frame number ((fn + 1) & 0x7FF) and LICH index (mod 6)
+ * carry across calls. */
+typedef struct qrl_m17_tx qrl_m17_tx;
+int  qrl_m17_tx_create(int n_channels, int max_steps, int device, qrl_m17_tx** out);
+int  qrl_m17_tx_destroy(qrl_m17_tx*);
+int  qrl_m17_tx_set_stream(qrl_m17_tx*, void* cuda_stream);
+int  qrl_m17_tx_set_lsf(qrl_m17_tx*, int channel, const unsigned char* lsf28);
+int  qrl_m17_tx_work(qrl_m17_tx*, const unsigned char* ops, const unsigned char* payloads, int K, int on_device);
+/* out_host [n_channels][cap] (may be NULL), counts_host [n_channels]; synchronises */
+int  qrl_m17_tx_read(qrl_m17_tx*, unsigned char* out_host, long cap, int* counts_host);
+int  qrl_m17_tx_out_device(qrl_m17_tx*, void** out, long* stride, int** counts);
+int  qrl_m17_tx_sync(qrl_m17_tx*);
+long qrl_m17_tx_launch_count(qrl_m17_tx*);
+
 /* ---- stand-alone kernels exposed for tests / micro-benchmarks ---- */
 /* batched decimating FIR (stage 1 alone): x [C][T] device, y [C][ceil(T/D)] device; zero history */
 int qrl_fir_decim_ccf_device(const float* taps, int ntaps, int D, const float* x_dev, long T, long x_stride,

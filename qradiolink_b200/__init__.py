@@ -17,3 +17,4 @@ from .framing import Deframer, DeframerBB, MODE_FRAMING, SYNC_1K, SYNC_NARROW, S
 from .frontend import Frontend, TxCombiner, TxFrontend  # noqa: F401
 from .spectrum import Spectrum  # noqa: F401
 from .mmdvm import MmdvmDemod, MmdvmMod, MmdvmChannelsRx, MmdvmChannelsTx, mmdvm_tag_item  # noqa: F401
+from .m17 import M17Decoder, M17Encoder, m17_lsf, m17_callsign, m17_crc16  # noqa: F401

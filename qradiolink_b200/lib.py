@@ -151,6 +151,24 @@ SYMBOLS = {
     "qrl_dfbb_read": (_i, [_vp, _vp, _l, _vp]),
     "qrl_dfbb_sync": (_i, [_vp]),
     "qrl_dfbb_launch_count": (_l, [_vp]),
+    "qrl_m17_rx_create": (_i, [_i, _i, _i, C.POINTER(_vp)]),
+    "qrl_m17_rx_destroy": (_i, [_vp]),
+    "qrl_m17_rx_set_stream": (_i, [_vp, _vp]),
+    "qrl_m17_rx_work": (_i, [_vp, _vp, _vp, _i, _i, _i]),
+    "qrl_m17_rx_reset": (_i, [_vp, _i]),
+    "qrl_m17_rx_read": (_i, [_vp, _vp, _vp]),
+    "qrl_m17_rx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp)]),
+    "qrl_m17_rx_sync": (_i, [_vp]),
+    "qrl_m17_rx_launch_count": (_l, [_vp]),
+    "qrl_m17_tx_create": (_i, [_i, _i, _i, C.POINTER(_vp)]),
+    "qrl_m17_tx_destroy": (_i, [_vp]),
+    "qrl_m17_tx_set_stream": (_i, [_vp, _vp]),
+    "qrl_m17_tx_set_lsf": (_i, [_vp, _i, _vp]),
+    "qrl_m17_tx_work": (_i, [_vp, _vp, _vp, _i, _i]),
+    "qrl_m17_tx_read": (_i, [_vp, _vp, _l, _vp]),
+    "qrl_m17_tx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_l), C.POINTER(_vp)]),
+    "qrl_m17_tx_sync": (_i, [_vp]),
+    "qrl_m17_tx_launch_count": (_l, [_vp]),
 }
 
 

@@ -121,7 +121,7 @@ def build(out_dir):
         open(os.path.join(out_dir, name.replace(".cu", ".cpp") if name.endswith(".cu") else name), "w").write(text)
     open(os.path.join(out_dir, "qrl_tma.cuh"), "w").write('#pragma once\n#include <cuda_runtime.h>   // the fake one: pulls in qrl_tma_emu.hpp\n')
     lib = os.path.join(out_dir, "libqrl_b200_emu.so")
-    srcs = [os.path.join(out_dir, f) for f in ("qrl_b200.cpp", "qrl_pfb.cpp", "qrl_deframer.cpp", "qrl_spectrum.cpp")]
+    srcs = [os.path.join(out_dir, f) for f in ("qrl_b200.cpp", "qrl_pfb.cpp", "qrl_deframer.cpp", "qrl_spectrum.cpp", "qrl_m17.cpp")]
     cmd = ["g++", "-std=c++20", "-O" + os.environ.get("QRL_EMU_OPT", "1"), "-ffp-contract=off", "-fno-fast-math", "-pthread", "-fPIC", "-shared", "-Wno-unknown-pragmas",
            "-I", os.path.join(HERE, "fake_cuda"), "-I", HERE, "-I", out_dir, "-o", lib] + srcs
     if os.environ.get("QRL_EMU_ASAN"):      # AddressSanitizer build (CPU memcheck): LD_PRELOAD=$(gcc -print-file-name=libasan.so), ASAN_OPTIONS=detect_leaks=0
