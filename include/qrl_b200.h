@@ -488,6 +488,42 @@ int  qrl_m17_tx_out_device(qrl_m17_tx*, void** out, long* stride, int** counts);
 int  qrl_m17_tx_sync(qrl_m17_tx*);
 long qrl_m17_tx_launch_count(qrl_m17_tx*);
 
+/* ---- DMR burst decoder (qrl_dmr.cu): gr_dmr_sink's burst search and the per-burst work of DMRFrame (constructor, setDownlink,
+ * validate), CDMREMB::putData and, when ambe_fec is set, CAMBEFEC::regenerateDMR (/root/reference/src/gr/gr_dmr_sink.cpp,
+ * src/DMR/dmrframe.cpp, src/DMR/dmrcontrol.cpp:225-271) for a batch of channels.  Input: QRL_DEMOD_DMR's port 2, one hard bit per byte,
+ * [n_channels][stride] with per-channel counts (count <= max_bits) -- exactly qrl_rx_port_device(handle, 2, ...) -- or host arrays of
+ * the same layout (on_device = 0).  With on_device = 1 the caller guarantees 0 <= counts[c] <= stride (port 2 does); host input is
+ * checked, and stride may not exceed max_bits there.  Output, per channel in the order of gr_dmr_sink's _frame_buffer, up to max_bursts records of
+ * QRL_DMR_RECORD_BYTES (72) bytes:
+ *    0 int64  position: stream index of the burst's last bit, counted from create / reset
+ *    8 u8     ts_index (the sink buffer the burst was cut from), 9 frame_type (0 data, 1 voice, 2 voice sync), 10 FN (setFN),
+ *   11 u8     downlink, 12 cach_decoded, 13 AT, 14 slot number, 15 LCSS (setDownlink)
+ *   16 u8     colour code (255 for voice bursts), 17 data type (DT_VOICE 0xF1 / DT_VOICE_SYNC 0xF0 for voice bursts)
+ *   18 u8     validate(), 19 FLCO, 20 FID, 21 EMB colour code, 22 EMB PI, 23 EMB LCSS (voice bursts B-F; 0 otherwise)
+ *   24 u32    src ID, 28 u32 dst ID (as validate() leaves them)
+ *   32 int32  AMBE error count of regenerateDMR (-1: ambe_fec off or not a voice burst)
+ *   36 u8[3]  CACH bytes, 39 u8[33] burst bytes, as the reference leaves them (data bursts re-encoded by a successful validate(),
+ *             voice bursts regenerated by the AMBE FEC when it is on)
+ * Bursts beyond max_bursts advance the state but are not stored (qrl_dmr_rx_dropped counts them); the DMRTiming calls the reference
+ * makes for them (set_slot_times) cannot be replayed, so size max_bursts for a call's worst case (one burst per 288 bits).  Sink state carries across calls;
+ * records are valid until the next work call. */
+#define QRL_DMR_RECORD_BYTES 72
+typedef struct qrl_dmr_rx qrl_dmr_rx;
+int  qrl_dmr_rx_create(int n_channels, long max_bits, int max_bursts, int ambe_fec, int device, qrl_dmr_rx** out);
+int  qrl_dmr_rx_destroy(qrl_dmr_rx*);
+int  qrl_dmr_rx_set_stream(qrl_dmr_rx*, void* cuda_stream);
+int  qrl_dmr_rx_work(qrl_dmr_rx*, const unsigned char* bits, const int* counts, long stride, int on_device);
+int  qrl_dmr_rx_record_bytes(qrl_dmr_rx*);
+/* records_host [n_channels][max_bursts][72] (may be NULL), counts_host [n_channels]; synchronises */
+int  qrl_dmr_rx_read(qrl_dmr_rx*, unsigned char* records_host, int* counts_host);
+int  qrl_dmr_rx_out_device(qrl_dmr_rx*, void** records, int** counts);
+/* bursts not stored because a call found more than max_bursts, per channel, since create / that channel's reset; synchronises */
+int  qrl_dmr_rx_dropped(qrl_dmr_rx*, int* dropped_host);
+/* gr_dmr_sink's constructor state for one channel (-1 = all): slots idle, buffers empty, position 0 */
+int  qrl_dmr_rx_reset(qrl_dmr_rx*, int channel);
+int  qrl_dmr_rx_sync(qrl_dmr_rx*);
+long qrl_dmr_rx_launch_count(qrl_dmr_rx*);
+
 /* ---- stand-alone kernels exposed for tests / micro-benchmarks ---- */
 /* batched decimating FIR (stage 1 alone): x [C][T] device, y [C][ceil(T/D)] device; zero history */
 int qrl_fir_decim_ccf_device(const float* taps, int ntaps, int D, const float* x_dev, long T, long x_stride,

@@ -47,19 +47,6 @@ std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
 
 using HandleBase = QrlHandleBase;       // qrl_handle.hpp: shared by every handle type of the library
 
-// a device pointer handed to a *_work call must live on the handle's device (a pointer from another GPU would fault inside a kernel
-// long after the call returned)
-int check_device_ptr(HandleBase* h, const void* p, const char* who)
-{
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return QRL_OK; }
-    if (a.type == cudaMemoryTypeDevice && a.device != h->device) {
-        set_err(h, std::string(who) + ": the device pointer belongs to GPU " + std::to_string(a.device) + ", the handle to GPU " + std::to_string(h->device));
-        return QRL_EINVAL;
-    }
-    return QRL_OK;
-}
-
 // the atan, tanh, MMSE and sine lookup tables, once per device (keyed by this function)
 int upload_tables(HandleBase* h)
 {

@@ -123,6 +123,19 @@ int handle_close(H* h)
     return QRL_OK;
 }
 
+// a device pointer handed to a *_work call must live on the handle's device (a pointer from another GPU would fault inside a kernel
+// long after the call returned)
+inline int check_device_ptr(QrlHandleBase* h, const void* p, const char* who)
+{
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return QRL_OK; }
+    if (a.type == cudaMemoryTypeDevice && a.device != h->device) {
+        set_err(h, std::string(who) + ": the device pointer belongs to GPU " + std::to_string(a.device) + ", the handle to GPU " + std::to_string(h->device));
+        return QRL_EINVAL;
+    }
+    return QRL_OK;
+}
+
 // *_set_stream: the handle's work so far drains, then it runs on the caller's stream; NULL = back to a stream of its own
 inline int handle_set_stream(QrlHandleBase* h, void* s)
 {

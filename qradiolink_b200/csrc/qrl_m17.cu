@@ -18,6 +18,7 @@
 // spec's randomizer sequence.  Where the reference decoder has a quirk (the Viterbi chainback, segment numbers 6 and 7) the kernels
 // restate its observable result.
 #include "../../include/qrl_b200.h"
+#include "qrl_golay.cuh"
 #include "qrl_handle.hpp"
 
 #include <cuda_runtime.h>
@@ -38,19 +39,9 @@ __device__ const unsigned char kRandomizer[46] = {
     0xd6, 0xb5, 0xe2, 0x30, 0x82, 0xff, 0x84, 0x62, 0xba, 0x4e, 0x96, 0x90, 0xd8, 0x98, 0xdd, 0x5d, 0x0c, 0xc8, 0x52, 0x43, 0x91, 0x1d, 0xf8,
     0x6e, 0x68, 0x2f, 0x35, 0xda, 0x14, 0xea, 0xcd, 0x76, 0x19, 0x8d, 0xd5, 0x80, 0xd1, 0x33, 0x87, 0x13, 0x57, 0x18, 0x2d, 0x29, 0x78, 0xc3 };
 
-// ---- Golay(24,12): the 12 check bits of data d are ((d(x) x^11 mod g(x)) << 1) | overall parity, g(x) = 0xC75 (the (23,12) cyclic
-// code, extended).  enc[i] = the check bits of data bit i; dec = its transpose, which is also its inverse (the code is self-dual).
+// ---- Golay(24,12): golay_check (qrl_golay.cuh) gives the 12 check bits of data d.  enc[i] = the check bits of data bit i; dec = its
+// transpose, which is also its inverse (the code is self-dual).
 struct GolayRows { uint16_t enc[12], dec[12]; };
-
-__host__ __device__ constexpr uint16_t golay_check(uint32_t d)
-{
-    uint32_t r = d << 11;
-    for (int b = 22; b >= 11; b--)
-        if (r >> b & 1u) r ^= 0xC75u << (b - 11);
-    int par = 0;
-    for (int b = 0; b < 12; b++) par += static_cast<int>((d >> b) & 1u) + static_cast<int>((r >> b) & 1u);
-    return static_cast<uint16_t>((r << 1) | (par & 1));
-}
 
 constexpr GolayRows make_golay_rows()
 {

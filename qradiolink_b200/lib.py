@@ -169,6 +169,17 @@ SYMBOLS = {
     "qrl_m17_tx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_l), C.POINTER(_vp)]),
     "qrl_m17_tx_sync": (_i, [_vp]),
     "qrl_m17_tx_launch_count": (_l, [_vp]),
+    "qrl_dmr_rx_create": (_i, [_i, _l, _i, _i, _i, C.POINTER(_vp)]),
+    "qrl_dmr_rx_destroy": (_i, [_vp]),
+    "qrl_dmr_rx_set_stream": (_i, [_vp, _vp]),
+    "qrl_dmr_rx_work": (_i, [_vp, _vp, _vp, _l, _i]),
+    "qrl_dmr_rx_record_bytes": (_i, [_vp]),
+    "qrl_dmr_rx_read": (_i, [_vp, _vp, _vp]),
+    "qrl_dmr_rx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp)]),
+    "qrl_dmr_rx_dropped": (_i, [_vp, _vp]),
+    "qrl_dmr_rx_reset": (_i, [_vp, _i]),
+    "qrl_dmr_rx_sync": (_i, [_vp]),
+    "qrl_dmr_rx_launch_count": (_l, [_vp]),
 }
 
 
