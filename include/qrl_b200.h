@@ -81,7 +81,10 @@ enum qrl_param {
     QRL_PARAM_AGC_ATTACK = 8,         /* gr_demod_ssb::set_agc_attack / gr_demod_am::set_agc_attack (gr_demod_ssb.cpp:108-111, gr_demod_am.cpp:94-97) */
     QRL_PARAM_AGC_DECAY = 9,          /* gr_demod_ssb::set_agc_decay / gr_demod_am::set_agc_decay */
     QRL_PARAM_GAIN = 10,              /* gr_demod_ssb::set_gain (gr_demod_ssb.cpp:118-121): the IF gain in front of the side-band filter */
-    QRL_PARAM_RSSI = 6,               /* 1: keep the RSSI tap of rssi_block.cpp:25-45 on port 0 up to date (read with qrl_rx_rssi) */
+    QRL_PARAM_RSSI = 6,               /* 1: keep the RSSI tap of rssi_block.cpp:25-45 on port 0 up to date (read with qrl_rx_rssi).
+                                         Whenever it goes from 0 to 1 (the first switch-on, mid-stream or not, and every one after
+                                         a switch-off) the tap starts afresh: its values are those of rssi_block constructed at that
+                                         moment and fed port 0 from the next qrl_rx_work on. */
     QRL_PARAM_OVERLAP_CALLS = 5       /* 1: the loop / FEC tail of qrl_rx_work call k runs under the parallel stages of call
                                          k+1 (streaming use).  Output ports are double-buffered; the results of a call are
                                          ordered on the caller's stream only after qrl_rx_join (or qrl_rx_sync /
@@ -113,6 +116,12 @@ int qrl_rx_destroy(qrl_rx* h);
 /* run all kernels of this handle on an existing CUDA stream (cudaStream_t); NULL = the handle's own stream */
 int qrl_rx_set_stream(qrl_rx* h, void* cuda_stream);
 int qrl_rx_set_param(qrl_rx* h, int channel /* -1 = all */, int key, double value);
+/* Restart every channel's stream at sample 0; waits for everything the handle has in flight.  Afterwards every port of every call
+ * is bit-identical to a handle created with the same arguments and given the settings now in force before its first call.  Those
+ * settings are: each channel's carrier offset; squelch, filter width and CTCSS; AGC attack and decay, and the IF gain; RSSI on or
+ * off; overlapped calls; the stream set with qrl_rx_set_stream.  Everything carried by the stream restarts: histories, rings, loop
+ * states, counts, the rotator phase (0 at the first sample after the reset) and the RSSI window.  Until the next qrl_rx_work,
+ * qrl_rx_rssi reads -180 + level. */
 int qrl_rx_reset(qrl_rx* h);
 /* iq: [n_channels][T] interleaved float (re,im) = gr_complex; channel stride = `stride` complex samples.
  * on_device != 0: iq is a device pointer (already in HBM). Otherwise host memory (pinned or pageable);

@@ -1447,6 +1447,12 @@ int qrl_rx_reset(qrl_rx* h)
     }
     QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
     QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+    if (!h->rot.empty()) {
+        // the carrier offsets stay in force, the rotator's phase restarts: 0 at the first sample after the reset
+        h->rot_active = false;
+        for (RotState& r : h->rot) { r.base = 0; r.n_base = 0; h->rot_active = h->rot_active || r.inc != 0; }
+        if (h->d_rot) QRL_CK(cudaMemcpyAsync(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    }
     QRL_CK(cudaStreamSynchronize(h->stream));   // the staging vectors above go out of scope
     h->n_in = 0; h->n1 = 0; h->n_in_s = 0; h->n1_s = 0; h->hist_cur = 0; h->port0_n = 0; h->prev_nsub = 0; h->rssi_n = 0;
     return QRL_OK;
@@ -1481,16 +1487,25 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
 {
     if (!h) return QRL_EINVAL;
     if (key == QRL_PARAM_RSSI) {
-        if (value != 0.0 && !h->d_rssi_ring) {
+        const bool on = value != 0.0;
+        if (on && !h->d_rssi_ring) {
             int rc;
             if ((rc = dev_alloc(h, &h->d_rssi_ring, static_cast<size_t>(4096) * h->C))) return rc;
             if ((rc = dev_alloc(h, &h->d_rssi_y, h->C))) return rc;
             if ((rc = dev_alloc(h, &h->d_rssi_db, h->C))) return rc;
             h->zero_list.emplace_back(h->d_rssi_ring, sizeof(float) * 4096 * h->C);
             h->zero_list.emplace_back(h->d_rssi_y, sizeof(float) * h->C);
+        }
+        if (on && !h->rssi_on) {
+            // every switch-on starts the tap afresh, as an rssi_block constructed now and fed port 0 from the next call on: the |x|^2
+            // ring and the IIR value of an earlier switch-on would otherwise reach into the new window.  The memsets follow the
+            // last call's rssi_kernel (every call ends with the handle's stream waiting for the parallel stream it ran on).
+            if (int rc = rx_join_host(h)) return rc;
+            QRL_CK(cudaMemsetAsync(h->d_rssi_ring, 0, sizeof(float) * 4096 * h->C, h->stream));
+            QRL_CK(cudaMemsetAsync(h->d_rssi_y, 0, sizeof(float) * h->C, h->stream));
             h->rssi_n = 0;
         }
-        h->rssi_on = value != 0.0;
+        h->rssi_on = on;
         return QRL_OK;
     }
     if (key == QRL_PARAM_OVERLAP_CALLS) {

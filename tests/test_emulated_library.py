@@ -145,6 +145,50 @@ def test_mmdvm_tx_zero_idle_through_the_emulated_library(emu_qrl, oracle, single
     TM.zero_idle_case(emu_qrl, oracle, single, q=1)
 
 
+def test_rx_reset_restarts_the_rotator_phase_through_the_emulated_library(emu_qrl):
+    """qrl_rx_reset keeps each channel's carrier offset and restarts its phase at 0 (tests/test_gpu_rx_reset.py on every chain): a
+    2500 Hz offset set after the first 20 000 samples, then a reset, must leave the next stream bit-identical to a fresh handle that
+    had the offset before its first call"""
+    from tests import siggen
+    X = siggen.gen_nbfm_channels(1, 100000, seed0=5500)
+    a = emu_qrl.make_gr_demod_nbfm(125, 1000000, 1700, 5000, n_channels=1, max_samples=50000)
+    b = emu_qrl.make_gr_demod_nbfm(125, 1000000, 1700, 5000, n_channels=1, max_samples=50000)
+    try:
+        a.work(X[:, :20000])
+        a.set_carrier_offset(2500.0)
+        a.work(X[:, 20000:50000])
+        a.reset()
+        b.set_carrier_offset(2500.0)
+        for blk in (a, b):
+            blk.work(X[:, 50000:])
+        for p in range(2):
+            g, w = a.read_port(p)[0], b.read_port(p)[0]
+            assert len(g) == len(w) > 0 and np.array_equal(g.view(np.uint8), w.view(np.uint8)), p
+    finally:
+        a.close(); b.close()
+
+
+def test_rssi_switched_off_and_on_restarts_the_tap_through_the_emulated_library(emu_qrl, oracle):
+    """QRL_PARAM_RSSI from 0 to 1 starts the tap afresh (tests/test_gpu_rx_reset.py): on for a loud call, off for a call 40 dB
+    quieter, on again; the next call must read what rssi_block constructed at the re-enable reads"""
+    from tests import siggen
+    X = siggen.gen_nbfm_channels(1, 72000, seed0=5600)
+    X[:, 50000:] *= np.float32(0.01)
+    blk = emu_qrl.make_gr_demod_nbfm(125, 1000000, 1700, 5000, n_channels=1, max_samples=50000)
+    try:
+        blk.enable_rssi(True)
+        blk.work(X[:, :50000])
+        blk.enable_rssi(False)
+        blk.work(X[:, 50000:70000])
+        blk.enable_rssi(True)
+        blk.work(X[:, 70000:])
+        p0 = blk.read_port(0)[0]
+        want = oracle.Rssi(0.0).work(p0)
+        assert len(p0) > 0 and abs(float(blk.rssi()[0]) - want) < 1e-3, (float(blk.rssi()[0]), want)
+    finally:
+        blk.close()
+
+
 def test_qpsk_chain_through_the_emulated_library(emu_qrl, oracle):
     """The QPSK-250k chain's loop kernels hand blocks between warps through 3-deep shared-memory rings (AGC -> Costas -> bulk store;
     symbol sync -> second Costas -> feed-forward epilogue): a short ragged stream through the real host code and kernels, ports

@@ -198,7 +198,7 @@ def representatives(Cn, spots):
     for c in range(Cn):
         if c not in spots and c % P not in reps:
             reps[c % P] = c
-    assert len(reps) == P
+    assert len(reps) == min(P, Cn - len(spots))       # every class has one (a handle of fewer than P plain channels: each its own)
     return reps
 
 
@@ -301,11 +301,14 @@ def concat_calls(calls, nports, Cn):
     return [[np.concatenate([calls[k][p][c] for k in range(len(calls))]) for c in range(Cn)] for p in range(nports)]
 
 
-def oracle_ports(name, O, B, spots, c, cuts, events):
-    key = (name, B.shape[1], c % P, spots.get(c), tuple(cuts), tuple((k, hz) for (k, ch, hz) in events if ch in (-1, c)))
+def oracle_ports(name, O, B, spots, c, cuts, events, setters=()):
+    """setters: (PARAM key, value) applied before the first sample"""
+    key = (name, B.shape[1], c % P, spots.get(c), tuple(cuts), tuple((k, hz) for (k, ch, hz) in events if ch in (-1, c)), tuple(setters))
     if key not in _ORACLE:
         x = host_channel(B, spots, c)
         rx = RX[name][1](O)
+        for pkey, value in setters:
+            rx.set_param(pkey, value)
         for k, (lo, hi) in enumerate(cuts):
             for (ek, ch, hz) in events:
                 if ek == k and ch in (-1, c):
@@ -315,8 +318,8 @@ def oracle_ports(name, O, B, spots, c, cuts, events):
     return _ORACLE[key]
 
 
-def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True):
-    """got[p][c]: the whole stream of port p on channel c"""
+def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True, setters=()):
+    """got[p][c]: the whole stream of port p on channel c; setters: (PARAM key, value) the handle had before its first sample"""
     nports, fr = RX[name][2], RX[name][5]
     mins = [m * cuts[-1][1] // RX[name][3] for m in RX[name][4]]         # the minimum lengths scale with the stream's length
     Cn = len(got[0])
@@ -326,7 +329,7 @@ def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True):
             if c not in spots:
                 assert np.array_equal(got[p][c], got[p][reps[c % P]]), "%s: port %d of channel %d differs from channel %d" % (name, p, c, reps[c % P])
     for c in sorted(set(reps.values()) | set(spots)):
-        want = oracle_ports(name, O, B, spots, c, cuts, events)
+        want = oracle_ports(name, O, B, spots, c, cuts, events, setters)
         for p in range(nports):
             g, w = got[p][c], want[p]
             n = min(len(g), len(w))
