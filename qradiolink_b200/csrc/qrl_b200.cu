@@ -80,6 +80,7 @@ struct qrl_rx : HandleBase {
     long long n_in_s = 0, n1_s = 0;   // progress of the per-slice stages behind it (equal to the above between calls)
     bool fir_group_forced = false;     // QRL_FIR_GROUP given: keep it in overlap mode too
     int fir_group = 4;                 // stage-1 launches cover this many slices (bigger launches, same pipeline depth)
+    bool fsk_fused = false;            // fsk_fm_fused(): stage 1 runs inside the per-slice front-end kernel (decided at create)
     Ring r1;
     // stage 2: channel / shaping filter on the complex stream (port 0)
     float* d_taps2 = nullptr; int ntaps2 = 0; size_t taps2_cap = 0;     // floats allocated for d_taps2 (set_filter_width redesigns)
@@ -453,6 +454,9 @@ struct Slice {
     cudaStream_t sp;            // stream of the parallel stages
     dim3 gtile;                 // kTileThreads-thread CTAs over the new outputs, one row per channel
     int groups;                 // CTAs of 32 channels (the loop kernels)
+    // the call's input as stage 1 reads it (the fused 4FSK-FM front end runs stage 1 slice by slice): T samples per channel from x
+    // (row stride xstride), the first of them absolute input sample n_in0, the history in front of it in hist
+    const float2* x; long long xstride, T, n_in0; const float2* hist;
 };
 
 // `to` runs on behind everything queued on `from` so far
@@ -477,6 +481,38 @@ int launch_channel_filter(qrl_rx* h, const Slice& s, cudaStream_t st, const Ring
 {
     return launch_fir_ccf(h, st, static_cast<const float2*>(in.d), in.mask, in.stride, static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                           h->d_taps2, h->ntaps2, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0, interleaved);
+}
+
+// 4FSK-FM with the register-tiled /50 stage 1 and filters that fit the kernel's shared memory: the whole receive front end of a slice
+// is one fsk_fm_frontend_kernel launch (QRL_FSK_FRONTEND=0 keeps stage 1, the channel filter and the demodulator as three launches)
+bool fsk_fm_fused(const qrl_rx* h)
+{
+    if (const char* e = getenv("QRL_FSK_FRONTEND")) { if (e[0] == '0') return false; }
+    // the first strip of a slice reads the halo in front of the slice from r1 while the slice's last strips store the halo behind it
+    // there: a slice (at most n1max outputs) plus its halo must fit the ring, or the two ranges alias
+    const long long halo = h->ntaps3 + h->ntaps2 - 1;
+    return h->kind == QRL_DEMOD_4FSK && h->flag && !h->m17 && !h->dmr && h->L1 == 1 && h->D1 == 50 && h->Q1 == 9 && !h->fir_group_forced &&
+           h->ntaps2 >= 8 && h->ntaps2 <= 256 && h->ntaps3 >= 8 && h->ntaps3 <= 512 &&
+           static_cast<long long>(h->r1.mask) + 1 >= h->n1max + halo;
+}
+
+// stage 1, channel filter (-> port 0), quadrature demod and RRC (-> r4) of a slice in one launch on the parallel stream.  A strip is
+// two chunks of stage-1 outputs, its halo included (halo / strip stays under 10 % at the 4FSK-2k filters).
+int launch_fsk_frontend(qrl_rx* h, const Slice& s)
+{
+    constexpr int D = 50, Q = 9, NOUT1 = 64;
+    const int halo = h->ntaps3 + h->ntaps2 - 1;
+    const int strip = 2 * FF_CH - halo;
+    const size_t smem = sizeof(float) * FskFrontendSmem<D, Q, NOUT1>(h->ntaps2, h->ntaps3).floats;
+    auto kern = fsk_fm_frontend_kernel<D, Q, NOUT1>;
+    if (int rc = smem_opt_in(h, kern, 120 * 1024)) return rc;
+    dim3 g(static_cast<unsigned>((s.n_new + strip - 1) / strip), h->C);
+    kern<<<g, FF_NT, smem, s.sp>>>(s.x, s.xstride, s.T, s.hist, h->H, h->d_taps1, s.n_in0, h->rot_fused ? h->d_rot : nullptr,
+        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->d_taps2, h->ntaps2, h->d_port0, h->port0_cap, s.k_call0,
+        h->d_taps3, h->ntaps3, h->qd_gain, static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, s.k0, s.k1, strip);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    return QRL_OK;
 }
 
 // one symbol-sync launch on `st` over the input ring `in` up to k1 (opting the instance in to `smem_max` bytes first); only the
@@ -696,13 +732,8 @@ int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
 int slice_4fsk(qrl_rx* h, const Slice& s)
 {
     cudaEvent_t pe;
-    if (s.n_new > 0) {
-        // ---- stage 2: channel filter -> ring + port 0
-        pe = h->prof.begin(1, s.sp);
-        if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
-        h->prof.end(pe);
-        // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
-        // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
+    // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
+    auto wait_r4_free = [&]() -> int {
         if (h->overlap && h->prev_nsub > 0) {
             // the slots [k0, k1) overwrite the samples cap older; the previous call's symbol sync of slice q has
             // consumed everything up to prev_k1[q] - lookahead
@@ -711,6 +742,21 @@ int slice_4fsk(qrl_rx* h, const Slice& s)
             for (int j = 0; j < h->prev_nsub; j++) if (h->prev_k1[j] - 64 < must) q = j;      // not yet safe after slice j alone
             if (q >= 0) QRL_CK(cudaStreamWaitEvent(s.sp, h->ev_c[std::min(q + 1, h->prev_nsub - 1)], 0));
         }
+        return QRL_OK;
+    };
+    if (s.n_new > 0 && h->fsk_fused) {
+        // ---- stages 1-3 in one launch (profiled as stage 1)
+        if (int rc = wait_r4_free()) return rc;
+        pe = h->prof.begin(0, s.sp);
+        if (int rc = launch_fsk_frontend(h, s)) return rc;
+        h->prof.end(pe);
+    } else if (s.n_new > 0) {
+        // ---- stage 2: channel filter -> ring + port 0
+        pe = h->prof.begin(1, s.sp);
+        if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
+        h->prof.end(pe);
+        // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
+        if (int rc = wait_r4_free()) return rc;
         pe = h->prof.begin(2, s.sp);
         if (h->flag) {
             if (int rc = launch_qdemod_fir(h, s.sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
@@ -1373,6 +1419,7 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
     if (kind == QRL_DEMOD_QPSK) h->nsub = qrl_rx::kMaxSub;
     if (const char* e = getenv("QRL_NSUB")) { int v = atoi(e); if (v >= 1 && v <= qrl_rx::kMaxSub) { h->nsub = v; h->nsub_forced = true; } }
     if (const char* e = getenv("QRL_FIR_GROUP")) { int v = atoi(e); if (v >= 1 && v <= qrl_rx::kMaxSub) { h->fir_group = v; h->fir_group_forced = true; } }
+    h->fsk_fused = fsk_fm_fused(h);
     if ((rc = qrl_rx_reset(h))) return fail(rc);
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
@@ -1767,6 +1814,10 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     int nsub = (h->overlap && !h->nsub_forced) ? 2 : h->nsub;
     if (T < 32768L * nsub) nsub = static_cast<int>(std::max<long>(1, T / 32768));
     const long long k_call0 = h->n1;
+    const long long n_in0 = h->n_in;
+    const float2* hist0 = h->d_hist[h->hist_cur];
+    // the fused 4FSK-FM front end runs stage 1 inside its per-slice launches: here only the history advances, once for the call
+    const bool whole_call = (h->overlap && !h->fir_group_forced) || h->fsk_fused;
     h->port0_n = 0;
     for (int i = 0; i < nsub; i++) {
         // slice boundaries on multiples of 2*D: the slice base stays 16-byte aligned (TMA bulk fill) and every slice
@@ -1781,16 +1832,16 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         // stage-1 launch schedule: slice 0 alone (the loop stage starts as early as possible), then fir_group slices
         // per launch (bigger launches run closer to the HBM roofline)
         // (overlapped calls: the pipeline is already full, one launch for the whole call)
-        const bool fir_here = h->overlap && !h->fir_group_forced ? (i == 0) : ((i == 0) || ((i - 1) % h->fir_group == 0));
+        const bool fir_here = whole_call ? (i == 0) : ((i == 0) || ((i - 1) % h->fir_group == 0));
         if (fir_here) {
-            const long long tg1 = cut(h->overlap && !h->fir_group_forced ? nsub : (i == 0 ? 1 : std::min(i + h->fir_group, nsub)));
+            const long long tg1 = cut(whole_call ? nsub : (i == 0 ? 1 : std::min(i + h->fir_group, nsub)));
             const long long Tg = tg1 - t0;
             const float2* xg = x + t0;
             const long long Ng = h->n_in + Tg;
             const long long kg0 = h->n1;
             const long long kg1 = (Ng * h->L1 + h->D1 - 1) / h->D1;       // outputs i with floor(i M / L) <= N - 1
-            pe = h->prof.begin(0, sp);
-            int rc = stage1(h, xg, xstride, Tg, kg0, kg1);
+            pe = h->fsk_fused ? nullptr : h->prof.begin(0, sp);
+            int rc = h->fsk_fused ? QRL_OK : stage1(h, xg, xstride, Tg, kg0, kg1);
             if (!rc && h->kind == QRL_DEMOD_SSB && kg1 > kg0) {
                 // gr_demod_ssb's multiply_const_cc(_if_gain) sits between the resampler and the side-band filter: the gain is applied
                 // to the samples as they pass (8 ksps), so after set_gain the filter's history keeps the old gain, like the reference's
@@ -1817,7 +1868,8 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         const long long n_new = k1 - k0;
         h->port0_n += static_cast<long>(n_new);
         const Slice s{ i, k0, k1, n_new, k_call0, h->d_nsoft + static_cast<size_t>(i) * h->C, sp,
-                       dim3(static_cast<unsigned>((std::max<long long>(n_new, 1) + kTileThreads - 1) / kTileThreads), h->C), (h->C + 31) / 32 };
+                       dim3(static_cast<unsigned>((std::max<long long>(n_new, 1) + kTileThreads - 1) / kTileThreads), h->C), (h->C + 31) / 32,
+                       x, xstride, T, n_in0, hist0 };
         int rc;
         switch (h->kind) {
         case QRL_DEMOD_DSSS: rc = slice_dsss(h, s); break;

@@ -119,72 +119,66 @@ __device__ __forceinline__ unsigned char qrl_soft_u8(float v, float scale)
 // front-end rotator state (gr_demod_base's rotator_cc): exact Q32 phase, phase = base + inc * (n_abs - n_base)
 struct RotState { unsigned inc, base; long long n_base; };
 
-// rot != nullptr: the carrier-offset rotator is applied to the window in shared memory right after the fill (same arithmetic as
-// rotator_kernel, sample by sample), so a non-zero offset costs no extra pass over HBM (8.16 B per input sample instead of 24);
-// the history tail then holds ALREADY ROTATED samples (frontend_hist_kernel), like the reference's resampler history.
-template <int D, int Q, int K, int NOUT, int NWARPS>
-__global__ void __launch_bounds__(NWARPS * 32)
-fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
-                      const float2* __restrict__ hist, int H,
-                      const float* __restrict__ taps_padded,   // Q*D floats, zero padded
-                      float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
-                      long long n_in_before, long long k0, long long k1, const RotState* __restrict__ rot = nullptr)
+// The per-tile arithmetic of the register-tiled stage 1, shared by fir_decim_poly_kernel and fsk_fm_frontend_kernel: one tile =
+// NOUT consecutive outputs from a window of (NOUT + Q - 1) D samples in shared memory.
+template <int D, int Q>
+struct FirPolyShape {
+    static constexpr int R = (D + 31) / 32;          // branch rounds per lane
+};
+
+// per-lane taps: tap[rho][q] = h[D q + r], r = lane + 32 rho (zero beyond the filter / beyond D)
+template <int D, int Q>
+__device__ __forceinline__ void fir_poly_load_taps(const float* __restrict__ taps_padded, int lane, float (&tap)[FirPolyShape<D, Q>::R][Q])
 {
-    static_assert(K == 8, "transposed butterfly below is written for 2K = 16 values");
-    constexpr int R = (D + 31) / 32;                 // branch rounds per lane
-    constexpr int W = (NOUT + Q - 1) * D;            // samples in the strip window
-    constexpr int WC = (W + 3) & ~1;                 // bulk-copy length: even (16-byte multiple), >= W + 1
-    extern __shared__ __align__(128) float2 xs_raw[];   // WC samples
-    __shared__ __align__(8) uint64_t fill_bar;
-
-    const int c = blockIdx.y;
-    const long long kbase = k0 + static_cast<long long>(blockIdx.x) * NOUT;
-    if (kbase >= k1) return;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-
-    // per-lane taps: tap[rho][q] = h[D q + r], r = lane + 32 rho (zero beyond the filter / beyond D)
-    float tap[R][Q];
 #pragma unroll
-    for (int rho = 0; rho < R; rho++) {
+    for (int rho = 0; rho < FirPolyShape<D, Q>::R; rho++) {
         const int r = lane + 32 * rho;
 #pragma unroll
         for (int q = 0; q < Q; q++) tap[rho][q] = (r < D) ? taps_padded[D * q + r] : 0.0f;
     }
+}
 
-    // window covers absolute samples [A0, A0 + W); the copy starts one sample early when that makes the
-    // global source 16-byte aligned (S0 even relative to the 16-byte aligned channel base)
-    const long long A0 = D * kbase - (static_cast<long long>(Q) * D - 1);
-    const float2* iqc = iq + static_cast<long long>(c) * iq_stride;
-    const float2* hc = hist + static_cast<long long>(c) * H;
-    const long long i0 = A0 - n_in_before;                       // index of the window start in this call's input
-    const int shift = static_cast<int>(i0 & 1);                  // 1 -> start the bulk copy at i0 - 1
-    const float2* xs = xs_raw + shift;
-    const bool bulk = (i0 - shift >= 0) && (i0 - shift + WC <= T) && ((iq_stride & 1) == 0) &&
-                      ((reinterpret_cast<unsigned long long>(iq) & 15ull) == 0);
-    if (bulk) {
-        if (threadIdx.x == 0) { mbar_init(&fill_bar, 1); mbar_fence_init(); }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            mbar_expect_tx(&fill_bar, WC * 8);
-            bulk_g2s(xs_raw, iqc + (i0 - shift), WC * 8, &fill_bar);
-        }
-        mbar_wait(&fill_bar, 0);
-    } else {
+// where the window of the tile starting at output kbase sits: it covers absolute samples [A0, A0 + W); the copy starts one sample
+// early when that makes the global source 16-byte aligned (S0 even relative to the 16-byte aligned channel base).  bulk: the whole
+// copy lies inside this call's input and can be one bulk copy.
+template <int D, int Q, int NOUT>
+struct FirPolyWindow {
+    static constexpr int W = (NOUT + Q - 1) * D;     // samples in the window
+    static constexpr int WC = (W + 3) & ~1;          // bulk-copy length: even (16-byte multiple), >= W + 1
+    long long i0;                                    // index of the window start in this call's input
+    int shift;                                       // 1 -> the bulk copy starts at i0 - 1
+    bool bulk;
+    __device__ __forceinline__ FirPolyWindow(const float2* iq, long long iq_stride, long long T, long long n_in_before, long long kbase)
+    {
+        i0 = D * kbase - (static_cast<long long>(Q) * D - 1) - n_in_before;
+        shift = static_cast<int>(i0 & 1);
+        bulk = (i0 - shift >= 0) && (i0 - shift + WC <= T) && ((iq_stride & 1) == 0) &&
+               ((reinterpret_cast<unsigned long long>(iq) & 15ull) == 0);
+    }
+    // thread 0: queue the bulk copy of the window into xs_raw, completing on `bar`
+    __device__ __forceinline__ void issue(float2* xs_raw, const float2* iqc, uint64_t* bar) const
+    {
+        mbar_expect_tx(bar, WC * 8);
+        bulk_g2s(xs_raw, iqc + (i0 - shift), WC * 8, bar);
+    }
+    // every thread: element-wise fill (window edges: before this call's input the channel's history, else zeros)
+    __device__ __forceinline__ void fill(float2* xs_raw, const float2* iqc, long long T, const float2* hc, int H, int nthreads) const
+    {
         float2* xw = xs_raw + shift;
-        for (int idx = threadIdx.x; idx < W; idx += NWARPS * 32) {
+        for (int idx = threadIdx.x; idx < W; idx += nthreads) {
             const long long i = i0 + idx;
             float2 v = make_float2(0.0f, 0.0f);
             if (i >= 0) { if (i < T) v = __ldg(iqc + i); }
             else if (H + i >= 0) v = hc[H + i];
             xw[idx] = v;
         }
-        __syncthreads();
     }
-    if (rot) {
-        // rotate this call's samples of the window in place (history samples were rotated when they were new)
-        const RotState r = rot[c];
+    // every thread: rotate this call's samples of the window in place (same arithmetic as rotator_kernel, sample by sample; history
+    // samples were rotated when they were new)
+    __device__ __forceinline__ void rotate(float2* xs_raw, const RotState& r, long long T, long long n_in_before, int nthreads) const
+    {
         float2* xw = xs_raw + shift;
-        for (int idx = threadIdx.x; idx < W; idx += NWARPS * 32) {
+        for (int idx = threadIdx.x; idx < W; idx += nthreads) {
             const long long i = i0 + idx;
             if (i < 0 || i >= T) continue;
             const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_in_before + i - r.n_base);
@@ -194,10 +188,16 @@ fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long l
             const float2 x = xw[idx];
             xw[idx] = make_float2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
         }
-        __syncthreads();
     }
+};
 
-    float* outc = reinterpret_cast<float*>(out_ring + static_cast<long long>(c) * ring_stride);
+// the tile's outputs from its window xs (= xs_raw + shift): warp w computes the K-output blocks b = w, w + NWARPS, ...; lane partials
+// meet in the transposed butterfly; store(i, comp, value) receives output i of the tile (component comp) from the even lanes
+template <int D, int Q, int K, int NOUT, int NWARPS, class Store>
+__device__ __forceinline__ void fir_poly_tile(const float2* xs, const float (&tap)[FirPolyShape<D, Q>::R][Q], int lane, int warp, Store store)
+{
+    static_assert(K == 8, "transposed butterfly below is written for 2K = 16 values");
+    constexpr int R = FirPolyShape<D, Q>::R;
     for (int b = warp; b < NOUT / K; b += NWARPS) {
         float2 acc[K];                                // (re, im) pairs: one ffma2() (two FFMA) per tap and output
 #pragma unroll
@@ -258,10 +258,54 @@ fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long l
         // lane l (even) now holds value v = l >> 1  -> output i = v >> 1, component v & 1
         if ((lane & 1) == 0) {
             const int v = lane >> 1;
-            const long long k = kbase + K * b + (v >> 1);
-            if (k < k1) outc[2 * (k & ring_mask) + (v & 1)] = a[0];
+            store(K * b + (v >> 1), v & 1, a[0]);
         }
     }
+}
+
+// rot != nullptr: the carrier-offset rotator is applied to the window in shared memory right after the fill (same arithmetic as
+// rotator_kernel, sample by sample), so a non-zero offset costs no extra pass over HBM (8.16 B per input sample instead of 24);
+// the history tail then holds ALREADY ROTATED samples (frontend_hist_kernel), like the reference's resampler history.
+template <int D, int Q, int K, int NOUT, int NWARPS>
+__global__ void __launch_bounds__(NWARPS * 32)
+fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
+                      const float2* __restrict__ hist, int H,
+                      const float* __restrict__ taps_padded,   // Q*D floats, zero padded
+                      float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
+                      long long n_in_before, long long k0, long long k1, const RotState* __restrict__ rot = nullptr)
+{
+    extern __shared__ __align__(128) float2 xs_raw[];   // WC samples
+    __shared__ __align__(8) uint64_t fill_bar;
+
+    const int c = blockIdx.y;
+    const long long kbase = k0 + static_cast<long long>(blockIdx.x) * NOUT;
+    if (kbase >= k1) return;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+    float tap[FirPolyShape<D, Q>::R][Q];
+    fir_poly_load_taps<D, Q>(taps_padded, lane, tap);
+
+    const float2* iqc = iq + static_cast<long long>(c) * iq_stride;
+    const FirPolyWindow<D, Q, NOUT> win(iq, iq_stride, T, n_in_before, kbase);
+    if (win.bulk) {
+        if (threadIdx.x == 0) { mbar_init(&fill_bar, 1); mbar_fence_init(); }
+        __syncthreads();
+        if (threadIdx.x == 0) win.issue(xs_raw, iqc, &fill_bar);
+        mbar_wait(&fill_bar, 0);
+    } else {
+        win.fill(xs_raw, iqc, T, hist + static_cast<long long>(c) * H, H, NWARPS * 32);
+        __syncthreads();
+    }
+    if (rot) {
+        win.rotate(xs_raw, rot[c], T, n_in_before, NWARPS * 32);
+        __syncthreads();
+    }
+
+    float* outc = reinterpret_cast<float*>(out_ring + static_cast<long long>(c) * ring_stride);
+    fir_poly_tile<D, Q, K, NOUT, NWARPS>(xs_raw + win.shift, tap, lane, warp, [&](int i, int comp, float v) {
+        const long long k = kbase + i;
+        if (k < k1) outc[2 * (k & ring_mask) + comp] = v;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -402,35 +446,14 @@ __global__ void fir_ccf_ring_kernel(const float2* __restrict__ in, unsigned in_m
     if (lin) lin[static_cast<long long>(c) * lin_stride + (a - lin_base)] = y;
 }
 
-// Register-tiled form of fir_ccf_ring_kernel (round 2): one CTA = NT * K consecutive outputs of one channel.  The tile's samples
-// (+ ntaps - 1 of history) and the taps sit in shared memory; thread t owns K consecutive outputs and walks the samples oldest
-// first, so every sample is loaded once (one LDS.64) and meets K taps that slide through a register window (one broadcast LDS.32
-// per step): 2 LDS per K ffma2() instead of 2 loads per ffma2().  Per output the accumulation order is the ring kernel's (tap index
-// descending = oldest sample first): results are bit-identical.  Sample index i lives at i + i / 16 (one pad slot per 16): the K-strided
-// LDS.64 of a half-warp then hit distinct bank pairs.
-template <int K, int NT>
-__global__ void __launch_bounds__(NT)
-fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                          float2* __restrict__ out, unsigned out_mask, long long out_stride,
-                          const float* __restrict__ taps, int ntaps, long long a0, long long a1,
-                          float2* __restrict__ lin, long long lin_stride, long long lin_base, int out_interleaved)
+// The per-thread arithmetic of the register-tiled complex ring filter, shared by fir_ccf_ring_tiled_kernel and
+// fsk_fm_frontend_kernel: outputs base .. base + K - 1 of a tile whose samples (ntaps - 1 of history first) sit in xs in the padded
+// layout (index i at i + i / 16), taps in hs.  base must be a multiple of K.
+template <int K>
+__device__ __forceinline__ void ccf_tile_outputs(const float* hs, const float2* xs, int ntaps, int base, float2 (&acc)[K])
 {
-    extern __shared__ __align__(16) float sm_tl[];
-    constexpr int TILE = K * NT;
-    float* hs = sm_tl;                                                    // ntaps floats (rounded up to even)
-    float2* xs = reinterpret_cast<float2*>(sm_tl + ((ntaps + 1) & ~1));   // (TILE + ntaps - 1) samples, padded layout
-    const int c = blockIdx.y;
-    const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
-    if (tile0 >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
-    const int span = TILE + ntaps - 1;
-    for (int i = threadIdx.x; i < span; i += NT) xs[i + (i >> 4)] = x[(tile0 - (ntaps - 1) + i) & in_mask];
-    __syncthreads();
-    float2 acc[K];
 #pragma unroll
     for (int i = 0; i < K; i++) acc[i] = make_float2(0.0f, 0.0f);
-    const int base = K * threadIdx.x;                  // xs index of the oldest sample of my output 0
     // step t meets sample base + t with tap j = i + (ntaps - 1) - t for output i; w[i] holds that tap (slides by one per step)
     float w[K];
 #pragma unroll
@@ -490,6 +513,36 @@ fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long 
 #pragma unroll
         for (int i = u; i < K; i++) ffma2(acc[i], w[i], v);
     }
+}
+
+// Register-tiled form of fir_ccf_ring_kernel (round 2): one CTA = NT * K consecutive outputs of one channel.  The tile's samples
+// (+ ntaps - 1 of history) and the taps sit in shared memory; thread t owns K consecutive outputs and walks the samples oldest
+// first, so every sample is loaded once (one LDS.64) and meets K taps that slide through a register window (one broadcast LDS.32
+// per step): 2 LDS per K ffma2() instead of 2 loads per ffma2().  Per output the accumulation order is the ring kernel's (tap index
+// descending = oldest sample first): results are bit-identical.  Sample index i lives at i + i / 16 (one pad slot per 16): the K-strided
+// LDS.64 of a half-warp then hit distinct bank pairs.
+template <int K, int NT>
+__global__ void __launch_bounds__(NT)
+fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
+                          float2* __restrict__ out, unsigned out_mask, long long out_stride,
+                          const float* __restrict__ taps, int ntaps, long long a0, long long a1,
+                          float2* __restrict__ lin, long long lin_stride, long long lin_base, int out_interleaved)
+{
+    extern __shared__ __align__(16) float sm_tl[];
+    constexpr int TILE = K * NT;
+    float* hs = sm_tl;                                                    // ntaps floats (rounded up to even)
+    float2* xs = reinterpret_cast<float2*>(sm_tl + ((ntaps + 1) & ~1));   // (TILE + ntaps - 1) samples, padded layout
+    const int c = blockIdx.y;
+    const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
+    if (tile0 >= a1) return;
+    const float2* x = in + static_cast<long long>(c) * in_stride;
+    for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
+    const int span = TILE + ntaps - 1;
+    for (int i = threadIdx.x; i < span; i += NT) xs[i + (i >> 4)] = x[(tile0 - (ntaps - 1) + i) & in_mask];
+    __syncthreads();
+    const int base = K * threadIdx.x;                  // xs index of the oldest sample of my output 0
+    float2 acc[K];
+    ccf_tile_outputs<K>(hs, xs, ntaps, base, acc);
 #pragma unroll
     for (int i = 0; i < K; i++) {
         const long long a = tile0 + base + i;
@@ -500,42 +553,23 @@ fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long 
     }
 }
 
-// quadrature_demod_cf + real FIR, register-tiled like the kernel above (K outputs per thread, taps through a register window).
-// The CTA first demodulates its tile + ntaps - 1 of history into shared memory, then filters from there.
-template <int K, int NT>
-__global__ void __launch_bounds__(NT)
-qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                            float* __restrict__ out, unsigned out_mask, long long out_stride,
-                            const float* __restrict__ taps, int ntaps, float gain, long long a0, long long a1)
+// quadrature_demod_cf of one sample: gain * arg(cur conj(prev))
+__device__ __forceinline__ float qdemod_sample(float2 cur, float2 prev, float gain)
 {
-    extern __shared__ __align__(16) float sm_tl[];
-    constexpr int TILE = K * NT;
-    float* hs = sm_tl;                         // ntaps
-    float* ds = sm_tl + ntaps;                 // TILE + ntaps - 1 demodulated samples, index i at i + i / 32
-    const int c = blockIdx.y;
-    const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
-    if (tile0 >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
-    const int span = TILE + ntaps - 1;
-    for (int i = threadIdx.x; i < span; i += NT) {
-        const long long n = tile0 - (ntaps - 1) + i;       // absolute demod index
-        float d = 0.0f;
-        if (n >= 0 && n < a1) {
-            const float2 cur = x[n & in_mask];
-            float2 prev = make_float2(0.0f, 0.0f);
-            if (n >= 1) prev = x[(n - 1) & in_mask];
-            const float re = cur.x * prev.x + cur.y * prev.y;
-            const float im = cur.y * prev.x - cur.x * prev.y;
-            d = gain * qrl_fast_atan2f(im, re);
-        }
-        ds[i + (i >> 5)] = d;
-    }
-    __syncthreads();
-    float acc[K], w[K];
+    const float re = cur.x * prev.x + cur.y * prev.y;
+    const float im = cur.y * prev.x - cur.x * prev.y;
+    return gain * qrl_fast_atan2f(im, re);
+}
+
+// The per-thread arithmetic of the register-tiled real FIR behind the demodulator, shared by qdemod_fir_fff_tiled_kernel and
+// fsk_fm_frontend_kernel: outputs base .. base + K - 1 from demodulated samples in ds (ntaps - 1 of history first, index i at
+// i + i / 32), taps in hs.  base must be a multiple of K.
+template <int K>
+__device__ __forceinline__ void fff_tile_outputs(const float* hs, const float* ds, int ntaps, int base, float (&acc)[K])
+{
+    float w[K];
 #pragma unroll
     for (int i = 0; i < K; i++) { acc[i] = 0.0f; w[i] = 0.0f; }
-    const int base = K * threadIdx.x;
 #pragma unroll
     for (int t = 0; t < K - 1; t++) {
 #pragma unroll
@@ -547,7 +581,7 @@ qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, lon
         for (int i = 0; i <= t; i++) acc[i] = fmaf(w[i], v, acc[i]);
     }
     // (main phase: a few shifting steps, then K steps per iteration with the window rotating through the registers -- see
-    // fir_ccf_ring_tiled_kernel)
+    // ccf_tile_outputs)
     auto shift_steps = [&](int ta, int tb) {
         for (int t = ta; t < tb; t++) {
 #pragma unroll
@@ -584,11 +618,218 @@ qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, lon
 #pragma unroll
         for (int i = u; i < K; i++) acc[i] = fmaf(w[i], v, acc[i]);
     }
+}
+
+// quadrature_demod_cf + real FIR, register-tiled like the kernel above (K outputs per thread, taps through a register window).
+// The CTA first demodulates its tile + ntaps - 1 of history into shared memory, then filters from there.
+template <int K, int NT>
+__global__ void __launch_bounds__(NT)
+qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
+                            float* __restrict__ out, unsigned out_mask, long long out_stride,
+                            const float* __restrict__ taps, int ntaps, float gain, long long a0, long long a1)
+{
+    extern __shared__ __align__(16) float sm_tl[];
+    constexpr int TILE = K * NT;
+    float* hs = sm_tl;                         // ntaps
+    float* ds = sm_tl + ntaps;                 // TILE + ntaps - 1 demodulated samples, index i at i + i / 32
+    const int c = blockIdx.y;
+    const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
+    if (tile0 >= a1) return;
+    const float2* x = in + static_cast<long long>(c) * in_stride;
+    for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
+    const int span = TILE + ntaps - 1;
+    for (int i = threadIdx.x; i < span; i += NT) {
+        const long long n = tile0 - (ntaps - 1) + i;       // absolute demod index
+        float d = 0.0f;
+        if (n >= 0 && n < a1) {
+            float2 prev = make_float2(0.0f, 0.0f);
+            if (n >= 1) prev = x[(n - 1) & in_mask];
+            d = qdemod_sample(x[n & in_mask], prev, gain);
+        }
+        ds[i + (i >> 5)] = d;
+    }
+    __syncthreads();
+    const int base = K * threadIdx.x;
+    float acc[K];
+    fff_tile_outputs<K>(hs, ds, ntaps, base, acc);
 #pragma unroll
     for (int i = 0; i < K; i++) {
         const long long a = tile0 + base + i;
         if (a >= a1) break;
         out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc[i];
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The 4FSK-FM receive front end in one kernel per slice: stage 1 (rational_resampler_ccf(1, D) with the carrier rotator), the
+// channel filter (-> port 0), quadrature_demod_cf and the RRC (-> the symbol sync's channel-interleaved ring) for the stage-1
+// outputs [k0, k1), without the intermediate rings.  One CTA owns a strip of `strip` consecutive outputs of one channel and walks it
+// in chunks of FF_CH stage-1 outputs: the chunk's stage-1 outputs come from NOUT1-output tiles whose windows are bulk-copied two
+// deep (the copy of the next tile runs under this tile's FIR and under the chunk's filters), and the filters run from shared memory,
+// carrying ntaps2 - 1 stage-1 outputs, one channel-filter output and ntaps3 - 1 demodulated samples from chunk to chunk.  Every
+// output meets the same taps in the same order as in fir_decim_poly_kernel -> fir_ccf_ring_tiled_kernel ->
+// qdemod_fir_fff_tiled_kernel (the same device functions): the results are bit-identical.
+//
+// Halo rule: a strip needs the halo = (ntaps3 - 1) + 1 + (ntaps2 - 1) stage-1 outputs before it.  The first strip of a slice reads
+// them from r1, and every strip stores its outputs k >= k1 - halo there, so the next slice (or the next call) finds them; every other
+// strip recomputes its halo from the input.  r1 is zeroed at create and reset: at stream start the halo is zeros, as the ring
+// filters read it.
+// ------------------------------------------------------------------------------------------------
+constexpr int FF_CH = 2048;            // stage-1 outputs per chunk = FF_NT threads x 8 outputs per filter pass
+constexpr int FF_NT = 256;
+
+// shared-memory layout of fsk_fm_frontend_kernel, in floats: two stage-1 windows, the stage-1 outputs (padded: i at i + i / 16), the
+// channel-filter outputs, the demodulated samples (padded: i at i + i / 32), the two tap sets; every part starts 16-byte aligned
+template <int D, int Q, int NOUT1>
+struct FskFrontendSmem {
+    int y1, y2, ds, hs2, hs3, floats;
+    __host__ __device__ FskFrontendSmem(int ntaps2, int ntaps3)
+    {
+        constexpr int WC = FirPolyWindow<D, Q, NOUT1>::WC;
+        const int n1 = ntaps2 - 1 + FF_CH, n3 = ntaps3 - 1 + FF_CH;
+        y1 = 2 * 2 * WC;
+        y2 = y1 + 2 * ((n1 + (n1 >> 4) + 2) & ~1);
+        ds = y2 + 2 * (FF_CH + 2);
+        hs2 = ds + ((n3 + (n3 >> 5) + 4) & ~3);
+        hs3 = hs2 + ((ntaps2 + 3) & ~3);
+        floats = hs3 + ((ntaps3 + 3) & ~3);
+    }
+};
+
+template <int D, int Q, int NOUT1>
+__global__ void __launch_bounds__(FF_NT, 2)
+fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long long T, const float2* __restrict__ hist, int H,
+                       const float* __restrict__ taps1, long long n_in_before, const RotState* __restrict__ rot,
+                       float2* __restrict__ r1, unsigned r1_mask, long long r1_stride,
+                       const float* __restrict__ taps2, int ntaps2, float2* __restrict__ port0, long long port0_stride, long long port0_base,
+                       const float* __restrict__ taps3, int ntaps3, float gain,
+                       float* __restrict__ r4, unsigned r4_mask, long long r4_stride,
+                       long long k0, long long k1, int strip)
+{
+    constexpr int K = 8, NWARPS = FF_NT / 32, TPC = FF_CH / NOUT1;
+    using Win = FirPolyWindow<D, Q, NOUT1>;
+    static_assert(FF_CH == K * FF_NT && FF_CH % NOUT1 == 0, "a chunk is one filter pass and whole stage-1 tiles");
+    extern __shared__ __align__(128) float ff_sm[];
+    __shared__ __align__(8) uint64_t bar[2];
+
+    const int c = blockIdx.y;
+    const long long a = k0 + static_cast<long long>(blockIdx.x) * strip;
+    if (a >= k1) return;
+    const long long b = a + strip < k1 ? a + strip : k1;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int G2 = ntaps2 - 1, G3 = ntaps3 - 1, halo = G3 + 1 + G2;
+    const long long v0 = a - halo;                            // first stage-1 output of the strip's stream (chunk 0 starts here)
+    const long long keep_from = a > k1 - halo ? a : k1 - halo;
+    const bool first = blockIdx.x == 0;
+
+    const FskFrontendSmem<D, Q, NOUT1> L(ntaps2, ntaps3);
+    float2* const win0 = reinterpret_cast<float2*>(ff_sm);   // window of stage-1 tile t at win0 + (t & 1) WC
+    float2* y1 = reinterpret_cast<float2*>(ff_sm + L.y1);    // stage-1 output u0 - G2 + l at l + l / 16
+    float2* y2 = reinterpret_cast<float2*>(ff_sm + L.y2);    // channel-filter output u0 - 1 + l at l
+    float* ds = ff_sm + L.ds;                                  // demodulated sample u0 - G3 + l at l + l / 32
+    float* hs2 = ff_sm + L.hs2;
+    float* hs3 = ff_sm + L.hs3;
+
+    float tap[FirPolyShape<D, Q>::R][Q];
+    fir_poly_load_taps<D, Q>(taps1, lane, tap);
+    for (int i = threadIdx.x; i < ntaps2; i += FF_NT) hs2[i] = taps2[i];
+    for (int i = threadIdx.x; i < ntaps3; i += FF_NT) hs3[i] = taps3[i];
+    // chunk 0 starts without carried history: what it reads there only reaches outputs before the strip, which are not stored
+    for (int l = threadIdx.x; l < G2; l += FF_NT) y1[l + (l >> 4)] = make_float2(0.0f, 0.0f);
+    for (int l = threadIdx.x; l < G3; l += FF_NT) ds[l + (l >> 5)] = 0.0f;
+    if (threadIdx.x == 0) y2[0] = make_float2(0.0f, 0.0f);
+    const float2* r1c = r1 + static_cast<long long>(c) * r1_stride;
+    if (first) {
+        for (int l = threadIdx.x; l < halo; l += FF_NT) {
+            const int li = G2 + l;
+            y1[li + (li >> 4)] = r1c[(v0 + l) & r1_mask];
+        }
+    }
+    if (threadIdx.x == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); mbar_fence_init(); }
+    __syncthreads();
+
+    const float2* iqc = iq + static_cast<long long>(c) * iq_stride;
+    const float2* hc = hist + static_cast<long long>(c) * H;
+    const RotState rs = rot ? rot[c] : RotState{ 0u, 0u, 0 };
+    const int t_lo = first ? halo / NOUT1 : 0;                 // the first strip takes its halo tiles from r1
+    const int t_hi = static_cast<int>((b - v0 + NOUT1 - 1) / NOUT1);
+    auto prefetch = [&](int t) {                              // thread 0, window t & 1 free
+        if (t >= t_hi) return;
+        const Win w(iq, iq_stride, T, n_in_before, v0 + static_cast<long long>(NOUT1) * t);
+        if (w.bulk) { fence_proxy_async(); w.issue(win0 + (t & 1) * Win::WC, iqc, &bar[t & 1]); }
+    };
+    if (threadIdx.x == 0) { prefetch(t_lo); prefetch(t_lo + 1); }
+    unsigned parity = 0;                                       // bit s: phase of the next completion of bar[s]
+    float2* r1w = r1 + static_cast<long long>(c) * r1_stride;
+
+    int t = t_lo;
+    for (long long u0 = v0; u0 < b; u0 += FF_CH) {
+        // ---- stage 1: the chunk's outputs [u0, u0 + FF_CH) -> y1 (and the slice's last `halo` of them -> r1)
+        const int t_end = min(t_hi, static_cast<int>((u0 - v0) / NOUT1) + TPC);
+        for (; t < t_end; t++) {
+            const long long kbase = v0 + static_cast<long long>(NOUT1) * t;
+            const Win w(iq, iq_stride, T, n_in_before, kbase);
+            float2* xw = win0 + (t & 1) * Win::WC;
+            if (w.bulk) {
+                mbar_wait(&bar[t & 1], (parity >> (t & 1)) & 1u);
+                parity ^= 1u << (t & 1);
+            } else {
+                w.fill(xw, iqc, T, hc, H, FF_NT);
+                __syncthreads();
+            }
+            if (rot) {
+                w.rotate(xw, rs, T, n_in_before, FF_NT);
+                __syncthreads();
+            }
+            fir_poly_tile<D, Q, K, NOUT1, NWARPS>(xw + w.shift, tap, lane, warp, [&](int i, int comp, float v) {
+                const long long k = kbase + i;
+                if (k >= b || (first && k < a)) return;
+                const int li = G2 + static_cast<int>(k - u0);
+                reinterpret_cast<float*>(y1 + li + (li >> 4))[comp] = v;
+                if (k >= keep_from) reinterpret_cast<float*>(r1w + (k & r1_mask))[comp] = v;
+            });
+            __syncthreads();                                   // window t & 1 consumed
+            if (threadIdx.x == 0) prefetch(t + 2);
+        }
+        const int base = K * threadIdx.x;
+        // ---- channel filter: outputs [u0, u0 + FF_CH) -> y2, and port 0 for the strip's own
+        {
+            float2 acc[K];
+            ccf_tile_outputs<K>(hs2, y1, ntaps2, base, acc);
+            float2* p0 = port0 + static_cast<long long>(c) * port0_stride - port0_base;
+#pragma unroll
+            for (int i = 0; i < K; i++) {
+                y2[1 + base + i] = acc[i];
+                const long long n = u0 + base + i;
+                if (n >= a && n < b) p0[n] = acc[i];
+            }
+        }
+        __syncthreads();
+        // ---- quadrature_demod_cf: 0 before stream index 0, the previous sample of index 0 is 0
+        for (int m = threadIdx.x; m < FF_CH; m += FF_NT) {
+            const long long n = u0 + m;
+            float d = 0.0f;
+            if (n >= 0) d = qdemod_sample(y2[m + 1], n >= 1 ? y2[m] : make_float2(0.0f, 0.0f), gain);
+            const int li = G3 + m;
+            ds[li + (li >> 5)] = d;
+        }
+        __syncthreads();
+        // ---- RRC: outputs [u0, u0 + FF_CH) -> r4 for the strip's own
+        {
+            float acc[K];
+            fff_tile_outputs<K>(hs3, ds, ntaps3, base, acc);
+#pragma unroll
+            for (int i = 0; i < K; i++) {
+                const long long n = u0 + base + i;
+                if (n >= a && n < b) r4[(static_cast<long long>(c >> 5) * r4_stride + (n & r4_mask)) * 32 + (c & 31)] = acc[i];
+            }
+        }
+        __syncthreads();
+        // ---- carry the filters' history into the next chunk
+        for (int l = threadIdx.x; l < G2; l += FF_NT) { const int sl = FF_CH + l; y1[l + (l >> 4)] = y1[sl + (sl >> 4)]; }
+        for (int l = threadIdx.x; l < G3; l += FF_NT) { const int sl = FF_CH + l; ds[l + (l >> 5)] = ds[sl + (sl >> 5)]; }
+        if (threadIdx.x == 0) y2[0] = y2[FF_CH];
+        __syncthreads();
     }
 }
 
