@@ -506,10 +506,10 @@ int launch_fsk_frontend(qrl_rx* h, const Slice& s)
     const size_t smem = sizeof(float) * FskFrontendSmem<D, Q, NOUT1>(h->ntaps2, h->ntaps3).floats;
     auto kern = fsk_fm_frontend_kernel<D, Q, NOUT1>;
     if (int rc = smem_opt_in(h, kern, 120 * 1024)) return rc;
-    dim3 g(static_cast<unsigned>((s.n_new + strip - 1) / strip), h->C);
+    const unsigned g = static_cast<unsigned>((s.n_new + strip - 1) / strip * h->C);     // strip-major, channel fastest
     kern<<<g, FF_NT, smem, s.sp>>>(s.x, s.xstride, s.T, s.hist, h->H, h->d_taps1, s.n_in0, h->rot_fused ? h->d_rot : nullptr,
         static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->d_taps2, h->ntaps2, h->d_port0, h->port0_cap, s.k_call0,
-        h->d_taps3, h->ntaps3, h->qd_gain, static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, s.k0, s.k1, strip);
+        h->d_taps3, h->ntaps3, h->qd_gain, static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, s.k0, s.k1, strip, h->C);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;

@@ -704,7 +704,7 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
                        const float* __restrict__ taps2, int ntaps2, float2* __restrict__ port0, long long port0_stride, long long port0_base,
                        const float* __restrict__ taps3, int ntaps3, float gain,
                        float* __restrict__ r4, unsigned r4_mask, long long r4_stride,
-                       long long k0, long long k1, int strip)
+                       long long k0, long long k1, int strip, int C)
 {
     constexpr int K = 8, NWARPS = FF_NT / 32, TPC = FF_CH / NOUT1;
     using Win = FirPolyWindow<D, Q, NOUT1>;
@@ -712,15 +712,20 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
     extern __shared__ __align__(128) float ff_sm[];
     __shared__ __align__(8) uint64_t bar[2];
 
-    const int c = blockIdx.y;
-    const long long a = k0 + static_cast<long long>(blockIdx.x) * strip;
+    // block j * C + c: strip j of channel c.  The channel runs fastest, so the CTAs in flight cover every channel at the same strips,
+    // and the 32 channels that share a 128-byte line of r4 write it within a short time, while it is still in L2.  In channel-major
+    // order the writes to one line arrive up to a wave apart, after the input stream has moved through L2, and the kernel takes
+    // 5 % longer per call; with the filters skipped the two orders time the same (DESIGN §6).
+    const int c = static_cast<int>(blockIdx.x % C);
+    const long long j = blockIdx.x / C;
+    const long long a = k0 + j * strip;
     if (a >= k1) return;
     const long long b = a + strip < k1 ? a + strip : k1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G2 = ntaps2 - 1, G3 = ntaps3 - 1, halo = G3 + 1 + G2;
     const long long v0 = a - halo;                            // first stage-1 output of the strip's stream (chunk 0 starts here)
     const long long keep_from = a > k1 - halo ? a : k1 - halo;
-    const bool first = blockIdx.x == 0;
+    const bool first = j == 0;
 
     const FskFrontendSmem<D, Q, NOUT1> L(ntaps2, ntaps3);
     float2* const win0 = reinterpret_cast<float2*>(ff_sm);   // window of stage-1 tile t at win0 + (t & 1) WC
