@@ -533,6 +533,70 @@ int  qrl_dmr_rx_reset(qrl_dmr_rx*, int channel);
 int  qrl_dmr_rx_sync(qrl_dmr_rx*);
 long qrl_dmr_rx_launch_count(qrl_dmr_rx*);
 
+/* ---- DMR burst encoder (qrl_dmr.cu): DMRControl's transmit side (/root/reference/src/DMR/dmrcontrol.cpp:19-223) as gr_modem drives
+ * it (src/gr_modem.cpp:676-678 startTransmission's CSBK, 710-717 endTransmission, 747-764 transmitDMRHeader, 766-802 transmitDMR),
+ * the burst encoders behind DMRFrame (src/DMR/dmrframe.cpp:20-34, 88-96, 399-421, 460-501) and gr_dmr_source's framing
+ * (src/gr/gr_dmr_source.cpp:58-126), for a batch of channels.
+ * Settings (qrl_dmr_tx_set_config, channel -1 = all; QRL_EINVAL for a value out of range): colour code 0-15, timeslot 1 or 2, 24-bit
+ * source and destination IDs, private_call (0: FLCO_GROUP, 1: FLCO_USER_USER, from dmr_call_type), codec2 (FID 0xC2 on the voice LC:
+ * !Settings::dmr_vocoder, dmrcontrol.cpp:29-31, 85-86) and up to 27 talker-alias bytes (the UTF-8 prefix DMRControl copies into _ta_tx,
+ * dmrcontrol.cpp:33-35, 49-51; zero padded).  They take effect where the reference reads them: every CSBK, header and terminator op
+ * reads colour code, slot, IDs and call type, every voice burst colour code and slot (dmrcontrol.cpp:87-89, 104-110, 122-127, 147-148);
+ * the header op snapshots the voice LC, _FLCO_TX and the embedded LC (getVoiceHeader, :80-86) and the talker alias (initVoiceTX,
+ * :44-52); create and reset snapshot all of them (the constructor, :19-36).  qrl_dmr_tx_create starts every channel in the constructor
+ * state of the default config (colour code 1, slot 1, source 1, destination 9, group call, codec2 = 1, no alias: settings.cpp:85-94);
+ * qrl_dmr_tx_reset(channel, -1 = all) puts a channel into the constructor state of the config in force, byte position 0.
+ * Work: ops [n_channels][K] and audio [n_channels][K][9] (one 9-byte vocoder frame per op), K <= max_ops (QRL_ERANGE otherwise); host
+ * arrays, or device arrays with on_device = 1.  One op is one call of the reference:
+ *   0 none (so is any value above 4);
+ *   1 CSBK: getStartCSBK, 3 CSBK bursts (CSBKO_BSDWNACT with LB set, CBF 0, data1 0, src, dst; CRC-CCITT ^ 0xA5A5, BPTC(196,96));
+ *   2 voice header: getVoiceHeader, 2 LC header bursts (RS(12,9) ^ 0x969696, BPTC), then initVoiceTX (FN 0, superframe 0, active);
+ *   3 audio: transmitDMR with the op's vocoder frame.  Dropped while idle.  Otherwise the frame joins the pending ones; at three,
+ *     getTxAudio makes either one voice burst (FN 0: voice sync; FN 1-5: EMB + embedded-LC fragment) or, when ending at FN 0, the
+ *     terminator, the terminator again and two empty frames; FN runs 0-5, the superframe 0-4, superframes 1-4 carry the talker-alias LCs;
+ *   4 stop: stopVoiceTX, no burst; it sets the ending state even from idle, as the reference does.
+ * Output, valid until the next work call: bytes [n_channels][stride = max_ops * 4 * 72], every burst its 33 frame bytes then 39 zero
+ * bytes as gr_dmr_source::set_data appends them, counts in bytes -- with equal counts on every channel, the input of
+ * qrl_tx_work(QRL_MOD_DMR, ..., on_device = 1) as it stands; and per channel up to max_ops * 4 records of QRL_DMR_TX_RECORD_BYTES (16):
+ *    0 int64  position of the burst's first byte in the channel's byte stream since create / reset
+ *    8 u8     slot number the frame carries (the configured slot; 0 for the two empty frames): gr_dmr_source's get_slot_times argument
+ *    9 u8     kind: 1 CSBK, 2 LC header, 3 voice sync (FN 0), 4 voice (FN 1-5), 5 terminator with LC, 6 empty
+ *   10 u8     FN, 11 u8 LCSS of the embedded fragment (FN 1: 1, FN 2-3: 3, FN 4: 2, otherwise 0)
+ *   12 int32  index of the op (within the call) that produced the burst
+ * An adapter attaches gr_dmr_source's tags from a record: tx_time on byte `position` (DMRTiming::get_slot_times(slot) on the host) and
+ * zero_samples on byte position + 33 with 780 samples (qrl_tx_zero_samples).  All syncs are the MS-sourced words (duplex = false).
+ * Where the reference is undefined or accidental, this is the definition:
+ *   - DMRFrame(uint8_t) leaves _data_type uninitialised, so transmitDMR's DT_TERMINATOR_WITH_LC test reads garbage for a voice frame:
+ *     here a voice burst is never a terminator;
+ *   - the two empty frames are 33 zero bytes with slot 0;
+ *   - the terminator is a fresh CDMRLC(_FLCO_TX, src, dst): FID 0 even for codec2 (getVoiceTerminator, :120-128);
+ *   - FN 5 carries CDMREmbeddedData::getData's null fragment, LCSS 0;
+ *   - up to two pending vocoder frames carry across calls; a terminator drops them (clearTxAudio), a new header does not.
+ * State (counters, snapshots, pending frames, byte position) carries across calls. */
+#define QRL_DMR_TX_RECORD_BYTES 16
+typedef struct qrl_dmr_tx_config {
+    int color_code;                  /* 0-15 */
+    int timeslot;                    /* 1 or 2 */
+    unsigned src_id, dst_id;         /* 24 bit */
+    int private_call;                /* 0: FLCO_GROUP, 1: FLCO_USER_USER */
+    int codec2;                      /* 1: FID 0xC2 on the voice LC (Settings::dmr_vocoder == 0) */
+    int talker_alias_len;            /* 0-27 */
+    unsigned char talker_alias[28];  /* the first talker_alias_len bytes are used */
+} qrl_dmr_tx_config;
+typedef struct qrl_dmr_tx qrl_dmr_tx;
+int  qrl_dmr_tx_create(int n_channels, int max_ops, int device, qrl_dmr_tx** out);
+int  qrl_dmr_tx_destroy(qrl_dmr_tx*);
+int  qrl_dmr_tx_set_stream(qrl_dmr_tx*, void* cuda_stream);
+int  qrl_dmr_tx_set_config(qrl_dmr_tx*, int channel, const qrl_dmr_tx_config* cfg);
+int  qrl_dmr_tx_reset(qrl_dmr_tx*, int channel);
+int  qrl_dmr_tx_work(qrl_dmr_tx*, const unsigned char* ops, const unsigned char* audio, int K, int on_device);
+/* bytes_host [n_channels][cap] (may be NULL), records_host [n_channels][max_ops * 4][16] (may be NULL), counts_host [n_channels]
+ * (bytes; records = counts / 72); synchronises */
+int  qrl_dmr_tx_read(qrl_dmr_tx*, unsigned char* bytes_host, long cap, unsigned char* records_host, int* counts_host);
+int  qrl_dmr_tx_out_device(qrl_dmr_tx*, void** bytes, long* stride, int** counts, void** records);
+int  qrl_dmr_tx_sync(qrl_dmr_tx*);
+long qrl_dmr_tx_launch_count(qrl_dmr_tx*);
+
 /* ---- stand-alone kernels exposed for tests / micro-benchmarks ---- */
 /* batched decimating FIR (stage 1 alone): x [C][T] device, y [C][ceil(T/D)] device; zero history */
 int qrl_fir_decim_ccf_device(const float* taps, int ntaps, int D, const float* x_dev, long T, long x_stride,

@@ -18,4 +18,4 @@ from .frontend import Frontend, TxCombiner, TxFrontend  # noqa: F401
 from .spectrum import Spectrum  # noqa: F401
 from .mmdvm import MmdvmDemod, MmdvmMod, MmdvmChannelsRx, MmdvmChannelsTx, mmdvm_tag_item  # noqa: F401
 from .m17 import M17Decoder, M17Encoder, m17_lsf, m17_callsign, m17_crc16  # noqa: F401
-from .dmr import DmrBurstDecoder, DMR_RECORD  # noqa: F401
+from .dmr import DmrBurstDecoder, DMR_RECORD, DmrBurstEncoder, DMR_TX_RECORD, dmr_tx_config  # noqa: F401

@@ -256,17 +256,24 @@ __device__ __forceinline__ uint32_t gf_mul(uint32_t a, uint32_t b)
     return r & 0xFFu;
 }
 
-// CRS129::check on 9 data bytes + 3 parity bytes
-__device__ bool rs129_ok(const unsigned char* m)
+// CRS129::encode of 9 data bytes: par[2], par[1], par[0] are the parity bytes 9, 10, 11 of the codeword
+__device__ void rs129_parity(const unsigned char* m, uint32_t* par)
 {
     const uint32_t G[3] = { 64, 56, 14 };
-    uint32_t par[3] = { 0, 0, 0 };
+    par[0] = par[1] = par[2] = 0;
     for (int i = 0; i < 9; i++) {
         const uint32_t d = m[i] ^ par[2];
         par[2] = par[1] ^ gf_mul(G[2], d);
         par[1] = par[0] ^ gf_mul(G[1], d);
         par[0] = gf_mul(G[0], d);
     }
+}
+
+// CRS129::check on 9 data bytes + 3 parity bytes
+__device__ bool rs129_ok(const unsigned char* m)
+{
+    uint32_t par[3];
+    rs129_parity(m, par);
     return m[9] == par[2] && m[10] == par[1] && m[11] == par[0];
 }
 
@@ -603,6 +610,269 @@ dmr_decode_kernel(int C, int max_bursts, const int* __restrict__ counts, unsigne
     }
 }
 
+// ================================================================================================ transmit
+// DMRControl's transmit state machine as gr_modem drives it, and the burst encoders behind DMRFrame (see qrl_b200.h, qrl_dmr_tx_*).
+constexpr int kTxBurst = 72;                 // gr_dmr_source: 33 frame bytes + 39 zero bytes
+constexpr int kTxRec = QRL_DMR_TX_RECORD_BYTES;
+enum { TX_IDLE = 0, TX_ACTIVE = 1, TX_ENDING = 2 };
+enum { OPX_NONE = 0, OPX_CSBK = 1, OPX_HEADER = 2, OPX_AUDIO = 3, OPX_STOP = 4 };
+enum { BK_CSBK = 1, BK_LC_HEADER = 2, BK_VOICE_SYNC = 3, BK_VOICE = 4, BK_TERMINATOR = 5, BK_EMPTY = 6 };
+
+struct DmrTxCfg {                            // the Settings fields DMRControl reads, per channel
+    unsigned char cc, slot, flco, fid;       // fid: 0xC2 when the voice is codec2 (!dmr_vocoder)
+    uint32_t src, dst;
+    unsigned char ta[27];                    // talker alias, zero padded
+};
+struct DmrTxState {                          // DMRControl's transmit members, plus the byte position of gr_dmr_source's stream
+    long long pos;
+    unsigned char state, fn, sf, npend, flco_tx;
+    unsigned char lc_tx[9], emb_lc[9], ta[27];
+    unsigned char pend[18];                  // _tx_frames: up to two 9-byte vocoder frames wait for a third
+};
+struct DmrTxBurst {                          // what the encode warp needs beyond the channel's settings
+    unsigned char kind, fn, lcss, cc;
+    unsigned char lc[9];                     // LC header / terminator: the full LC; voice FN 1-4: the embedded LC
+    unsigned char pad[3];
+    int audio[3];                            // the three vocoder frames: op index of this call (>= 0) or carried frame -1 - j
+};
+struct DmrTxRecord { long long pos; unsigned char slot, kind, fn, lcss; int op; };
+static_assert(sizeof(DmrTxRecord) == kTxRec, "record layout");
+
+__host__ __device__ inline void lc_bytes(unsigned char* o, uint32_t flco, uint32_t fid, uint32_t options, uint32_t src, uint32_t dst)
+{
+    o[0] = static_cast<unsigned char>(flco & 0x3Fu); o[1] = static_cast<unsigned char>(fid); o[2] = static_cast<unsigned char>(options);
+    o[3] = static_cast<unsigned char>(dst >> 16); o[4] = static_cast<unsigned char>(dst >> 8); o[5] = static_cast<unsigned char>(dst);
+    o[6] = static_cast<unsigned char>(src >> 16); o[7] = static_cast<unsigned char>(src >> 8); o[8] = static_cast<unsigned char>(src);
+}
+
+// DMRControl's constructor with the channel's settings in force; channel < 0 = every channel
+__global__ void dmr_tx_reset_kernel(int C, int channel, const DmrTxCfg* __restrict__ cfgs, DmrTxState* __restrict__ states)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C || (channel >= 0 && c != channel)) return;
+    const DmrTxCfg g = cfgs[c];
+    DmrTxState s = {};
+    s.flco_tx = g.flco;
+    lc_bytes(s.lc_tx, g.flco, g.fid, 0, g.src, g.dst);
+    for (int i = 0; i < 9; i++) s.emb_lc[i] = s.lc_tx[i];
+    for (int i = 0; i < 27; i++) s.ta[i] = g.ta[i];
+    states[c] = s;
+}
+
+// one thread per channel, in op order: the state machine of DMRControl (dmrcontrol.cpp:44-223) under gr_modem's calls
+// (gr_modem.cpp:676-678, 710-717, 747-802).  Writes a descriptor and a record per burst and the channel's byte count; the vocoder
+// frames still waiting at the end of the call are copied into the state, the ones carried in are left in `prev` for the encoder.
+__global__ void dmr_tx_scan_kernel(int C, int K, const unsigned char* __restrict__ ops, const unsigned char* __restrict__ audio,
+                                   const DmrTxCfg* __restrict__ cfgs, DmrTxState* __restrict__ states, unsigned char* __restrict__ prev,
+                                   DmrTxBurst* __restrict__ bursts, unsigned char* __restrict__ recs, int max_bursts, int* __restrict__ counts)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const DmrTxCfg g = cfgs[c];
+    DmrTxState s = states[c];
+    for (int i = 0; i < 18; i++) prev[static_cast<long long>(c) * 18 + i] = s.pend[i];
+    int psrc[3] = { -1, -2, 0 };
+    int nb = 0;
+    DmrTxBurst* bo = bursts + static_cast<long long>(c) * max_bursts;
+    DmrTxRecord* ro = reinterpret_cast<DmrTxRecord*>(recs) + static_cast<long long>(c) * max_bursts;
+    auto emit = [&](int kind, int slot, int fn, int lcss, const unsigned char* lc, int k) {
+        DmrTxBurst d = {};
+        d.kind = static_cast<unsigned char>(kind); d.fn = static_cast<unsigned char>(fn); d.lcss = static_cast<unsigned char>(lcss);
+        d.cc = g.cc;
+        if (lc)
+            for (int i = 0; i < 9; i++) d.lc[i] = lc[i];
+        for (int j = 0; j < 3; j++) d.audio[j] = psrc[j];
+        bo[nb] = d;
+        DmrTxRecord r;
+        r.pos = s.pos; r.slot = static_cast<unsigned char>(slot); r.kind = d.kind; r.fn = d.fn; r.lcss = d.lcss; r.op = k;
+        ro[nb] = r;
+        s.pos += kTxBurst;
+        nb++;
+    };
+    for (int k = 0; k < K; k++) {
+        const int op = ops[static_cast<long long>(c) * K + k];
+        if (op == OPX_CSBK) {                                       // getStartCSBK: three CSBK frames
+            for (int i = 0; i < 3; i++) emit(BK_CSBK, g.slot, 0, 0, nullptr, k);
+        } else if (op == OPX_HEADER) {                              // getVoiceHeader (LC snapshot, two frames), initVoiceTX
+            s.flco_tx = g.flco;
+            lc_bytes(s.lc_tx, g.flco, g.fid, 0, g.src, g.dst);
+            for (int i = 0; i < 9; i++) s.emb_lc[i] = s.lc_tx[i];
+            for (int i = 0; i < 2; i++) emit(BK_LC_HEADER, g.slot, 0, 0, s.lc_tx, k);
+            s.fn = 0; s.sf = 0; s.state = TX_ACTIVE;
+            for (int i = 0; i < 27; i++) s.ta[i] = g.ta[i];
+        } else if (op == OPX_STOP) {                                // stopVoiceTX, from any state
+            s.state = TX_ENDING;
+        } else if (op == OPX_AUDIO && s.state != TX_IDLE) {         // transmitDMR: addTxAudio, then getTxAudio at three frames
+            psrc[s.npend++] = k;
+            if (s.npend < 3) continue;
+            if (s.state == TX_ENDING && s.fn == 0) {                // the terminator twice, two empty frames; clearTxAudio
+                unsigned char lc[9];
+                lc_bytes(lc, s.flco_tx, 0, 0, g.src, g.dst);
+                emit(BK_TERMINATOR, g.slot, 0, 0, lc, k);
+                emit(BK_TERMINATOR, g.slot, 0, 0, lc, k);
+                emit(BK_EMPTY, 0, 0, 0, nullptr, k);
+                emit(BK_EMPTY, 0, 0, 0, nullptr, k);
+                s.npend = 0; s.state = TX_IDLE; s.sf = 0;
+                continue;
+            }
+            const int fn = s.fn;
+            emit(fn == 0 ? BK_VOICE_SYNC : BK_VOICE, g.slot, fn, fn == 1 ? 1 : fn == 4 ? 2 : (fn == 2 || fn == 3) ? 3 : 0, s.emb_lc, k);
+            s.npend = 0;
+            if (++s.fn > 5) {                                       // superframe: the voice LC, then the talker-alias LCs
+                s.fn = 0;
+                s.sf = s.sf >= 4 ? 0 : s.sf + 1;
+                if (s.sf == 0) {
+                    for (int i = 0; i < 9; i++) s.emb_lc[i] = s.lc_tx[i];
+                } else {
+                    const int i = (s.sf - 1) * 6;
+                    const uint32_t flco = 3u + s.sf;
+                    const unsigned char* t = s.ta;
+                    if (s.sf == 1)
+                        lc_bytes(s.emb_lc, flco, 0, (1u << 6) | (0x1Bu << 1), static_cast<uint32_t>(t[i + 3]) << 16 | t[i + 4] << 8 | t[i + 5],
+                                 static_cast<uint32_t>(t[i]) << 16 | t[i + 1] << 8 | t[i + 2]);
+                    else
+                        lc_bytes(s.emb_lc, flco, 0, t[i], static_cast<uint32_t>(t[i + 4]) << 16 | t[i + 5] << 8 | t[i + 6],
+                                 static_cast<uint32_t>(t[i + 1]) << 16 | t[i + 2] << 8 | t[i + 3]);
+                }
+            }
+        }
+    }
+    // the frames still waiting: from this call's audio or carried in
+    unsigned char pend[18];
+    for (int j = 0; j < s.npend; j++)
+        for (int i = 0; i < 9; i++)
+            pend[9 * j + i] = psrc[j] >= 0 ? audio[(static_cast<long long>(c) * K + psrc[j]) * 9 + i] : s.pend[9 * (-1 - psrc[j]) + i];
+    for (int i = 0; i < 9 * s.npend; i++) s.pend[i] = pend[i];
+    states[c] = s;
+    counts[c] = nb * kTxBurst;
+}
+
+// Hamming(16,11,4) of a row of the embedded LC: the (15,11) checks of the BPTC rows plus overall parity (CHamming::encode16114)
+__device__ __forceinline__ void ham16_encode(unsigned char* d)
+{
+    const uint32_t p = ham15_parity(d);
+    uint32_t all = 0;
+    for (int k = 0; k < 4; k++) { d[11 + k] = (p >> k) & 1u; all ^= (p >> k) & 1u; }
+    for (int i = 0; i < 11; i++) all ^= d[i];
+    d[15] = static_cast<unsigned char>(all);
+}
+
+// one warp per burst (S warps share a channel's bursts): 33 frame bytes + 39 zero bytes at the burst's place in the stream
+__global__ void __launch_bounds__(128)
+dmr_tx_encode_kernel(int C, int K, int S, const unsigned char* __restrict__ audio, const unsigned char* __restrict__ prev,
+                     const DmrTxCfg* __restrict__ cfgs, const DmrTxBurst* __restrict__ bursts, int max_bursts, const int* __restrict__ counts,
+                     unsigned char* __restrict__ out, long long stride)
+{
+    __shared__ unsigned char s_fb[4][264];
+    __shared__ unsigned char s_d[4][196];
+    __shared__ unsigned char s_pl[4][28];
+    __shared__ unsigned char s_emb[4][128];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long gw = static_cast<long long>(blockIdx.x) * 4 + w;
+    const int c = static_cast<int>(gw / S), s0 = static_cast<int>(gw % S);
+    if (c >= C) return;
+    const int nb = counts[c] / kTxBurst;
+    unsigned char* fb = s_fb[w];
+    unsigned char* pl = s_pl[w];
+    for (int b = s0; b < nb; b += S) {
+        const DmrTxBurst d = bursts[static_cast<long long>(c) * max_bursts + b];
+        uint32_t* o = reinterpret_cast<uint32_t*>(out + static_cast<long long>(c) * stride + static_cast<long long>(b) * kTxBurst);
+        if (d.kind == BK_EMPTY) {                                   // DMRFrame(DMRFrameTypeData): 33 zero bytes
+            if (lane < kTxBurst / 4) o[lane] = 0;
+            continue;
+        }
+        if (d.kind == BK_CSBK || d.kind == BK_LC_HEADER || d.kind == BK_TERMINATOR) {
+            const uint32_t dt = d.kind == BK_CSBK ? DT_CSBK : d.kind == BK_LC_HEADER ? DT_VOICE_LC_HEADER : DT_TERMINATOR_WITH_LC;
+            if (lane == 0) {
+                if (d.kind == BK_CSBK) {                            // CDMRCSBK::get: BSDWNACT with LB, FID / data1 / CBF 0, CRC ^ 0xA5A5
+                    const DmrTxCfg& g = cfgs[c];
+                    lc_bytes(pl + 1, 0, 0, 0, g.src, g.dst);            // dst at 4-6, src at 7-9
+                    pl[0] = 0x80u | 0x38u;
+                    const uint32_t crc = crc_ccitt(pl, 10);
+                    pl[10] = static_cast<unsigned char>((crc >> 8) ^ 0xA5u); pl[11] = static_cast<unsigned char>((crc & 0xFFu) ^ 0xA5u);
+                } else {                                            // CDMRFullLC::encode: RS(12,9) parity ^ the type's mask
+                    const unsigned char m = d.kind == BK_LC_HEADER ? 0x96 : 0x99;
+                    for (int i = 0; i < 9; i++) pl[i] = d.lc[i];
+                    uint32_t par[3];
+                    rs129_parity(pl, par);
+                    pl[9] = static_cast<unsigned char>(par[2] ^ m); pl[10] = static_cast<unsigned char>(par[1] ^ m);
+                    pl[11] = static_cast<unsigned char>(par[0] ^ m);
+                }
+            }
+            __syncwarp();
+            bptc_encode(pl, s_d[w], fb, lane);
+            // CDMRSlotType::getData (Golay(20,8) of colour code and data type) and CSync::addDMRDataSync (MS sourced)
+            const uint32_t st = (static_cast<uint32_t>(d.cc) << 4) | dt, w20 = (st << 12) | golay_check(st);
+            for (int i = lane; i < 68; i += 32) {
+                if (i < 20) fb[i < 10 ? 98 + i : 146 + i] = static_cast<unsigned char>((w20 >> (19 - i)) & 1u);
+                else fb[88 + i] = static_cast<unsigned char>((kMsData >> (67 - i)) & 1u);
+            }
+        } else {                                                    // voice: setVoice, then the sync or the EMB + embedded fragment
+            if (lane < 27) {
+                const int src = d.audio[lane / 9];
+                pl[lane] = src >= 0 ? audio[(static_cast<long long>(c) * K + src) * 9 + lane % 9]
+                                    : prev[static_cast<long long>(c) * 18 + 9 * (-1 - src) + lane % 9];
+            }
+            __syncwarp();
+            for (int i = lane; i < 216; i += 32) fb[i < 108 ? i : i + 48] = (pl[i >> 3] >> (7 - (i & 7))) & 1u;
+            if (d.fn == 0) {
+                for (int i = lane; i < 48; i += 32) fb[108 + i] = static_cast<unsigned char>((kMsVoice >> (47 - i)) & 1u);
+            } else {
+                unsigned char* e = s_emb[w];
+                if (d.fn <= 4) {
+                    // CDMREmbeddedData::encodeEmbeddedData: the 72 LC bits in rows of 11 / 10, the 5-bit checksum (sum of the bytes
+                    // mod 31) in column 10 of rows 2-6, Hamming(16,11,4) rows, column parity in row 7
+                    uint32_t sum = 0;
+                    for (int i = 0; i < 9; i++) sum += d.lc[i];
+                    const uint32_t crc = sum % 31u;
+                    for (int a = lane; a < 128; a += 32) {
+                        const int r = a >> 4, col = a & 15;
+                        int j = -1;
+                        uint32_t v = 0;
+                        if (r < 2 && col < 11) j = 11 * r + col;
+                        else if (r >= 2 && r < 7 && col < 10) j = 22 + 10 * (r - 2) + col;
+                        else if (r >= 2 && r < 7 && col == 10) v = (crc >> (6 - r)) & 1u;
+                        if (j >= 0) v = (d.lc[j >> 3] >> (7 - (j & 7))) & 1u;
+                        e[a] = static_cast<unsigned char>(v);
+                    }
+                    __syncwarp();
+                    if (lane < 7) ham16_encode(e + 16 * lane);
+                    __syncwarp();
+                    if (lane < 16) {
+                        uint32_t p = 0;
+                        for (int r = 0; r < 7; r++) p ^= e[16 * r + lane];
+                        e[112 + lane] = static_cast<unsigned char>(p);
+                    }
+                    __syncwarp();
+                    // packed downwards in columns: raw bit a is data bit 16 a mod 127 (bit 127 stays); fragment FN - 1 of 32 bits
+                    const int a = 32 * (d.fn - 1) + lane;
+                    fb[116 + lane] = e[a == 127 ? 127 : (16 * a) % 127];
+                } else {
+                    fb[116 + lane] = 0;                             // FN 5: CDMREmbeddedData::getData's null fragment
+                }
+                // CDMREMB::getData: QR(16,7) of colour code, PI 0, LCSS = the (15,7) QR code (g = 0x139) plus overall parity
+                const uint32_t v = (static_cast<uint32_t>(d.cc) << 3) | d.lcss;
+                const uint32_t code = (v << 8) | poly_mod(v << 8, 14, 0x139u, 8);
+                const uint32_t w16 = (code << 1) | (__popc(code) & 1u);
+                if (lane < 16) fb[lane < 8 ? 108 + lane : 140 + lane] = static_cast<unsigned char>((w16 >> (15 - lane)) & 1u);
+            }
+        }
+        __syncwarp();
+        if (lane < kTxBurst / 4) {
+            uint32_t word = 0;
+            for (int q = 0; q < 4; q++) {
+                const int m = 4 * lane + q;
+                uint32_t v = 0;
+                if (m < 33)
+                    for (int i = 0; i < 8; i++) v = (v << 1) | fb[8 * m + i];
+                word |= v << (8 * q);
+            }
+            o[lane] = word;
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace
 
 struct qrl_dmr_rx : QrlHandleBase {
@@ -730,5 +1000,165 @@ int qrl_dmr_rx_sync(qrl_dmr_rx* h)
 }
 
 long qrl_dmr_rx_launch_count(qrl_dmr_rx* h) { return h ? h->launches : 0; }
+
+}  // extern "C"
+
+// ================================================================================================ transmit handle
+struct qrl_dmr_tx : QrlHandleBase {
+    int C = 0, max_ops = 0, max_bursts = 0;
+    long out_stride = 0;
+    DmrTxCfg* d_cfg = nullptr;
+    DmrTxState* d_state = nullptr;
+    DmrTxBurst* d_bursts = nullptr;
+    unsigned char *d_recs = nullptr, *d_out = nullptr, *d_prev = nullptr, *d_ops = nullptr, *d_audio = nullptr;
+    int* d_counts = nullptr;
+};
+
+namespace {
+int tx_config(qrl_dmr_tx* h, const qrl_dmr_tx_config* in, DmrTxCfg* out)
+{
+    if (in->color_code < 0 || in->color_code > 15 || (in->timeslot != 1 && in->timeslot != 2) || in->src_id > 0xFFFFFFu ||
+        in->dst_id > 0xFFFFFFu || (in->private_call != 0 && in->private_call != 1) || (in->codec2 != 0 && in->codec2 != 1) ||
+        in->talker_alias_len < 0 || in->talker_alias_len > 27) {
+        set_err(h, "qrl_dmr_tx_set_config: colour code 0-15, timeslot 1 or 2, 24-bit IDs, private_call and codec2 0 or 1, "
+                   "talker_alias_len 0-27");
+        return QRL_EINVAL;
+    }
+    *out = DmrTxCfg{};
+    out->cc = static_cast<unsigned char>(in->color_code); out->slot = static_cast<unsigned char>(in->timeslot);
+    out->flco = in->private_call ? 3 : 0; out->fid = in->codec2 ? 0xC2 : 0;
+    out->src = in->src_id; out->dst = in->dst_id;
+    for (int i = 0; i < in->talker_alias_len; i++) out->ta[i] = in->talker_alias[i];
+    return QRL_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int qrl_dmr_tx_destroy(qrl_dmr_tx* h)
+{
+    if (!h) return QRL_EINVAL;
+    return handle_close(h);
+}
+
+int qrl_dmr_tx_set_config(qrl_dmr_tx* h, int channel, const qrl_dmr_tx_config* cfg)
+{
+    if (!h || !cfg) { set_err(h, "qrl_dmr_tx_set_config: bad argument"); return QRL_EINVAL; }
+    if (channel < -1 || channel >= h->C) { set_err(h, "qrl_dmr_tx_set_config: channel out of range"); return QRL_ERANGE; }
+    DmrTxCfg g;
+    if (int rc = tx_config(h, cfg, &g)) return rc;
+    QRL_CK(cudaSetDevice(h->device));
+    const int n = channel < 0 ? h->C : 1;
+    std::vector<DmrTxCfg> v(n, g);
+    QRL_CK(cudaMemcpyAsync(h->d_cfg + (channel < 0 ? 0 : channel), v.data(), sizeof(DmrTxCfg) * n, cudaMemcpyHostToDevice, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_reset(qrl_dmr_tx* h, int channel)
+{
+    if (!h) return QRL_EINVAL;
+    if (channel < -1 || channel >= h->C) { set_err(h, "qrl_dmr_tx_reset: channel out of range"); return QRL_ERANGE; }
+    QRL_CK(cudaSetDevice(h->device));
+    dmr_tx_reset_kernel<<<(h->C + 127) / 128, 128, 0, h->stream>>>(h->C, channel, h->d_cfg, h->d_state);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_create(int n_channels, int max_ops, int device, qrl_dmr_tx** out)
+{
+    if (!out || n_channels < 1 || max_ops < 1) { set_err(nullptr, "qrl_dmr_tx_create: bad argument"); return QRL_EINVAL; }
+    *out = nullptr;
+    if (int rc = check_device("qrl_dmr_tx_create", device)) return rc;
+    qrl_dmr_tx* h = new qrl_dmr_tx();
+    h->C = n_channels; h->max_ops = max_ops; h->max_bursts = 4 * max_ops; h->out_stride = static_cast<long>(h->max_bursts) * kTxBurst;
+    auto fail = [&](int rc) { return create_failed(h, qrl_dmr_tx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (rc) return fail(rc);
+    const size_t C = static_cast<size_t>(n_channels), B = C * h->max_bursts;
+    if ((rc = dev_alloc(h, &h->d_cfg, C)) || (rc = dev_alloc(h, &h->d_state, C)) || (rc = dev_alloc(h, &h->d_bursts, B)) ||
+        (rc = dev_alloc(h, &h->d_recs, B * kTxRec)) || (rc = dev_alloc(h, &h->d_out, C * h->out_stride, false)) ||
+        (rc = dev_alloc(h, &h->d_prev, C * 18)) || (rc = dev_alloc(h, &h->d_ops, C * max_ops)) ||
+        (rc = dev_alloc(h, &h->d_audio, C * max_ops * 9)) || (rc = dev_alloc(h, &h->d_counts, C)))
+        return fail(rc);
+    qrl_dmr_tx_config def = {};
+    def.color_code = 1; def.timeslot = 1; def.src_id = 1; def.dst_id = 9; def.private_call = 0; def.codec2 = 1;
+    if ((rc = qrl_dmr_tx_set_config(h, -1, &def)) || (rc = qrl_dmr_tx_reset(h, -1))) return fail(rc);
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create: state init failed"); return fail(QRL_ECUDA); }
+    *out = h;
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_set_stream(qrl_dmr_tx* h, void* cuda_stream)
+{
+    if (!h) return QRL_EINVAL;
+    return handle_set_stream(h, cuda_stream);
+}
+
+int qrl_dmr_tx_work(qrl_dmr_tx* h, const unsigned char* ops, const unsigned char* audio, int K, int on_device)
+{
+    if (!h || !ops || !audio) { set_err(h, "qrl_dmr_tx_work: bad argument"); return QRL_EINVAL; }
+    if (K < 0 || K > h->max_ops) { set_err(h, "qrl_dmr_tx_work: K must be between 0 and max_ops"); return QRL_ERANGE; }
+    QRL_CK(cudaSetDevice(h->device));
+    const unsigned char *d_ops = ops, *d_audio = audio;
+    if (on_device) {
+        int rc;
+        if ((rc = check_device_ptr(h, ops, "qrl_dmr_tx_work")) || (rc = check_device_ptr(h, audio, "qrl_dmr_tx_work"))) return rc;
+    } else {
+        if (K > 0) {
+            QRL_CK(cudaMemcpyAsync(h->d_ops, ops, static_cast<size_t>(h->C) * K, cudaMemcpyHostToDevice, h->stream));
+            QRL_CK(cudaMemcpyAsync(h->d_audio, audio, static_cast<size_t>(h->C) * K * 9, cudaMemcpyHostToDevice, h->stream));
+        }
+        d_ops = h->d_ops; d_audio = h->d_audio;
+    }
+    dmr_tx_scan_kernel<<<(h->C + 127) / 128, 128, 0, h->stream>>>(h->C, K, d_ops, d_audio, h->d_cfg, h->d_state, h->d_prev, h->d_bursts,
+                                                                   h->d_recs, h->max_bursts, h->d_counts);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    if (K > 0) {
+        // S warps per channel walk its bursts with stride S: steady voice makes one burst per three ops, a terminator four per op
+        const int S = std::min(8, h->max_bursts);
+        const long long warps = static_cast<long long>(h->C) * S;
+        dmr_tx_encode_kernel<<<static_cast<unsigned>((warps + 3) / 4), 128, 0, h->stream>>>(h->C, K, S, d_audio, h->d_prev, h->d_cfg, h->d_bursts,
+                                                                                         h->max_bursts, h->d_counts, h->d_out, h->out_stride);
+        h->launches++;
+        QRL_CK(cudaGetLastError());
+    }
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_read(qrl_dmr_tx* h, unsigned char* bytes_host, long cap, unsigned char* records_host, int* counts_host)
+{
+    if (!h || !counts_host) { set_err(h, "qrl_dmr_tx_read: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpyAsync(counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    if (bytes_host && cap > 0)
+        QRL_CK(cudaMemcpy2DAsync(bytes_host, static_cast<size_t>(cap), h->d_out, static_cast<size_t>(h->out_stride),
+                                 static_cast<size_t>(cap < h->out_stride ? cap : h->out_stride), h->C, cudaMemcpyDeviceToHost, h->stream));
+    if (records_host)
+        QRL_CK(cudaMemcpyAsync(records_host, h->d_recs, static_cast<size_t>(h->C) * h->max_bursts * kTxRec, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_out_device(qrl_dmr_tx* h, void** bytes, long* stride, int** counts, void** records)
+{
+    if (!h) return QRL_EINVAL;
+    if (bytes) *bytes = h->d_out;
+    if (stride) *stride = h->out_stride;
+    if (counts) *counts = h->d_counts;
+    if (records) *records = h->d_recs;
+    return QRL_OK;
+}
+
+int qrl_dmr_tx_sync(qrl_dmr_tx* h)
+{
+    if (!h) return QRL_EINVAL;
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+
+long qrl_dmr_tx_launch_count(qrl_dmr_tx* h) { return h ? h->launches : 0; }
 
 }  // extern "C"

@@ -180,6 +180,16 @@ SYMBOLS = {
     "qrl_dmr_rx_reset": (_i, [_vp, _i]),
     "qrl_dmr_rx_sync": (_i, [_vp]),
     "qrl_dmr_rx_launch_count": (_l, [_vp]),
+    "qrl_dmr_tx_create": (_i, [_i, _i, _i, C.POINTER(_vp)]),
+    "qrl_dmr_tx_destroy": (_i, [_vp]),
+    "qrl_dmr_tx_set_stream": (_i, [_vp, _vp]),
+    "qrl_dmr_tx_set_config": (_i, [_vp, _i, _vp]),
+    "qrl_dmr_tx_reset": (_i, [_vp, _i]),
+    "qrl_dmr_tx_work": (_i, [_vp, _vp, _vp, _i, _i]),
+    "qrl_dmr_tx_read": (_i, [_vp, _vp, _l, _vp, _vp]),
+    "qrl_dmr_tx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_l), C.POINTER(_vp), C.POINTER(_vp)]),
+    "qrl_dmr_tx_sync": (_i, [_vp]),
+    "qrl_dmr_tx_launch_count": (_l, [_vp]),
 }
 
 
