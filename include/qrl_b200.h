@@ -533,6 +533,50 @@ int  qrl_dmr_rx_reset(qrl_dmr_rx*, int channel);
 int  qrl_dmr_rx_sync(qrl_dmr_rx*);
 long qrl_dmr_rx_launch_count(qrl_dmr_rx*);
 
+/* ---- DMR direct-mode (DMO) burst decoder (qrl_dmr.cu): gr_dmr_dmo_sink (the reference's src/gr/gr_dmr_dmo_sink.cpp, after MMDVM's
+ * DMRDMORX) and then the per-burst work of qrl_dmr_rx, for a batch of channels.  This is what gr_modem reads when Settings::dmr_mode is
+ * DMR_MODE_DMO (radio to radio, no repeater).  Input: QRL_DEMOD_DMR's port 3, the RRC symbol filter's float output at 24 ksps,
+ * 5 samples per symbol: [n_channels][stride] floats, channel c takes counts[c] samples (counts == NULL: every channel takes n, which is
+ * port 3's case: it has port 0's count on every channel and qrl_rx_port_device returns no count array for it).  0 <= n <= max_samples,
+ * stride >= n; on_device = 1: samples (and counts, if given) are device pointers and the caller guarantees 0 <= counts[c] <= n (the
+ * kernel clamps to that range); host counts are checked.
+ * The sink runs per sample: a 1440-sample ring, the MS data / voice sync searched at every sample while idle (at most 2 of the 24 sign
+ * bits wrong, then at most 3 of the 48 sliced sync bits wrong, accepted only above the best correlation so far), then only at the
+ * accepted sync's sample +-1; 269 samples after the sync, 132 symbols are sliced with the average of the last four centres and
+ * thresholds, and the state machine on the sync kind writes a frame or not.  BS syncs are never matched.  As in the reference, the
+ * slice starts 654 samples before the end pointer, so its last symbol comes from the ring slot after the end pointer, which holds the
+ * sample from 1439 samples earlier: the last dibit of byte 32 is not the burst's.  Every float operation
+ * rounds as the reference's separate SSE multiplies and adds do, in its order; NaN, -0 and denormal samples behave as on the host.
+ * Where the reference is undefined the handle defines: the ring, the five sign registers, the four centres and thresholds and the
+ * sync kind are zero at create and reset (the reference's constructor leaves them uninitialised).
+ * Output, per channel in the order gr_dmr_dmo_sink::writeFrame pushes them, up to max_bursts records of QRL_DMR_RECORD_BYTES in
+ * qrl_dmr_rx's layout, with these DMO values:
+ *    position: stream index of the sample whose processing wrote the frame, counted from create / reset
+ *    ts_index 0, downlink 0, cach_decoded 0, AT 0, LCSS 0, CACH bytes 0 (DMRFrame's defaults; the sink calls setDownlink(false))
+ *    slot number 2 and colour code the sink's m_colorCode (writeFrame's setSlotNo(2), setColorCode: on every frame, voice included;
+ *    0 after a reset); FN the sink's m_n (0 for syncs and headers, cycling 1..5, 0 for voice bursts without sync)
+ *    data type from DMRFrame's constructor (its CDMRSlotType for data frames, DT_VOICE / DT_VOICE_SYNC otherwise); validate(), IDs,
+ *    EMB, AMBE error count and burst bytes as qrl_dmr_rx.
+ * Bursts beyond max_bursts advance the state but are not stored (qrl_dmr_dmo_rx_dropped counts them).  A burst can follow 270
+ * samples after a reset, so max_bursts = max_samples / 270 + 2 never drops.  State carries across calls; records are valid until the
+ * next work call. */
+typedef struct qrl_dmr_dmo_rx qrl_dmr_dmo_rx;
+int  qrl_dmr_dmo_rx_create(int n_channels, long max_samples, int max_bursts, int ambe_fec, int device, qrl_dmr_dmo_rx** out);
+int  qrl_dmr_dmo_rx_destroy(qrl_dmr_dmo_rx*);
+int  qrl_dmr_dmo_rx_set_stream(qrl_dmr_dmo_rx*, void* cuda_stream);
+int  qrl_dmr_dmo_rx_work(qrl_dmr_dmo_rx*, const float* samples, long n, const int* counts, long stride, int on_device);
+int  qrl_dmr_dmo_rx_record_bytes(qrl_dmr_dmo_rx*);
+/* records_host [n_channels][max_bursts][72] (may be NULL), counts_host [n_channels]; synchronises */
+int  qrl_dmr_dmo_rx_read(qrl_dmr_dmo_rx*, unsigned char* records_host, int* counts_host);
+int  qrl_dmr_dmo_rx_out_device(qrl_dmr_dmo_rx*, void** records, int** counts);
+/* bursts not stored because a call found more than max_bursts, per channel, since create / that channel's reset; synchronises */
+int  qrl_dmr_dmo_rx_dropped(qrl_dmr_dmo_rx*, int* dropped_host);
+/* gr_dmr_dmo_sink's constructor state for one channel (-1 = all), with ring, registers and position zero.  This is not the sink's own
+ * partial reset(), which the state machine runs after a CSBK, a terminator or 13 bursts without sync */
+int  qrl_dmr_dmo_rx_reset(qrl_dmr_dmo_rx*, int channel);
+int  qrl_dmr_dmo_rx_sync(qrl_dmr_dmo_rx*);
+long qrl_dmr_dmo_rx_launch_count(qrl_dmr_dmo_rx*);
+
 /* ---- DMR burst encoder (qrl_dmr.cu): DMRControl's transmit side (/root/reference/src/DMR/dmrcontrol.cpp:19-223) as gr_modem drives
  * it (src/gr_modem.cpp:676-678 startTransmission's CSBK, 710-717 endTransmission, 747-764 transmitDMRHeader, 766-802 transmitDMR),
  * the burst encoders behind DMRFrame (src/DMR/dmrframe.cpp:20-34, 88-96, 399-421, 460-501) and gr_dmr_source's framing

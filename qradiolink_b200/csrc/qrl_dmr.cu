@@ -1,4 +1,4 @@
-// qrl_dmr.cu -- the DMR burst decoder on the device, part of libqrl_b200.so.
+// qrl_dmr.cu -- the DMR burst decoders (repeater and direct mode) and encoder on the device, part of libqrl_b200.so.
 //
 // qrl_dmr_rx_* takes QRL_DEMOD_DMR's port 2 (the hard bits gr_demod_base feeds to gr_dmr_sink, /root/reference/src/gr_demod_base.cpp:814)
 // and returns, per burst, what DMRControl::addFrames reads of a DMRFrame.  Two kernels:
@@ -463,7 +463,7 @@ __device__ __forceinline__ int ambe_bit(int f, int t)
 __device__ __forceinline__ uint32_t be24(const unsigned char* p) { return static_cast<uint32_t>(p[0]) << 16 | p[1] << 8 | p[2]; }
 
 __global__ void __launch_bounds__(128)
-dmr_decode_kernel(int C, int max_bursts, const int* __restrict__ counts, unsigned char* __restrict__ out, int ambe_fec)
+dmr_decode_kernel(int C, int max_bursts, const int* __restrict__ counts, unsigned char* __restrict__ out, int ambe_fec, int dmo)
 {
     __shared__ unsigned char s_fb[4][264];
     __shared__ unsigned char s_d[4][196];
@@ -598,8 +598,10 @@ dmr_decode_kernel(int C, int max_bursts, const int* __restrict__ counts, unsigne
         r[39 + j] = static_cast<unsigned char>(v);
     }
     if (lane == 0) {
-        r[12] = static_cast<unsigned char>(cach_ok); r[13] = static_cast<unsigned char>(at); r[14] = static_cast<unsigned char>(slot);
-        r[15] = static_cast<unsigned char>(lcss); r[16] = static_cast<unsigned char>(cc); r[17] = static_cast<unsigned char>(dt);
+        // gr_dmr_dmo_sink::writeFrame sets the slot number and colour code after the constructor: the DMO sink wrote them already
+        r[12] = static_cast<unsigned char>(cach_ok); r[13] = static_cast<unsigned char>(at);
+        if (!dmo) { r[14] = static_cast<unsigned char>(slot); r[16] = static_cast<unsigned char>(cc); }
+        r[15] = static_cast<unsigned char>(lcss); r[17] = static_cast<unsigned char>(dt);
         r[18] = static_cast<unsigned char>(valid); r[19] = static_cast<unsigned char>(flco); r[20] = static_cast<unsigned char>(fid);
         r[21] = static_cast<unsigned char>(ecc); r[22] = static_cast<unsigned char>(epi); r[23] = static_cast<unsigned char>(elcss);
         for (int b = 0; b < 4; b++) {
@@ -607,6 +609,239 @@ dmr_decode_kernel(int C, int max_bursts, const int* __restrict__ counts, unsigne
             r[28 + b] = static_cast<unsigned char>(dst >> (8 * b));
             r[32 + b] = static_cast<unsigned char>(static_cast<uint32_t>(ambe) >> (8 * b));
         }
+    }
+}
+
+// ================================================================================================ direct-mode (DMO) burst search
+// gr_dmr_dmo_sink::processSample (MMDVM's DMRDMORX) on QRL_DEMOD_DMR's port 3: 24 ksps floats, 5 samples per symbol.  The sink keeps a
+// 1440-sample ring (60 ms, one DMO burst period); every sign bit the reference shifts into its five per-phase registers is the sign of
+// a ring sample, so the ring alone is saved between calls.  All float arithmetic is separate multiplies and adds in the reference's
+// order (this file is compiled with -fmad=false), so every decision rounds as the reference's SSE code does.
+constexpr int kDmoRing = 1440;                 // DMO_BUFFER_LENGTH_SAMPLES
+constexpr uint32_t kDmoNoEnd = 9999;           // NOENDPTR
+constexpr uint32_t kMsDataSym = 0x76286Eu, kMsVoiceSym = 0x89D791u;     // sign patterns of the MS syncs' 24 symbols (+3 = 1)
+enum { DMO_NONE = 0, DMO_DATA = 1, DMO_VOICE = 2 };                      // RECV_NONE / RECV_DATA / RECV_VOICE
+enum { CTRL_NONE = 0x00, CTRL_VOICE = 0x20, CTRL_DATA = 0x40 };
+
+struct DmoChan {
+    long long pos;               // samples consumed since create / reset; m_dataPtr = pos mod 1440, m_bitPtr = pos mod 5
+    float max_corr, centre[4], threshold[4];
+    uint32_t sync_ptr, end_ptr, avg_ptr, sync_count, state, control, n, cc;
+    int dropped;
+};
+
+struct DmoCand {                 // correlateSync at one sample, before its acceptance test
+    uint32_t kind;               // 0: the prefilter failed; CTRL_DATA / CTRL_VOICE
+    float corr, centre, threshold;
+    bool bytes_ok;               // the sliced sync is within MAX_SYNC_BYTES_ERRS of the sync bytes
+};
+
+__device__ __forceinline__ uint32_t dmo_dibit(float v, float centre, float threshold)
+{
+    const float s = v - centre;
+    return s < -threshold ? 3u : s < 0.0f ? 2u : s < threshold ? 0u : 1u;
+}
+
+// correlateSync's sample-local part at ring index d (the ring holds the sample of d and the 115 before it)
+__device__ DmoCand dmo_correlate(const float* ring, uint32_t d)
+{
+    DmoCand c = { 0u, 0.0f, 0.0f, 0.0f, false };
+    const uint32_t p0 = (d + kDmoRing - 115) % kDmoRing;
+    uint32_t reg = 0;
+    for (int i = 0; i < 24; i++) reg = (reg << 1) | (ring[(p0 + 5 * i) % kDmoRing] > 0.0f ? 1u : 0u);
+    const bool data = __popc(reg ^ kMsDataSym) <= 2, voice = __popc(reg ^ kMsVoiceSym) <= 2;
+    if (!data && !voice) return c;
+    const uint32_t sym = data ? kMsDataSym : kMsVoiceSym;
+    float corr = 0.0f, mn = 100.0f, mx = -100.0f;
+    for (int i = 0; i < 24; i++) {
+        const float val = ring[(p0 + 5 * i) % kDmoRing];
+        if (val > mx) mx = val;
+        if (val < mn) mn = val;
+        corr = corr + ((sym >> (23 - i) & 1u) ? 3.0f : -3.0f) * val;      // float(corrVal) * val, rounded, then the add
+    }
+    const float centre = (mx + mn) / 2.0f;
+    const float threshold = (mx - centre) / 2.0f;
+    uint64_t bits = 0;
+    for (int i = 0; i < 24; i++) bits = (bits << 2) | dmo_dibit(ring[(p0 + 5 * i) % kDmoRing], centre, threshold);
+    c.kind = data ? CTRL_DATA : CTRL_VOICE;
+    c.corr = corr; c.centre = centre; c.threshold = threshold;
+    const uint64_t e = bits ^ (data ? kMsData : kMsVoice);
+    c.bytes_ok = __popc(static_cast<uint32_t>(e)) + __popc(static_cast<uint32_t>(e >> 32)) <= 3;
+    return c;
+}
+
+// the acceptance branch of correlateSync (corr > m_maxCorr and the byte check passed)
+__device__ __forceinline__ void dmo_accept(DmoChan& s, const DmoCand& c, uint32_t d, bool first)
+{
+    if (first) {
+        for (int i = 0; i < 4; i++) { s.threshold[i] = c.threshold; s.centre[i] = c.centre; }
+        s.avg_ptr = 0;
+    } else {
+        s.threshold[s.avg_ptr] = c.threshold; s.centre[s.avg_ptr] = c.centre;
+        s.avg_ptr = (s.avg_ptr + 1) & 3u;
+    }
+    s.max_corr = c.corr;
+    s.control = c.kind;
+    s.sync_ptr = d;
+    s.end_ptr = (d + 269) % kDmoRing;           // DMR_SLOT_TYPE_LENGTH_SAMPLES / 2 + DMR_INFO_LENGTH_SAMPLES / 2 - 1
+}
+
+__device__ __forceinline__ void dmo_sink_reset(DmoChan& s)     // gr_dmr_dmo_sink::reset(): the partial reset of the state machine
+{
+    s.sync_ptr = 0; s.max_corr = 0.0f; s.sync_count = 0; s.state = DMO_NONE; s.end_ptr = kDmoNoEnd; s.cc = 0; s.n = 0;
+}
+
+__global__ void __launch_bounds__(128)
+dmr_dmo_sink_kernel(int C, const float* __restrict__ x, long long stride, int n_all, const int* __restrict__ counts,
+                    DmoChan* __restrict__ chans, float* __restrict__ rings, unsigned char* __restrict__ out, int max_bursts,
+                    int* __restrict__ out_counts)
+{
+    __shared__ float s_ring[4][kDmoRing];
+    __shared__ unsigned char s_frame[4][36];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int c = blockIdx.x * 4 + w;
+    if (c >= C) return;
+    float* ring = s_ring[w];
+    float* ring_g = rings + static_cast<long long>(c) * kDmoRing;
+    for (int i = lane; i < kDmoRing; i += 32) ring[i] = ring_g[i];
+    DmoChan s = chans[c];                   // every lane holds the same copy of the state
+    const float* in = x + static_cast<long long>(c) * stride;
+    const int n = counts ? min(max(counts[c], 0), n_all) : n_all;
+    uint32_t d = static_cast<uint32_t>(s.pos % kDmoRing);
+    int nrec = 0;
+    __syncwarp();
+    // the end of a slot at ring index d, sample p of this call (processSample's m_dataPtr == m_endPtr branch)
+    auto end_event = [&](int p) {
+        const float centre = (s.centre[0] + s.centre[1] + s.centre[2] + s.centre[3]) / 4.0f;
+        const float threshold = (s.threshold[0] + s.threshold[1] + s.threshold[2] + s.threshold[3]) / 4.0f;
+        const uint32_t p0 = (s.end_ptr + kDmoRing - 660 + 5 + 1) % kDmoRing;
+        for (int j = lane; j < 33; j += 32) {
+            uint32_t v = 0;
+            for (int k = 0; k < 4; k++) v = (v << 2) | dmo_dibit(ring[(p0 + 5 * (4 * j + k)) % kDmoRing], centre, threshold);
+            s_frame[w][j] = static_cast<unsigned char>(v);
+        }
+        __syncwarp();
+        const unsigned char* fr = s_frame[w];
+        int ftype = -1;                    // the frame writeFrame is called with, if any
+        bool do_reset = false;
+        if (s.control == CTRL_DATA) {
+            // CDMRSlotType2::decode: the same 19 bits and the same (19,8) syndrome table as DMRFrame's CDMRSlotType
+            const uint32_t code = (static_cast<uint32_t>(fr[12] & 0x3Fu) << 13) | (static_cast<uint32_t>(fr[13] >> 4) << 9) |
+                                  (static_cast<uint32_t>(fr[19] & 0x0Fu) << 5) | ((static_cast<uint32_t>(fr[20]) >> 3) & 0x1Fu);
+            const uint32_t st = ((code ^ d_golay19_err[poly_mod(code, 18, 0xC75u, 11)]) >> 11) & 0xFFu;
+            const uint32_t dt = st & 0xFu;
+            s.cc = st >> 4; s.sync_count = 0; s.n = 0;
+            if (dt == DT_DATA_HEADER) { s.state = DMO_DATA; ftype = FT_DATA; }
+            else if (dt == DT_RATE_12_DATA || dt == DT_RATE_34_DATA || dt == 0x0Au) { if (s.state == DMO_DATA) ftype = FT_DATA; }
+            else if (dt == DT_VOICE_LC_HEADER || dt == DT_VOICE_PI_HEADER) { s.state = DMO_VOICE; ftype = FT_DATA; }
+            else if (dt == DT_TERMINATOR_WITH_LC) { if (s.state == DMO_VOICE) { ftype = FT_DATA; do_reset = true; } }
+            else { ftype = FT_DATA; do_reset = true; }
+        } else if (s.control == CTRL_VOICE) {
+            s.state = DMO_VOICE; s.sync_count = 0; s.n = 0;
+            ftype = FT_VOICE_SYNC;
+        } else {
+            if (s.state != DMO_NONE && ++s.sync_count >= 13) dmo_sink_reset(s);
+            if (s.state == DMO_VOICE) { s.n = s.n >= 5 ? 0 : s.n + 1; ftype = FT_VOICE; }
+            else if (s.state == DMO_DATA) ftype = FT_DATA;
+        }
+        if (ftype >= 0) {
+            if (nrec < max_bursts) {
+                unsigned char* r = out + (static_cast<long long>(c) * max_bursts + nrec) * kRec;
+                for (int j = lane; j < 33; j += 32) r[39 + j] = fr[j];
+                if (lane == 0) {
+                    const long long at = s.pos + p;
+                    for (int b = 0; b < 8; b++) r[b] = static_cast<unsigned char>(at >> (8 * b));
+                    r[8] = 0; r[9] = static_cast<unsigned char>(ftype); r[10] = static_cast<unsigned char>(s.n); r[11] = 0;
+                    r[14] = 2; r[16] = static_cast<unsigned char>(s.cc);
+                    r[36] = r[37] = r[38] = 0;
+                }
+            } else {
+                s.dropped++;
+            }
+            nrec++;
+        }
+        if (do_reset) dmo_sink_reset(s);
+        s.max_corr = 0.0f;
+        s.control = CTRL_NONE;
+        __syncwarp();
+    };
+    int p = 0;
+    while (p < n) {
+        if (s.state == DMO_NONE) {
+            // searching: correlateSync(true) at every sample.  Lane l takes sample p + l; the step ends at the first sample whose
+            // candidate beats m_maxCorr or that meets the (possibly stale) end pointer
+            const int k = min(32, n - p);
+            const uint32_t dl = (d + lane) % kDmoRing;
+            float old = 0.0f;
+            if (lane < k) { old = ring[dl]; ring[dl] = in[p + lane]; }
+            __syncwarp();
+            DmoCand cd = { 0u, 0.0f, 0.0f, 0.0f, false };
+            if (lane < k) cd = dmo_correlate(ring, dl);
+            const bool ev = lane < k && ((cd.kind && cd.corr > s.max_corr && cd.bytes_ok) || dl == s.end_ptr);
+            const uint32_t evs = __ballot_sync(0xffffffffu, ev);
+            const int used = evs ? __ffs(evs) : k;
+            __syncwarp();
+            if (lane >= used && lane < k) ring[dl] = old;     // samples after the event are not in the ring yet
+            if (evs) {
+                const int e = used - 1;
+                const uint32_t de = (d + e) % kDmoRing;
+                DmoCand ce;
+                ce.kind = __shfl_sync(0xffffffffu, cd.kind, e);
+                ce.corr = __shfl_sync(0xffffffffu, cd.corr, e);
+                ce.centre = __shfl_sync(0xffffffffu, cd.centre, e);
+                ce.threshold = __shfl_sync(0xffffffffu, cd.threshold, e);
+                ce.bytes_ok = __shfl_sync(0xffffffffu, static_cast<int>(cd.bytes_ok), e) != 0;
+                if (ce.kind && ce.corr > s.max_corr && ce.bytes_ok) dmo_accept(s, ce, de, true);
+                __syncwarp();
+                if (de == s.end_ptr) end_event(p + e);
+            }
+            __syncwarp();
+            p += used;
+            d = (d + used) % kDmoRing;
+        } else {
+            // locked: correlateSync(false) only at m_syncPtr - 1 .. m_syncPtr + 1, so jump to that window or the end pointer
+            const uint32_t t_in = (d + kDmoRing + 1 - s.sync_ptr) % kDmoRing;            // 0..2: d lies in the window
+            const uint32_t t_win = t_in <= 2 ? 0u : (s.sync_ptr + kDmoRing - 1 - d) % kDmoRing;
+            const uint32_t t_end = s.end_ptr == kDmoNoEnd ? 0xFFFFFFFFu : (s.end_ptr + kDmoRing - d) % kDmoRing;
+            const int m = static_cast<int>(min(static_cast<uint32_t>(n - p), min(t_win, t_end)));
+            for (int j = lane; j < m; j += 32) ring[(d + j) % kDmoRing] = in[p + j];
+            p += m;
+            d = (d + m) % kDmoRing;
+            __syncwarp();
+            if (p >= n) break;
+            // one sample, as processSample takes it
+            if (lane == 0) ring[d] = in[p];
+            __syncwarp();
+            if ((d + kDmoRing + 1 - s.sync_ptr) % kDmoRing <= 2) {
+                const DmoCand cd = dmo_correlate(ring, d);
+                if (cd.kind && cd.corr > s.max_corr && cd.bytes_ok) dmo_accept(s, cd, d, false);
+            }
+            if (d == s.end_ptr) end_event(p);
+            __syncwarp();
+            p += 1;
+            d = (d + 1) % kDmoRing;
+        }
+    }
+    s.pos += n;
+    __syncwarp();
+    for (int i = lane; i < kDmoRing; i += 32) ring_g[i] = ring[i];
+    if (lane == 0) {
+        chans[c] = s;
+        out_counts[c] = min(nrec, max_bursts);
+    }
+}
+
+__global__ void dmr_dmo_reset_kernel(int C, int channel, DmoChan* __restrict__ chans, float* __restrict__ rings)
+{
+    // the constructor's state, with the members it leaves uninitialised (ring, bit registers, centre, threshold, control) zero
+    const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const int c = static_cast<int>(i / kDmoRing), k = static_cast<int>(i % kDmoRing);
+    if (c >= C || (channel >= 0 && c != channel)) return;
+    rings[i] = 0.0f;
+    if (k == 0) {
+        DmoChan s = {};
+        s.end_ptr = kDmoNoEnd;
+        chans[c] = s;
     }
 }
 
@@ -943,7 +1178,7 @@ int qrl_dmr_rx_work(qrl_dmr_rx* h, const unsigned char* bits, const int* counts,
     h->launches++;
     QRL_CK(cudaGetLastError());
     const long long warps = static_cast<long long>(h->C) * h->max_bursts;
-    dmr_decode_kernel<<<static_cast<unsigned>((warps + 3) / 4), 128, 0, h->stream>>>(h->C, h->max_bursts, h->d_counts, h->d_out, h->ambe_fec);
+    dmr_decode_kernel<<<static_cast<unsigned>((warps + 3) / 4), 128, 0, h->stream>>>(h->C, h->max_bursts, h->d_counts, h->d_out, h->ambe_fec, 0);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
@@ -1000,6 +1235,146 @@ int qrl_dmr_rx_sync(qrl_dmr_rx* h)
 }
 
 long qrl_dmr_rx_launch_count(qrl_dmr_rx* h) { return h ? h->launches : 0; }
+
+}  // extern "C"
+
+// ================================================================================================ DMO receive handle
+struct qrl_dmr_dmo_rx : QrlHandleBase {
+    int C = 0, max_bursts = 0, ambe_fec = 0;
+    long max_samples = 0;
+    DmoChan* d_chans = nullptr;
+    float* d_rings = nullptr;
+    unsigned char* d_out = nullptr;
+    int* d_counts = nullptr;
+    float* d_stage = nullptr;
+    int* d_stage_counts = nullptr;
+};
+
+extern "C" {
+
+int qrl_dmr_dmo_rx_destroy(qrl_dmr_dmo_rx* h)
+{
+    if (!h) return QRL_EINVAL;
+    return handle_close(h);
+}
+
+int qrl_dmr_dmo_rx_reset(qrl_dmr_dmo_rx* h, int channel)
+{
+    if (!h) return QRL_EINVAL;
+    if (channel < -1 || channel >= h->C) { set_err(h, "qrl_dmr_dmo_rx_reset: channel out of range"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
+    const long long n = static_cast<long long>(h->C) * kDmoRing;
+    dmr_dmo_reset_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, h->stream>>>(h->C, channel, h->d_chans, h->d_rings);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_create(int n_channels, long max_samples, int max_bursts, int ambe_fec, int device, qrl_dmr_dmo_rx** out)
+{
+    if (!out || n_channels < 1 || max_samples < 1 || max_bursts < 1) { set_err(nullptr, "qrl_dmr_dmo_rx_create: bad argument"); return QRL_EINVAL; }
+    *out = nullptr;
+    if (int rc = check_device("qrl_dmr_dmo_rx_create", device)) return rc;
+    qrl_dmr_dmo_rx* h = new qrl_dmr_dmo_rx();
+    h->C = n_channels; h->max_samples = max_samples; h->max_bursts = max_bursts; h->ambe_fec = ambe_fec ? 1 : 0;
+    auto fail = [&](int rc) { return create_failed(h, qrl_dmr_dmo_rx_destroy, rc); };
+    int rc = handle_open(h, device);
+    if (rc) return fail(rc);
+    const size_t C = static_cast<size_t>(n_channels);
+    if ((rc = upload_dmr_tables(h)) || (rc = dev_alloc(h, &h->d_chans, C)) || (rc = dev_alloc(h, &h->d_rings, C * kDmoRing)) ||
+        (rc = dev_alloc(h, &h->d_out, C * max_bursts * kRec)) || (rc = dev_alloc(h, &h->d_counts, C)) ||
+        (rc = dev_alloc(h, &h->d_stage, C * static_cast<size_t>(max_samples), false)) || (rc = dev_alloc(h, &h->d_stage_counts, C)))
+        return fail(rc);
+    if ((rc = qrl_dmr_dmo_rx_reset(h, -1))) return fail(rc);
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create: state init failed"); return fail(QRL_ECUDA); }
+    *out = h;
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_set_stream(qrl_dmr_dmo_rx* h, void* cuda_stream)
+{
+    if (!h) return QRL_EINVAL;
+    return handle_set_stream(h, cuda_stream);
+}
+
+int qrl_dmr_dmo_rx_work(qrl_dmr_dmo_rx* h, const float* samples, long n, const int* counts, long stride, int on_device)
+{
+    if (!h || !samples || n < 0 || n > h->max_samples || stride < n) {
+        set_err(h, "qrl_dmr_dmo_rx_work: bad argument (0 <= n <= max_samples, stride >= n)");
+        return QRL_EINVAL;
+    }
+    QRL_CK(cudaSetDevice(h->device));
+    const float* d_x = samples;
+    const int* d_cnt = counts;
+    long d_stride = stride;
+    if (on_device) {
+        int rc;
+        if ((rc = check_device_ptr(h, samples, "qrl_dmr_dmo_rx_work")) || (counts && (rc = check_device_ptr(h, counts, "qrl_dmr_dmo_rx_work"))))
+            return rc;
+    } else {
+        if (counts)
+            for (int c = 0; c < h->C; c++)
+                if (counts[c] < 0 || counts[c] > n) { set_err(h, "qrl_dmr_dmo_rx_work: bad count"); return QRL_EINVAL; }
+        if (n > 0)
+            QRL_CK(cudaMemcpy2DAsync(h->d_stage, sizeof(float) * n, samples, sizeof(float) * stride, sizeof(float) * n, h->C,
+                                     cudaMemcpyHostToDevice, h->stream));
+        if (counts) {
+            QRL_CK(cudaMemcpyAsync(h->d_stage_counts, counts, sizeof(int) * h->C, cudaMemcpyHostToDevice, h->stream));
+            d_cnt = h->d_stage_counts;
+        }
+        d_x = h->d_stage; d_stride = n;
+    }
+    dmr_dmo_sink_kernel<<<(h->C + 3) / 4, 128, 0, h->stream>>>(h->C, d_x, d_stride, static_cast<int>(n), d_cnt, h->d_chans, h->d_rings,
+                                                              h->d_out, h->max_bursts, h->d_counts);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    const long long warps = static_cast<long long>(h->C) * h->max_bursts;
+    dmr_decode_kernel<<<static_cast<unsigned>((warps + 3) / 4), 128, 0, h->stream>>>(h->C, h->max_bursts, h->d_counts, h->d_out, h->ambe_fec, 1);
+    h->launches++;
+    QRL_CK(cudaGetLastError());
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_record_bytes(qrl_dmr_dmo_rx* h) { return h ? kRec : 0; }
+
+int qrl_dmr_dmo_rx_read(qrl_dmr_dmo_rx* h, unsigned char* records_host, int* counts_host)
+{
+    if (!h || !counts_host) { set_err(h, "qrl_dmr_dmo_rx_read: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
+    QRL_CK(cudaMemcpyAsync(counts_host, h->d_counts, sizeof(int) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    if (records_host)
+        QRL_CK(cudaMemcpyAsync(records_host, h->d_out, static_cast<size_t>(h->C) * h->max_bursts * kRec, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_out_device(qrl_dmr_dmo_rx* h, void** records, int** counts)
+{
+    if (!h) return QRL_EINVAL;
+    if (records) *records = h->d_out;
+    if (counts) *counts = h->d_counts;
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_dropped(qrl_dmr_dmo_rx* h, int* dropped_host)
+{
+    if (!h || !dropped_host) { set_err(h, "qrl_dmr_dmo_rx_dropped: bad argument"); return QRL_EINVAL; }
+    QRL_CK(cudaSetDevice(h->device));
+    std::vector<DmoChan> ch(h->C);
+    QRL_CK(cudaMemcpyAsync(ch.data(), h->d_chans, sizeof(DmoChan) * h->C, cudaMemcpyDeviceToHost, h->stream));
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    for (int c = 0; c < h->C; c++) dropped_host[c] = ch[c].dropped;
+    return QRL_OK;
+}
+
+int qrl_dmr_dmo_rx_sync(qrl_dmr_dmo_rx* h)
+{
+    if (!h) return QRL_EINVAL;
+    QRL_CK(cudaStreamSynchronize(h->stream));
+    return QRL_OK;
+}
+
+long qrl_dmr_dmo_rx_launch_count(qrl_dmr_dmo_rx* h) { return h ? h->launches : 0; }
 
 }  // extern "C"
 

@@ -93,6 +93,82 @@ class DmrBurstDecoder(Handle):
         return self.read() if collect else None
 
 
+class DmrDmoBurstDecoder(Handle):
+    """gr_dmr_dmo_sink + DMRFrame decoding (DMR direct mode) for n_channels channels of up to max_samples port-3 samples per call;
+    up to max_bursts records per channel and call (default max_samples // 270 + 2, which never drops), in DMR_RECORD's layout with
+    slot number 2, the sink's colour code and FN, position = the index of the sample that completed the burst.  ambe_fec as for
+    DmrBurstDecoder.  Sink state carries across calls."""
+    ABI = "dmr_dmo_rx"
+
+    def __init__(self, n_channels, max_samples, max_bursts=None, ambe_fec=False, device=0):
+        self._L = load_library()
+        self.n_channels, self.max_samples = int(n_channels), int(max_samples)
+        self.max_bursts = self.max_samples // 270 + 2 if max_bursts is None else int(max_bursts)
+        self._create(self._L.qrl_dmr_dmo_rx_create, self.n_channels, self.max_samples, self.max_bursts, int(bool(ambe_fec)), device)
+
+    set_stream = Handle._set_stream
+    sync = Handle._sync
+    launches = property(Handle._launches)
+
+    def reset(self, channel=-1):
+        """gr_dmr_dmo_sink's constructor state for one channel (-1: every channel), ring and position zero"""
+        check(self._L.qrl_dmr_dmo_rx_reset(self._h, int(channel)), self._h, "qrl_dmr_dmo_rx_reset")
+
+    def dropped(self):
+        d = np.zeros(self.n_channels, np.int32)
+        check(self._L.qrl_dmr_dmo_rx_dropped(self._h, _p(d)), self._h, "qrl_dmr_dmo_rx_dropped")
+        return d
+
+    def out_device(self):
+        """device pointers of the last call's [n_channels][max_bursts][72] records and [n_channels] counts"""
+        r, c = C.c_void_p(), C.c_void_p()
+        check(self._L.qrl_dmr_dmo_rx_out_device(self._h, C.byref(r), C.byref(c)), self._h, "qrl_dmr_dmo_rx_out_device")
+        return r, c
+
+    def read(self):
+        """list per channel of a DMR_RECORD array, one entry per burst of the last call"""
+        rec = np.zeros((self.n_channels, self.max_bursts), DMR_RECORD)
+        cnt = np.zeros(self.n_channels, np.int32)
+        check(self._L.qrl_dmr_dmo_rx_read(self._h, _p(rec), _p(cnt)), self._h, "qrl_dmr_dmo_rx_read")
+        return [rec[c, :cnt[c]].copy() for c in range(self.n_channels)]
+
+    def work(self, samples, counts=None, collect=True):
+        """samples: [n_channels][n] float32 (every channel takes n, or counts[c]) or a list of per-channel arrays"""
+        if isinstance(samples, (list, tuple)):
+            n = max([len(x) for x in samples] + [0])
+            buf = np.zeros((self.n_channels, max(n, 1)), np.float32)
+            cnt = np.zeros(self.n_channels, np.int32)
+            for c, x in enumerate(samples):
+                buf[c, :len(x)] = x
+                cnt[c] = len(x)
+        else:
+            buf = np.ascontiguousarray(samples, np.float32)
+            n = buf.shape[1]
+            cnt = None if counts is None else np.ascontiguousarray(counts, np.int32)
+        if buf.shape[0] != self.n_channels or (cnt is not None and cnt.shape != (self.n_channels,)):
+            raise ValueError("samples must be [n_channels][n] with n_channels counts")
+        check(self._L.qrl_dmr_dmo_rx_work(self._h, _p(buf), n, None if cnt is None else _p(cnt), buf.shape[1], 0), self._h,
+              "qrl_dmr_dmo_rx_work")
+        return self.read() if collect else None
+
+    def work_device(self, samples_ptr, n, stride, counts_ptr=None):
+        """[n_channels][stride] float32 samples (and optionally [n_channels] int32 counts) already in this handle's GPU memory"""
+        check(self._L.qrl_dmr_dmo_rx_work(self._h, C.c_void_p(samples_ptr), int(n), None if counts_ptr is None else C.c_void_p(counts_ptr),
+                                          int(stride), 1), self._h, "qrl_dmr_dmo_rx_work")
+
+    def work_from_demod(self, rx_block, collect=True):
+        """decode the DMR demodulator's last port-3 output in place on the device (qrl_rx_port_device); every channel takes port 0's
+        count, which is port 3's"""
+        data, cap, none = C.c_void_p(), C.c_long(), C.c_void_p()
+        # reading port 0's counts waits for the demodulator's call (the two handles run on different streams) before the sink reads
+        # port 3; the data stays in HBM
+        cnt = np.zeros(rx_block.n_channels, np.int32)
+        check(self._L.qrl_rx_read_port(rx_block._h, 0, None, 0, _p(cnt), 0), rx_block._h, "qrl_rx_read_port")
+        check(self._L.qrl_rx_port_device(rx_block._h, 3, C.byref(data), C.byref(cap), C.byref(none)), rx_block._h, "qrl_rx_port_device")
+        check(self._L.qrl_dmr_dmo_rx_work(self._h, data, int(cnt[0]), None, cap.value, 1), self._h, "qrl_dmr_dmo_rx_work")
+        return self.read() if collect else None
+
+
 # ---------------------------------------------------------------------------------------------------------------- transmit
 OP_NONE, OP_CSBK, OP_HEADER, OP_AUDIO, OP_STOP = 0, 1, 2, 3, 4
 KIND_CSBK, KIND_LC_HEADER, KIND_VOICE_SYNC, KIND_VOICE, KIND_TERMINATOR, KIND_EMPTY = 1, 2, 3, 4, 5, 6

@@ -180,6 +180,17 @@ SYMBOLS = {
     "qrl_dmr_rx_reset": (_i, [_vp, _i]),
     "qrl_dmr_rx_sync": (_i, [_vp]),
     "qrl_dmr_rx_launch_count": (_l, [_vp]),
+    "qrl_dmr_dmo_rx_create": (_i, [_i, _l, _i, _i, _i, C.POINTER(_vp)]),
+    "qrl_dmr_dmo_rx_destroy": (_i, [_vp]),
+    "qrl_dmr_dmo_rx_set_stream": (_i, [_vp, _vp]),
+    "qrl_dmr_dmo_rx_work": (_i, [_vp, _vp, _l, _vp, _l, _i]),
+    "qrl_dmr_dmo_rx_record_bytes": (_i, [_vp]),
+    "qrl_dmr_dmo_rx_read": (_i, [_vp, _vp, _vp]),
+    "qrl_dmr_dmo_rx_out_device": (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp)]),
+    "qrl_dmr_dmo_rx_dropped": (_i, [_vp, _vp]),
+    "qrl_dmr_dmo_rx_reset": (_i, [_vp, _i]),
+    "qrl_dmr_dmo_rx_sync": (_i, [_vp]),
+    "qrl_dmr_dmo_rx_launch_count": (_l, [_vp]),
     "qrl_dmr_tx_create": (_i, [_i, _i, _i, C.POINTER(_vp)]),
     "qrl_dmr_tx_destroy": (_i, [_vp]),
     "qrl_dmr_tx_set_stream": (_i, [_vp, _vp]),
