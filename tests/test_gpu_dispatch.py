@@ -174,12 +174,14 @@ RX = {
              lambda O: O.Rx(O.DEMOD_DSSS, 25, 1000000, 1700, 150, 0), 4, 3 << 20, (16000, 20, 0, 0), None),
 }
 
+# Rows outside RX run through the harness below when passed as `row`: RX's six fields plus a seventh, gen(O, T) -> (the P base
+# signals, payloads or None) (tests/reference_instances.py: the reference instances RX does not hold).  `name` then only keys the caches.
 _BASES, _ORACLE = {}, {}
 
 
-def bases(name, O, T):
+def bases(name, O, T, row=None):
     if (name, T) not in _BASES:
-        _BASES[(name, T)] = _gen(name, O, T)
+        _BASES[(name, T)] = row[6](O, T) if row is not None and len(row) > 6 else _gen(name, O, T)
     return _BASES[(name, T)]
 
 
@@ -301,12 +303,13 @@ def concat_calls(calls, nports, Cn):
     return [[np.concatenate([calls[k][p][c] for k in range(len(calls))]) for c in range(Cn)] for p in range(nports)]
 
 
-def oracle_ports(name, O, B, spots, c, cuts, events, setters=()):
+def oracle_ports(name, O, B, spots, c, cuts, events, setters=(), row=None):
     """setters: (PARAM key, value) applied before the first sample"""
+    row = row or RX[name]
     key = (name, B.shape[1], c % P, spots.get(c), tuple(cuts), tuple((k, hz) for (k, ch, hz) in events if ch in (-1, c)), tuple(setters))
     if key not in _ORACLE:
         x = host_channel(B, spots, c)
-        rx = RX[name][1](O)
+        rx = row[1](O)
         for pkey, value in setters:
             rx.set_param(pkey, value)
         for k, (lo, hi) in enumerate(cuts):
@@ -314,14 +317,15 @@ def oracle_ports(name, O, B, spots, c, cuts, events, setters=()):
                 if ek == k and ch in (-1, c):
                     rx.set_carrier_offset(hz)
             rx.work(x[lo:hi])
-        _ORACLE[key] = [rx.port(p) for p in range(RX[name][2])]
+        _ORACLE[key] = [rx.port(p) for p in range(row[2])]
     return _ORACLE[key]
 
 
-def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True, setters=()):
+def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True, setters=(), row=None):
     """got[p][c]: the whole stream of port p on channel c; setters: (PARAM key, value) the handle had before its first sample"""
-    nports, fr = RX[name][2], RX[name][5]
-    mins = [m * cuts[-1][1] // RX[name][3] for m in RX[name][4]]         # the minimum lengths scale with the stream's length
+    row = row or RX[name]
+    nports, fr = row[2], row[5]
+    mins = [m * cuts[-1][1] // row[3] for m in row[4]]         # the minimum lengths scale with the stream's length
     Cn = len(got[0])
     reps = representatives(Cn, spots)
     for p in range(nports):
@@ -329,7 +333,7 @@ def check_rx(name, O, B, payloads, got, spots, cuts, events=(), frames=True, set
             if c not in spots:
                 assert np.array_equal(got[p][c], got[p][reps[c % P]]), "%s: port %d of channel %d differs from channel %d" % (name, p, c, reps[c % P])
     for c in sorted(set(reps.values()) | set(spots)):
-        want = oracle_ports(name, O, B, spots, c, cuts, events, setters)
+        want = oracle_ports(name, O, B, spots, c, cuts, events, setters, row)
         for p in range(nports):
             g, w = got[p][c], want[p]
             n = min(len(g), len(w))
@@ -352,17 +356,18 @@ def equal_cuts(T, K):
     return [(k * (T // K), (k + 1) * (T // K)) for k in range(K)]
 
 
-def run_case(qrl, O, name, Cn, T=None, cuts=None, overlap=False, events=(), profile=False, frames=True):
+def run_case(qrl, O, name, Cn, T=None, cuts=None, overlap=False, events=(), profile=False, frames=True, row=None):
     """build the slab, run one handle, check everything; returns the handle (caller closes).  Overlapped: the handle reads after every
     call; a serialised twin gives every call's reference ports; two more overlapped handles issue the calls back to back, one read
     every second call and one read only after the last, so the calls in between really run under each other's tails"""
-    T = T or RX[name][3]
-    B, payloads = bases(name, O, T)
+    row = row or RX[name]
+    T = T or row[3]
+    B, payloads = bases(name, O, T, row)
     spots = spot_shifts(Cn)
     cuts = cuts or ragged(T)
     maxs = max(hi - lo for lo, hi in cuts)
     X = make_slab(B, Cn, spots)
-    blk = RX[name][0](qrl, Cn, maxs)
+    blk = row[0](qrl, Cn, maxs)
     try:
         if profile:
             assert blk._L.qrl_rx_profile(blk._h, 1) == 0
@@ -370,7 +375,7 @@ def run_case(qrl, O, name, Cn, T=None, cuts=None, overlap=False, events=(), prof
             blk.set_overlap(True)
         calls = run_rx(blk, X, cuts, events)
         if overlap:         # every call equals the serialised handle's
-            ser = RX[name][0](qrl, Cn, maxs)
+            ser = row[0](qrl, Cn, maxs)
             try:
                 want = run_rx(ser, X, cuts, events)
             finally:
@@ -379,7 +384,7 @@ def run_case(qrl, O, name, Cn, T=None, cuts=None, overlap=False, events=(), prof
                 if read_every == 1:
                     got_calls = calls
                 else:
-                    b2b = RX[name][0](qrl, Cn, maxs)
+                    b2b = row[0](qrl, Cn, maxs)
                     try:
                         b2b.set_overlap(True)
                         got_calls = run_rx(b2b, X, cuts, events, read_every=read_every)
@@ -391,7 +396,7 @@ def run_case(qrl, O, name, Cn, T=None, cuts=None, overlap=False, events=(), prof
                             for c in range(Cn):
                                 assert np.array_equal(got_calls[k][p][c], want[k][p][c]), (name, read_every, k, p, c)
         got = concat_calls(calls, blk.nports, Cn)
-        check_rx(name, O, B, payloads, got, spots, cuts, events, frames=frames and T == RX[name][3])
+        check_rx(name, O, B, payloads, got, spots, cuts, events, frames=frames and T == row[3], row=row)
     except BaseException:
         blk.close()
         raise

@@ -104,13 +104,18 @@ def test_freedv_rx_setters_mid_stream(qrl):
 
 @pytest.mark.parametrize("sb", [0, 1])
 def test_freedv_tx_parity_and_bb_gain(qrl, sb):
+    tx_parity_case(qrl, 300, sb)
+
+
+def tx_parity_case(qrl, lo, sb):
+    """make_gr_mod_freedv(125, 1e6, 1700, 2700, lo, ..., sb) against the oracle over ragged calls with two bb_gain changes"""
     C, n = 3, 9000
     rng = np.random.default_rng(950 + sb)
     t = np.arange(n) / 8000.0
     S = np.stack([(5000 * np.sin(2 * np.pi * (500 + 300 * c) * t) + 1500 * rng.standard_normal(n)).astype(np.int16) for c in range(C)])
     S[:, 3000:3600] = 0
-    tx = qrl.make_gr_mod_freedv(125, 1000000, 1700, 2700, 300, 0, sb, n_channels=C, max_items=4000)
-    ors = [FO.FreedvTx(125, 1000000, 2700, 300, sb) for _ in range(C)]
+    tx = qrl.make_gr_mod_freedv(125, 1000000, 1700, 2700, lo, 0, sb, n_channels=C, max_items=4000)
+    ors = [FO.FreedvTx(125, 1000000, 2700, lo, sb) for _ in range(C)]
     a, i, sizes = 0, 0, [1, 4000, 511, 1, 2000, 2487]
     gains = {4001: 0.5, 6513: 1.7}
     while a < n:
