@@ -44,6 +44,7 @@ std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
         for (int k = 0; k < nt; k++) { const size_t j = p + static_cast<size_t>(k) * L; if (j < taps.size()) a[p * nt + k] = taps[j]; }
     return a;
 }
+int arms_nt(const std::vector<float>& taps, int L) { return (static_cast<int>(taps.size()) + L - 1) / L; }
 
 using HandleBase = QrlHandleBase;       // qrl_handle.hpp: shared by every handle type of the library
 
@@ -64,10 +65,17 @@ int upload_tables(HandleBase* h)
 }  // namespace
 
 // =====================================================================================================
+// the receive chains (DESIGN.md section 5): rx_create picks one from the demod kind and its flag, and one create function per chain
+// family designs its taps and rings; qrl_rx_work runs the chain's slice function
+enum class RxChain { Nbfm, Am, Wbfm, Ssb, Freedv, Dsss, Bpsk, Fsk2Fm, Fsk2Bank, Gmsk, Fsk4Fm, Fsk4Bank, M17, Dmr, Qpsk };
 struct qrl_rx : HandleBase {
-    int kind = 0, sps = 0, samp_rate = 0, carrier_freq = 0, filter_width = 0, flag = 0, C = 0;
+    RxChain chain = RxChain::Nbfm;
+    int samp_rate = 0, C = 0;
+    bool lsb = false;                  // SSB, FreeDV: the lower side band
     long Tmax = 0;
-    int nports = 3;
+    // ports: 0 the channel filter's output (complex), 1 symbols (complex), audio (float) or modem samples (int16), 2 and 3 the
+    // decoders' bytes (DMR: port 3 the symbol filter's floats, one per port-0 sample)
+    int nports = 3, port1_isz = 8, port3_isz = 1;
     // stage 1 (rational_resampler_ccf(1, D))
     int D1 = 1, L1 = 1, Q1 = 1, ntaps1 = 0, H = 0, hist_cur = 0;
     float* d_taps1 = nullptr;
@@ -101,8 +109,8 @@ struct qrl_rx : HandleBase {
     DsssParams dsp{}; DsssState* d_ds = nullptr; float* d_ds_arms = nullptr; float2* d_ds_taps = nullptr;
     Ring ds_a, ds_c, ds_d; long long ds_o_call0 = 0;
     Ring r3;
-    int sym_sps = 0;
-    // BPSK / 2FSK: fll_band_edge_cc + second (delayed) decoder
+    // BPSK, 2FSK (not GMSK), QPSK above 4 samples per symbol: fll_band_edge_cc behind stage 1; BPSK / 2FSK: second (delayed) decoder
+    bool fll = false;
     FllParams fllp{};
     FllState* d_fll = nullptr; float2* d_fll_hist = nullptr; float* d_fll_taps = nullptr;
     Ring rf;                       // FLL output (channel-major complex)
@@ -122,7 +130,6 @@ struct qrl_rx : HandleBase {
     SsbParams ssbp{};
     SsbState* d_ssb = nullptr;
     Ring rclip, rstr;
-    float* d_taps2c = nullptr;     // complex side-band filter taps
     // NBFM audio chain
     NbfmParams nbp{};
     NbfmState* d_nb = nullptr;
@@ -136,10 +143,7 @@ struct qrl_rx : HandleBase {
     SymSyncState* d_ss = nullptr;
     float* d_ss_scratch = nullptr; int* d_ss_hdr = nullptr; long long ss_chunk_cap = 0, ss_chunk_off = 0;   // external symbol-sync epilogue
     cudaStream_t s_epi = nullptr;                        // wide-partition stream of the external epilogue
-    bool gmsk = false;                                   // 2FSK code path running as gr_demod_gmsk (no FLL)
-    bool m17 = false;                                    // 4FSK (fm) code path running as gr_demod_m17 (x3/125 front end, hard bits)
     int nt_arm1 = 0;                                     // taps per arm of a generic rational stage 1 (L1 > 1)
-    bool dmr = false;                                    // M17 code path running as gr_demod_dmr (plain M&M detector, x0.9, float port 3)
     float* d_port3f = nullptr;                           // gr_demod_dmr port 3: symbol filter output, [C][port0_cap] floats
     // RSSI tap on port 0 (QRL_PARAM_RSSI): ring of |x|^2, carried IIR value, latest dB value per channel
     bool rssi_on = false; float* d_rssi_ring = nullptr; float* d_rssi_y = nullptr; float* d_rssi_db = nullptr; long long rssi_n = 0;
@@ -433,7 +437,7 @@ int symsync_maxs(const SymSyncParams& p, int CH)
 }
 
 // dynamic shared memory of the 4FSK-FM symbol sync with the external epilogue: NST input stages of CH rows x 32 channels, the tap
-// table, two symbol windows and the header; rep adds the replicated (conflict-free) interpolator bank.  rx_create chooses ss_ch and
+// table, two symbol windows and the header; rep adds the replicated (conflict-free) interpolator bank.  create_4fsk chooses ss_ch and
 // sizes the epilogue scratch with it, and the launch uses it, so the two always agree.
 size_t symsync_ext_smem(const SymSyncParams& p, int CH, int NST, bool rep)
 {
@@ -483,6 +487,9 @@ int launch_channel_filter(qrl_rx* h, const Slice& s, cudaStream_t st, const Ring
                           h->d_taps2, h->ntaps2, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0, interleaved);
 }
 
+// gr_demod_m17, gr_demod_dmr: the symbol sync's epilogue writes two hard bits per symbol to port 2, no decoder behind them
+bool hard_bits(const qrl_rx* h) { return h->chain == RxChain::M17 || h->chain == RxChain::Dmr; }
+
 // 4FSK-FM with the register-tiled /50 stage 1 and filters that fit the kernel's shared memory: the whole receive front end of a slice
 // is one fsk_fm_frontend_kernel launch (QRL_FSK_FRONTEND=0 keeps stage 1, the channel filter and the demodulator as three launches)
 bool fsk_fm_fused(const qrl_rx* h)
@@ -491,7 +498,7 @@ bool fsk_fm_fused(const qrl_rx* h)
     // the first strip of a slice reads the halo in front of the slice from r1 while the slice's last strips store the halo behind it
     // there: a slice (at most n1max outputs) plus its halo must fit the ring, or the two ranges alias
     const long long halo = h->ntaps3 + h->ntaps2 - 1;
-    return h->kind == QRL_DEMOD_4FSK && h->flag && !h->m17 && !h->dmr && h->L1 == 1 && h->D1 == 50 && h->Q1 == 9 && !h->fir_group_forced &&
+    return h->chain == RxChain::Fsk4Fm && h->L1 == 1 && h->D1 == 50 && h->Q1 == 9 && !h->fir_group_forced &&
            h->ntaps2 >= 8 && h->ntaps2 <= 256 && h->ntaps3 >= 8 && h->ntaps3 <= 512 &&
            static_cast<long long>(h->r1.mask) + 1 >= h->n1max + halo;
 }
@@ -573,7 +580,7 @@ int slice_analog(qrl_rx* h, const Slice& s)
     cudaEvent_t pe;
     if (s.n_new > 0) {
         pe = h->prof.begin(1, s.sp);
-        if (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_WBFM) {
+        if (h->chain == RxChain::Nbfm || h->chain == RxChain::Wbfm) {
             if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
         } else {
             fir_ccc_ring_kernel<<<s.gtile, kTileThreads, sizeof(float) * 2 * h->ntaps2, s.sp>>>(
@@ -587,15 +594,15 @@ int slice_analog(qrl_rx* h, const Slice& s)
     if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
     pe = h->prof.begin(3, h->s_loop);
     const size_t fat = h->nbfm_split ? 120 * 1024 : 0;       // one CTA per SM, and never next to a de-emphasis CTA
-    switch (h->kind) {
-    case QRL_DEMOD_SSB:
+    switch (h->chain) {
+    case RxChain::Ssb:
         ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb,
             static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
             static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
             static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
             h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
         break;
-    case QRL_DEMOD_FREEDV:
+    case RxChain::Freedv:
         freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
             static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
             static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
@@ -633,20 +640,20 @@ int slice_analog(qrl_rx* h, const Slice& s)
 // two decoders
 int slice_fll_bpsk_2fsk(qrl_rx* h, const Slice& s)
 {
-    const bool bpsk = h->kind == QRL_DEMOD_BPSK;
+    const bool bpsk = h->chain == RxChain::Bpsk;
     if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
     cudaEvent_t pe = h->prof.begin(1, h->s_loop);
-    if (!h->gmsk) launch_fll(h, s);
+    if (h->fll) launch_fll(h, s);
     h->prof.end(pe);
     if (s.n_new > 0) {
         // ---- channel filter / RRC on the FLL output -> port 0 (+ ring: channel-major for 2FSK, interleaved for BPSK)
         pe = h->prof.begin(2, h->s_loop);
-        if (int rc = launch_channel_filter(h, s, h->s_loop, h->gmsk ? h->r1 : h->rf, bpsk ? 1 : 0)) return rc;     // GMSK: no FLL
-        if (!bpsk && h->flag) {
+        if (int rc = launch_channel_filter(h, s, h->s_loop, h->fll ? h->rf : h->r1, bpsk ? 1 : 0)) return rc;     // GMSK: no FLL
+        if (h->chain == RxChain::Fsk2Fm || h->chain == RxChain::Gmsk) {
             if (int rc = launch_qdemod_fir(h, h->s_loop, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                            static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
                                            h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
-        } else if (!bpsk) {
+        } else if (h->chain == RxChain::Fsk2Bank) {
             fsk_bank_kernel<2><<<s.gtile, kTileThreads, sizeof(float) * 4 * h->nt_bank, h->s_loop>>>(
                 static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, s.k0, s.k1,
                 static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
@@ -695,9 +702,10 @@ int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
 {
     cudaEvent_t pe = h->prof.begin(3, h->s_loop);
     const int maxs = symsync_maxs(h->ssp, CH);
-    const bool rep = symsync_ext_smem(h->ssp, CH, NST, true) <= 220 * 1024 && !h->dmr;
+    const bool dmr = h->chain == RxChain::Dmr;
+    const bool rep = symsync_ext_smem(h->ssp, CH, NST, true) <= 220 * 1024 && !dmr;
     // gr_demod_dmr: TED_MUELLER_AND_MULLER instead of the modified detector -> generic recurrence, variant 3
-    auto kern = h->dmr ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>
+    auto kern = dmr ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>
               : rep ? symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 2>
                     : symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 1>;
     // overlapped calls: the previous call's Viterbi of slice i still reads d_nsoft[i], its epilogue scratch region i
@@ -715,13 +723,13 @@ int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
     if (se != h->s_loop || h->overlap) QRL_CK(cudaEventRecord(h->ev_c[s.i], h->s_loop));
     if (se != h->s_loop) QRL_CK(cudaStreamWaitEvent(se, h->ev_c[s.i], 0));
     pe = h->prof.begin(5, se);
-    auto epi = h->dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
+    auto epi = dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
     if (chunk_bound > 0)        // (counted in h->launches with the symbol sync it finishes)
         epi<<<dim3(chunk_bound, s.groups), dim3(32, 8), 0, se>>>(
             h->ssp, h->C, scratch_i, static_cast<int>(h->ss_chunk_cap), maxs, hdr_i,
             h->d_port1, h->port1_cap, static_cast<int>(h->port1_cap),
             static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
-            h->m17 ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
+            hard_bits(h) ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
     h->prof.end(pe);
     QRL_CK(cudaEventRecord(h->ev_b[s.i], se));
     return QRL_OK;
@@ -731,6 +739,7 @@ int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
 // stream, then the decoder (M17: none)
 int slice_4fsk(qrl_rx* h, const Slice& s)
 {
+    const bool fm = h->chain != RxChain::Fsk4Bank;      // FM discriminator (4FSK, M17, DMR) or band-pass bank
     cudaEvent_t pe;
     // overlapped calls: this slice overwrites ring slots the previous call's symbol sync (slices i, i+1) read
     auto wait_r4_free = [&]() -> int {
@@ -758,11 +767,11 @@ int slice_4fsk(qrl_rx* h, const Slice& s)
         // ---- stage 3: quadrature demod + RRC   |   band-pass bank + discriminator + symbol filter
         if (int rc = wait_r4_free()) return rc;
         pe = h->prof.begin(2, s.sp);
-        if (h->flag) {
+        if (fm) {
             if (int rc = launch_qdemod_fir(h, s.sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
                                            static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
                                            h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
-            if (h->dmr) {      // gr_demod_dmr.cpp:103: the symbol filter output is port 3
+            if (h->chain == RxChain::Dmr) {      // gr_demod_dmr.cpp:103: the symbol filter output is port 3
                 ring_to_port_f32_kernel<<<dim3(static_cast<unsigned>((s.k1 - s.k0 + 31) / 32), s.groups), dim3(32, 8), 0, s.sp>>>(
                     static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, h->C, s.k0, s.k1,
                     h->d_port3f, h->port0_cap, s.k0 - s.k_call0);
@@ -781,7 +790,7 @@ int slice_4fsk(qrl_rx* h, const Slice& s)
     }
     // ---- stage 4: symbol sync (+ phase mod + soft bits) on the loop stream
     if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
-    if (h->flag) {
+    if (fm) {
         const int rc = h->ss_ch == 512 ? symsync_4fsk_ext<512, 2>(h, s) : symsync_4fsk_ext<256, 3>(h, s);
         if (rc) return rc;
     } else {
@@ -797,7 +806,7 @@ int slice_4fsk(qrl_rx* h, const Slice& s)
     // ---- stage 5: Viterbi + descrambler on the FEC stream
     QRL_CK(cudaStreamWaitEvent(h->s_fec, h->ev_b[s.i], 0));
     // gr_demod_m17 has no FEC: the epilogue wrote the hard bits of port 2 (s_fec joins it at the end)
-    if (!h->m17) launch_viterbi(h, s.nsoft_i, false);
+    if (!hard_bits(h)) launch_viterbi(h, s.nsoft_i, false);
     if (h->overlap) QRL_CK(cudaEventRecord(h->ev_v[s.i], h->s_fec));
     return QRL_OK;
 }
@@ -837,7 +846,7 @@ int qpsk_symsync(qrl_rx* h, const Slice& s)
 // the second loop stream, then the decoder
 int slice_qpsk(qrl_rx* h, const Slice& s)
 {
-    if (h->d_fll) {     // sps > 4: fll_band_edge_cc between resampler and shaping filter (sequential, on the loop stream)
+    if (h->fll) {       // sps > 4: fll_band_edge_cc between resampler and shaping filter (sequential, on the loop stream)
         if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
         launch_fll(h, s);
         if (int rc = hand_off(h, h->ev_c[s.i], h->s_loop, s.sp)) return rc;
@@ -846,7 +855,7 @@ int slice_qpsk(qrl_rx* h, const Slice& s)
     if (s.n_new > 0) {
         // ---- stage 2: RRC shaping filter -> interleaved ring + port 0
         pe = h->prof.begin(1, s.sp);
-        if (int rc = launch_channel_filter(h, s, s.sp, h->d_fll ? h->rf : h->r1, 1)) return rc;
+        if (int rc = launch_channel_filter(h, s, s.sp, h->fll ? h->rf : h->r1, 1)) return rc;
         h->prof.end(pe);
     }
     // ---- stage 3: agc2 + costas "PLL" per sample on the loop stream
@@ -870,6 +879,476 @@ int slice_qpsk(qrl_rx* h, const Slice& s)
     if (int rc2 = hand_off(h, h->ev_b[s.i], h->s_loop2, h->s_fec)) return rc2;
     launch_viterbi(h, s.nsoft_i, false);
     return QRL_OK;
+}
+
+// ---- receive create.  rx_create opens the handle and hands it to the create function of its chain: the tap design and loop constants
+// (gr_demod_*.cpp), stage 1 through rx_stage1, and the chain's own rings and states.  rx_create then adds the ports, the symbol-sync and
+// decoder states, the streams and the SM partition.
+
+// stage 1 (rational_resampler_ccf(L1, D1)): its taps (L1 > 1: arms), the double-buffered history and the ring r1; then the channel /
+// shaping filter taps (complex2: complex taps) with room for set_filter_width redesigns, and the demodulator taps
+int rx_stage1(qrl_rx* h, const std::vector<float>& taps1, const std::vector<float>& taps2, bool complex2, const std::vector<float>& taps3)
+{
+    h->ntaps1 = static_cast<int>(taps1.size());
+    h->Q1 = (h->ntaps1 + h->D1 - 1) / h->D1;
+    std::vector<float> tp;
+    if (h->L1 == 2) {               // 105 taps per arm, 128 history samples kept
+        tp = make_arms(taps1, 2, 105);
+        h->H = 128;
+    } else if (h->L1 > 2) {         // shape-generic rational resampler
+        h->nt_arm1 = arms_nt(taps1, h->L1);
+        tp = make_arms(taps1, h->L1, h->nt_arm1);
+        h->H = h->nt_arm1 + 8;
+    } else {
+        h->H = std::max(h->Q1 * h->D1, h->D1 == 2 ? 56 : 0);
+        tp = taps1;
+        tp.resize(h->H, 0.0f);
+    }
+    int rc = upload_floats(h, &h->d_taps1, tp);
+    if (!rc) rc = dev_alloc(h, &h->d_hist[0], static_cast<size_t>(h->H) * h->C);
+    if (!rc) rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C);
+    if (rc) return rc;
+    h->n1max = h->Tmax * h->L1 / h->D1 + 2;
+    h->ntaps2 = static_cast<int>(taps2.size()) / (complex2 ? 2 : 1);
+    h->ntaps3 = static_cast<int>(taps3.size());
+    std::vector<float> t2(std::max<size_t>(taps2.size(), 512), 0.0f);     // room for set_filter_width redesigns
+    std::copy(taps2.begin(), taps2.end(), t2.begin());
+    h->taps2_cap = t2.size();
+    if ((rc = upload_floats(h, &h->d_taps2, t2))) return rc;
+    if (!taps3.empty() && (rc = upload_floats(h, &h->d_taps3, taps3))) return rc;
+    return make_ring(h, &h->r1, sizeof(float2), h->n1max + std::max(512, static_cast<int>(taps2.size())) + 8);
+}
+
+// fll_band_edge_cc between stage 1 and the channel / shaping filter: its taps, state and history, and its output ring rf
+int rx_fll(qrl_rx* h, int sym_sps, float rolloff)
+{
+    h->fll = true;
+    int rc = upload_floats(h, &h->d_fll_taps, fll_design(static_cast<float>(sym_sps), rolloff, h->fllp.N));
+    if (!rc) rc = dev_alloc(h, &h->d_fll, h->C);
+    if (!rc) rc = dev_alloc(h, &h->d_fll_hist, static_cast<size_t>(32) * h->C);
+    if (rc) return rc;
+    h->zero_list.emplace_back(h->d_fll_hist, sizeof(float2) * 32 * h->C);
+    h->zero_list.emplace_back(h->d_fll, sizeof(FllState) * h->C);
+    return make_ring(h, &h->rf, sizeof(float2), h->n1max + 512 + 8);
+}
+
+// the symbol sync's period bounds sps +- dev, its window lookahead and its first whole step (alpha set by clock_loop_gains)
+void symsync_periods(SymSyncParams& p, float dev)
+{
+    p.max_period = p.sps + dev; p.min_period = p.sps - dev;
+    p.lookahead = 8 + static_cast<int>(ceilf(p.max_period)) + 1;
+    p.n0 = static_cast<int>(floorf(p.min_period - fabsf(p.alpha)));
+    p.fl0 = static_cast<float>(p.n0);
+}
+
+// QPSK, BPSK and the 4FSK band-pass bank run their symbol sync in 128-row windows
+int check_window_128(qrl_rx* h)
+{
+    if (h->ssp.lookahead > 0 && symsync_stride(128, h->ssp.lookahead) < 32) {
+        set_err(h, "symbol-sync lookahead does not fit the 128-row window of the complex-symbol kernels");
+        return QRL_EINVAL;
+    }
+    return QRL_OK;
+}
+
+// QPSK / BPSK: shaping-filter output and loop output are channel-interleaved complex rings; the agc2 + Costas state
+int psk_rings(qrl_rx* h)
+{
+    int rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 600, true);
+    if (!rc) rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true);
+    if (!rc) rc = dev_alloc(h, &h->d_ac, h->C);
+    return rc;
+}
+
+// gr_demod_4fsk.cpp:46-84 (sps ladder), :98-107 (resampler), :108-109 (filter), :125-131 (demod, RRC, sync).  gr_demod_m17.cpp:30-113 is
+// the FM chain behind a x3 / 125 rational resampler (24 ksps, 5 samples per symbol) with a hard-decision bit tail instead of the FEC.
+// gr_demod_dmr.cpp:32-112 is that M17 chain again with its own stage-1 taps, no IF filter, a 0.2 roll-off symbol filter tapped as (float)
+// port 3, the PLAIN Mueller & Mueller detector in the symbol sync and x0.9 in front of the phase modulator.
+int create_4fsk(qrl_rx* h, int sps, int samp_rate, int filter_width, int& sym_sps)
+{
+    const bool dmr = h->chain == RxChain::Dmr, m17 = hard_bits(h), fm = h->chain != RxChain::Fsk4Bank;
+    int decimation = 1, interpolation = 1, nfilts = 0, tsr = 0;
+    if (dmr) { tsr = 24000; sym_sps = 5; decimation = 125; interpolation = 3; nfilts = 25 * sym_sps; }           // gr_demod_dmr.cpp:38-45
+    else if (m17) { tsr = 24000; sym_sps = 5; decimation = 125; interpolation = 3; nfilts = 50 * sym_sps; }      // gr_demod_m17.cpp:37-48
+    else if (sps == 1) { tsr = 80000; sym_sps = sps * 8; decimation = 25; interpolation = 2; nfilts = 32 * sym_sps; }
+    else if (sps == 5) { tsr = 20000; sym_sps = sps * 2; decimation = 50; nfilts = 25 * sym_sps; }
+    else if (sps == 10) { tsr = 10000; sym_sps = sps; decimation = 100; nfilts = 25 * sym_sps; }
+    else if (sps == 2) { decimation = 2; sym_sps = 5; tsr = 500000; nfilts = 50 * sym_sps; }
+    else { set_err(h, "make_gr_demod_4fsk: unsupported sps"); return QRL_EINVAL; }
+    h->tsr = tsr;
+    if ((nfilts % 2) == 0) nfilts += 1;
+    const std::vector<float> taps1 = dmr ? low_pass_2(3, 3.0 * samp_rate, 5000, 2000, 60, WIN_BLACKMAN_HARRIS)       // gr_demod_dmr.cpp:54-55
+                                         : low_pass(interpolation, static_cast<double>(interpolation) * samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
+    h->D1 = decimation; h->L1 = interpolation;
+    const std::vector<float> taps2 = dmr ? std::vector<float>{ 1.0f }     // no IF filter in gr_demod_dmr: the stage runs as a 1-tap pass-through
+                                   : m17 ? low_pass(1, tsr, filter_width, filter_width, WIN_BLACKMAN_HARRIS)       // gr_demod_m17.cpp:58-59
+                                         : low_pass(1, tsr, filter_width, filter_width / 2, WIN_BLACKMAN_HARRIS);
+    const std::vector<float> taps3 = dmr ? root_raised_cosine(1, tsr, tsr / sym_sps, 0.2, nfilts)                  // gr_demod_dmr.cpp:61-62
+                                         : root_raised_cosine(1.5, tsr, tsr / sym_sps, m17 ? 0.5 : 0.2, nfilts);
+    const float m17_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
+    h->qd_gain = dmr ? static_cast<float>(tsr / (kPi / 2 * m17_rate))                               // gr_demod_dmr.cpp:71
+                     : static_cast<float>(sym_sps / (1 * kPi));
+    const float dev = dmr ? 0.06f : (m17 ? 500.0f / m17_rate : 0.05f);                              // gr_demod_m17.cpp:67-70, gr_demod_dmr.cpp:68
+    clock_loop_gains(dmr ? static_cast<float>(2 * kPi / 100.0f)
+                         : (m17 ? static_cast<float>(2 * kPi / (m17_rate / 50)) : static_cast<float>(2 * kPi / 200.0f)), 1.0f, 0.2869f,
+                     h->ssp.alpha, h->ssp.beta);
+    if (dmr) h->ssp.sym_scale = 0.9f;                                                               // gr_demod_dmr.cpp:72
+    h->ssp.sps = static_cast<float>(sym_sps);
+    h->ssp.pm_sens = static_cast<float>(kPi / 2);
+    h->ssp.soft_scale = 128.0f;
+    symsync_periods(h->ssp, dev);
+    h->nports = dmr ? 4 : 3;
+    if (dmr) h->port3_isz = 4;
+    int rc;
+    if (!fm) {     // gr_demod_4fsk.cpp:110-124: four complex band-pass filters + discriminator + symbol filter
+        int rs = 0, bw = 0;
+        if (sps == 1) { rs = 10000; bw = 4000; } else if (sps == 5) { rs = 2000; bw = 4000; } else if (sps == 10) { rs = 1000; bw = 2000; }
+        else { set_err(h, "make_gr_demod_4fsk: non-FM variant needs sps 1, 5 or 10"); return QRL_EINVAL; }
+        const int fw = filter_width;
+        const double lo[4] = { double(-fw), double(-fw + rs), 0.0, double(fw - rs) }, hi[4] = { double(-fw + rs), 0.0, double(fw - rs), double(fw) };
+        std::vector<float> bank;
+        for (int b = 0; b < 4; b++) {
+            std::vector<float> t = complex_band_pass(1, tsr, lo[b], hi[b], bw, WIN_BLACKMAN_HARRIS);
+            h->nt_bank = static_cast<int>(t.size() / 2);
+            bank.insert(bank.end(), t.begin(), t.end());
+        }
+        if ((rc = upload_floats(h, &h->d_bank_taps, bank))) return rc;
+        std::vector<float> sf = low_pass(1.0, tsr, tsr / sym_sps, tsr / sym_sps / 20, WIN_BLACKMAN_HARRIS);
+        h->nt_symf = static_cast<int>(sf.size());
+        if ((rc = upload_floats(h, &h->d_symf_taps, sf))) return rc;
+    }
+    if ((rc = rx_stage1(h, taps1, taps2, false, taps3))) return rc;
+    if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + h->ntaps3 + 64))) return rc;
+    // two calls deep when the block may run with overlapped calls (the producer of call k+1 must not wait for the consumer of call k)
+    if ((rc = make_ring(h, &h->r4, sizeof(float), (fm ? 2 : 1) * h->n1max + 600, true))) return rc;
+    if (!fm) {
+        if ((rc = make_ring(h, &h->rbank, sizeof(float2), h->n1max + h->nt_symf + 16))) return rc;
+        if ((rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true))) return rc;
+        return check_window_128(h);
+    }
+    // scratch of the external symbol-sync epilogue: [groups][chunks][maxs + 2][32] floats + a 128-int header per group
+    // window size: 512 rows x 2 stages when the replicated interpolator bank still fits next to it, else 256 x 3
+    h->ss_ch = symsync_ext_smem(h->ssp, 512, 2, true) <= 220 * 1024 ? 512 : 256;
+    if (const char* e = getenv("QRL_SS_CH")) { const int v = atoi(e); if (v == 512 || v == 256) h->ss_ch = v; }
+    const int maxs = symsync_maxs(h->ssp, h->ss_ch);
+    h->ss_chunk_cap = h->n1max / symsync_stride(h->ss_ch, h->ssp.lookahead) + 4 + 3 * qrl_rx::kMaxSub;
+    const size_t groups = (h->C + 31) / 32;
+    if ((rc = dev_alloc(h, &h->d_ss_scratch, groups * h->ss_chunk_cap * (maxs + 2) * 32))) return rc;
+    return dev_alloc(h, &h->d_ss_hdr, groups * 128 * qrl_rx::kMaxSub);
+}
+
+// gr_demod_2fsk.cpp:39-130 (fm variant; band filters :88-100).  gr_demod_gmsk.cpp:30-134 is the FM chain without the band-edge FLL, with
+// a plain low-pass as symbol filter and its own clock-loop constants.
+int create_2fsk(qrl_rx* h, int sps, int samp_rate, int filter_width, int& sym_sps)
+{
+    const bool gmsk = h->chain == RxChain::Gmsk, band = h->chain == RxChain::Fsk2Bank;
+    int decim, nfilts, interp = 1, tsr;
+    if (sps == 10) { tsr = 20000; sym_sps = sps; decim = 50; nfilts = 35 * sym_sps; }
+    else if (sps >= 5) { tsr = 40000; sym_sps = sps * 2; decim = 25; nfilts = 35 * sym_sps; }
+    else if (sps == 1) { tsr = 80000; sym_sps = 4; decim = 25; interp = 2; nfilts = 125 * sym_sps; }
+    else { set_err(h, "make_gr_demod_2fsk: unsupported sps"); return QRL_EINVAL; }
+    h->tsr = tsr;
+    h->L1 = interp; h->D1 = decim;
+    if ((nfilts % 2) == 0) nfilts += 1;
+    int rc;
+    if (band) {     // gr_demod_2fsk.cpp:88-100: upper (-fw,0) / lower (0,fw) band filters, ratio detector, symbol filter
+        std::vector<float> bank = complex_band_pass(1, tsr, -filter_width, 0, filter_width, WIN_BLACKMAN_HARRIS);
+        std::vector<float> lower = complex_band_pass(1, tsr, 0, filter_width, filter_width, WIN_BLACKMAN_HARRIS);
+        h->nt_bank = static_cast<int>(bank.size() / 2);
+        bank.insert(bank.end(), lower.begin(), lower.end());
+        if ((rc = upload_floats(h, &h->d_bank_taps, bank))) return rc;
+        std::vector<float> sf = low_pass(1.0, tsr, tsr / sym_sps, tsr / sym_sps, WIN_HAMMING);
+        h->nt_symf = static_cast<int>(sf.size());
+        if ((rc = upload_floats(h, &h->d_symf_taps, sf))) return rc;
+    }
+    const std::vector<float> taps3 = gmsk ? low_pass(1, tsr, tsr / sym_sps, tsr / sym_sps, WIN_HAMMING)      // gr_demod_gmsk.cpp:88-90
+                                          : root_raised_cosine(1, tsr, tsr / sym_sps, 0.2, nfilts);
+    h->qd_gain = static_cast<float>(sym_sps / (1 * kPi / 2));
+    const float symbol_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
+    const float sps_dev = gmsk ? 0.05f : 200.0f / symbol_rate;                                    // gr_demod_gmsk.cpp:79-84
+    clock_loop_gains(gmsk ? static_cast<float>(2 * kPi / 200.0f) : static_cast<float>(2 * kPi / (symbol_rate / 10)), 1.0f, 0.2869f,
+                     h->ssp.alpha, h->ssp.beta);
+    h->ssp.sps = static_cast<float>(sym_sps);
+    h->ssp.soft_scale = 128.0f;
+    symsync_periods(h->ssp, sps_dev);
+    h->nports = 4;
+    rc = rx_stage1(h, low_pass(interp, static_cast<double>(interp) * samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                   low_pass(1, tsr, filter_width, filter_width, WIN_BLACKMAN_HARRIS), false, taps3);
+    if (!rc && !gmsk) {
+        h->fllp.N = 16;
+        control_loop_gains(static_cast<float>(24 * kPi / 100), h->fllp.alpha, h->fllp.beta);
+        h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sym_sps)); h->fllp.min_freq = -h->fllp.max_freq;
+        rc = rx_fll(h, sym_sps, 0.1f);
+    }
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + h->ntaps3 + 64);
+    if (!rc) rc = make_ring(h, &h->r4, sizeof(float), h->n1max + 600, true);
+    if (!rc && band) rc = make_ring(h, &h->rbank, sizeof(float), h->n1max + h->nt_symf + 16);
+    return rc;
+}
+
+// gr_demod_bpsk.cpp:40-76
+int create_bpsk(qrl_rx* h, int sps, int samp_rate, int& sym_sps)
+{
+    const int tsr = 20000;
+    h->tsr = tsr; sym_sps = sps;
+    h->D1 = 50;
+    h->acp.attack = 1e-1f; h->acp.decay = 1e-1f; h->acp.ref = 1.0f; h->acp.max_gain = 65536.0f; h->acp.order = 0;
+    const float gain_mu = 0.05f, gain_omega = 0.005f;
+    h->ssp.loop_kind = LOOP_CRMM;
+    h->ssp.sps = static_cast<float>(sps);
+    h->ssp.gain_omega = gain_omega * gain_omega; h->ssp.gain_mu = gain_mu;
+    h->ssp.omega_mid = static_cast<float>(sps); h->ssp.omega_lim = 0.001f * static_cast<float>(sps);
+    h->ssp.lookahead = 24;
+    h->ssp.max_period = static_cast<float>(sps) + 1.0f; h->ssp.min_period = static_cast<float>(sps) - 1.0f;   // bounds for buffer sizing only
+    h->ssp.alpha = 0.0f;
+    control_loop_gains(static_cast<float>(2 * kPi / 200), h->ssp.costas_alpha, h->ssp.costas_beta);
+    h->ssp.soft_scale = 64.0f;
+    h->fllp.N = 32;
+    control_loop_gains(static_cast<float>(8 * kPi / 100), h->fllp.alpha, h->fllp.beta);
+    h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sps)); h->fllp.min_freq = -h->fllp.max_freq;
+    h->nports = 4;
+    int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS), root_raised_cosine(sps, sps, 1, 0.35, 15 * sps), false, {});
+    if (!rc) rc = rx_fll(h, sps, 0.35f);
+    if (!rc) rc = psk_rings(h);
+    if (!rc) rc = check_window_128(h);
+    return rc;
+}
+
+// gr_demod_qpsk.cpp:46-71 (sps ladder), :98-103 (resampler), :106-110 (RRC), :104,113-118 (agc, sync, costas)
+int create_qpsk(qrl_rx* h, int sps, int samp_rate, int& sym_sps)
+{
+    int decimation, tsr; float costas_bw = static_cast<float>(kPi / 200);
+    if (sps > 4 && sps < 125) { decimation = 25; sym_sps = sps * 4 / 25; tsr = 40000; }
+    else if (sps >= 125) { decimation = 100; sym_sps = sps / 25; tsr = 10000; }
+    else { decimation = 2; sym_sps = sps; tsr = 500000; costas_bw = static_cast<float>(kPi / 400); }
+    h->tsr = tsr;
+    h->D1 = decimation;
+    h->acp.attack = 1.0f; h->acp.decay = 1e-1f; h->acp.ref = 1.0f; h->acp.max_gain = 65536.0f;
+    control_loop_gains(static_cast<float>(kPi / 200 / sym_sps), h->acp.alpha, h->acp.beta);
+    h->acp.order = 4; h->acp.use_snr = 1;
+    const float symbol_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
+    const float sps_dev = 200.0f / symbol_rate;
+    clock_loop_gains(static_cast<float>(2 * kPi / (symbol_rate / 10)), 1.0f, 0.2869f, h->ssp.alpha, h->ssp.beta);
+    h->ssp.sps = static_cast<float>(sym_sps);
+    control_loop_gains(costas_bw, h->ssp.costas_alpha, h->ssp.costas_beta);
+    const float th = static_cast<float>(-3 * kPi / 4);
+    h->ssp.rot_r = cosf(th); h->ssp.rot_i = sinf(th);
+    h->ssp.soft_scale = 48.0f;
+    symsync_periods(h->ssp, sps_dev);
+    h->nports = 3;
+    int rc = rx_stage1(h, low_pass_2(1, static_cast<double>(samp_rate), tsr / 2, tsr / 10, 60, WIN_BLACKMAN_HARRIS),
+                       root_raised_cosine(sym_sps, sym_sps, 1, 0.35, 11 * sym_sps), false, {});
+    if (!rc && sps > 4) {      // gr_demod_qpsk.cpp:105,130-134: FLL between the resampler and the shaping filter
+        h->fllp.N = 32;
+        control_loop_gains(static_cast<float>(2 * kPi / 100), h->fllp.alpha, h->fllp.beta);
+        h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sym_sps)); h->fllp.min_freq = -h->fllp.max_freq;
+        rc = rx_fll(h, sym_sps, 0.35f);
+    }
+    if (!rc) rc = psk_rings(h);
+    if (!rc) rc = check_window_128(h);
+    return rc;
+}
+
+// gr_demod_dsss.cpp:32-124 (instance gr_demod_base.cpp:218: make_gr_demod_dsss(25, 1e6, 1700, 150)); sps = items per chip at 5200 sps
+int create_dsss(qrl_rx* h, int sps, int samp_rate, int filter_width)
+{
+    const int tsr = 20000;
+    h->tsr = tsr;
+    h->D1 = 50;
+    const std::vector<float> tif = low_pass(1, 20000, 5200 / 2, 5200 / 2, WIN_BLACKMAN_HARRIS);       // rational_resampler_ccf(13, 50)
+    const std::vector<float> taps2 = low_pass(1, 5200, filter_width, 1200, WIN_BLACKMAN_HARRIS);
+    DsssParams& d = h->dsp;
+    d.nt_arm = (static_cast<int>(tif.size()) + 12) / 13; d.nt2 = static_cast<int>(taps2.size());
+    d.N = sps * 13; d.ntaps = d.N + 11 * sps;
+    if (sps < 1 || d.nt_arm > 8 || d.nt2 > 64 || d.ntaps > 640 || d.N + d.ntaps - 1 > kDsssChunk) {
+        set_err(h, "make_gr_demod_dsss: sps / filter_width outside what the chain kernel holds in shared memory"); return QRL_EINVAL;
+    }
+    int rc = upload_floats(h, &h->d_ds_arms, make_arms(tif, 13, d.nt_arm));
+    if (rc) return rc;
+    {   // dsss_decoder_cc_impl.cc:60-96: reversed Barker-13, `sps` items per chip, shaped by RRC(1, sps, 1, 0.35f, 11 sps); the block's
+        // fir_filter_ccc keeps the taps reversed (what is uploaded)
+        static const int barker_13[13] = { 1, 1, 1, 1, 1, 0, 0, 1, 1, 0, 1, 0, 1 };
+        const int extra = 11 * sps, total = d.N + 2 * extra;
+        std::vector<float> cs(total, 0.0f);
+        for (int i = 0; i < 13; i++) { const float cv = barker_13[13 - (i + 1)] == 0 ? -1.0f : 1.0f; for (int k = 0; k < sps; k++) cs[extra + i * sps + k] = cv; }
+        const std::vector<float> rrc = root_raised_cosine(1, sps, 1.0, static_cast<double>(0.350f), extra);
+        const int nr = static_cast<int>(rrc.size());
+        std::vector<float> t(2 * static_cast<size_t>(d.ntaps));
+        for (int i = 0; i < d.ntaps; i++) {
+            float acc = 0.0f, acci = 0.0f;
+            for (int k = 0; k < nr; k++) { acc = acc + cs[i + k] * rrc[nr - 1 - k]; acci = acci + 0.0f * rrc[nr - 1 - k]; }
+            t[2 * (d.ntaps - 1 - i)] = acc; t[2 * (d.ntaps - 1 - i) + 1] = acci;
+        }
+        float* tp = nullptr;
+        if ((rc = upload_floats(h, &tp, t))) return rc;
+        h->d_ds_taps = reinterpret_cast<float2*>(tp);
+    }
+    control_loop_gains(static_cast<float>(kPi / 200), d.pll_alpha, d.pll_beta);
+    control_loop_gains(static_cast<float>(2 * kPi / 100), d.costas_alpha, d.costas_beta);
+    d.agc_attack = 1e-1f; d.agc_decay = 1e-1f; d.agc_ref = 1.0f; d.agc_max = 65536.0f;
+    const float gain_mu = 0.05f, gain_omega = 0.005f;
+    d.gain_omega = gain_omega * gain_omega; d.gain_mu = gain_mu; d.omega_mid = 1.0f; d.omega_lim = 0.005f * 1.0f; d.soft_scale = 64.0f;
+    h->nports = 4;
+    rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS), taps2, false, {});
+    if (rc) return rc;
+    const long long n5 = h->n1max * 13 / 50 + 8;
+    if ((rc = make_ring(h, &h->ds_a, sizeof(float2), n5 + 2048))) return rc;
+    if ((rc = make_ring(h, &h->ds_c, sizeof(float2), n5 + 2048))) return rc;
+    if ((rc = make_ring(h, &h->ds_d, sizeof(float2), n5 / h->dsp.N + 128))) return rc;
+    return dev_alloc(h, &h->d_ds, h->C);
+}
+
+// gr_demod_nbfm.cpp:39-66
+int create_nbfm(qrl_rx* h, int samp_rate, int filter_width)
+{
+    const int tsr = 20000;
+    h->tsr = tsr;
+    h->D1 = 50;
+    h->qd_gain = static_cast<float>(tsr / (4 * kPi * filter_width));
+    h->nports = 2; h->port1_isz = 4;
+    int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                       low_pass_2(1, tsr, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS), false, {});
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (rc) return rc;
+    std::vector<float> audio_rs = low_pass_2(2, 2 * tsr, 3600, 250, 60, WIN_BLACKMAN_HARRIS);
+    std::vector<float> audio_f = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
+    const int nt_arm = arms_nt(audio_rs, 2);
+    rc = upload_floats(h, &h->d_arm_taps, make_arms(audio_rs, 2, nt_arm));
+    if (!rc) rc = upload_floats(h, &h->d_audio_taps, audio_f);
+    if (rc) return rc;
+    const int ramp = 320;
+    std::vector<float> env(ramp + 1);
+    for (int k = 0; k <= ramp; k++) env[k] = static_cast<float>(0.5 - std::cos(kPi * k / ramp) / 2.0);
+    if ((rc = upload_floats(h, &h->d_env, env))) return rc;
+    double a[2], b[2];
+    deemph_taps(tsr, 50e-6, a, b);
+    h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = ramp; h->nbp.sq_gate = 1;
+    h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
+    h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 2.0f;
+    if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return rc;
+    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return rc;
+    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return rc;
+    if ((rc = dev_alloc(h, &h->d_nb, h->C))) return rc;
+    // analog::ctcss_squelch_ff::make(8000, 88.5, 0.01, 8000, 160, true) (gr_demod_nbfm.cpp:60), out of the graph until set_ctcss(f)
+    if ((rc = make_ring(h, &h->rq, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 64))) return rc;
+    h->ctc.on = 0; h->ctc.len = 8000; h->ctc.ramp = 160; h->ctc.gate = 1; h->ctc.level = 0.01f;
+    std::vector<double> ce(h->ctc.ramp + 1);
+    for (int k = 0; k <= h->ctc.ramp; k++) ce[k] = 0.5 - std::cos(kPi * k / h->ctc.ramp) / 2.0;       // squelch_base_ff envelope (double)
+    if ((rc = dev_alloc(h, &h->d_cenv, ce.size(), false))) return rc;
+    if (cudaMemcpy(h->d_cenv, ce.data(), sizeof(double) * ce.size(), cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "envelope upload failed"); return QRL_ECUDA; }
+    // (an FP64 instruction occupies an SM's FP64 pipe for ~64 cycles whatever its lane count, so two recurrences only overlap on
+    // DIFFERENT SMs: both kernels then ask for more than half an SM's shared memory, which keeps their CTAs one per SM and apart, and
+    // the split is used while each kernel's C CTAs fit the SMs at once -- on an H100 it is faster up to 128 channels, slower at 160)
+    int n_sm = 0;
+    if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess) { set_err(h, "SM count query failed"); return QRL_ECUDA; }
+    if (h->C <= n_sm && !getenv("QRL_NBFM_NO_SPLIT")) {
+        if ((rc = make_ring(h, &h->raud, sizeof(float), h->n1max * 2 / 5 + 64))) return rc;
+        if ((rc = dev_alloc(h, &h->d_nb2, h->C))) return rc;
+        h->zero_list.emplace_back(h->d_nb2, sizeof(NbfmDeemphState) * h->C);
+        h->nbfm_split = true;
+    }
+    return QRL_OK;
+}
+
+// gr_demod_am.cpp:35-70: the NBFM audio kernel in detector mode 1
+int create_am(qrl_rx* h, int samp_rate, int filter_width)
+{
+    const int tsr = 20000;
+    h->tsr = tsr;
+    h->D1 = 50;
+    h->nports = 2; h->port1_isz = 4;
+    int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                       complex_band_pass_2(1, tsr, -filter_width, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (rc) return rc;
+    std::vector<float> audio_rs = low_pass(2, 2 * tsr, 3600, 600, WIN_BLACKMAN_HARRIS);
+    std::vector<float> audio_f = low_pass(1, 8000, 3600, 300, WIN_BLACKMAN_HARRIS);
+    const int nt_arm = arms_nt(audio_rs, 2);
+    rc = upload_floats(h, &h->d_arm_taps, make_arms(audio_rs, 2, nt_arm));
+    if (!rc) rc = upload_floats(h, &h->d_audio_taps, audio_f);
+    if (rc) return rc;
+    if ((rc = upload_floats(h, &h->d_env, std::vector<float>{ 1.0f, 1.0f }))) return rc;
+    h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = 0; h->nbp.sq_gate = 1;
+    h->nbp.qd_gain = 0.0f; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
+    h->nbp.b0 = 1.0; h->nbp.b1 = -1.0; h->nbp.a1 = -0.9999; h->nbp.out_gain = 1.0f;      // iir_filter_ffd({1,-1},{0,0.9999}), old style
+    h->nbp.mode = 1; h->nbp.agc_attack = 1e-1f; h->nbp.agc_decay = 1e-1f; h->nbp.agc_ref = 1.0f; h->nbp.agc_max = 65536.0f; h->nbp.am_gain = 0.99f;
+    if ((rc = make_ring(h, &h->rg, sizeof(float2), 64))) return rc;
+    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return rc;
+    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return rc;
+    return dev_alloc(h, &h->d_nb, h->C);
+}
+
+// gr_demod_wbfm.cpp:35-64: the analog audio kernel in mode 2
+int create_wbfm(qrl_rx* h, int samp_rate, int filter_width)
+{
+    const int tsr = 200000;
+    h->tsr = tsr;
+    h->D1 = 5;
+    h->qd_gain = static_cast<float>(tsr / (2 * kPi * filter_width));
+    h->nports = 2; h->port1_isz = 4;
+    int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                       low_pass_2(1, tsr, filter_width, 600, 90, WIN_BLACKMAN_HARRIS), false, {});
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (rc) return rc;
+    std::vector<float> audio_rs = low_pass(1, tsr, 4000, 2000, WIN_BLACKMAN_HARRIS);
+    if ((rc = upload_floats(h, &h->d_audio_taps, audio_rs))) return rc;
+    if ((rc = upload_floats(h, &h->d_arm_taps, std::vector<float>{ 0.0f, 0.0f }))) return rc;
+    if ((rc = upload_floats(h, &h->d_env, std::vector<float>{ 1.0f, 1.0f }))) return rc;
+    double a[2], b[2];
+    deemph_taps(8000, 50e-6, a, b);                        // the reference designs them for 8 kHz (:39) and runs them at 200 ksps
+    h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = 0; h->nbp.sq_gate = 1;
+    h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = 1; h->nbp.nt_audio = static_cast<int>(audio_rs.size());
+    h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 1.0f;
+    h->nbp.mode = 2; h->nbp.am_gain = 0.9f;
+    if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return rc;
+    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + 16))) return rc;
+    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max + h->nbp.nt_audio + 16))) return rc;
+    return dev_alloc(h, &h->d_nb, h->C);
+}
+
+// gr_demod_ssb.cpp:37-61; sps = decimation (125)
+int create_ssb(qrl_rx* h, int sps, int samp_rate, int filter_width)
+{
+    const int tsr = 8000;
+    h->tsr = tsr;
+    h->D1 = sps;
+    h->nports = 2; h->port1_isz = 4;
+    int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                       h->lsb ? complex_band_pass_2(1, tsr, -filter_width, -200, 200, 90, WIN_BLACKMAN_HARRIS)
+                              : complex_band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (rc) return rc;
+    std::vector<float> audio_f = band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
+    if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return rc;
+    h->ssbp.sq_alpha = 0.01; h->ssbp.sq_threshold = std::pow(10.0, -140 / 10.0);
+    h->ssbp.attack = 1e-1f; h->ssbp.decay = 1e-1f; h->ssbp.ref = 0.25f; h->ssbp.max_gain = 65536.0f;
+    h->ssbp.clip = 0.95f; h->ssbp.emax = static_cast<float>(1 / (std::sqrt(0.5) / 2)); h->ssbp.out_gain = 1.333f;
+    h->ssbp.nt_audio = static_cast<int>(audio_f.size());
+    if ((rc = make_ring(h, &h->rclip, sizeof(float2), h->n1max + 16))) return rc;
+    if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->ssbp.nt_audio + 16))) return rc;
+    return dev_alloc(h, &h->d_ssb, h->C);
+}
+
+// gr_demod_freedv.cpp:40-54; sps = decimation to 8 ksps.  The stage-1 taps are low_pass(sps, ...): DC gain sps.  :57-77: agc2_ff(1e-1,
+// 1e-3, 0.5, 1) (max gain 65536) -> band_pass_2(1, 8000, 200, 3500, 200, 90, BH) -> x0.1 -> float_to_short(1, 32768); the
+// feedforward_agc_cc of :56 is never connected
+int create_freedv(qrl_rx* h, int sps, int samp_rate, int filter_width, int low_cutoff)
+{
+    const int tsr = 8000;
+    h->tsr = tsr;
+    h->D1 = sps;
+    h->nports = 2; h->port1_isz = 2;
+    int rc = rx_stage1(h, low_pass(sps, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
+                       h->lsb ? complex_band_pass_2(1, tsr, -filter_width, -low_cutoff, 200, 90, WIN_BLACKMAN_HARRIS)
+                              : complex_band_pass_2(1, tsr, low_cutoff, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
+    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (rc) return rc;
+    std::vector<float> audio_f = band_pass_2(1, tsr, 200, 3500, 200, 90, WIN_BLACKMAN_HARRIS);
+    if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return rc;
+    h->fdp.attack = 1e-1f; h->fdp.decay = 1e-3f; h->fdp.ref = 0.5f; h->fdp.max_gain = 65536.0f;
+    h->fdp.nt_audio = static_cast<int>(audio_f.size());
+    if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->fdp.nt_audio + 16))) return rc;
+    return dev_alloc(h, &h->d_fdv, h->C);
 }
 
 }  // namespace
@@ -900,481 +1379,77 @@ static int check_freedv_args(const char* who, int sps, int samp_rate, int filter
     return QRL_OK;
 }
 
-static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+static int rx_create(int kind, int sps, int samp_rate, int filter_width, int flag, int low_cutoff,
                      int n_channels, long max_samples, int device, qrl_rx** out);
 
-int qrl_rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag,
+int qrl_rx_create(int kind, int sps, int samp_rate, int /*carrier_freq*/, int filter_width, int flag,
                   int n_channels, long max_samples, int device, qrl_rx** out)
 {
     if (kind == QRL_DEMOD_FREEDV) { set_err(nullptr, "qrl_rx_create: QRL_DEMOD_FREEDV takes a low cutoff: use qrl_rx_create_freedv"); return QRL_EINVAL; }
-    return rx_create(kind, sps, samp_rate, carrier_freq, filter_width, flag, 0, n_channels, max_samples, device, out);
+    return rx_create(kind, sps, samp_rate, filter_width, flag, 0, n_channels, max_samples, device, out);
 }
 
-int qrl_rx_create_freedv(int sps, int samp_rate, int carrier_freq, int filter_width, int low_cutoff, int sb,
+int qrl_rx_create_freedv(int sps, int samp_rate, int /*carrier_freq*/, int filter_width, int low_cutoff, int sb,
                          int n_channels, long max_samples, int device, qrl_rx** out)
 {
     int rc = check_freedv_args("qrl_rx_create_freedv", sps, samp_rate, filter_width, low_cutoff);
     if (rc) return rc;
-    return rx_create(QRL_DEMOD_FREEDV, sps, samp_rate, carrier_freq, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_samples, device, out);
+    return rx_create(QRL_DEMOD_FREEDV, sps, samp_rate, filter_width, sb ? 1 : 0, low_cutoff, n_channels, max_samples, device, out);
 }
 
-static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int filter_width, int flag, int low_cutoff,
+static int rx_create(int kind, int sps, int samp_rate, int filter_width, int flag, int low_cutoff,
                      int n_channels, long max_samples, int device, qrl_rx** out)
 {
     if (!out || n_channels <= 0 || max_samples <= 0) { set_err(nullptr, "qrl_rx_create: bad argument"); return QRL_EINVAL; }
     *out = nullptr;
     if (int rc = check_device("qrl_rx_create", device)) return rc;
-    // gr_demod_gmsk.cpp:30-134 is the 2FSK (fm) chain without the band-edge FLL, with a plain low-pass as symbol filter and its
-    // own clock-loop constants: it runs through the 2FSK code path
-    const bool gmsk = (kind == QRL_DEMOD_GMSK);
-    if (gmsk) { kind = QRL_DEMOD_2FSK; flag = 1; }
-    // gr_demod_m17.cpp:30-113 is the 4FSK (fm) chain behind a x3 / 125 rational resampler (24 ksps, 5 samples per symbol) with a
-    // hard-decision bit tail instead of the FEC: it runs through the 4FSK code path
-    // gr_demod_dmr.cpp:32-112 is that M17 chain again with its own stage-1 taps, no IF filter, a 0.2 roll-off symbol filter tapped as
-    // (float) port 3, the PLAIN Mueller & Mueller detector in the symbol sync and x0.9 in front of the phase modulator
-    const bool dmr = (kind == QRL_DEMOD_DMR);
-    const bool m17 = (kind == QRL_DEMOD_M17) || dmr;
-    if (m17) { kind = QRL_DEMOD_4FSK; flag = 1; }
-    if (dmr) { carrier_freq = 0; filter_width = 5000; }
     qrl_rx* h = new qrl_rx();
-    h->kind = kind; h->sps = sps; h->samp_rate = samp_rate; h->carrier_freq = carrier_freq;
-    h->filter_width = filter_width; h->flag = flag; h->C = n_channels; h->Tmax = max_samples;
-    h->gmsk = gmsk; h->m17 = m17; h->dmr = dmr;
+    h->samp_rate = samp_rate; h->C = n_channels; h->Tmax = max_samples;
     auto fail = [&](int rc) { return create_failed(h, qrl_rx_destroy, rc); };
     int rc = handle_open(h, device);
     if (!rc) rc = upload_tables(h);
     if (rc) return fail(rc);
-
-    std::vector<float> taps1, taps2, taps3;
-    int tsr = 0, sym_sps = 0;
-    if (kind == QRL_DEMOD_4FSK) {
-        // gr_demod_4fsk.cpp:46-84 (sps ladder), :98-107 (resampler), :108-109 (filter), :125-131 (demod, RRC, sync)
-        int decimation = 1, interpolation = 1, nfilts = 0;
-        if (dmr) { tsr = 24000; sym_sps = 5; decimation = 125; interpolation = 3; nfilts = 25 * sym_sps; }           // gr_demod_dmr.cpp:38-45
-        else if (m17) { tsr = 24000; sym_sps = 5; decimation = 125; interpolation = 3; nfilts = 50 * sym_sps; }      // gr_demod_m17.cpp:37-48
-        else if (sps == 1) { tsr = 80000; sym_sps = sps * 8; decimation = 25; interpolation = 2; nfilts = 32 * sym_sps; }
-        else if (sps == 5) { tsr = 20000; sym_sps = sps * 2; decimation = 50; nfilts = 25 * sym_sps; }
-        else if (sps == 10) { tsr = 10000; sym_sps = sps; decimation = 100; nfilts = 25 * sym_sps; }
-        else if (sps == 2) { decimation = 2; sym_sps = 5; tsr = 500000; nfilts = 50 * sym_sps; }
-        else { set_err(h, "make_gr_demod_4fsk: unsupported sps"); return fail(QRL_EINVAL); }
-        if ((nfilts % 2) == 0) nfilts += 1;
-        taps1 = dmr ? low_pass_2(3, 3.0 * samp_rate, 5000, 2000, 60, WIN_BLACKMAN_HARRIS)              // gr_demod_dmr.cpp:54-55
-                    : low_pass(interpolation, static_cast<double>(interpolation) * samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = decimation; h->L1 = interpolation;
-        taps2 = dmr ? std::vector<float>{ 1.0f }                // no IF filter in gr_demod_dmr: the stage runs as a 1-tap pass-through
-              : m17 ? low_pass(1, tsr, filter_width, filter_width, WIN_BLACKMAN_HARRIS)                 // gr_demod_m17.cpp:58-59
-                    : low_pass(1, tsr, filter_width, filter_width / 2, WIN_BLACKMAN_HARRIS);
-        taps3 = dmr ? root_raised_cosine(1, tsr, tsr / sym_sps, 0.2, nfilts)                            // gr_demod_dmr.cpp:61-62
-                    : root_raised_cosine(1.5, tsr, tsr / sym_sps, m17 ? 0.5 : 0.2, nfilts);
-        const float m17_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
-        h->qd_gain = dmr ? static_cast<float>(tsr / (kPi / 2 * m17_rate))                               // gr_demod_dmr.cpp:71
-                         : static_cast<float>(sym_sps / (1 * kPi));
-        const float dev = dmr ? 0.06f : (m17 ? 500.0f / m17_rate : 0.05f);                              // gr_demod_m17.cpp:67-70, gr_demod_dmr.cpp:68
-        clock_loop_gains(dmr ? static_cast<float>(2 * kPi / 100.0f)
-                             : (m17 ? static_cast<float>(2 * kPi / (m17_rate / 50)) : static_cast<float>(2 * kPi / 200.0f)), 1.0f, 0.2869f,
-                         h->ssp.alpha, h->ssp.beta);
-        if (dmr) h->ssp.sym_scale = 0.9f;                                                               // gr_demod_dmr.cpp:72
-        h->ssp.sps = static_cast<float>(sym_sps);
-        h->ssp.max_period = h->ssp.sps + dev; h->ssp.min_period = h->ssp.sps - dev;
-        h->ssp.lookahead = 8 + static_cast<int>(ceilf(h->ssp.max_period)) + 1;
-        h->ssp.pm_sens = static_cast<float>(kPi / 2);
-        h->ssp.soft_scale = 128.0f;
-        h->ssp.n0 = static_cast<int>(floorf(h->ssp.min_period - fabsf(h->ssp.alpha)));
-        h->ssp.fl0 = static_cast<float>(h->ssp.n0);
-        h->nports = dmr ? 4 : 3;
-        if (!flag) {     // gr_demod_4fsk.cpp:110-124: four complex band-pass filters + discriminator + symbol filter
-            int rs = 0, bw = 0;
-            if (sps == 1) { rs = 10000; bw = 4000; } else if (sps == 5) { rs = 2000; bw = 4000; } else if (sps == 10) { rs = 1000; bw = 2000; }
-            else { set_err(h, "make_gr_demod_4fsk: non-FM variant needs sps 1, 5 or 10"); return fail(QRL_EINVAL); }
-            const int fw = filter_width;
-            const double lo[4] = { double(-fw), double(-fw + rs), 0.0, double(fw - rs) }, hi[4] = { double(-fw + rs), 0.0, double(fw - rs), double(fw) };
-            std::vector<float> bank;
-            for (int b = 0; b < 4; b++) {
-                std::vector<float> t = complex_band_pass(1, tsr, lo[b], hi[b], bw, WIN_BLACKMAN_HARRIS);
-                h->nt_bank = static_cast<int>(t.size() / 2);
-                bank.insert(bank.end(), t.begin(), t.end());
-            }
-            if ((rc = upload_floats(h, &h->d_bank_taps, bank))) return fail(rc);
-            std::vector<float> sf = low_pass(1.0, tsr, tsr / sym_sps, tsr / sym_sps / 20, WIN_BLACKMAN_HARRIS);
-            h->nt_symf = static_cast<int>(sf.size());
-            if ((rc = upload_floats(h, &h->d_symf_taps, sf))) return fail(rc);
-        }
-    } else if (kind == QRL_DEMOD_QPSK) {
-        // gr_demod_qpsk.cpp:46-71 (sps ladder), :98-103 (resampler), :106-110 (RRC), :104,113-118 (agc, sync, costas)
-        int decimation; float costas_bw = static_cast<float>(kPi / 200);
-        if (sps > 4 && sps < 125) { decimation = 25; sym_sps = sps * 4 / 25; tsr = 40000; }
-        else if (sps >= 125) { decimation = 100; sym_sps = sps / 25; tsr = 10000; }
-        else { decimation = 2; sym_sps = sps; tsr = 500000; costas_bw = static_cast<float>(kPi / 400); }
-        if (sps > 4) {      // gr_demod_qpsk.cpp:105,130-134: FLL between the resampler and the shaping filter
-            h->fllp.N = 32;
-            control_loop_gains(static_cast<float>(2 * kPi / 100), h->fllp.alpha, h->fllp.beta);
-            h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sym_sps)); h->fllp.min_freq = -h->fllp.max_freq;
-        }
-        taps1 = low_pass_2(1, static_cast<double>(samp_rate), tsr / 2, tsr / 10, 60, WIN_BLACKMAN_HARRIS);
-        h->D1 = decimation;
-        taps2 = root_raised_cosine(sym_sps, sym_sps, 1, 0.35, 11 * sym_sps);
-        h->acp.attack = 1.0f; h->acp.decay = 1e-1f; h->acp.ref = 1.0f; h->acp.max_gain = 65536.0f;
-        control_loop_gains(static_cast<float>(kPi / 200 / sym_sps), h->acp.alpha, h->acp.beta);
-        h->acp.order = 4; h->acp.use_snr = 1;
-        const float symbol_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
-        const float sps_dev = 200.0f / symbol_rate;
-        clock_loop_gains(static_cast<float>(2 * kPi / (symbol_rate / 10)), 1.0f, 0.2869f, h->ssp.alpha, h->ssp.beta);
-        h->ssp.sps = static_cast<float>(sym_sps);
-        h->ssp.max_period = h->ssp.sps + sps_dev; h->ssp.min_period = h->ssp.sps - sps_dev;
-        h->ssp.lookahead = 8 + static_cast<int>(ceilf(h->ssp.max_period)) + 1;
-        control_loop_gains(costas_bw, h->ssp.costas_alpha, h->ssp.costas_beta);
-        const float th = static_cast<float>(-3 * kPi / 4);
-        h->ssp.rot_r = cosf(th); h->ssp.rot_i = sinf(th);
-        h->ssp.soft_scale = 48.0f;
-        h->ssp.n0 = static_cast<int>(floorf(h->ssp.min_period - fabsf(h->ssp.alpha)));
-        h->ssp.fl0 = static_cast<float>(h->ssp.n0);
-        h->nports = 3;
-    } else if (kind == QRL_DEMOD_2FSK) {
-        // gr_demod_2fsk.cpp:39-130 (fm variant)
-        int decim, nfilts, interp = 1;
-        if (sps == 10) { tsr = 20000; sym_sps = sps; decim = 50; nfilts = 35 * sym_sps; }
-        else if (sps >= 5) { tsr = 40000; sym_sps = sps * 2; decim = 25; nfilts = 35 * sym_sps; }
-        else if (sps == 1) { tsr = 80000; sym_sps = 4; decim = 25; interp = 2; nfilts = 125 * sym_sps; }
-        else { set_err(h, "make_gr_demod_2fsk: unsupported sps"); return fail(QRL_EINVAL); }
-        h->L1 = interp;
-        if ((nfilts % 2) == 0) nfilts += 1;
-        if (!flag) {     // gr_demod_2fsk.cpp:88-100: upper (-fw,0) / lower (0,fw) band filters, ratio detector, symbol filter
-            std::vector<float> bank = complex_band_pass(1, tsr, -filter_width, 0, filter_width, WIN_BLACKMAN_HARRIS);
-            std::vector<float> lower = complex_band_pass(1, tsr, 0, filter_width, filter_width, WIN_BLACKMAN_HARRIS);
-            h->nt_bank = static_cast<int>(bank.size() / 2);
-            bank.insert(bank.end(), lower.begin(), lower.end());
-            if ((rc = upload_floats(h, &h->d_bank_taps, bank))) return fail(rc);
-            std::vector<float> sf = low_pass(1.0, tsr, tsr / sym_sps, tsr / sym_sps, WIN_HAMMING);
-            h->nt_symf = static_cast<int>(sf.size());
-            if ((rc = upload_floats(h, &h->d_symf_taps, sf))) return fail(rc);
-        }
-        taps1 = low_pass(interp, static_cast<double>(interp) * samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = decim;
-        taps2 = low_pass(1, tsr, filter_width, filter_width, WIN_BLACKMAN_HARRIS);
-        taps3 = gmsk ? low_pass(1, tsr, tsr / sym_sps, tsr / sym_sps, WIN_HAMMING)            // gr_demod_gmsk.cpp:88-90
-                     : root_raised_cosine(1, tsr, tsr / sym_sps, 0.2, nfilts);
-        h->qd_gain = static_cast<float>(sym_sps / (1 * kPi / 2));
-        const float symbol_rate = static_cast<float>(tsr) / static_cast<float>(sym_sps);
-        const float sps_dev = gmsk ? 0.05f : 200.0f / symbol_rate;                                    // gr_demod_gmsk.cpp:79-84
-        clock_loop_gains(gmsk ? static_cast<float>(2 * kPi / 200.0f) : static_cast<float>(2 * kPi / (symbol_rate / 10)), 1.0f, 0.2869f,
-                         h->ssp.alpha, h->ssp.beta);
-        h->ssp.sps = static_cast<float>(sym_sps);
-        h->ssp.max_period = h->ssp.sps + sps_dev; h->ssp.min_period = h->ssp.sps - sps_dev;
-        h->ssp.lookahead = 8 + static_cast<int>(ceilf(h->ssp.max_period)) + 1;
-        h->ssp.soft_scale = 128.0f;
-        h->ssp.n0 = static_cast<int>(floorf(h->ssp.min_period - fabsf(h->ssp.alpha)));
-        h->ssp.fl0 = static_cast<float>(h->ssp.n0);
-        h->fllp.N = 16;
-        control_loop_gains(static_cast<float>(24 * kPi / 100), h->fllp.alpha, h->fllp.beta);
-        h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sym_sps)); h->fllp.min_freq = -h->fllp.max_freq;
-        h->nports = 4;
-    } else if (kind == QRL_DEMOD_BPSK) {
-        // gr_demod_bpsk.cpp:40-76
-        tsr = 20000; sym_sps = sps;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = 50;
-        taps2 = root_raised_cosine(sps, sps, 1, 0.35, 15 * sps);
-        h->acp.attack = 1e-1f; h->acp.decay = 1e-1f; h->acp.ref = 1.0f; h->acp.max_gain = 65536.0f; h->acp.order = 0;
-        const float gain_mu = 0.05f, gain_omega = 0.005f;
-        h->ssp.loop_kind = LOOP_CRMM;
-        h->ssp.sps = static_cast<float>(sps);
-        h->ssp.gain_omega = gain_omega * gain_omega; h->ssp.gain_mu = gain_mu;
-        h->ssp.omega_mid = static_cast<float>(sps); h->ssp.omega_lim = 0.001f * static_cast<float>(sps);
-        h->ssp.lookahead = 24;
-        h->ssp.max_period = static_cast<float>(sps) + 1.0f; h->ssp.min_period = static_cast<float>(sps) - 1.0f;   // bounds for buffer sizing only
-        h->ssp.alpha = 0.0f;
-        control_loop_gains(static_cast<float>(2 * kPi / 200), h->ssp.costas_alpha, h->ssp.costas_beta);
-        h->ssp.soft_scale = 64.0f;
-        h->fllp.N = 32;
-        control_loop_gains(static_cast<float>(8 * kPi / 100), h->fllp.alpha, h->fllp.beta);
-        h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sps)); h->fllp.min_freq = -h->fllp.max_freq;
-        h->nports = 4;
-    } else if (kind == QRL_DEMOD_DSSS) {
-        // gr_demod_dsss.cpp:32-124 (instance gr_demod_base.cpp:218: make_gr_demod_dsss(25, 1e6, 1700, 150)); sps = items per chip at 5200 sps
-        tsr = 20000; sym_sps = 2;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = 50;
-        const std::vector<float> tif = low_pass(1, 20000, 5200 / 2, 5200 / 2, WIN_BLACKMAN_HARRIS);       // rational_resampler_ccf(13, 50)
-        taps2 = low_pass(1, 5200, filter_width, 1200, WIN_BLACKMAN_HARRIS);
-        DsssParams& d = h->dsp;
-        d.nt_arm = (static_cast<int>(tif.size()) + 12) / 13; d.nt2 = static_cast<int>(taps2.size());
-        d.N = sps * 13; d.ntaps = d.N + 11 * sps;
-        if (sps < 1 || d.nt_arm > 8 || d.nt2 > 64 || d.ntaps > 640 || d.N + d.ntaps - 1 > kDsssChunk) {
-            set_err(h, "make_gr_demod_dsss: sps / filter_width outside what the chain kernel holds in shared memory"); return fail(QRL_EINVAL);
-        }
-        if ((rc = upload_floats(h, &h->d_ds_arms, make_arms(tif, 13, d.nt_arm)))) return fail(rc);
-        {   // dsss_decoder_cc_impl.cc:60-96: reversed Barker-13, `sps` items per chip, shaped by RRC(1, sps, 1, 0.35f, 11 sps); the block's
-            // fir_filter_ccc keeps the taps reversed (what is uploaded)
-            static const int barker_13[13] = { 1, 1, 1, 1, 1, 0, 0, 1, 1, 0, 1, 0, 1 };
-            const int extra = 11 * sps, total = d.N + 2 * extra;
-            std::vector<float> cs(total, 0.0f);
-            for (int i = 0; i < 13; i++) { const float cv = barker_13[13 - (i + 1)] == 0 ? -1.0f : 1.0f; for (int k = 0; k < sps; k++) cs[extra + i * sps + k] = cv; }
-            const std::vector<float> rrc = root_raised_cosine(1, sps, 1.0, static_cast<double>(0.350f), extra);
-            const int nr = static_cast<int>(rrc.size());
-            std::vector<float> t(2 * static_cast<size_t>(d.ntaps));
-            for (int i = 0; i < d.ntaps; i++) {
-                float acc = 0.0f, acci = 0.0f;
-                for (int k = 0; k < nr; k++) { acc = acc + cs[i + k] * rrc[nr - 1 - k]; acci = acci + 0.0f * rrc[nr - 1 - k]; }
-                t[2 * (d.ntaps - 1 - i)] = acc; t[2 * (d.ntaps - 1 - i) + 1] = acci;
-            }
-            float* tp = nullptr;
-            if ((rc = upload_floats(h, &tp, t))) return fail(rc);
-            h->d_ds_taps = reinterpret_cast<float2*>(tp);
-        }
-        control_loop_gains(static_cast<float>(kPi / 200), d.pll_alpha, d.pll_beta);
-        control_loop_gains(static_cast<float>(2 * kPi / 100), d.costas_alpha, d.costas_beta);
-        d.agc_attack = 1e-1f; d.agc_decay = 1e-1f; d.agc_ref = 1.0f; d.agc_max = 65536.0f;
-        const float gain_mu = 0.05f, gain_omega = 0.005f;
-        d.gain_omega = gain_omega * gain_omega; d.gain_mu = gain_mu; d.omega_mid = 1.0f; d.omega_lim = 0.005f * 1.0f; d.soft_scale = 64.0f;
-        h->ssp.lookahead = 0; h->ssp.sps = 2.0f;
-        h->nports = 4;
-    } else if (kind == QRL_DEMOD_SSB) {
-        // gr_demod_ssb.cpp:37-61; flag = sb (0 USB, 1 LSB); sps = decimation (125)
-        tsr = 8000; sym_sps = 2;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = sps;
-        taps2 = flag ? complex_band_pass_2(1, tsr, -filter_width, -200, 200, 90, WIN_BLACKMAN_HARRIS)
-                     : complex_band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        h->nports = 2;
-    } else if (kind == QRL_DEMOD_FREEDV) {
-        // gr_demod_freedv.cpp:40-54; flag = sb (0 USB, 1 LSB); sps = decimation to 8 ksps.  The stage-1 taps are low_pass(sps, ...): DC gain sps
-        tsr = 8000; sym_sps = 2;
-        taps1 = low_pass(sps, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = sps;
-        taps2 = flag ? complex_band_pass_2(1, tsr, -filter_width, -low_cutoff, 200, 90, WIN_BLACKMAN_HARRIS)
-                     : complex_band_pass_2(1, tsr, low_cutoff, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        h->nports = 2;
-    } else if (kind == QRL_DEMOD_WBFM) {
-        // gr_demod_wbfm.cpp:35-54
-        tsr = 200000; sym_sps = 2;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = 5;
-        taps2 = low_pass_2(1, tsr, filter_width, 600, 90, WIN_BLACKMAN_HARRIS);
-        h->qd_gain = static_cast<float>(tsr / (2 * kPi * filter_width));
-        h->nports = 2;
-    } else if (kind == QRL_DEMOD_AM) {
-        // gr_demod_am.cpp:35-56
-        tsr = 20000; sym_sps = 2;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = 50;
-        taps2 = complex_band_pass_2(1, tsr, -filter_width, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        h->nports = 2;
-    } else if (kind == QRL_DEMOD_NBFM) {
-        // gr_demod_nbfm.cpp:39-66
-        tsr = 20000; sym_sps = 2;
-        taps1 = low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS);
-        h->D1 = 50;
-        taps2 = low_pass_2(1, tsr, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS);
-        h->qd_gain = static_cast<float>(tsr / (4 * kPi * filter_width));
-        h->nports = 2;
-    } else {
-        set_err(h, "qrl_rx_create: demod kind " + std::to_string(kind) + " not built");
-        return fail(QRL_EINVAL);
+    int sym_sps = 2;        // stage-1 samples per symbol (the audio chains: 2)
+    switch (kind) {
+    case QRL_DEMOD_4FSK: h->chain = flag ? RxChain::Fsk4Fm : RxChain::Fsk4Bank; rc = create_4fsk(h, sps, samp_rate, filter_width, sym_sps); break;
+    case QRL_DEMOD_M17: h->chain = RxChain::M17; rc = create_4fsk(h, sps, samp_rate, filter_width, sym_sps); break;
+    case QRL_DEMOD_DMR: h->chain = RxChain::Dmr; rc = create_4fsk(h, sps, samp_rate, filter_width, sym_sps); break;
+    case QRL_DEMOD_2FSK: h->chain = flag ? RxChain::Fsk2Fm : RxChain::Fsk2Bank; rc = create_2fsk(h, sps, samp_rate, filter_width, sym_sps); break;
+    case QRL_DEMOD_GMSK: h->chain = RxChain::Gmsk; rc = create_2fsk(h, sps, samp_rate, filter_width, sym_sps); break;
+    case QRL_DEMOD_BPSK: h->chain = RxChain::Bpsk; rc = create_bpsk(h, sps, samp_rate, sym_sps); break;
+    case QRL_DEMOD_QPSK: h->chain = RxChain::Qpsk; rc = create_qpsk(h, sps, samp_rate, sym_sps); break;
+    case QRL_DEMOD_DSSS: h->chain = RxChain::Dsss; rc = create_dsss(h, sps, samp_rate, filter_width); break;
+    case QRL_DEMOD_NBFM: h->chain = RxChain::Nbfm; rc = create_nbfm(h, samp_rate, filter_width); break;
+    case QRL_DEMOD_AM: h->chain = RxChain::Am; rc = create_am(h, samp_rate, filter_width); break;
+    case QRL_DEMOD_WBFM: h->chain = RxChain::Wbfm; rc = create_wbfm(h, samp_rate, filter_width); break;
+    case QRL_DEMOD_SSB: h->chain = RxChain::Ssb; h->lsb = flag != 0; rc = create_ssb(h, sps, samp_rate, filter_width); break;
+    case QRL_DEMOD_FREEDV: h->chain = RxChain::Freedv; h->lsb = flag != 0; rc = create_freedv(h, sps, samp_rate, filter_width, low_cutoff); break;
+    default: set_err(h, "qrl_rx_create: demod kind " + std::to_string(kind) + " not built"); rc = QRL_EINVAL;
     }
-    h->sym_sps = sym_sps; h->tsr = tsr;
-
-    // ---- stage 1 buffers
-    h->ntaps1 = static_cast<int>(taps1.size());
-    h->Q1 = (h->ntaps1 + h->D1 - 1) / h->D1;
-    int padded = std::max(h->Q1 * h->D1, h->D1 == 2 ? 56 : 0);
-    std::vector<float> tp(padded, 0.0f);
-    std::copy(taps1.begin(), taps1.end(), tp.begin());
-    if (h->L1 == 2) {       // rational_resampler arms: arm[p][k] = taps[p + k L], 105 taps per arm
-        const int nt = 105;
-        tp.assign(2 * nt, 0.0f);
-        for (int p = 0; p < 2; p++) for (int k = 0; k < nt; k++) { const size_t j = p + 2 * k; if (j < taps1.size()) tp[p * nt + k] = taps1[j]; }
-        padded = 128;       // history samples kept
-    } else if (h->L1 > 2) {   // shape-generic rational resampler: arm[p][k] = taps[p + k L]
-        const int nt = (static_cast<int>(taps1.size()) + h->L1 - 1) / h->L1;
-        tp.assign(static_cast<size_t>(h->L1) * nt, 0.0f);
-        for (int p = 0; p < h->L1; p++) for (int k = 0; k < nt; k++) { const size_t j = p + static_cast<size_t>(k) * h->L1; if (j < taps1.size()) tp[p * nt + k] = taps1[j]; }
-        h->nt_arm1 = nt;
-        padded = nt + 8;
-    }
-    if ((rc = upload_floats(h, &h->d_taps1, tp))) return fail(rc);
-    h->H = padded;
-    if ((rc = dev_alloc(h, &h->d_hist[0], static_cast<size_t>(h->H) * h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C))) return fail(rc);
-    h->n1max = h->Tmax * h->L1 / h->D1 + 2;
-    // ---- rings
-    h->ntaps2 = static_cast<int>(taps2.size()) / ((kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM || kind == QRL_DEMOD_FREEDV) ? 2 : 1);
-    h->ntaps3 = static_cast<int>(taps3.size());
-    {
-        std::vector<float> t2(std::max<size_t>(taps2.size(), 512), 0.0f);     // room for set_filter_width redesigns
-        std::copy(taps2.begin(), taps2.end(), t2.begin());
-        if ((rc = upload_floats(h, &h->d_taps2, t2))) return fail(rc);
-        h->taps2_cap = t2.size();
-    }
-    if (!taps3.empty() && (rc = upload_floats(h, &h->d_taps3, taps3))) return fail(rc);
-    if ((rc = make_ring(h, &h->r1, sizeof(float2), h->n1max + std::max(512, static_cast<int>(taps2.size())) + 8))) return fail(rc);
-    if (kind == QRL_DEMOD_SSB) {
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
-        std::vector<float> audio_f = band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
-        if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return fail(rc);
-        h->ssbp.sq_alpha = 0.01; h->ssbp.sq_threshold = std::pow(10.0, -140 / 10.0);
-        h->ssbp.attack = 1e-1f; h->ssbp.decay = 1e-1f; h->ssbp.ref = 0.25f; h->ssbp.max_gain = 65536.0f;
-        h->ssbp.clip = 0.95f; h->ssbp.emax = static_cast<float>(1 / (std::sqrt(0.5) / 2)); h->ssbp.out_gain = 1.333f;
-        h->ssbp.nt_audio = static_cast<int>(audio_f.size());
-        if ((rc = make_ring(h, &h->rclip, sizeof(float2), h->n1max + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->ssbp.nt_audio + 16))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_ssb, h->C))) return fail(rc);
-    } else if (kind == QRL_DEMOD_FREEDV) {
-        // gr_demod_freedv.cpp:57-77: agc2_ff(1e-1, 1e-3, 0.5, 1) (max gain 65536) -> band_pass_2(1, 8000, 200, 3500, 200, 90, BH) -> x0.1 ->
-        // float_to_short(1, 32768); the feedforward_agc_cc of :56 is never connected
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
-        std::vector<float> audio_f = band_pass_2(1, tsr, 200, 3500, 200, 90, WIN_BLACKMAN_HARRIS);
-        if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return fail(rc);
-        h->fdp.attack = 1e-1f; h->fdp.decay = 1e-3f; h->fdp.ref = 0.5f; h->fdp.max_gain = 65536.0f;
-        h->fdp.nt_audio = static_cast<int>(audio_f.size());
-        if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->fdp.nt_audio + 16))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_fdv, h->C))) return fail(rc);
-    } else if (kind == QRL_DEMOD_WBFM) {
-        // gr_demod_wbfm.cpp:39-64: the analog audio kernel in mode 2
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
-        std::vector<float> audio_rs = low_pass(1, tsr, 4000, 2000, WIN_BLACKMAN_HARRIS);
-        if ((rc = upload_floats(h, &h->d_audio_taps, audio_rs))) return fail(rc);
-        if ((rc = upload_floats(h, &h->d_arm_taps, std::vector<float>{ 0.0f, 0.0f }))) return fail(rc);
-        if ((rc = upload_floats(h, &h->d_env, std::vector<float>{ 1.0f, 1.0f }))) return fail(rc);
-        double a[2], b[2];
-        deemph_taps(8000, 50e-6, a, b);                        // the reference designs them for 8 kHz (:39) and runs them at 200 ksps
-        h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = 0; h->nbp.sq_gate = 1;
-        h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = 1; h->nbp.nt_audio = static_cast<int>(audio_rs.size());
-        h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 1.0f;
-        h->nbp.mode = 2; h->nbp.am_gain = 0.9f;
-        if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max + h->nbp.nt_audio + 16))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_nb, h->C))) return fail(rc);
-    } else if (kind == QRL_DEMOD_AM) {
-        // gr_demod_am.cpp:41-70: the NBFM audio kernel in detector mode 1
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
-        std::vector<float> audio_rs = low_pass(2, 2 * tsr, 3600, 600, WIN_BLACKMAN_HARRIS);
-        std::vector<float> audio_f = low_pass(1, 8000, 3600, 300, WIN_BLACKMAN_HARRIS);
-        const int nt_arm = (static_cast<int>(audio_rs.size()) + 1) / 2;
-        std::vector<float> arms(2 * nt_arm, 0.0f);
-        for (int pp = 0; pp < 2; pp++)
-            for (int k = 0; k < nt_arm; k++) { const size_t j = pp + 2 * k; arms[pp * nt_arm + k] = j < audio_rs.size() ? audio_rs[j] : 0.0f; }
-        if ((rc = upload_floats(h, &h->d_arm_taps, arms))) return fail(rc);
-        if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return fail(rc);
-        if ((rc = upload_floats(h, &h->d_env, std::vector<float>{ 1.0f, 1.0f }))) return fail(rc);
-        h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = 0; h->nbp.sq_gate = 1;
-        h->nbp.qd_gain = 0.0f; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
-        h->nbp.b0 = 1.0; h->nbp.b1 = -1.0; h->nbp.a1 = -0.9999; h->nbp.out_gain = 1.0f;      // iir_filter_ffd({1,-1},{0,0.9999}), old style
-        h->nbp.mode = 1; h->nbp.agc_attack = 1e-1f; h->nbp.agc_decay = 1e-1f; h->nbp.agc_ref = 1.0f; h->nbp.agc_max = 65536.0f; h->nbp.am_gain = 0.99f;
-        if ((rc = make_ring(h, &h->rg, sizeof(float2), 64))) return fail(rc);
-        if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_nb, h->C))) return fail(rc);
-    } else if (kind == QRL_DEMOD_NBFM) {
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64))) return fail(rc);
-        std::vector<float> audio_rs = low_pass_2(2, 2 * tsr, 3600, 250, 60, WIN_BLACKMAN_HARRIS);
-        std::vector<float> audio_f = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
-        const int nt_arm = (static_cast<int>(audio_rs.size()) + 1) / 2;
-        std::vector<float> arms(2 * nt_arm, 0.0f);
-        for (int pp = 0; pp < 2; pp++)
-            for (int k = 0; k < nt_arm; k++) { const size_t j = pp + 2 * k; arms[pp * nt_arm + k] = j < audio_rs.size() ? audio_rs[j] : 0.0f; }
-        if ((rc = upload_floats(h, &h->d_arm_taps, arms))) return fail(rc);
-        if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return fail(rc);
-        const int ramp = 320;
-        std::vector<float> env(ramp + 1);
-        for (int k = 0; k <= ramp; k++) env[k] = static_cast<float>(0.5 - std::cos(kPi * k / ramp) / 2.0);
-        if ((rc = upload_floats(h, &h->d_env, env))) return fail(rc);
-        double a[2], b[2];
-        deemph_taps(tsr, 50e-6, a, b);
-        h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = ramp; h->nbp.sq_gate = 1;
-        h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
-        h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 2.0f;
-        if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return fail(rc);
-        if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_nb, h->C))) return fail(rc);
-        if (kind == QRL_DEMOD_NBFM) {
-            // analog::ctcss_squelch_ff::make(8000, 88.5, 0.01, 8000, 160, true) (gr_demod_nbfm.cpp:60), out of the graph until set_ctcss(f)
-            if ((rc = make_ring(h, &h->rq, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 64))) return fail(rc);
-            h->ctc.on = 0; h->ctc.len = 8000; h->ctc.ramp = 160; h->ctc.gate = 1; h->ctc.level = 0.01f;
-            std::vector<double> ce(h->ctc.ramp + 1);
-            for (int k = 0; k <= h->ctc.ramp; k++) ce[k] = 0.5 - std::cos(kPi * k / h->ctc.ramp) / 2.0;       // squelch_base_ff envelope (double)
-            if ((rc = dev_alloc(h, &h->d_cenv, ce.size(), false))) return fail(rc);
-            if (cudaMemcpy(h->d_cenv, ce.data(), sizeof(double) * ce.size(), cudaMemcpyHostToDevice) != cudaSuccess) { set_err(h, "envelope upload failed"); return fail(QRL_ECUDA); }
-        }
-        // (an FP64 instruction occupies an SM's FP64 pipe for ~64 cycles whatever its lane count, so two recurrences only overlap on
-        // DIFFERENT SMs: both kernels then ask for more than half an SM's shared memory, which keeps their CTAs one per SM and apart, and
-        // the split is used while each kernel's C CTAs fit the SMs at once -- on an H100 it is faster up to 128 channels, slower at 160)
-        int n_sm = 0;
-        if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess) { set_err(h, "SM count query failed"); return fail(QRL_ECUDA); }
-        if (kind == QRL_DEMOD_NBFM && h->C <= n_sm && !getenv("QRL_NBFM_NO_SPLIT")) {
-            if ((rc = make_ring(h, &h->raud, sizeof(float), h->n1max * 2 / 5 + 64))) return fail(rc);
-            if ((rc = dev_alloc(h, &h->d_nb2, h->C))) return fail(rc);
-            h->zero_list.emplace_back(h->d_nb2, sizeof(NbfmDeemphState) * h->C);
-            h->nbfm_split = true;
-        }
-    } else if (kind == QRL_DEMOD_DSSS) {
-        const long long n5 = h->n1max * 13 / 50 + 8;
-        if ((rc = make_ring(h, &h->ds_a, sizeof(float2), n5 + 2048))) return fail(rc);
-        if ((rc = make_ring(h, &h->ds_c, sizeof(float2), n5 + 2048))) return fail(rc);
-        if ((rc = make_ring(h, &h->ds_d, sizeof(float2), n5 / h->dsp.N + 128))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_ds, h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_vs2, h->C))) return fail(rc);
-    } else if (kind == QRL_DEMOD_4FSK || kind == QRL_DEMOD_2FSK) {
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + h->ntaps3 + 64))) return fail(rc);
-        // two calls deep when the block may run with overlapped calls (the producer of call k+1 must not wait for the
-        // consumer of call k)
-        if ((rc = make_ring(h, &h->r4, sizeof(float), (flag && kind == QRL_DEMOD_4FSK ? 2 : 1) * h->n1max + 600, true))) return fail(rc);
-        if (flag && kind == QRL_DEMOD_4FSK) {
-            // scratch of the external symbol-sync epilogue: [groups][chunks][maxs + 2][32] floats + a 128-int header per group
-            // window size: 512 rows x 2 stages when the replicated interpolator bank still fits next to it, else 256 x 3
-            h->ss_ch = symsync_ext_smem(h->ssp, 512, 2, true) <= 220 * 1024 ? 512 : 256;
-            if (const char* e = getenv("QRL_SS_CH")) { const int v = atoi(e); if (v == 512 || v == 256) h->ss_ch = v; }
-            const int maxs = symsync_maxs(h->ssp, h->ss_ch);
-            h->ss_chunk_cap = h->n1max / symsync_stride(h->ss_ch, h->ssp.lookahead) + 4 + 3 * qrl_rx::kMaxSub;
-            const size_t groups = (h->C + 31) / 32;
-            if ((rc = dev_alloc(h, &h->d_ss_scratch, groups * h->ss_chunk_cap * (maxs + 2) * 32))) return fail(rc);
-            if ((rc = dev_alloc(h, &h->d_ss_hdr, groups * 128 * qrl_rx::kMaxSub))) return fail(rc);
-        }
-        if (!flag) {
-            if ((rc = make_ring(h, &h->rbank, kind == QRL_DEMOD_4FSK ? sizeof(float2) : sizeof(float), h->n1max + h->nt_symf + 16))) return fail(rc);
-            if (kind == QRL_DEMOD_4FSK && (rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true))) return fail(rc);
-        }
-    } else {   // QPSK / BPSK: shaping-filter output and loop output are channel-interleaved complex rings
-        if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 600, true))) return fail(rc);
-        if ((rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_ac, h->C))) return fail(rc);
-    }
-    const bool has_fll = kind == QRL_DEMOD_BPSK || kind == QRL_DEMOD_2FSK || (kind == QRL_DEMOD_QPSK && sps > 4);
-    if (has_fll) {
-        const float fsps = static_cast<float>(sym_sps);
-        std::vector<float> ft = fll_design(fsps, kind == QRL_DEMOD_2FSK ? 0.1f : 0.35f, h->fllp.N);
-        if ((rc = upload_floats(h, &h->d_fll_taps, ft))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_fll, h->C))) return fail(rc);
-        if ((rc = dev_alloc(h, &h->d_fll_hist, static_cast<size_t>(32) * h->C))) return fail(rc);
-        h->zero_list.emplace_back(h->d_fll_hist, sizeof(float2) * 32 * h->C);
-        h->zero_list.emplace_back(h->d_fll, sizeof(FllState) * h->C);
-        if ((rc = make_ring(h, &h->rf, sizeof(float2), h->n1max + 512 + 8))) return fail(rc);
-        if (kind != QRL_DEMOD_QPSK && (rc = dev_alloc(h, &h->d_vs2, h->C))) return fail(rc);
-    }
-    if ((rc = make_ring(h, &h->r5, 1, 2 * h->n1max + 1024))) return fail(rc);
+    if (rc) return fail(rc);
+    // ---- ports (port 1: at most one symbol per sym_sps - 1 stage-1 samples), the soft bits and the symbol-sync and decoder states
     h->port0_cap = h->n1max;
     if ((rc = dev_alloc(h, &h->d_port0, static_cast<size_t>(h->port0_cap) * h->C))) return fail(rc);
     h->port1_cap = h->n1max / std::max(1, sym_sps - 1) + 64;
     if ((rc = dev_alloc(h, &h->d_port1, static_cast<size_t>(h->port1_cap) * h->C))) return fail(rc);
     h->d_port1f = reinterpret_cast<float*>(h->d_port1);
     if ((rc = dev_alloc(h, &h->d_port1_cnt, h->C))) return fail(rc);
-    h->port2_cap = (h->m17 ? 2 : 1) * h->port1_cap + 160;      // M17: two hard bits per symbol, no rate-1/2 decoder behind them
-    if ((rc = dev_alloc(h, &h->d_port2, static_cast<size_t>(h->port2_cap) * h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_port2_cnt, h->C))) return fail(rc);
-    if (h->dmr) {
+    if (h->nports > 2) {        // the symbol chains: soft bits (u8) -> decoder -> port 2
+        if ((rc = make_ring(h, &h->r5, 1, 2 * h->n1max + 1024))) return fail(rc);
+        h->port2_cap = (hard_bits(h) ? 2 : 1) * h->port1_cap + 160;      // M17: two hard bits per symbol, no rate-1/2 decoder behind them
+        if ((rc = dev_alloc(h, &h->d_port2, static_cast<size_t>(h->port2_cap) * h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_port2_cnt, h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_vs, h->C))) return fail(rc);
+        // (DSSS: the chain kernel carries its own clock recovery)
+        if (h->chain != RxChain::Dsss && (rc = dev_alloc(h, &h->d_ss, h->C))) return fail(rc);
+    }
+    if (h->port3_isz == 4) {
         if ((rc = dev_alloc(h, &h->d_port3f, static_cast<size_t>(h->port0_cap) * h->C))) return fail(rc);
-    } else if (h->nports == 4) {
+    } else if (h->nports == 4) {    // the second decoder, behind delay(1)
         if ((rc = dev_alloc(h, &h->d_port3, static_cast<size_t>(h->port2_cap) * h->C))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_port3_cnt, h->C))) return fail(rc);
+        if ((rc = dev_alloc(h, &h->d_vs2, h->C))) return fail(rc);
     }
-    if ((rc = dev_alloc(h, &h->d_ss, h->C))) return fail(rc);
-    if (h->ssp.lookahead > 0 && symsync_stride(128, h->ssp.lookahead) < 32 &&
-        (kind == QRL_DEMOD_QPSK || kind == QRL_DEMOD_BPSK || (kind == QRL_DEMOD_4FSK && !flag))) {
-        set_err(h, "symbol-sync lookahead does not fit the 128-row window of the complex-symbol kernels");
-        return fail(QRL_EINVAL);
-    }
-    if ((rc = dev_alloc(h, &h->d_vs, h->C))) return fail(rc);
     if ((rc = dev_alloc(h, &h->d_nsoft, static_cast<size_t>(qrl_rx::kMaxSub) * h->C))) return fail(rc);
     {
         int lo = 0, hi = 0;
@@ -1384,9 +1459,10 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         const int groups = (h->C + 31) / 32;
         // analog blocks: one CTA per channel whose thread 0 runs the double-precision recurrences (squelch power, de-emphasis): they want
         // an SM (its FP64 pipe) each, up to half the machine
-        const bool analog_kind = kind == QRL_DEMOD_NBFM || kind == QRL_DEMOD_SSB || kind == QRL_DEMOD_AM || kind == QRL_DEMOD_WBFM ||
-                                 kind == QRL_DEMOD_FREEDV;
-        const int big_ctas = (kind == QRL_DEMOD_QPSK) ? 2 * groups : (analog_kind ? (h->nbfm_split ? 2 * h->C : std::min(h->C, 44)) : groups);
+        const bool analog_kind = h->chain == RxChain::Nbfm || h->chain == RxChain::Ssb || h->chain == RxChain::Am || h->chain == RxChain::Wbfm ||
+                                 h->chain == RxChain::Freedv;
+        const bool qpsk = h->chain == RxChain::Qpsk;
+        const int big_ctas = qpsk ? 2 * groups : (analog_kind ? (h->nbfm_split ? 2 * h->C : std::min(h->C, 44)) : groups);
         unsigned loop_sms = static_cast<unsigned>(std::min(48, 8 * ((big_ctas + 4 + 7) / 8)));
         if (const char* e = getenv("QRL_LOOP_SMS")) { int v = atoi(e); if (v >= 8 && v <= 64) loop_sms = static_cast<unsigned>(v); }
         // Many channels (more loop CTAs than a 48-SM partition holds one per SM): the loop kernels have enough warps in flight to
@@ -1396,8 +1472,8 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
         if (const char* e = getenv("QRL_MANY_CHANNELS")) h->many = e[0] == '1';
         // QPSK (per-sample loops, 2 loop CTAs per 32 channels + a heavy Viterbi load): runs WITHOUT a private partition, so that the
         // decoder gets the whole machine and the loop CTAs spread over more SMs; QRL_QPSK_PARTITION=1 brings the partition back.
-        bool want_partition = kind != QRL_DEMOD_QPSK;
-        if (const char* e = getenv("QRL_QPSK_PARTITION")) { if (kind == QRL_DEMOD_QPSK) want_partition = e[0] == '1'; }
+        bool want_partition = !qpsk;
+        if (const char* e = getenv("QRL_QPSK_PARTITION")) { if (qpsk) want_partition = e[0] == '1'; }
         if (h->many || !want_partition || !make_sm_partition(h, loop_sms, hi, !analog_kind && groups <= 2)) {
             h->s_par = nullptr; h->sm_loop = 0; h->sm_par = 0;
             if (h->s_loop == nullptr)
@@ -1416,7 +1492,7 @@ static int rx_create(int kind, int sps, int samp_rate, int carrier_freq, int fil
     }
     // QPSK: the call ends with the symbol sync + Viterbi of the last slice behind the per-sample loop (no overlapped calls for this
     // chain): the finest slicing the event arrays allow keeps that tail short
-    if (kind == QRL_DEMOD_QPSK) h->nsub = qrl_rx::kMaxSub;
+    if (h->chain == RxChain::Qpsk) h->nsub = qrl_rx::kMaxSub;
     if (const char* e = getenv("QRL_NSUB")) { int v = atoi(e); if (v >= 1 && v <= qrl_rx::kMaxSub) { h->nsub = v; h->nsub_forced = true; } }
     if (const char* e = getenv("QRL_FIR_GROUP")) { int v = atoi(e); if (v >= 1 && v <= qrl_rx::kMaxSub) { h->fir_group = v; h->fir_group_forced = true; } }
     h->fsk_fused = fsk_fm_fused(h);
@@ -1450,8 +1526,8 @@ int qrl_rx_reset(qrl_rx* h)
         ss[c].mu = (h->ssp.loop_kind == LOOP_CRMM) ? 0.5f : 0.0f;          // clock_recovery_mm_cc(omega, g_omega, mu = 0.5, ...)
         vs[c].rd = 0; vs[c].start_state = 0; vs[c].descr_reg = 0x7F;
     }
-    QRL_CK(cudaMemcpyAsync(h->d_ss, ss.data(), sizeof(SymSyncState) * h->C, cudaMemcpyHostToDevice, h->stream));
-    QRL_CK(cudaMemcpyAsync(h->d_vs, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    if (h->d_ss) QRL_CK(cudaMemcpyAsync(h->d_ss, ss.data(), sizeof(SymSyncState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    if (h->d_vs) QRL_CK(cudaMemcpyAsync(h->d_vs, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
     if (h->d_vs2) QRL_CK(cudaMemcpyAsync(h->d_vs2, vs.data(), sizeof(ViterbiState) * h->C, cudaMemcpyHostToDevice, h->stream));
     if (h->d_port3_cnt) QRL_CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
     QRL_CK(cudaMemsetAsync(h->d_hist[0], 0, sizeof(float2) * h->H * h->C, h->stream));
@@ -1493,7 +1569,7 @@ int qrl_rx_reset(qrl_rx* h)
         QRL_CK(cudaMemcpyAsync(h->d_ac, ac.data(), sizeof(AgcCostasState) * h->C, cudaMemcpyHostToDevice, h->stream));
     }
     QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
-    QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+    if (h->d_port2_cnt) QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
     if (!h->rot.empty()) {
         // the carrier offsets stay in force, the rotator's phase restarts: 0 at the first sample after the reset
         h->rot_active = false;
@@ -1557,7 +1633,7 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
     }
     if (key == QRL_PARAM_OVERLAP_CALLS) {
         // only the path whose ring reuse is fenced for it: real-symbol 4FSK (external soft-bit epilogue)
-        if (!(h->kind == QRL_DEMOD_4FSK && h->flag) || h->dmr) { set_err(h, "QRL_PARAM_OVERLAP_CALLS: not supported for this block"); return QRL_EINVAL; }
+        if (h->chain != RxChain::Fsk4Fm && h->chain != RxChain::M17) { set_err(h, "QRL_PARAM_OVERLAP_CALLS: not supported for this block"); return QRL_EINVAL; }
         QRL_CK(cudaStreamSynchronize(h->stream));
         { int rc = rx_join_host(h); if (rc) return rc; }
         const bool on = value != 0.0;
@@ -1595,7 +1671,7 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
     // ---- run-time setters of the analog blocks.  Kernel parameters travel by value with every launch, so a plain host-side update is
     // enough for scalars; new taps are uploaded after everything in flight has drained and meet the true sample history (the rings)
     // from the next qrl_rx_work on.
-    const bool nbfm = h->kind == QRL_DEMOD_NBFM, ssb = h->kind == QRL_DEMOD_SSB, am = h->kind == QRL_DEMOD_AM, wbfm = h->kind == QRL_DEMOD_WBFM;
+    const bool nbfm = h->chain == RxChain::Nbfm, ssb = h->chain == RxChain::Ssb, am = h->chain == RxChain::Am, wbfm = h->chain == RxChain::Wbfm;
     auto quiesce = [&]() -> int { QRL_CK(cudaStreamSynchronize(h->stream)); return rx_join_host(h); };
     auto upload = [&](float* dst, const std::vector<float>& t) -> int {
         int rc = quiesce(); if (rc) return rc;
@@ -1617,7 +1693,7 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
         return QRL_OK;
     }
     if (key == QRL_PARAM_GAIN && ssb) { h->if_gain = static_cast<float>(value); return QRL_OK; }      // gr_demod_ssb::set_gain (:118-121): _if_gain->set_k
-    if (h->kind == QRL_DEMOD_FREEDV) {
+    if (h->chain == RxChain::Freedv) {
         // gr_demod_freedv::set_agc_attack / set_agc_decay (:85-93): the agc2_ff rates, from the next sample on
         if (key == QRL_PARAM_AGC_ATTACK) { h->fdp.attack = static_cast<float>(value); return QRL_OK; }
         if (key == QRL_PARAM_AGC_DECAY) { h->fdp.decay = static_cast<float>(value); return QRL_OK; }
@@ -1665,12 +1741,11 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
         std::vector<float> t;
         if (nbfm || wbfm) t = low_pass(1, h->tsr, fw, 1200, WIN_BLACKMAN_HARRIS);                       // gr_demod_nbfm.cpp:82-90, gr_demod_wbfm.cpp:77-85
         else if (am) t = complex_band_pass(1, h->tsr, -fw, fw, 1200, WIN_BLACKMAN_HARRIS);              // gr_demod_am.cpp:84-92
-        else t = h->flag ? complex_band_pass_2(1, h->tsr, -fw, -200, 200, 90, WIN_BLACKMAN_HARRIS)      // gr_demod_ssb.cpp:89-101
-                         : complex_band_pass_2(1, h->tsr, 200, fw, 200, 90, WIN_BLACKMAN_HARRIS);
+        else t = h->lsb ? complex_band_pass_2(1, h->tsr, -fw, -200, 200, 90, WIN_BLACKMAN_HARRIS)       // gr_demod_ssb.cpp:89-101
+                        : complex_band_pass_2(1, h->tsr, 200, fw, 200, 90, WIN_BLACKMAN_HARRIS);
         if (t.size() > h->taps2_cap) { set_err(h, "set_filter_width: out of range (filter longer than the block was sized for)"); return QRL_EINVAL; }
         int rc = upload(h->d_taps2, t); if (rc) return rc;
         h->ntaps2 = static_cast<int>(t.size()) / ((ssb || am) ? 2 : 1);
-        h->filter_width = fw;
         if (nbfm) h->qd_gain = static_cast<float>(h->tsr / (4 * kPi * fw));
         if (wbfm) h->qd_gain = static_cast<float>(h->tsr / (2 * kPi * fw));
         h->nbp.qd_gain = h->qd_gain;
@@ -1772,7 +1847,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
     // stage-1 ring and its history, which nothing behind the channel filter reads (the channel filter runs on the same stream), so it
     // does not touch the double-buffered ports that tail still owns.  Waiting first put the FIR (about 0.8 ms at 64 x 2^22) behind
     // call k-2's last Viterbi slice, on the loop that sets the step; now it runs under that tail.
-    const bool early_fir = h->overlap && !h->fir_group_forced && h->kind == QRL_DEMOD_4FSK && !seam;
+    const bool early_fir = h->overlap && !h->fir_group_forced && !seam;
     if (h->overlap) {
         h->call_parity ^= 1;
         std::swap(h->d_port0, h->alt_port0); std::swap(h->d_port1, h->alt_port1); std::swap(h->d_port2, h->alt_port2);
@@ -1792,7 +1867,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
             if (seam) for (int j = 0; j < 3; j++) QRL_CK(cudaStreamWaitEvent(h->stream, h->ev_tail[h->call_parity ^ 1][j], 0));
         }
         QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
-        QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
+        if (h->d_port2_cnt) QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
         if (h->d_port3_cnt) QRL_CK(cudaMemsetAsync(h->d_port3_cnt, 0, sizeof(int) * h->C, h->stream));
         QRL_CK(cudaEventRecord(h->ev_start, h->stream));
         QRL_CK(cudaStreamWaitEvent(h->s_loop, h->ev_start, 0));
@@ -1842,7 +1917,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
             const long long kg1 = (Ng * h->L1 + h->D1 - 1) / h->D1;       // outputs i with floor(i M / L) <= N - 1
             pe = h->fsk_fused ? nullptr : h->prof.begin(0, sp);
             int rc = h->fsk_fused ? QRL_OK : stage1(h, xg, xstride, Tg, kg0, kg1);
-            if (!rc && h->kind == QRL_DEMOD_SSB && kg1 > kg0) {
+            if (!rc && h->chain == RxChain::Ssb && kg1 > kg0) {
                 // gr_demod_ssb's multiply_const_cc(_if_gain) sits between the resampler and the side-band filter: the gain is applied
                 // to the samples as they pass (8 ksps), so after set_gain the filter's history keeps the old gain, like the reference's
                 dim3 gs(static_cast<unsigned>((kg1 - kg0 + 255) / 256), h->C);
@@ -1871,17 +1946,17 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                        dim3(static_cast<unsigned>((std::max<long long>(n_new, 1) + kTileThreads - 1) / kTileThreads), h->C), (h->C + 31) / 32,
                        x, xstride, T, n_in0, hist0 };
         int rc;
-        switch (h->kind) {
-        case QRL_DEMOD_DSSS: rc = slice_dsss(h, s); break;
-        case QRL_DEMOD_SSB: case QRL_DEMOD_FREEDV: case QRL_DEMOD_AM: case QRL_DEMOD_NBFM: case QRL_DEMOD_WBFM: rc = slice_analog(h, s); break;
-        case QRL_DEMOD_BPSK: case QRL_DEMOD_2FSK: rc = slice_fll_bpsk_2fsk(h, s); break;      // (GMSK runs as 2FSK)
-        case QRL_DEMOD_4FSK: rc = slice_4fsk(h, s); break;                                    // (M17 and DMR run as 4FSK)
-        default: rc = slice_qpsk(h, s); break;
+        switch (h->chain) {
+        case RxChain::Dsss: rc = slice_dsss(h, s); break;
+        case RxChain::Nbfm: case RxChain::Am: case RxChain::Wbfm: case RxChain::Ssb: case RxChain::Freedv: rc = slice_analog(h, s); break;
+        case RxChain::Bpsk: case RxChain::Fsk2Fm: case RxChain::Fsk2Bank: case RxChain::Gmsk: rc = slice_fll_bpsk_2fsk(h, s); break;
+        case RxChain::Fsk4Fm: case RxChain::Fsk4Bank: case RxChain::M17: case RxChain::Dmr: rc = slice_4fsk(h, s); break;
+        default: rc = slice_qpsk(h, s); break;      // Qpsk
         }
         if (rc) return rc;
     }
     if (!began) { int rc = begin_call(); if (rc) return rc; }     // every slice was empty
-    if (h->kind == QRL_DEMOD_DSSS) {          // port 0 holds 5200 sps items (13 / 50 of the stage-1 items counted in the loop)
+    if (h->chain == RxChain::Dsss) {          // port 0 holds 5200 sps items (13 / 50 of the stage-1 items counted in the loop)
         const long long o_end = (h->n1_s * 13 + 49) / 50;
         h->port0_n = static_cast<long>(o_end - h->ds_o_call0);
         h->ds_o_call0 = o_end;
@@ -1965,11 +2040,7 @@ int qrl_rx_num_ports(const qrl_rx* h) { return h ? h->nports : QRL_EINVAL; }
 int qrl_rx_port_itemsize(const qrl_rx* h, int port)
 {
     if (!h || port < 0 || port >= h->nports) return QRL_EINVAL;
-    if (port == 0) return 8;
-    if (port == 1 && h->kind == QRL_DEMOD_FREEDV) return 2;        // int16 modem samples
-    if (port == 1) return (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_SSB || h->kind == QRL_DEMOD_AM || h->kind == QRL_DEMOD_WBFM) ? 4 : 8;
-    if (port == 3 && h->dmr) return 4;
-    return 1;
+    return port == 0 ? 8 : port == 1 ? h->port1_isz : port == 3 ? h->port3_isz : 1;
 }
 
 int qrl_rx_port_device(qrl_rx* h, int port, void** data, long* cap, int** counts)
@@ -1978,11 +2049,10 @@ int qrl_rx_port_device(qrl_rx* h, int port, void** data, long* cap, int** counts
     if (port == 0) { *data = h->d_port0; *cap = h->port0_cap; *counts = nullptr; }
     else if (port == 1) {
         *data = h->d_port1; *counts = h->d_port1_cnt;
-        *cap = (h->kind == QRL_DEMOD_NBFM || h->kind == QRL_DEMOD_SSB || h->kind == QRL_DEMOD_AM || h->kind == QRL_DEMOD_WBFM) ? 2 * h->port1_cap : h->port1_cap;      // float view of the same buffer
-        if (h->kind == QRL_DEMOD_FREEDV) *cap = 4 * h->port1_cap;                                                                   // int16 view
+        *cap = h->port1_cap * (8 / h->port1_isz);       // the complex buffer seen as floats or int16
     }
     else if (port == 2) { *data = h->d_port2; *cap = h->port2_cap; *counts = h->d_port2_cnt; }
-    else if (h->dmr) { *data = h->d_port3f; *cap = h->port0_cap; *counts = nullptr; }      // one float per port-0 sample
+    else if (h->port3_isz == 4) { *data = h->d_port3f; *cap = h->port0_cap; *counts = nullptr; }      // one float per port-0 sample
     else { *data = h->d_port3; *cap = h->port2_cap; *counts = h->d_port3_cnt; }
     return QRL_OK;
 }
@@ -2120,7 +2190,6 @@ struct qrl_tx : HandleBase {
 namespace {
 // the interpolator and resampler kernels stage a whole arm table (L arms of nt taps) in shared memory
 bool arms_fit(int L, int nt) { return static_cast<size_t>(L) * nt * sizeof(float) <= 40 * 1024; }
-int arms_nt(const std::vector<float>& taps, int L) { return (static_cast<int>(taps.size()) + L - 1) / L; }
 // register-tiled interpolator shapes.  tx_create pads a shorter arm table to the instance's taps per arm, so the same predicate
 // picks the instance in qrl_tx_work: interp_fir_ccf_rt_kernel<20, 35, 8, 16> (4FSK's final x20), interp_fir_ccf_kernel<4, 16, 8, 64> (QPSK)
 constexpr int kFskRtL = 20, kFskRtNT = 35, kQpskRtL = 4, kQpskRtNT = 16;

@@ -16,7 +16,8 @@ import numpy as np
 import pytest
 
 from tests.golden import cases
-from tests.test_gpu_dispatch import TX, tx_bases
+from tests import test_gpu_dispatch as D
+from tests.test_gpu_dispatch import RX, TX, tx_bases
 
 pytestmark = pytest.mark.timeout(900)      # pytest-timeout: a scheduling bug in the emulator must fail, not hang the tier
 
@@ -37,6 +38,31 @@ def emu_qrl(tmp_path_factory):
     assert L.device_count() == 1
     yield q
     L._LIB_PATH, L._LIB = saved
+
+
+def rx_through_the_emulated_library(qrl, O, name, row, T):
+    """2 channels, a 1-sample call and cuts that are no multiple of the decimation, every port bit-identical to the oracle under the
+    length rules of test_gpu_dispatch.check_rx: port 0 as long as the oracle's, the others within SLACK, and empty only where the row's
+    minimum length scaled to T is 0 and the oracle's port is empty too.  row: a row of test_gpu_dispatch.RX or of its form; the stream
+    is the first T samples of the row's base signals"""
+    B, _ = D.bases(name, O, row[3], row)
+    X = np.ascontiguousarray(B[:2, :T])
+    cuts = [(0, 1), (1, 30001), (30001, 30078), (30078, T)]
+    blk = row[0](qrl, 2, max(hi - lo for lo, hi in cuts))
+    try:
+        got = D.concat_calls(D.run_rx(blk, X, cuts), blk.nports, 2)
+    finally:
+        blk.close()
+    for c in range(2):
+        rx = row[1](O)
+        for lo, hi in cuts:
+            rx.work(X[c, lo:hi])
+        for p in range(blk.nports):
+            g, w = got[p][c], rx.port(p)
+            n = min(len(g), len(w))
+            filled = n > 0 or (row[4][p] * T // row[3] == 0 and len(g) == len(w) == 0)
+            assert abs(len(g) - len(w)) <= D.SLACK and filled and (p > 0 or len(g) == len(w)), (name, c, p, len(g), len(w))
+            assert np.array_equal(g[:n], w[:n]), "%s: port %d of channel %d differs from the oracle" % (name, p, c)
 
 
 # the cheaper golden cases (the 250 ksps QPSK chain takes minutes under emulation: GPU tier only)
@@ -214,3 +240,15 @@ def test_qpsk_chain_through_the_emulated_library(emu_qrl, oracle):
             assert n >= len(w) - (160 if p == 2 else 8), (c, p, len(g), len(w))
             assert np.array_equal(g[:n], w[:n]), (c, p)
         assert len(np.concatenate(acc[2][c])) > 3000           # several Viterbi frames came out
+
+
+# stream lengths of the RX rows (default 60 000 samples, long enough for the first Viterbi frames): 4FSK-1K needs 120 000 for its
+# first; the 250 ksps QPSK and 4FSK-100K chains, the slowest under emulation, decode within 40 000
+RX_T = {"4fsk1k": 120000, "qpsk": 40000, "4fsk100k": 40000}
+
+
+@pytest.mark.parametrize("name", sorted(RX))
+def test_rx_chain_through_the_emulated_library(emu_qrl, oracle, name):
+    """every receive chain of the GPU tier's channel-count table -- its create path, slice function and ports -- on the host-thread
+    build, against the oracle"""
+    rx_through_the_emulated_library(emu_qrl, oracle, name, RX[name], RX_T.get(name, 60000))

@@ -14,7 +14,7 @@ import pytest
 from tests import reference_instances as R
 from tests import siggen
 from tests import test_gpu_dispatch as D
-from tests.test_emulated_library import emu_qrl  # noqa: F401  (module-scoped fixture: the emulated build)
+from tests.test_emulated_library import emu_qrl, rx_through_the_emulated_library  # noqa: F401  (emu_qrl: module-scoped fixture)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = os.environ.get("QRL_REFERENCE", "/root/reference")      # where oracle/Makefile's REF points by default
@@ -46,24 +46,7 @@ def test_rx_instance_through_the_emulated_library(emu_qrl, oracle, name):  # noq
     """2 channels, a 1-sample call and cuts that are no multiple of the decimation, every port bit-identical to the oracle (the
     length rules of test_gpu_dispatch.check_rx)"""
     row = EMU_ROWS[name]
-    T = EMU_T.get(name, row[3])
-    B, _ = D.bases(name, oracle, row[3], row)
-    X = np.ascontiguousarray(B[:2, :T])
-    cuts = [(0, 1), (1, 30001), (30001, 30078), (30078, T)]
-    blk = row[0](emu_qrl, 2, max(hi - lo for lo, hi in cuts))
-    try:
-        got = D.concat_calls(D.run_rx(blk, X, cuts), blk.nports, 2)
-    finally:
-        blk.close()
-    for c in range(2):
-        rx = row[1](oracle)
-        for lo, hi in cuts:
-            rx.work(X[c, lo:hi])
-        for p in range(blk.nports):
-            g, w = got[p][c], rx.port(p)
-            n = min(len(g), len(w))
-            assert abs(len(g) - len(w)) <= D.SLACK and n > 0 and (p > 0 or len(g) == len(w)), (name, c, p, len(g), len(w))
-            assert np.array_equal(g[:n], w[:n]), "%s: port %d of channel %d differs from the oracle" % (name, p, c)
+    rx_through_the_emulated_library(emu_qrl, oracle, name, row, EMU_T.get(name, row[3]))
 
 
 # ------------------------------------------------------------------ the lean QPSK symbol sync's proof at every QPSK instance
