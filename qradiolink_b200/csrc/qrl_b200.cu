@@ -62,6 +62,40 @@ int upload_tables(HandleBase* h)
     });
 }
 
+// the Q32 phase increment of a rotator turning `cycles` of a full turn per sample (the offset over the rate it runs at)
+unsigned rot_inc(double cycles) { return static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(cycles * 4294967296.0)))); }
+
+// a handle's carrier-offset rotators, one rotator_cc per channel (DESIGN.md §2): the host table, its device copy (allocated zeroed)
+// and whether any channel rotates
+struct Rotators {
+    std::vector<RotState> host; RotState* d = nullptr; bool active = false;
+    int alloc(HandleBase* h, int C) { host.assign(C, RotState{ 0u, 0u, 0 }); return dev_alloc(h, &d, C); }
+    // from absolute sample n_abs on, channel `channel` (every channel for channel < 0) turns by `inc` per sample, the phase kept
+    // continuous
+    void retune(int channel, unsigned inc, long long n_abs)
+    {
+        active = false;
+        for (int c = 0; c < static_cast<int>(host.size()); c++) {
+            RotState& r = host[c];
+            if (channel < 0 || c == channel) {
+                r.base = r.base + r.inc * static_cast<unsigned>(n_abs - r.n_base);
+                r.n_base = n_abs;
+                r.inc = inc;
+            }
+            active = active || r.inc != 0 || r.base != 0;
+        }
+    }
+    // the offsets stay in force, the phase restarts: 0 at absolute sample 0
+    void restart() { active = false; for (RotState& r : host) { r.base = 0; r.n_base = 0; active = active || r.inc != 0; } }
+    // the table to the device once the handle's stream has drained, so no kernel that reads it is in flight there
+    int upload(HandleBase* h) const
+    {
+        QRL_CK(cudaStreamSynchronize(h->stream));
+        QRL_CK(cudaMemcpy(d, host.data(), sizeof(RotState) * host.size(), cudaMemcpyHostToDevice));
+        return QRL_OK;
+    }
+};
+
 }  // namespace
 
 // =====================================================================================================
@@ -117,7 +151,7 @@ struct qrl_rx : HandleBase {
     ViterbiState* d_vs2 = nullptr;
     unsigned char* d_port3 = nullptr; int* d_port3_cnt = nullptr;
     // front-end rotator (carrier offset)
-    std::vector<RotState> rot; RotState* d_rot = nullptr; bool rot_active = false; float2* d_rot_buf = nullptr;
+    Rotators rot; float2* d_rot_buf = nullptr;   // rot.d is allocated by the first offset
     bool rot_fused = false;            // this call: the rotator runs inside the stage-1 kernel (register-tiled shapes)
     // non-FM FSK detectors: band-pass bank + symbol filter
     float* d_bank_taps = nullptr; int nt_bank = 0;
@@ -196,7 +230,7 @@ int launch_fir_poly(qrl_rx* h, const float2* iq, long long stride, long long T, 
     dim3 grid(static_cast<unsigned>((nout + NOUT - 1) / NOUT), h->C);
     fir_decim_poly_kernel<D, Q, K, NOUT, NWARPS><<<grid, NWARPS * 32, smem, h->par()>>>(
         iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
-        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1, h->rot_fused ? h->d_rot : nullptr);
+        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1, h->rot_fused ? h->rot.d : nullptr);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
@@ -325,23 +359,6 @@ bool make_sm_partition(qrl_rx* h, unsigned loop_sms, int prio, bool fec_on_par_d
     h->s_loop = a; h->s_fec = b; h->s_par = c; h->s_loop2 = d; h->s_epi = e2;
     h->sm_loop = static_cast<int>(grp.sm.smCount); h->sm_par = static_cast<int>(rest.sm.smCount);
     return true;
-}
-
-// a carrier-offset change: from input sample n_in on, channel `channel` (every channel for channel < 0) turns by `inc` per sample,
-// the phase kept continuous; returns whether any channel still rotates
-bool retune(std::vector<RotState>& rot, int channel, unsigned inc, long long n_in)
-{
-    bool active = false;
-    for (int c = 0; c < static_cast<int>(rot.size()); c++) {
-        RotState& r = rot[c];
-        if (channel < 0 || c == channel) {
-            r.base = r.base + r.inc * static_cast<unsigned>(n_in - r.n_base);
-            r.n_base = n_in;
-            r.inc = inc;
-        }
-        if (r.inc != 0 || r.base != 0) active = true;
-    }
-    return active;
 }
 
 // interleaved = channel-interleaved layout [ceil(C/32)][slots][32] (allocated for the padded channel count)
@@ -514,7 +531,7 @@ int launch_fsk_frontend(qrl_rx* h, const Slice& s)
     auto kern = fsk_fm_frontend_kernel<D, Q, NOUT1>;
     if (int rc = smem_opt_in(h, kern, 120 * 1024)) return rc;
     const unsigned g = static_cast<unsigned>((s.n_new + strip - 1) / strip * h->C);     // strip-major, channel fastest
-    kern<<<g, FF_NT, smem, s.sp>>>(s.x, s.xstride, s.T, s.hist, h->H, h->d_taps1, s.n_in0, h->rot_fused ? h->d_rot : nullptr,
+    kern<<<g, FF_NT, smem, s.sp>>>(s.x, s.xstride, s.T, s.hist, h->H, h->d_taps1, s.n_in0, h->rot_fused ? h->rot.d : nullptr,
         static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->d_taps2, h->ntaps2, h->d_port0, h->port0_cap, s.k_call0,
         h->d_taps3, h->ntaps3, h->qd_gain, static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, s.k0, s.k1, strip, h->C);
     h->launches++;
@@ -1570,11 +1587,9 @@ int qrl_rx_reset(qrl_rx* h)
     }
     QRL_CK(cudaMemsetAsync(h->d_port1_cnt, 0, sizeof(int) * h->C, h->stream));
     if (h->d_port2_cnt) QRL_CK(cudaMemsetAsync(h->d_port2_cnt, 0, sizeof(int) * h->C, h->stream));
-    if (!h->rot.empty()) {
-        // the carrier offsets stay in force, the rotator's phase restarts: 0 at the first sample after the reset
-        h->rot_active = false;
-        for (RotState& r : h->rot) { r.base = 0; r.n_base = 0; h->rot_active = h->rot_active || r.inc != 0; }
-        if (h->d_rot) QRL_CK(cudaMemcpyAsync(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice, h->stream));
+    if (h->rot.d) {                    // the carrier offsets stay in force, the phase is 0 at the first sample after the reset
+        h->rot.restart();
+        if (int rc = h->rot.upload(h)) return rc;
     }
     QRL_CK(cudaStreamSynchronize(h->stream));   // the staging vectors above go out of scope
     h->n_in = 0; h->n1 = 0; h->n_in_s = 0; h->n1_s = 0; h->hist_cur = 0; h->port0_n = 0; h->prev_nsub = 0; h->rssi_n = 0;
@@ -1659,14 +1674,10 @@ int qrl_rx_set_param(qrl_rx* h, int channel, int key, double value)
     }
     if (key == QRL_PARAM_CARRIER_OFFSET_HZ) {        // gr_demod_base::set_carrier_offset (:1220-1225): phase inc = 2 pi (-offset) / fs
         if (channel >= h->C) { set_err(h, "set_param: channel out of range"); return QRL_EINVAL; }
-        if (h->rot.empty()) h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
-        const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(-value / h->samp_rate * 4294967296.0))));
-        h->rot_active = retune(h->rot, channel, inc, h->n_in);
-        if (!h->d_rot) { int rc = dev_alloc(h, &h->d_rot, h->C); if (rc) return rc; }
-        QRL_CK(cudaStreamSynchronize(h->stream));
+        if (!h->rot.d) { int rc = h->rot.alloc(h, h->C); if (rc) return rc; }
+        h->rot.retune(channel, rot_inc(-value / h->samp_rate), h->n_in);
         if (h->overlap) { int rc = rx_join_host(h); if (rc) return rc; }
-        QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
-        return QRL_OK;
+        return h->rot.upload(h);
     }
     // ---- run-time setters of the analog blocks.  Kernel parameters travel by value with every launch, so a plain host-side update is
     // enough for scalars; new taps are uploaded after everything in flight has drained and meet the true sample history (the rings)
@@ -1831,11 +1842,11 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
         xstride = shared ? 0 : h->Tmax;
     }
     // carrier offset: inside the stage-1 kernel where it can rotate its window, else a separate pass
-    h->rot_fused = h->rot_active && stage1_fuses_rotator(h) && !getenv("QRL_ROTATOR_PASS");
-    if (h->rot_active && !h->rot_fused) {
+    h->rot_fused = h->rot.active && stage1_fuses_rotator(h) && !getenv("QRL_ROTATOR_PASS");
+    if (h->rot.active && !h->rot_fused) {
         if (!h->d_rot_buf) { int rc = dev_alloc(h, &h->d_rot_buf, static_cast<size_t>(h->Tmax) * h->C, false); if (rc) return rc; }
         dim3 g(static_cast<unsigned>(std::min<long long>((T + 255) / 256, 4096)), h->C);
-        rotator_kernel<<<g, 256, 0, h->stream>>>(h->d_rot, x, xstride, h->d_rot_buf, h->Tmax, T, h->n_in);
+        rotator_kernel<<<g, 256, 0, h->stream>>>(h->rot.d, x, xstride, h->d_rot_buf, h->Tmax, T, h->n_in);
         h->launches++;
         x = h->d_rot_buf; xstride = h->Tmax;
     }
@@ -1927,8 +1938,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
             h->prof.end(pe);
             if (rc) return rc;
             dim3 g((h->H + 127) / 128, h->C);
-            if (h->rot_fused) frontend_hist_kernel<<<g, 128, 0, sp>>>(h->d_rot, xg, xstride, Tg, h->n_in, h->d_hist[h->hist_cur], h->d_hist[h->hist_cur ^ 1], h->H);
-            else hist_update_kernel<<<g, 128, 0, sp>>>(xg, xstride, Tg, h->d_hist[h->hist_cur], h->d_hist[h->hist_cur ^ 1], h->H);
+            frontend_hist_kernel<<<g, 128, 0, sp>>>(h->rot_fused ? h->rot.d : nullptr, xg, xstride, Tg, h->n_in, h->d_hist[h->hist_cur], h->d_hist[h->hist_cur ^ 1], h->H);
             h->launches++;
             h->hist_cur ^= 1;
             h->n_in = Ng; h->n1 = kg1;
@@ -2935,7 +2945,7 @@ struct qrl_frontend : HandleBase {
     float2* d_hist[2] = { nullptr, nullptr };
     float2* d_in = nullptr; float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_in = 0, n1 = 0;
-    std::vector<RotState> rot; RotState* d_rot = nullptr; bool rot_active = false;
+    Rotators rot;
     // shared stream (stride 0): [max_in] host staging, and frontend_shared_kernel's chain-order taps [D][QP] and strip shape
     float2* d_in1 = nullptr;
     float* d_ht = nullptr; int QP = 0, Qmax = 0, NB = 0, n_sm = 0; size_t fs_smem = 0;
@@ -2969,8 +2979,7 @@ int qrl_frontend_create(int samp_rate, int n_channels, long max_in, int device, 
     if ((rc = dev_alloc(h, &h->d_hist[1], static_cast<size_t>(h->H) * h->C))) return fail(rc);
     h->out_stride = max_in / h->D + 2;
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_rot, h->C))) return fail(rc);
-    h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
+    if ((rc = h->rot.alloc(h, h->C))) return fail(rc);
     if (h->D <= FESH_DMAX) {
         h->Qmax = (h->ntaps - 1) / h->D + 1;
         h->QP = (h->Qmax + 3) & ~3;
@@ -3004,11 +3013,8 @@ int qrl_frontend_set_carrier_offset(qrl_frontend* h, int channel, double offset_
 {
     // gr_demod_base::set_carrier_offset (:1220-1225): rotator phase increment 2 pi (-offset) / samp_rate at the DEVICE rate
     if (!h || channel >= h->C) return QRL_EINVAL;
-    const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(-offset_hz / h->samp_rate * 4294967296.0))));
-    h->rot_active = retune(h->rot, channel, inc, h->n_in);
-    QRL_CK(cudaStreamSynchronize(h->stream));
-    QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
-    return QRL_OK;
+    h->rot.retune(channel, rot_inc(-offset_hz / h->samp_rate), h->n_in);
+    return h->rot.upload(h);
 }
 int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int on_device, long* n_out)
 {
@@ -3032,7 +3038,7 @@ int qrl_frontend_work(qrl_frontend* h, const float* iq, long T, long stride, int
     }
     const long long N = h->n_in + T;
     const long long k0 = h->n1, k1 = (N + h->D - 1) / h->D;              // outputs k with D k <= N - 1
-    const RotState* rs = h->rot_active ? h->d_rot : nullptr;
+    const RotState* rs = h->rot.active ? h->rot.d : nullptr;
     if (k1 > k0 && shared && h->D <= FESH_DMAX) {
         auto kern = frontend_shared_kernel<FESH_K, FESH_KC>;
         if (int rc = smem_opt_in(h, kern, FESH_SMEM)) return rc;
@@ -3117,7 +3123,7 @@ struct qrl_tx_frontend : HandleBase {
     float2* d_hist[2] = { nullptr, nullptr };
     float2* d_in = nullptr; float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_in = 0;
-    std::vector<RotState> rot; RotState* d_rot = nullptr; bool rot_active = false;
+    Rotators rot;
 };
 
 int qrl_tx_frontend_destroy(qrl_tx_frontend* h) { return h ? handle_close(h) : QRL_OK; }
@@ -3145,8 +3151,7 @@ int qrl_tx_frontend_create(int samp_rate, int n_channels, long max_in, int devic
     }
     h->out_stride = static_cast<long long>(max_in) * h->N;
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_rot, h->C))) return fail(rc);
-    h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
+    if ((rc = h->rot.alloc(h, h->C))) return fail(rc);
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
@@ -3160,11 +3165,8 @@ int qrl_tx_frontend_set_carrier_offset(qrl_tx_frontend* h, int channel, double o
 {
     // gr_mod_base::set_carrier_offset (:799-805): rotator_cc(2 pi offset / 1e6) at the modulators' 1 Msps, whatever the device rate
     if (!h || channel >= h->C) return QRL_EINVAL;
-    const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(offset_hz / 1e6 * 4294967296.0))));
-    h->rot_active = retune(h->rot, channel, inc, h->n_in);
-    QRL_CK(cudaStreamSynchronize(h->stream));
-    QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
-    return QRL_OK;
+    h->rot.retune(channel, rot_inc(offset_hz / 1e6), h->n_in);
+    return h->rot.upload(h);
 }
 int qrl_tx_frontend_work(qrl_tx_frontend* h, const float* iq, long n, long stride, int on_device, long* n_out)
 {
@@ -3177,7 +3179,7 @@ int qrl_tx_frontend_work(qrl_tx_frontend* h, const float* iq, long n, long strid
     QRL_CK(cudaSetDevice(h->device));
     const float2* x = reinterpret_cast<const float2*>(iq);
     long long xstride = stride;
-    const RotState* rs = h->rot_active ? h->d_rot : nullptr;
+    const RotState* rs = h->rot.active ? h->rot.d : nullptr;
     if (h->N == 1) {
         // the reference has no resampler at 1 Msps (gr_mod_base.cpp:260-293): the rotator alone, or a copy
         if (!rs) {
@@ -3258,7 +3260,7 @@ struct qrl_tx_combiner : HandleBase {
     float2* d_part = nullptr;                   // [nblk][range N]: block partial sums (nblk > 1)
     const float2** d_rows = nullptr; std::vector<const float2*> rows;
     long long n_out = 0;                        // absolute device-rate index of the next output
-    std::vector<RotState> rot; RotState* d_rot = nullptr;
+    Rotators rot;                               // rot.d is always passed: a channel with inc == base == 0 is not rotated
 };
 
 int qrl_tx_combiner_destroy(qrl_tx_combiner* h) { return h ? handle_close(h) : QRL_OK; }
@@ -3294,9 +3296,8 @@ int qrl_tx_combiner_create(int samp_rate, int n_channels, long max_in, int devic
     }
     if ((rc = dev_alloc(h, &h->d_y, static_cast<size_t>(max_in) * h->N, false))) return fail(rc);
     if ((rc = dev_alloc(h, &h->d_rows, h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_rot, h->C))) return fail(rc);
+    if ((rc = h->rot.alloc(h, h->C))) return fail(rc);
     h->rows.assign(h->C, nullptr);
-    h->rot.assign(h->C, RotState{ 0u, 0u, 0 });
     if (cudaStreamSynchronize(h->stream) != cudaSuccess) { set_err(h, "create sync failed"); return fail(QRL_ECUDA); }
     *out = h;
     return QRL_OK;
@@ -3313,11 +3314,8 @@ int qrl_tx_combiner_set_carrier_offset(qrl_tx_combiner* h, int channel, double o
         set_err(h, "qrl_tx_combiner_set_carrier_offset: bad channel or |offset| > samp_rate / 2");
         return QRL_EINVAL;
     }
-    const unsigned inc = static_cast<unsigned>(static_cast<int>(static_cast<long long>(std::rint(offset_hz / h->samp_rate * 4294967296.0))));
-    retune(h->rot, channel, inc, h->n_out);
-    QRL_CK(cudaStreamSynchronize(h->stream));
-    QRL_CK(cudaMemcpy(h->d_rot, h->rot.data(), sizeof(RotState) * h->C, cudaMemcpyHostToDevice));
-    return QRL_OK;
+    h->rot.retune(channel, rot_inc(offset_hz / h->samp_rate), h->n_out);
+    return h->rot.upload(h);
 }
 int qrl_tx_combiner_set_gain(qrl_tx_combiner* h, float bb_gain)
 {
@@ -3362,11 +3360,11 @@ int qrl_tx_combiner_work(qrl_tx_combiner* h, const float* const* rows, long n, i
         const long long pstride = h->range * h->N;
         if (h->N == 1) {
             dim3 g(static_cast<unsigned>(std::min<long long>((hi - lo + 255) / 256, 4096)), h->nblk);
-            tx_combiner_direct_kernel<<<g, 256, 0, h->stream>>>(h->d_rows, h->C, h->d_rot, lo, hi, h->n_out, dst, pstride, final, g1, g2);
+            tx_combiner_direct_kernel<<<g, 256, 0, h->stream>>>(h->d_rows, h->C, h->rot.d, lo, hi, h->n_out, dst, pstride, final, g1, g2);
         } else {
             const long long TM = static_cast<long long>(h->G) * TXC_R;
             dim3 g(static_cast<unsigned>((hi - lo + TM - 1) / TM), h->nblk);
-            kern<<<g, h->G * h->N, smem, h->stream>>>(h->d_rows, h->C, h->d_rot, n, lo, hi, h->n_out, h->d_hist[h->hist_cur],
+            kern<<<g, h->G * h->N, smem, h->stream>>>(h->d_rows, h->C, h->rot.d, n, lo, hi, h->n_out, h->d_hist[h->hist_cur],
                                                       hi == n ? h->d_hist[h->hist_cur ^ 1] : nullptr, h->H, h->d_arms, h->N, h->NTP, h->G,
                                                       dst, pstride, final, g1, g2);
         }

@@ -119,6 +119,17 @@ __device__ __forceinline__ unsigned char qrl_soft_u8(float v, float scale)
 // front-end rotator state (gr_demod_base's rotator_cc): exact Q32 phase, phase = base + inc * (n_abs - n_base)
 struct RotState { unsigned inc, base; long long n_base; };
 
+// x turned by the rotator's phase at absolute sample n_abs (DESIGN.md §2): the Q32 phase as a signed angle times pi / 2^31 in double,
+// rounded to float, qrl_sincosf, then (x cos - y sin, x sin + y cos).  Every kernel that rotates calls this, so they agree bit for bit.
+__device__ __forceinline__ float2 qrl_rotate(const RotState& r, long long n_abs, const float2& x)
+{
+    const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs - r.n_base);
+    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
+    float sn, cs;
+    qrl_sincosf(ang, sn, cs);
+    return make_float2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
+}
+
 // The per-tile arithmetic of the register-tiled stage 1, shared by fir_decim_poly_kernel and fsk_fm_frontend_kernel: one tile =
 // NOUT consecutive outputs from a window of (NOUT + Q - 1) D samples in shared memory.
 template <int D, int Q>
@@ -173,20 +184,14 @@ struct FirPolyWindow {
             xw[idx] = v;
         }
     }
-    // every thread: rotate this call's samples of the window in place (same arithmetic as rotator_kernel, sample by sample; history
-    // samples were rotated when they were new)
+    // every thread: rotate this call's samples of the window in place (history samples were rotated when they were new)
     __device__ __forceinline__ void rotate(float2* xs_raw, const RotState& r, long long T, long long n_in_before, int nthreads) const
     {
         float2* xw = xs_raw + shift;
         for (int idx = threadIdx.x; idx < W; idx += nthreads) {
             const long long i = i0 + idx;
             if (i < 0 || i >= T) continue;
-            const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_in_before + i - r.n_base);
-            const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-            float sn, cs;
-            qrl_sincosf(ang, sn, cs);
-            const float2 x = xw[idx];
-            xw[idx] = make_float2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
+            xw[idx] = qrl_rotate(r, n_in_before + i, xw[idx]);
         }
     }
 };
@@ -263,8 +268,8 @@ __device__ __forceinline__ void fir_poly_tile(const float2* xs, const float (&ta
     }
 }
 
-// rot != nullptr: the carrier-offset rotator is applied to the window in shared memory right after the fill (same arithmetic as
-// rotator_kernel, sample by sample), so a non-zero offset costs no extra pass over HBM (8.16 B per input sample instead of 24);
+// rot != nullptr: the carrier-offset rotator (qrl_rotate) is applied to the window in shared memory right after the fill, so a
+// non-zero offset costs no extra pass over HBM (8.16 B per input sample instead of 24);
 // the history tail then holds ALREADY ROTATED samples (frontend_hist_kernel), like the reference's resampler history.
 template <int D, int Q, int K, int NOUT, int NWARPS>
 __global__ void __launch_bounds__(NWARPS * 32)
@@ -3022,27 +3027,21 @@ __global__ void fir_fff_ring_kernel(const float* __restrict__ in, unsigned in_ma
     out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc;
 }
 
-// Front-end rotator (gr_demod_base's rotator_cc, carrier offset): out[c][n] = in[c][n] * exp(j theta), exact Q32 phase
-// phase = base[c] + inc[c] * (n_abs - n_base[c]).  Only launched when some channel has a non-zero offset (the
-// reference default is 0); it costs one extra pass over the slab -- fusing it needs complex stage-1 taps (next).
+// Front-end rotator (gr_demod_base's rotator_cc, carrier offset) as a pass of its own: out[c][n] = qrl_rotate(rs[c], n_abs0 + n,
+// in[c][n]).  Only launched when some channel has a non-zero offset (the reference default is 0); it costs one extra pass over the
+// slab -- fusing it needs complex stage-1 taps (next).
 __global__ void rotator_kernel(const RotState* __restrict__ rs, const float2* __restrict__ in, long long in_stride,
                                float2* __restrict__ out, long long out_stride, long long T, long long n_abs0)
 {
     const int c = blockIdx.y;
     const RotState r = rs[c];
-    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < T; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs0 + i - r.n_base);
-        const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-        float sn, cs;
-        qrl_sincosf(ang, sn, cs);
-        const float2 x = in[static_cast<long long>(c) * in_stride + i];
-        out[static_cast<long long>(c) * out_stride + i] = make_float2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
-    }
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < T; i += static_cast<long long>(gridDim.x) * blockDim.x)
+        out[static_cast<long long>(c) * out_stride + i] = qrl_rotate(r, n_abs0 + i, in[static_cast<long long>(c) * in_stride + i]);
 }
 
 // Front end at device rates >= 2 Msps (gr_demod_base.cpp:1303-1362): rotator_cc at the device rate fused into the /D decimating FIR
-// (83 taps at 2 Msps).  One CTA = 128 outputs of one channel: the window is rotated while it is loaded into shared memory (same Q32
-// phase arithmetic as rotator_kernel), the previous calls' tail comes ALREADY ROTATED from `hist` (a retune must not touch samples that
+// (83 taps at 2 Msps).  One CTA = 128 outputs of one channel: the window is rotated while it is loaded into shared memory
+// (qrl_rotate), the previous calls' tail comes ALREADY ROTATED from `hist` (a retune must not touch samples that
 // are already inside the filter, like the reference's resampler history); each thread then runs THE FIR order over its window.
 __global__ void __launch_bounds__(128)
 frontend_fir_kernel(const RotState* __restrict__ rs /* nullptr: no rotation */, const float2* __restrict__ in, long long in_stride, long long T,
@@ -3070,13 +3069,7 @@ frontend_fir_kernel(const RotState* __restrict__ rs /* nullptr: no rotation */, 
         if (li >= 0) {
             if (li < T) {
                 v = x[li];
-                if (rs) {
-                    const unsigned ph = r.base + r.inc * static_cast<unsigned>(a - r.n_base);
-                    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-                    float sn, cs;
-                    qrl_sincosf(ang, sn, cs);
-                    v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
-                }
+                if (rs) v = qrl_rotate(r, a, v);
             }
         } else if (H + li >= 0) v = hc[H + li];
         xs[i] = v;
@@ -3098,14 +3091,7 @@ __global__ void frontend_hist_kernel(const RotState* __restrict__ rs, const floa
     float2 v;
     if (li >= 0) {
         v = in[static_cast<long long>(c) * in_stride + li];
-        if (rs) {
-            const RotState r = rs[c];
-            const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs0 + li - r.n_base);
-            const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-            float sn, cs;
-            qrl_sincosf(ang, sn, cs);
-            v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
-        }
+        if (rs) v = qrl_rotate(rs[c], n_abs0 + li, v);
     } else v = old_hist[static_cast<long long>(c) * H + (H + li)];
     new_hist[static_cast<long long>(c) * H + i] = v;
 }
@@ -3114,8 +3100,8 @@ __global__ void frontend_hist_kernel(const RotState* __restrict__ rs, const floa
 // gr_demod_mmdvm_multi.cpp:68-123's wiring, one rotator + /D resampler per channel behind one source.  The outputs are those of
 // frontend_fir_kernel for each channel fed the shared stream, bit for bit; what changes is how the work is laid out:
 //   * one CTA = NB K consecutive outputs (a strip) of a group of CG channels.  The raw window of the strip is loaded from HBM into
-//     shared memory ONCE (coalesced 8-byte loads, any sample alignment), then for each channel of the group it is rotated (the
-//     same Q32 phase arithmetic as frontend_fir_kernel) into a polyphase-split copy xr[r][m] = x[D (kb - Qmax + 1 + m) - r].  The
+//     shared memory ONCE (coalesced 8-byte loads, any sample alignment), then for each channel of the group it is rotated
+//     (qrl_rotate) into a polyphase-split copy xr[r][m] = x[D (kb - Qmax + 1 + m) - r].  The
 //     first strip of a call takes its older samples from the channel's own already-rotated tail (frontend_hist_kernel);
 //   * phase 1: work item (branch r, block b) = K consecutive outputs of branch r.  With D <= 32 branch r is THE FIR order's slot r,
 //     accumulated oldest sample first: the taps sit in shared memory in chain order ht[r][s] = h[D (Q_r - 1 - s) + r], each chunk of
@@ -3160,13 +3146,7 @@ frontend_shared_kernel(const RotState* __restrict__ rs /* nullptr: no rotation *
             if (li >= 0) {
                 if (li < T) {
                     v = rw[i];
-                    if (rs) {
-                        const unsigned ph = r.base + r.inc * static_cast<unsigned>(a - r.n_base);
-                        const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-                        float sn, cs;
-                        qrl_sincosf(ang, sn, cs);
-                        v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
-                    }
+                    if (rs) v = qrl_rotate(r, a, v);
                 }
             } else if (H + li >= 0) v = hc[H + li];
             const int m = static_cast<int>((static_cast<float>(i) + 0.5f) * invD);   // i / D (exact: i < 2^16, D <= 32)
@@ -3231,7 +3211,7 @@ frontend_shared_kernel(const RotState* __restrict__ rs /* nullptr: no rotation *
 // rational_resampler_ccf(L, 1) with L = samp_rate / 1e6 and about 210 taps per arm, y[L m + p] = sum_k arm[p][k] x[m - k].
 // The arms are too long for interp_fir_ccf_rt_kernel's all-taps-in-registers shape, so:
 //   * one CTA = a tile of G R input positions m of one channel, all L phases.  The window is rotated while it is filled into shared
-//     memory (same Q32 phase arithmetic as frontend_fir_kernel); the previous calls' NTP - 1 samples come ALREADY ROTATED from `hist`
+//     memory (qrl_rotate); the previous calls' NTP - 1 samples come ALREADY ROTATED from `hist`
 //     (frontend_hist_kernel keeps that tail), so a retune never touches samples already inside the filter;
 //   * the arm table sits in shared memory as [NTP][L] (= the zero-padded tap array), so lanes on consecutive phases read consecutive
 //     words;
@@ -3264,13 +3244,7 @@ tx_frontend_interp_kernel(const RotState* __restrict__ rs /* nullptr: no rotatio
         if (li >= 0) {
             if (li < T) {
                 v = x[li];
-                if (rs) {
-                    const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs0 + li - r.n_base);
-                    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-                    float sn, cs;
-                    qrl_sincosf(ang, sn, cs);
-                    v = make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
-                }
+                if (rs) v = qrl_rotate(r, n_abs0 + li, v);
             }
         } else v = hc[H + li];
         xs[i] = v;
@@ -3310,16 +3284,11 @@ tx_frontend_interp_kernel(const RotState* __restrict__ rs /* nullptr: no rotatio
 // depend on the launch shape or on how a stream is chunked.
 constexpr int TXC_BLOCK = 8;
 
-// the device-rate NCO of one channel at absolute output index n_abs: the Q32 phase and qrl_sincosf of frontend_hist_kernel, applied
-// after the interpolator; a channel with inc == base == 0 is not rotated (bit-exact pass-through)
+// the device-rate NCO of one channel at absolute output index n_abs, applied after the interpolator; a channel with inc == base == 0
+// is not rotated (bit-exact pass-through)
 __device__ __forceinline__ float2 tx_combiner_rotate(const RotState& r, long long n_abs, float2 v)
 {
-    if (r.inc == 0u && r.base == 0u) return v;
-    const unsigned ph = r.base + r.inc * static_cast<unsigned>(n_abs - r.n_base);
-    const float ang = static_cast<float>(static_cast<double>(static_cast<int>(ph)) * (3.14159265358979323846 / 2147483648.0));
-    float sn, cs;
-    qrl_sincosf(ang, sn, cs);
-    return make_float2(v.x * cs - v.y * sn, v.x * sn + v.y * cs);
+    return (r.inc == 0u && r.base == 0u) ? v : qrl_rotate(r, n_abs, v);
 }
 
 // y = (S * g1) * g2 per component (scale2_linear_kernel's arithmetic: multiply_const_cc(1 / C) then multiply_const_cc(bb_gain))
@@ -3460,20 +3429,6 @@ __global__ void tx_combiner_sum_kernel(const float2* __restrict__ part, long lon
         }
         y[i] = tx_combiner_scale(t, g1, g2);
     }
-}
-
-// roll the stage-1 history: new_hist = last H samples of (old_hist ++ iq[0..T))
-__global__ void hist_update_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
-                                   const float2* __restrict__ old_hist, float2* __restrict__ new_hist, int H)
-{
-    const int c = blockIdx.y;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= H) return;
-    const long long src = T - H + i;     // index into iq; negative -> old history
-    float2 v;
-    if (src >= 0) v = iq[static_cast<long long>(c) * iq_stride + src];
-    else v = old_hist[static_cast<long long>(c) * H + (H + src)];
-    new_hist[static_cast<long long>(c) * H + i] = v;
 }
 
 // ================================================================================================
