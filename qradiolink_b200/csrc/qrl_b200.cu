@@ -23,12 +23,6 @@ using namespace qrl;
 
 namespace {
 
-struct Ring {
-    void* d = nullptr;
-    unsigned mask = 0;
-    long long stride = 0;   // items per channel (= capacity)
-};
-
 unsigned pow2_at_least(long long n)
 {
     unsigned long long c = 64;
@@ -47,6 +41,21 @@ std::vector<float> make_arms(const std::vector<float>& taps, int L, int nt)
 int arms_nt(const std::vector<float>& taps, int L) { return (static_cast<int>(taps.size()) + L - 1) / L; }
 
 using HandleBase = QrlHandleBase;       // qrl_handle.hpp: shared by every handle type of the library
+
+// a zeroed [C][capacity] stream ring of at least min_items items of per_item Ts each; interleaved: laid out [C / 32][capacity][32] for
+// the channel count rounded up to 32.  zero_list, when given, gets the buffer for the handle's reset to clear.
+template <class T>
+int make_ring(HandleBase* h, Ring<T>* r, int C, long long min_items, bool interleaved = false,
+              std::vector<std::pair<void*, size_t>>* zero_list = nullptr, int per_item = 1)
+{
+    const unsigned cap = pow2_at_least(min_items);
+    const size_t n = static_cast<size_t>(cap) * per_item * (interleaved ? static_cast<size_t>((C + 31) / 32) * 32 : static_cast<size_t>(C));
+    r->mask = cap - 1;
+    r->stride = cap;
+    const int rc = dev_alloc(h, &r->d, n);
+    if (!rc && zero_list) zero_list->emplace_back(r->d, n * sizeof(T));
+    return rc;
+}
 
 // the atan, tanh, MMSE and sine lookup tables, once per device (keyed by this function)
 int upload_tables(HandleBase* h)
@@ -123,31 +132,31 @@ struct qrl_rx : HandleBase {
     bool fir_group_forced = false;     // QRL_FIR_GROUP given: keep it in overlap mode too
     int fir_group = 4;                 // stage-1 launches cover this many slices (bigger launches, same pipeline depth)
     bool fsk_fused = false;            // fsk_fm_fused(): stage 1 runs inside the per-slice front-end kernel (decided at create)
-    Ring r1;
+    Ring<float2> r1;
     // stage 2: channel / shaping filter on the complex stream (port 0)
     float* d_taps2 = nullptr; int ntaps2 = 0; size_t taps2_cap = 0;     // floats allocated for d_taps2 (set_filter_width redesigns)
     float if_gain = 0.9f;              // gr_demod_ssb: multiply_const_cc(0.9) in front of the side-band filter (set_gain)
-    Ring r2;
+    Ring<float2> r2;
     float2* d_port0 = nullptr; long port0_cap = 0; long port0_n = 0;
     // stage 3: quadrature demod + RRC (4FSK-FM)
     float* d_taps3 = nullptr; int ntaps3 = 0; float qd_gain = 0;
-    Ring r4;
+    Ring<float> r4;
     // PSK chains: agc2 + costas "PLL" loop stage (per sample), output ring r3 (interleaved)
     AgcCostasParams acp{};
     AgcCostasState* d_ac = nullptr;
     // NBFM: de-emphasis recurrence in its own kernel on s_loop2 (overlaps the next slice's squelch recurrence)
-    NbfmDeemphState* d_nb2 = nullptr; Ring raud; bool nbfm_split = false;
+    NbfmDeemphState* d_nb2 = nullptr; Ring<float> raud; bool nbfm_split = false;
     // NBFM: stream between the 2/5 resampler and the audio filter (copy, or ctcss_squelch_ff after set_ctcss(f))
-    Ring rq; NbfmCtcss ctc{}; double* d_cenv = nullptr;
+    Ring<float> rq; NbfmCtcss ctc{}; double* d_cenv = nullptr;
     // gr_demod_dsss: one chain kernel behind stage 1 (dsss_chain_kernel)
     DsssParams dsp{}; DsssState* d_ds = nullptr; float* d_ds_arms = nullptr; float2* d_ds_taps = nullptr;
-    Ring ds_a, ds_c, ds_d; long long ds_o_call0 = 0;
-    Ring r3;
+    Ring<float2> ds_a, ds_c, ds_d; long long ds_o_call0 = 0;
+    Ring<float2> r3;
     // BPSK, 2FSK (not GMSK), QPSK above 4 samples per symbol: fll_band_edge_cc behind stage 1; BPSK / 2FSK: second (delayed) decoder
     bool fll = false;
     FllParams fllp{};
     FllState* d_fll = nullptr; float2* d_fll_hist = nullptr; float* d_fll_taps = nullptr;
-    Ring rf;                       // FLL output (channel-major complex)
+    Ring<float2> rf;               // FLL output (channel-major complex)
     ViterbiState* d_vs2 = nullptr;
     unsigned char* d_port3 = nullptr; int* d_port3_cnt = nullptr;
     // front-end rotator (carrier offset)
@@ -156,18 +165,18 @@ struct qrl_rx : HandleBase {
     // non-FM FSK detectors: band-pass bank + symbol filter
     float* d_bank_taps = nullptr; int nt_bank = 0;
     float* d_symf_taps = nullptr; int nt_symf = 0;
-    Ring rbank;                    // bank output (complex for 4FSK, float for 2FSK), channel-major
+    Ring<float> rbank;             // bank output (complex for 4FSK, float for 2FSK), channel-major
     // FreeDV: agc2_ff + audio band-pass + int16 conversion behind the side-band filter (AGC output ring: rstr)
     FreedvRxParams fdp{};
     FreedvRxState* d_fdv = nullptr;
     // SSB audio chain
     SsbParams ssbp{};
     SsbState* d_ssb = nullptr;
-    Ring rclip, rstr;
+    Ring<float2> rclip; Ring<float> rstr;
     // NBFM audio chain
     NbfmParams nbp{};
     NbfmState* d_nb = nullptr;
-    Ring rg, rd, rr;
+    Ring<float2> rg; Ring<float> rd, rr;
     float* d_env = nullptr; float* d_arm_taps = nullptr; float* d_audio_taps = nullptr;
     float* d_port1f = nullptr;
     int tsr = 0;
@@ -195,7 +204,7 @@ struct qrl_rx : HandleBase {
     long long prev_k1[16] = { 0 }, cur_k1[16] = { 0 }; int prev_nsub = 0;      // stage-1 sample index at the end of each slice
     int ss_ch = 256;                                     // rows per symbol-sync window (256 x 3 stages or 512 x 2)
     float2* d_port1 = nullptr; long port1_cap = 0; int* d_port1_cnt = nullptr;
-    Ring r5;   // soft bits (u8)
+    Ring<unsigned char> r5;   // soft bits
     ViterbiState* d_vs = nullptr;
     unsigned char* d_port2 = nullptr; long port2_cap = 0; int* d_port2_cnt = nullptr;
     long n1max = 0;
@@ -229,8 +238,7 @@ int launch_fir_poly(qrl_rx* h, const float2* iq, long long stride, long long T, 
     const long long nout = k1 - k0;
     dim3 grid(static_cast<unsigned>((nout + NOUT - 1) / NOUT), h->C);
     fir_decim_poly_kernel<D, Q, K, NOUT, NWARPS><<<grid, NWARPS * 32, smem, h->par()>>>(
-        iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
-        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1, h->rot_fused ? h->rot.d : nullptr);
+        iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->r1, h->n_in, k0, k1, h->rot_fused ? h->rot.d : nullptr);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
@@ -245,8 +253,7 @@ int launch_fir_d2(qrl_rx* h, const float2* iq, long long stride, long long T, lo
     const long long nout = k1 - k0;
     dim3 grid(static_cast<unsigned>((nout + NOUT - 1) / NOUT), h->C);
     fir_decim2_kernel<NTP, K, NTHREADS><<<grid, NTHREADS, smem, h->par()>>>(
-        iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
-        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
+        iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->r1, h->n_in, k0, k1);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
@@ -260,7 +267,7 @@ int launch_fir_resamp_2_25(qrl_rx* h, const float2* iq, long long stride, long l
     if (int rc = smem_opt_in(h, fir_resamp_ccf_kernel<L, M, NT, NOUT>, (int)smem)) return rc;
     dim3 grid(static_cast<unsigned>((k1 - k0 + NOUT - 1) / NOUT), h->C);
     fir_resamp_ccf_kernel<L, M, NT, NOUT><<<grid, 256, smem, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1,
-        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
+        h->r1, h->n_in, k0, k1);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
@@ -293,7 +300,7 @@ int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long
         const long long nout = k1 - k0;
         dim3 grid(static_cast<unsigned>((nout + 127) / 128), h->C);
         fir_resamp_hist_generic_kernel<<<grid, 128, 0, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->nt_arm1,
-            h->L1, h->D1, static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
+            h->L1, h->D1, h->r1, h->n_in, k0, k1);
         h->launches++;
         QRL_CK(cudaGetLastError());
         return QRL_OK;
@@ -305,7 +312,7 @@ int stage1(qrl_rx* h, const float2* iq, long long stride, long long T, long long
         const long long nout = k1 - k0;
         dim3 grid(static_cast<unsigned>((nout + 127) / 128), h->C);
         fir_decim_hist_generic_kernel<<<grid, 128, 0, h->par()>>>(iq, stride, T, h->d_hist[h->hist_cur], h->H, h->d_taps1, h->ntaps1, h->D1,
-            static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->n_in, k0, k1);
+            h->r1, h->n_in, k0, k1);
         h->launches++;
         QRL_CK(cudaGetLastError());
         return QRL_OK;
@@ -385,23 +392,9 @@ std::vector<float> fll_design(float sps, float rolloff, int N)
     return t;
 }
 
-int make_ring(qrl_rx* h, Ring* r, size_t isz, long long min_items, bool interleaved = false)
-{
-    unsigned cap = pow2_at_least(min_items);
-    r->mask = cap - 1;
-    r->stride = cap;
-    unsigned char* p = nullptr;
-    const size_t nch = interleaved ? static_cast<size_t>((h->C + 31) / 32) * 32 : static_cast<size_t>(h->C);
-    const size_t bytes = static_cast<size_t>(cap) * isz * nch;
-    int rc = dev_alloc(h, &p, bytes, true);
-    r->d = p;
-    if (!rc) h->zero_list.emplace_back(p, bytes);
-    return rc;
-}
-
 // low-rate stream filters: register-tiled instances for real calls, the one-thread-per-output kernels for slivers
-int launch_fir_ccf_c(HandleBase* h, int C, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
-                     const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
+int launch_fir_ccf(HandleBase* h, int C, cudaStream_t st, Ring<const float2> in, Ring<float2> out,
+                   const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
 {
     const long long n = a1 - a0;
     if (n <= 0) return QRL_OK;
@@ -413,22 +406,17 @@ int launch_fir_ccf_c(HandleBase* h, int C, cudaStream_t st, const float2* in, un
     }
     if (n >= 256 && smem <= 100 * 1024 && ntaps >= K) {      // (the tiled kernel's head / tail phases assume at least K taps)
         dim3 g(static_cast<unsigned>((n + TILE - 1) / TILE), C);
-        fir_ccf_ring_tiled_kernel<K, NT><<<g, NT, smem, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
+        fir_ccf_ring_tiled_kernel<K, NT><<<g, NT, smem, st>>>(in, out, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
     } else {
         dim3 g(static_cast<unsigned>((n + 255) / 256), C);
-        fir_ccf_ring_kernel<<<g, 256, sizeof(float) * ntaps, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
+        fir_ccf_ring_kernel<<<g, 256, sizeof(float) * ntaps, st>>>(in, out, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
     }
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
-int launch_fir_ccf(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float2* out, unsigned out_mask, long long out_stride,
-                   const float* taps, int ntaps, long long a0, long long a1, float2* lin, long long lin_stride, long long lin_base, int interleaved)
-{
-    return launch_fir_ccf_c(h, h->C, st, in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, a0, a1, lin, lin_stride, lin_base, interleaved);
-}
-int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_mask, long long in_stride, float* out, unsigned out_mask, long long out_stride,
-                      const float* taps, int ntaps, float gain, long long a0, long long a1)
+int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, Ring<const float2> in, Ring<float> out, const float* taps, int ntaps, float gain, long long a0,
+                      long long a1)
 {
     const long long n = a1 - a0;
     if (n <= 0) return QRL_OK;
@@ -437,10 +425,10 @@ int launch_qdemod_fir(qrl_rx* h, cudaStream_t st, const float2* in, unsigned in_
     const size_t smem = sizeof(float) * (ntaps + span + (span >> 5) + 2);
     if (n >= 256 && smem <= 48 * 1024 && ntaps >= K) {
         dim3 g(static_cast<unsigned>((n + TILE - 1) / TILE), h->C);
-        qdemod_fir_fff_tiled_kernel<K, NT><<<g, NT, smem, st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, gain, a0, a1);
+        qdemod_fir_fff_tiled_kernel<K, NT><<<g, NT, smem, st>>>(in, out, taps, ntaps, gain, a0, a1);
     } else {
         dim3 g(static_cast<unsigned>((n + 255) / 256), h->C);
-        qdemod_fir_fff_kernel<<<g, 256, sizeof(float) * (2 * ntaps + 256), st>>>(in, in_mask, in_stride, out, out_mask, out_stride, taps, ntaps, gain, a0, a1, nullptr, 0);
+        qdemod_fir_fff_kernel<<<g, 256, sizeof(float) * (2 * ntaps + 256), st>>>(in, out, taps, ntaps, gain, a0, a1);
     }
     h->launches++;
     QRL_CK(cudaGetLastError());
@@ -491,17 +479,14 @@ int hand_off(qrl_rx* h, cudaEvent_t ev, cudaStream_t from, cudaStream_t to)
 // fll_band_edge_cc (sequential, per sample) on the loop stream: r1 -> rf
 void launch_fll(qrl_rx* h, const Slice& s)
 {
-    fll_kernel<32><<<s.groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps,
-        static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, s.k1,
-        static_cast<float2*>(h->rf.d), h->rf.mask, h->rf.stride);
+    fll_kernel<32><<<s.groups, 32, 0, h->s_loop>>>(h->fllp, h->d_fll, h->d_fll_hist, h->C, h->d_fll_taps, h->r1, s.k1, h->rf);
     h->launches++;
 }
 
 // the channel / shaping filter of a slice on `st`: `in` -> r2 (channel-interleaved when `interleaved`) and port 0
-int launch_channel_filter(qrl_rx* h, const Slice& s, cudaStream_t st, const Ring& in, int interleaved)
+int launch_channel_filter(qrl_rx* h, const Slice& s, cudaStream_t st, Ring<const float2> in, int interleaved)
 {
-    return launch_fir_ccf(h, st, static_cast<const float2*>(in.d), in.mask, in.stride, static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                          h->d_taps2, h->ntaps2, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0, interleaved);
+    return launch_fir_ccf(h, h->C, st, in, h->r2, h->d_taps2, h->ntaps2, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0, interleaved);
 }
 
 // gr_demod_m17, gr_demod_dmr: the symbol sync's epilogue writes two hard bits per symbol to port 2, no decoder behind them
@@ -532,24 +517,24 @@ int launch_fsk_frontend(qrl_rx* h, const Slice& s)
     if (int rc = smem_opt_in(h, kern, 120 * 1024)) return rc;
     const unsigned g = static_cast<unsigned>((s.n_new + strip - 1) / strip * h->C);     // strip-major, channel fastest
     kern<<<g, FF_NT, smem, s.sp>>>(s.x, s.xstride, s.T, s.hist, h->H, h->d_taps1, s.n_in0, h->rot_fused ? h->rot.d : nullptr,
-        static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, h->d_taps2, h->ntaps2, h->d_port0, h->port0_cap, s.k_call0,
-        h->d_taps3, h->ntaps3, h->qd_gain, static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, s.k0, s.k1, strip, h->C);
+        h->r1, h->d_taps2, h->ntaps2, h->d_port0, h->port0_cap, s.k_call0,
+        h->d_taps3, h->ntaps3, h->qd_gain, h->r4, s.k0, s.k1, strip, h->C);
     h->launches++;
     QRL_CK(cudaGetLastError());
     return QRL_OK;
 }
 
 // one symbol-sync launch on `st` over the input ring `in` up to k1 (opting the instance in to `smem_max` bytes first); only the
-// 4FSK-FM symbol sync with the external epilogue passes the epilogue's scratch, chunk bound, chunk capacity and header
-template <class K>
-int launch_symsync(qrl_rx* h, K* kern, int smem_max, int grid, int threads, size_t smem, cudaStream_t st, const Ring& in, long long k1,
+// 4FSK-FM symbol sync with the external epilogue passes the epilogue's scratch, chunk bound, chunk capacity and header.  The kernel
+// reads its input, real (r4) or complex (r3), as rows of floats.
+template <class K, class T>
+int launch_symsync(qrl_rx* h, K* kern, int smem_max, int grid, int threads, size_t smem, cudaStream_t st, Ring<T> in, long long k1,
                    int maxs, long long* nsoft_i, float* scratch = nullptr, int chunk_bound = 0, int chunk_cap = 0, int* hdr = nullptr)
 {
     if (int rc = smem_opt_in(h, kern, smem_max)) return rc;
     kern<<<grid, threads, smem, st>>>(
-        h->ssp, h->d_ss, h->C, static_cast<const float*>(in.d), in.mask, in.stride, k1,
-        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, maxs, nsoft_i, scratch, chunk_bound, chunk_cap, hdr);
+        h->ssp, h->d_ss, h->C, Ring<const float>{ reinterpret_cast<const float*>(in.d), in.mask, in.stride }, k1,
+        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap), h->r5, maxs, nsoft_i, scratch, chunk_bound, chunk_cap, hdr);
     h->launches++;
     return QRL_OK;
 }
@@ -560,12 +545,10 @@ void launch_viterbi(qrl_rx* h, long long* nsoft_i, bool dual)
 {
     constexpr int CPB = 4;    // 4 channels (8 warps) per CTA
     cudaEvent_t pe = h->prof.begin(4, h->s_fec);
-    viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C,
-        static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+    viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs, nsoft_i, h->C, h->r5.d, h->r5.mask, h->r5.stride,
         h->d_port2, h->port2_cap, h->d_port2_cnt, static_cast<int>(h->port2_cap), 0);
     if (dual)
-        viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs2, nsoft_i, h->C,
-            static_cast<const unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+        viterbi_k7_kernel<CPB><<<(h->C + CPB - 1) / CPB, 64 * CPB, 0, h->s_fec>>>(h->d_vs2, nsoft_i, h->C, h->r5.d, h->r5.mask, h->r5.stride,
             h->d_port3, h->port2_cap, h->d_port3_cnt, static_cast<int>(h->port2_cap), 1);
     h->launches += dual ? 2 : 1;
     h->prof.end(pe);
@@ -576,13 +559,8 @@ int slice_dsss(qrl_rx* h, const Slice& s)
 {
     if (int rc = hand_off(h, h->ev_a[s.i], s.sp, h->s_loop)) return rc;
     cudaEvent_t pe = h->prof.begin(3, h->s_loop);
-    dsss_chain_kernel<<<h->C, 256, 0, h->s_loop>>>(h->dsp, h->d_ds, static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride, s.k1,
-        h->d_ds_arms, h->d_taps2, h->d_ds_taps,
-        static_cast<float2*>(h->ds_a.d), static_cast<float2*>(h->ds_c.d), h->ds_a.mask, h->ds_a.stride,
-        static_cast<float2*>(h->ds_d.d), h->ds_d.mask, h->ds_d.stride,
-        h->d_port0, h->port0_cap, h->ds_o_call0,
-        h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap),
-        static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride, s.nsoft_i);
+    dsss_chain_kernel<<<h->C, 256, 0, h->s_loop>>>(h->dsp, h->d_ds, h->r1, s.k1, h->d_ds_arms, h->d_taps2, h->d_ds_taps, h->ds_a, h->ds_c, h->ds_d,
+        h->d_port0, h->port0_cap, h->ds_o_call0, h->d_port1, h->port1_cap, h->d_port1_cnt, static_cast<int>(h->port1_cap), h->r5, s.nsoft_i);
     h->launches++;
     h->prof.end(pe);
     if (int rc = hand_off(h, h->ev_b[s.i], h->s_loop, h->s_fec)) return rc;
@@ -601,8 +579,7 @@ int slice_analog(qrl_rx* h, const Slice& s)
             if (int rc = launch_channel_filter(h, s, s.sp, h->r1, 0)) return rc;
         } else {
             fir_ccc_ring_kernel<<<s.gtile, kTileThreads, sizeof(float) * 2 * h->ntaps2, s.sp>>>(
-                static_cast<const float2*>(h->r1.d), h->r1.mask, h->r1.stride,
-                static_cast<float2*>(h->r2.d), h->r2.mask, h->r2.stride,
+                h->r1, h->r2,
                 h->d_taps2, h->ntaps2, 1.0f, s.k0, s.k1, h->d_port0, h->port0_cap, s.k_call0);
             h->launches++;
         }
@@ -613,16 +590,11 @@ int slice_analog(qrl_rx* h, const Slice& s)
     const size_t fat = h->nbfm_split ? 120 * 1024 : 0;       // one CTA per SM, and never next to a de-emphasis CTA
     switch (h->chain) {
     case RxChain::Ssb:
-        ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb,
-            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
-            static_cast<float2*>(h->rclip.d), h->rclip.mask, h->rclip.stride,
-            static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride,
+        ssb_audio_kernel<<<h->C, 128, 0, h->s_loop>>>(h->ssbp, h->d_ssb, h->r2, s.k1, h->rclip, h->rstr,
             h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
         break;
     case RxChain::Freedv:
-        freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv,
-            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
-            static_cast<float*>(h->rstr.d), h->rstr.mask, h->rstr.stride, h->d_audio_taps,
+        freedv_rx_tail_kernel<<<h->C, 128, sizeof(float) * h->fdp.nt_audio, h->s_loop>>>(h->fdp, h->d_fdv, h->r2, s.k1, h->rstr, h->d_audio_taps,
             reinterpret_cast<short*>(h->d_port1), 4 * h->port1_cap, h->d_port1_cnt, static_cast<int>(4 * h->port1_cap));
         break;
     default:    // AM, NBFM, WBFM (the de-emphasis ring and the CTCSS squelch ring only exist for NBFM; empty otherwise)
@@ -630,22 +602,16 @@ int slice_analog(qrl_rx* h, const Slice& s)
             int rc;
             if ((rc = smem_opt_in(h, nbfm_audio_kernel, 120 * 1024)) || (rc = smem_opt_in(h, nbfm_deemph_kernel, 120 * 1024))) return rc;
         }
-        nbfm_audio_kernel<<<h->C, 128, fat, h->s_loop>>>(h->nbp, h->d_nb,
-            static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1, h->d_env,
-            static_cast<float2*>(h->rg.d), h->rg.mask, h->rg.stride,
-            static_cast<float*>(h->rd.d), h->rd.mask, h->rd.stride,
-            static_cast<float*>(h->rr.d), h->rr.mask, h->rr.stride,
+        nbfm_audio_kernel<<<h->C, 128, fat, h->s_loop>>>(h->nbp, h->d_nb, h->r2, s.k1, h->d_env, h->rg, h->rd, h->rr,
             h->d_arm_taps, h->d_audio_taps, h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap),
-            h->nbfm_split ? static_cast<float*>(h->raud.d) : nullptr, h->raud.mask, h->raud.stride, h->nbfm_split ? s.nsoft_i : nullptr,
-            static_cast<float*>(h->rq.d), h->rq.mask, h->rq.stride, h->ctc, h->d_cenv);
+            h->raud, h->nbfm_split ? s.nsoft_i : nullptr, h->rq, h->ctc, h->d_cenv);
     }
     h->launches++;
     h->prof.end(pe);
     if (h->nbfm_split) {
         if (int rc = hand_off(h, h->ev_b[s.i], h->s_loop, h->s_loop2)) return rc;
         pe = h->prof.begin(5, h->s_loop2);
-        nbfm_deemph_kernel<<<h->C, 128, fat, h->s_loop2>>>(h->nbp.b0, h->nbp.b1, h->nbp.a1, h->nbp.out_gain, h->d_nb2,
-            static_cast<const float*>(h->raud.d), h->raud.mask, h->raud.stride, s.nsoft_i,
+        nbfm_deemph_kernel<<<h->C, 128, fat, h->s_loop2>>>(h->nbp.b0, h->nbp.b1, h->nbp.a1, h->nbp.out_gain, h->d_nb2, h->raud, s.nsoft_i,
             h->d_port1f, 2 * h->port1_cap, h->d_port1_cnt, static_cast<int>(2 * h->port1_cap));
         h->launches++;
         h->prof.end(pe);
@@ -667,16 +633,12 @@ int slice_fll_bpsk_2fsk(qrl_rx* h, const Slice& s)
         pe = h->prof.begin(2, h->s_loop);
         if (int rc = launch_channel_filter(h, s, h->s_loop, h->fll ? h->rf : h->r1, bpsk ? 1 : 0)) return rc;     // GMSK: no FLL
         if (h->chain == RxChain::Fsk2Fm || h->chain == RxChain::Gmsk) {
-            if (int rc = launch_qdemod_fir(h, h->s_loop, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                           static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
-                                           h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
+            if (int rc = launch_qdemod_fir(h, h->s_loop, h->r2, h->r4, h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
         } else if (h->chain == RxChain::Fsk2Bank) {
             fsk_bank_kernel<2><<<s.gtile, kTileThreads, sizeof(float) * 4 * h->nt_bank, h->s_loop>>>(
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, s.k0, s.k1,
-                static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
+                h->r2, h->d_bank_taps, h->nt_bank, s.k0, s.k1, h->rbank);
             fir_fff_ring_kernel<<<s.gtile, kTileThreads, sizeof(float) * h->nt_symf, h->s_loop>>>(
-                static_cast<const float*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
-                static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride, h->d_symf_taps, h->nt_symf, s.k0, s.k1);
+                h->rbank, h->r4, h->d_symf_taps, h->nt_symf, s.k0, s.k1);
             h->launches += 2;
         }
         h->prof.end(pe);
@@ -688,9 +650,7 @@ int slice_fll_bpsk_2fsk(qrl_rx* h, const Slice& s)
             const size_t smem = sizeof(float2) * (NST * CH + AC_NHB * (CH + 1)) * 32;      // every hand-off block + its padding row
             auto kern = agc_costas_kernel<CH, NST, 0, 0>;
             if (int rc = smem_opt_in(h, kern, 200 * 1024)) return rc;
-            kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
-                static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
+            kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C, h->r2.d, h->r2.mask, h->r2.stride, s.k1, h->r3.d, h->r3.mask, h->r3.stride);
             h->launches++;
         }
         // clock_recovery_mm_cc: its window bound is (CH + 1) / min_period symbols
@@ -743,9 +703,8 @@ int symsync_4fsk_ext(qrl_rx* h, const Slice& s)
     auto epi = dmr ? symsync_ext_epilogue_kernel<1> : symsync_ext_epilogue_kernel<0>;
     if (chunk_bound > 0)        // (counted in h->launches with the symbol sync it finishes)
         epi<<<dim3(chunk_bound, s.groups), dim3(32, 8), 0, se>>>(
-            h->ssp, h->C, scratch_i, static_cast<int>(h->ss_chunk_cap), maxs, hdr_i,
-            h->d_port1, h->port1_cap, static_cast<int>(h->port1_cap),
-            static_cast<unsigned char*>(h->r5.d), h->r5.mask, h->r5.stride,
+            h->ssp, h->C, scratch_i, static_cast<int>(h->ss_chunk_cap), maxs, hdr_i, h->d_port1, h->port1_cap, static_cast<int>(h->port1_cap),
+            h->r5.d, h->r5.mask, h->r5.stride,
             hard_bits(h) ? h->d_port2 : nullptr, h->port2_cap, static_cast<int>(h->port2_cap), h->d_port2_cnt, h->d_port1_cnt);
     h->prof.end(pe);
     QRL_CK(cudaEventRecord(h->ev_b[s.i], se));
@@ -785,23 +744,19 @@ int slice_4fsk(qrl_rx* h, const Slice& s)
         if (int rc = wait_r4_free()) return rc;
         pe = h->prof.begin(2, s.sp);
         if (fm) {
-            if (int rc = launch_qdemod_fir(h, s.sp, static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride,
-                                           static_cast<float*>(h->r4.d), h->r4.mask, h->r4.stride,
-                                           h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
+            if (int rc = launch_qdemod_fir(h, s.sp, h->r2, h->r4, h->d_taps3, h->ntaps3, h->qd_gain, s.k0, s.k1)) return rc;
             if (h->chain == RxChain::Dmr) {      // gr_demod_dmr.cpp:103: the symbol filter output is port 3
                 ring_to_port_f32_kernel<<<dim3(static_cast<unsigned>((s.k1 - s.k0 + 31) / 32), s.groups), dim3(32, 8), 0, s.sp>>>(
-                    static_cast<const float*>(h->r4.d), h->r4.mask, h->r4.stride, h->C, s.k0, s.k1,
-                    h->d_port3f, h->port0_cap, s.k0 - s.k_call0);
+                    h->r4, h->C, s.k0, s.k1, h->d_port3f, h->port0_cap, s.k0 - s.k_call0);
                 h->launches++;
             }
         } else {
             fsk_bank_kernel<4><<<s.gtile, kTileThreads, sizeof(float) * 8 * h->nt_bank, s.sp>>>(
-                static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, h->d_bank_taps, h->nt_bank, s.k0, s.k1,
-                static_cast<float*>(h->rbank.d), h->rbank.mask, h->rbank.stride);
+                h->r2, h->d_bank_taps, h->nt_bank, s.k0, s.k1, h->rbank);
             h->launches++;
-            if (int rc = launch_fir_ccf(h, s.sp, static_cast<const float2*>(h->rbank.d), h->rbank.mask, h->rbank.stride,
-                                        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride,
-                                        h->d_symf_taps, h->nt_symf, s.k0, s.k1, nullptr, 0, 0, 1)) return rc;
+            // the bank wrote complex items into rbank
+            const Ring<const float2> bank{ reinterpret_cast<const float2*>(h->rbank.d), h->rbank.mask, h->rbank.stride };
+            if (int rc = launch_fir_ccf(h, h->C, s.sp, bank, h->r3, h->d_symf_taps, h->nt_symf, s.k0, s.k1, nullptr, 0, 0, 1)) return rc;
         }
         h->prof.end(pe);
     }
@@ -837,9 +792,7 @@ int qpsk_agc_costas(qrl_rx* h, const Slice& s)
     auto kern = (h->acp.order == 4 && h->acp.use_snr) ? agc_costas_kernel<CH, NST, 4, 1> : agc_costas_kernel<CH, NST>;
     int rc;                                 // both instantiations, whichever this call takes
     if ((rc = smem_opt_in(h, agc_costas_kernel<CH, NST, 4, 1>, 200 * 1024)) || (rc = smem_opt_in(h, agc_costas_kernel<CH, NST>, 200 * 1024))) return rc;
-    kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C,
-        static_cast<const float2*>(h->r2.d), h->r2.mask, h->r2.stride, s.k1,
-        static_cast<float2*>(h->r3.d), h->r3.mask, h->r3.stride);
+    kern<<<s.groups, 96, smem, h->s_loop>>>(h->acp, h->d_ac, h->C, h->r2.d, h->r2.mask, h->r2.stride, s.k1, h->r3.d, h->r3.mask, h->r3.stride);
     h->launches++;
     return QRL_OK;
 }
@@ -933,7 +886,7 @@ int rx_stage1(qrl_rx* h, const std::vector<float>& taps1, const std::vector<floa
     h->taps2_cap = t2.size();
     if ((rc = upload_floats(h, &h->d_taps2, t2))) return rc;
     if (!taps3.empty() && (rc = upload_floats(h, &h->d_taps3, taps3))) return rc;
-    return make_ring(h, &h->r1, sizeof(float2), h->n1max + std::max(512, static_cast<int>(taps2.size())) + 8);
+    return make_ring(h, &h->r1, h->C, h->n1max + std::max(512, static_cast<int>(taps2.size())) + 8, false, &h->zero_list);
 }
 
 // fll_band_edge_cc between stage 1 and the channel / shaping filter: its taps, state and history, and its output ring rf
@@ -946,7 +899,7 @@ int rx_fll(qrl_rx* h, int sym_sps, float rolloff)
     if (rc) return rc;
     h->zero_list.emplace_back(h->d_fll_hist, sizeof(float2) * 32 * h->C);
     h->zero_list.emplace_back(h->d_fll, sizeof(FllState) * h->C);
-    return make_ring(h, &h->rf, sizeof(float2), h->n1max + 512 + 8);
+    return make_ring(h, &h->rf, h->C, h->n1max + 512 + 8, false, &h->zero_list);
 }
 
 // the symbol sync's period bounds sps +- dev, its window lookahead and its first whole step (alpha set by clock_loop_gains)
@@ -971,8 +924,8 @@ int check_window_128(qrl_rx* h)
 // QPSK / BPSK: shaping-filter output and loop output are channel-interleaved complex rings; the agc2 + Costas state
 int psk_rings(qrl_rx* h)
 {
-    int rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 600, true);
-    if (!rc) rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true);
+    int rc = make_ring(h, &h->r2, h->C, h->n1max + 600, true, &h->zero_list);
+    if (!rc) rc = make_ring(h, &h->r3, h->C, h->n1max + 600, true, &h->zero_list);
     if (!rc) rc = dev_alloc(h, &h->d_ac, h->C);
     return rc;
 }
@@ -1035,12 +988,12 @@ int create_4fsk(qrl_rx* h, int sps, int samp_rate, int filter_width, int& sym_sp
         if ((rc = upload_floats(h, &h->d_symf_taps, sf))) return rc;
     }
     if ((rc = rx_stage1(h, taps1, taps2, false, taps3))) return rc;
-    if ((rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + h->ntaps3 + 64))) return rc;
+    if ((rc = make_ring(h, &h->r2, h->C, h->n1max + h->ntaps3 + 64, false, &h->zero_list))) return rc;
     // two calls deep when the block may run with overlapped calls (the producer of call k+1 must not wait for the consumer of call k)
-    if ((rc = make_ring(h, &h->r4, sizeof(float), (fm ? 2 : 1) * h->n1max + 600, true))) return rc;
+    if ((rc = make_ring(h, &h->r4, h->C, (fm ? 2 : 1) * h->n1max + 600, true, &h->zero_list))) return rc;
     if (!fm) {
-        if ((rc = make_ring(h, &h->rbank, sizeof(float2), h->n1max + h->nt_symf + 16))) return rc;
-        if ((rc = make_ring(h, &h->r3, sizeof(float2), h->n1max + 600, true))) return rc;
+        if ((rc = make_ring(h, &h->rbank, h->C, h->n1max + h->nt_symf + 16, false, &h->zero_list, 2))) return rc;
+        if ((rc = make_ring(h, &h->r3, h->C, h->n1max + 600, true, &h->zero_list))) return rc;
         return check_window_128(h);
     }
     // scratch of the external symbol-sync epilogue: [groups][chunks][maxs + 2][32] floats + a 128-int header per group
@@ -1097,9 +1050,9 @@ int create_2fsk(qrl_rx* h, int sps, int samp_rate, int filter_width, int& sym_sp
         h->fllp.max_freq = static_cast<float>(2.0 * kPi * (2.0 / sym_sps)); h->fllp.min_freq = -h->fllp.max_freq;
         rc = rx_fll(h, sym_sps, 0.1f);
     }
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + h->ntaps3 + 64);
-    if (!rc) rc = make_ring(h, &h->r4, sizeof(float), h->n1max + 600, true);
-    if (!rc && band) rc = make_ring(h, &h->rbank, sizeof(float), h->n1max + h->nt_symf + 16);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + h->ntaps3 + 64, false, &h->zero_list);
+    if (!rc) rc = make_ring(h, &h->r4, h->C, h->n1max + 600, true, &h->zero_list);
+    if (!rc && band) rc = make_ring(h, &h->rbank, h->C, h->n1max + h->nt_symf + 16, false, &h->zero_list);
     return rc;
 }
 
@@ -1209,9 +1162,9 @@ int create_dsss(qrl_rx* h, int sps, int samp_rate, int filter_width)
     rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS), taps2, false, {});
     if (rc) return rc;
     const long long n5 = h->n1max * 13 / 50 + 8;
-    if ((rc = make_ring(h, &h->ds_a, sizeof(float2), n5 + 2048))) return rc;
-    if ((rc = make_ring(h, &h->ds_c, sizeof(float2), n5 + 2048))) return rc;
-    if ((rc = make_ring(h, &h->ds_d, sizeof(float2), n5 / h->dsp.N + 128))) return rc;
+    if ((rc = make_ring(h, &h->ds_a, h->C, n5 + 2048, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->ds_c, h->C, n5 + 2048, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->ds_d, h->C, n5 / h->dsp.N + 128, false, &h->zero_list))) return rc;
     return dev_alloc(h, &h->d_ds, h->C);
 }
 
@@ -1225,7 +1178,7 @@ int create_nbfm(qrl_rx* h, int samp_rate, int filter_width)
     h->nports = 2; h->port1_isz = 4;
     int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
                        low_pass_2(1, tsr, filter_width, 3500, 60, WIN_BLACKMAN_HARRIS), false, {});
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + 64, false, &h->zero_list);
     if (rc) return rc;
     std::vector<float> audio_rs = low_pass_2(2, 2 * tsr, 3600, 250, 60, WIN_BLACKMAN_HARRIS);
     std::vector<float> audio_f = low_pass_2(1, 8000, 3500, 200, 35, WIN_BLACKMAN_HARRIS);
@@ -1242,12 +1195,12 @@ int create_nbfm(qrl_rx* h, int samp_rate, int filter_width)
     h->nbp.sq_alpha = 0.01; h->nbp.sq_threshold = std::pow(10.0, -140 / 10.0); h->nbp.sq_ramp = ramp; h->nbp.sq_gate = 1;
     h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
     h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 2.0f;
-    if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return rc;
-    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return rc;
-    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return rc;
+    if ((rc = make_ring(h, &h->rg, h->C, h->n1max + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rd, h->C, h->n1max + nt_arm + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rr, h->C, h->n1max * 2 / 5 + h->nbp.nt_audio + 16, false, &h->zero_list))) return rc;
     if ((rc = dev_alloc(h, &h->d_nb, h->C))) return rc;
     // analog::ctcss_squelch_ff::make(8000, 88.5, 0.01, 8000, 160, true) (gr_demod_nbfm.cpp:60), out of the graph until set_ctcss(f)
-    if ((rc = make_ring(h, &h->rq, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 64))) return rc;
+    if ((rc = make_ring(h, &h->rq, h->C, h->n1max * 2 / 5 + h->nbp.nt_audio + 64, false, &h->zero_list))) return rc;
     h->ctc.on = 0; h->ctc.len = 8000; h->ctc.ramp = 160; h->ctc.gate = 1; h->ctc.level = 0.01f;
     std::vector<double> ce(h->ctc.ramp + 1);
     for (int k = 0; k <= h->ctc.ramp; k++) ce[k] = 0.5 - std::cos(kPi * k / h->ctc.ramp) / 2.0;       // squelch_base_ff envelope (double)
@@ -1259,7 +1212,7 @@ int create_nbfm(qrl_rx* h, int samp_rate, int filter_width)
     int n_sm = 0;
     if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess) { set_err(h, "SM count query failed"); return QRL_ECUDA; }
     if (h->C <= n_sm && !getenv("QRL_NBFM_NO_SPLIT")) {
-        if ((rc = make_ring(h, &h->raud, sizeof(float), h->n1max * 2 / 5 + 64))) return rc;
+        if ((rc = make_ring(h, &h->raud, h->C, h->n1max * 2 / 5 + 64, false, &h->zero_list))) return rc;
         if ((rc = dev_alloc(h, &h->d_nb2, h->C))) return rc;
         h->zero_list.emplace_back(h->d_nb2, sizeof(NbfmDeemphState) * h->C);
         h->nbfm_split = true;
@@ -1276,7 +1229,7 @@ int create_am(qrl_rx* h, int samp_rate, int filter_width)
     h->nports = 2; h->port1_isz = 4;
     int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
                        complex_band_pass_2(1, tsr, -filter_width, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + 64, false, &h->zero_list);
     if (rc) return rc;
     std::vector<float> audio_rs = low_pass(2, 2 * tsr, 3600, 600, WIN_BLACKMAN_HARRIS);
     std::vector<float> audio_f = low_pass(1, 8000, 3600, 300, WIN_BLACKMAN_HARRIS);
@@ -1289,9 +1242,9 @@ int create_am(qrl_rx* h, int samp_rate, int filter_width)
     h->nbp.qd_gain = 0.0f; h->nbp.nt_arm = nt_arm; h->nbp.nt_audio = static_cast<int>(audio_f.size());
     h->nbp.b0 = 1.0; h->nbp.b1 = -1.0; h->nbp.a1 = -0.9999; h->nbp.out_gain = 1.0f;      // iir_filter_ffd({1,-1},{0,0.9999}), old style
     h->nbp.mode = 1; h->nbp.agc_attack = 1e-1f; h->nbp.agc_decay = 1e-1f; h->nbp.agc_ref = 1.0f; h->nbp.agc_max = 65536.0f; h->nbp.am_gain = 0.99f;
-    if ((rc = make_ring(h, &h->rg, sizeof(float2), 64))) return rc;
-    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + nt_arm + 16))) return rc;
-    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max * 2 / 5 + h->nbp.nt_audio + 16))) return rc;
+    if ((rc = make_ring(h, &h->rg, h->C, 64, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rd, h->C, h->n1max + nt_arm + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rr, h->C, h->n1max * 2 / 5 + h->nbp.nt_audio + 16, false, &h->zero_list))) return rc;
     return dev_alloc(h, &h->d_nb, h->C);
 }
 
@@ -1305,7 +1258,7 @@ int create_wbfm(qrl_rx* h, int samp_rate, int filter_width)
     h->nports = 2; h->port1_isz = 4;
     int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
                        low_pass_2(1, tsr, filter_width, 600, 90, WIN_BLACKMAN_HARRIS), false, {});
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + 64, false, &h->zero_list);
     if (rc) return rc;
     std::vector<float> audio_rs = low_pass(1, tsr, 4000, 2000, WIN_BLACKMAN_HARRIS);
     if ((rc = upload_floats(h, &h->d_audio_taps, audio_rs))) return rc;
@@ -1317,9 +1270,9 @@ int create_wbfm(qrl_rx* h, int samp_rate, int filter_width)
     h->nbp.qd_gain = h->qd_gain; h->nbp.nt_arm = 1; h->nbp.nt_audio = static_cast<int>(audio_rs.size());
     h->nbp.b0 = b[0]; h->nbp.b1 = b[1]; h->nbp.a1 = a[1]; h->nbp.out_gain = 1.0f;
     h->nbp.mode = 2; h->nbp.am_gain = 0.9f;
-    if ((rc = make_ring(h, &h->rg, sizeof(float2), h->n1max + 16))) return rc;
-    if ((rc = make_ring(h, &h->rd, sizeof(float), h->n1max + 16))) return rc;
-    if ((rc = make_ring(h, &h->rr, sizeof(float), h->n1max + h->nbp.nt_audio + 16))) return rc;
+    if ((rc = make_ring(h, &h->rg, h->C, h->n1max + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rd, h->C, h->n1max + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rr, h->C, h->n1max + h->nbp.nt_audio + 16, false, &h->zero_list))) return rc;
     return dev_alloc(h, &h->d_nb, h->C);
 }
 
@@ -1333,7 +1286,7 @@ int create_ssb(qrl_rx* h, int sps, int samp_rate, int filter_width)
     int rc = rx_stage1(h, low_pass(1, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
                        h->lsb ? complex_band_pass_2(1, tsr, -filter_width, -200, 200, 90, WIN_BLACKMAN_HARRIS)
                               : complex_band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + 64, false, &h->zero_list);
     if (rc) return rc;
     std::vector<float> audio_f = band_pass_2(1, tsr, 200, filter_width, 200, 90, WIN_BLACKMAN_HARRIS);
     if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return rc;
@@ -1341,8 +1294,8 @@ int create_ssb(qrl_rx* h, int sps, int samp_rate, int filter_width)
     h->ssbp.attack = 1e-1f; h->ssbp.decay = 1e-1f; h->ssbp.ref = 0.25f; h->ssbp.max_gain = 65536.0f;
     h->ssbp.clip = 0.95f; h->ssbp.emax = static_cast<float>(1 / (std::sqrt(0.5) / 2)); h->ssbp.out_gain = 1.333f;
     h->ssbp.nt_audio = static_cast<int>(audio_f.size());
-    if ((rc = make_ring(h, &h->rclip, sizeof(float2), h->n1max + 16))) return rc;
-    if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->ssbp.nt_audio + 16))) return rc;
+    if ((rc = make_ring(h, &h->rclip, h->C, h->n1max + 16, false, &h->zero_list))) return rc;
+    if ((rc = make_ring(h, &h->rstr, h->C, h->n1max + h->ssbp.nt_audio + 16, false, &h->zero_list))) return rc;
     return dev_alloc(h, &h->d_ssb, h->C);
 }
 
@@ -1358,13 +1311,13 @@ int create_freedv(qrl_rx* h, int sps, int samp_rate, int filter_width, int low_c
     int rc = rx_stage1(h, low_pass(sps, samp_rate, tsr / 2, tsr / 2, WIN_BLACKMAN_HARRIS),
                        h->lsb ? complex_band_pass_2(1, tsr, -filter_width, -low_cutoff, 200, 90, WIN_BLACKMAN_HARRIS)
                               : complex_band_pass_2(1, tsr, low_cutoff, filter_width, 200, 90, WIN_BLACKMAN_HARRIS), true, {});
-    if (!rc) rc = make_ring(h, &h->r2, sizeof(float2), h->n1max + 64);
+    if (!rc) rc = make_ring(h, &h->r2, h->C, h->n1max + 64, false, &h->zero_list);
     if (rc) return rc;
     std::vector<float> audio_f = band_pass_2(1, tsr, 200, 3500, 200, 90, WIN_BLACKMAN_HARRIS);
     if ((rc = upload_floats(h, &h->d_audio_taps, audio_f))) return rc;
     h->fdp.attack = 1e-1f; h->fdp.decay = 1e-3f; h->fdp.ref = 0.5f; h->fdp.max_gain = 65536.0f;
     h->fdp.nt_audio = static_cast<int>(audio_f.size());
-    if ((rc = make_ring(h, &h->rstr, sizeof(float), h->n1max + h->fdp.nt_audio + 16))) return rc;
+    if ((rc = make_ring(h, &h->rstr, h->C, h->n1max + h->fdp.nt_audio + 16, false, &h->zero_list))) return rc;
     return dev_alloc(h, &h->d_fdv, h->C);
 }
 
@@ -1452,7 +1405,7 @@ static int rx_create(int kind, int sps, int samp_rate, int filter_width, int fla
     h->d_port1f = reinterpret_cast<float*>(h->d_port1);
     if ((rc = dev_alloc(h, &h->d_port1_cnt, h->C))) return fail(rc);
     if (h->nports > 2) {        // the symbol chains: soft bits (u8) -> decoder -> port 2
-        if ((rc = make_ring(h, &h->r5, 1, 2 * h->n1max + 1024))) return fail(rc);
+        if ((rc = make_ring(h, &h->r5, h->C, 2 * h->n1max + 1024, false, &h->zero_list))) return fail(rc);
         h->port2_cap = (hard_bits(h) ? 2 : 1) * h->port1_cap + 160;      // M17: two hard bits per symbol, no rate-1/2 decoder behind them
         if ((rc = dev_alloc(h, &h->d_port2, static_cast<size_t>(h->port2_cap) * h->C))) return fail(rc);
         if ((rc = dev_alloc(h, &h->d_port2_cnt, h->C))) return fail(rc);
@@ -1932,7 +1885,7 @@ static int rx_work_impl(qrl_rx* h, const void* iq_any, long T, long stride, int 
                 // gr_demod_ssb's multiply_const_cc(_if_gain) sits between the resampler and the side-band filter: the gain is applied
                 // to the samples as they pass (8 ksps), so after set_gain the filter's history keeps the old gain, like the reference's
                 dim3 gs(static_cast<unsigned>((kg1 - kg0 + 255) / 256), h->C);
-                scale2_ring_kernel<<<gs, 256, 0, sp>>>(static_cast<float2*>(h->r1.d), h->r1.mask, h->r1.stride, kg0, kg1, h->if_gain, 1.0f);
+                scale2_ring_kernel<<<gs, 256, 0, sp>>>(h->r1, kg0, kg1, h->if_gain, 1.0f);
                 h->launches++;
             }
             h->prof.end(pe);
@@ -2178,15 +2131,13 @@ struct qrl_tx : HandleBase {
     ZeroIdle zi;                                                      // gr_mod_dmr: gr_zero_idle_bursts(62)
     TxBitState* d_bits = nullptr;
     unsigned char* d_in = nullptr; size_t in_isz = 1;   // [C][max_items] staging of host input: bytes, float audio (NBFM / SSB / AM) or int16 (FreeDV)
-    float* d_sym = nullptr; unsigned sym_mask = 0; long long sym_stride = 0;    // float (4FSK) / float2 (QPSK)
-    float2* d_if = nullptr; unsigned if_mask = 0; long long if_stride = 0;
+    Ring<float> sym;                // float (4FSK) / float2 (QPSK) symbols
+    Ring<float2> if_;
     float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_sym = 0;           // symbols produced so far (absolute)
     TxAnalogState* d_an = nullptr;                                                 // analog modulators (NBFM / SSB / AM)
-    float* d_ra = nullptr; unsigned ra_mask = 0; long long ra_stride = 0;          // audio ring
-    float* d_rb = nullptr;                                                         // filtered audio ring (same geometry)
-    float2* d_rc = nullptr; unsigned rc_mask = 0; long long rc_stride = 0;         // SSB clip ring / NBFM IF-filter ring
-    float2* d_rs2 = nullptr;                                                       // SSB stretcher ring (same geometry as rc)
+    Ring<float> ra, rb;             // audio ring, filtered audio ring
+    Ring<float2> rc, rs2;           // SSB clip ring / NBFM IF-filter ring, SSB stretcher ring
     float* d_lpf = nullptr; int nt_lpf = 0; float* d_cfilt = nullptr; int nt_cfilt = 0;
     double pe_b0 = 0, pe_b1 = 0, pe_a1 = 0;
     long long n_audio = 0, n_mid = 0;        // audio samples consumed / mid-rate items produced (host mirror of the device counters)
@@ -2210,14 +2161,8 @@ struct TxDesign {
     std::vector<float> t1, t2, lpf, cfilt;     // prototypes of d_arms1 (L1 arms of nt1) and d_arms2 (L2 arms of nt2); d_lpf, d_cfilt as given
     long long sym = 0, if_ = 0, rc = 0, ra = 0, out = 0;      // items each ring must hold (0: the chain has no such ring); out_stride
     int sym_floats = 1;                                       // 2: complex symbols
-    bool rb = false, rs2 = false;                             // d_rb in d_ra's geometry, d_rs2 in d_rc's
+    bool rb = false, rs2 = false;                             // rb of ra's size, rs2 of rc's
 };
-// a [C][capacity] ring of at least min_items items, each `per_item` Ts
-extern "C++" template <class T> int tx_ring(qrl_tx* h, T** d, unsigned* mask, long long* stride, long long min_items, int per_item = 1)
-{
-    const unsigned cap = pow2_at_least(min_items); *mask = cap - 1; *stride = cap;
-    return dev_alloc(h, d, static_cast<size_t>(cap) * h->C * per_item);
-}
 void create_fsk(qrl_tx* h, TxDesign& d, int kind, int sps, int samp_rate, int fw)
 {
     if (kind == QRL_MOD_4FSK) {
@@ -2450,15 +2395,15 @@ int tx_create(int kind, int sps, int samp_rate, int fw, int flag, int low_cutoff
     if (!rc && !d.lpf.empty()) rc = upload_floats(h, &h->d_lpf, d.lpf);
     if (!rc && !d.cfilt.empty()) rc = upload_floats(h, &h->d_cfilt, d.cfilt);
     if (!rc) rc = dev_alloc(h, &h->d_in, h->in_isz * h->max_items * h->C);
-    if (!rc && d.sym) rc = tx_ring(h, &h->d_sym, &h->sym_mask, &h->sym_stride, d.sym, d.sym_floats);
-    if (!rc && d.if_) rc = tx_ring(h, &h->d_if, &h->if_mask, &h->if_stride, d.if_);
-    if (!rc && d.rc) rc = tx_ring(h, &h->d_rc, &h->rc_mask, &h->rc_stride, d.rc);
-    if (!rc && d.rs2) rc = dev_alloc(h, &h->d_rs2, static_cast<size_t>(h->rc_stride) * h->C);
+    if (!rc && d.sym) rc = make_ring(h, &h->sym, h->C, d.sym, false, nullptr, d.sym_floats);
+    if (!rc && d.if_) rc = make_ring(h, &h->if_, h->C, d.if_);
+    if (!rc && d.rc) rc = make_ring(h, &h->rc, h->C, d.rc);
+    if (!rc && d.rs2) rc = make_ring(h, &h->rs2, h->C, d.rc);
     if (!rc && d.ra) {      // the audio chains: audio ring and [C] states (AM: agc2_ff::make(1e-2, 1e-4, 1, 1), initial gain 1)
         std::vector<TxAnalogState> an(h->C);
         for (auto& a : an) { std::memset(&a, 0, sizeof a); a.agc = h->chain == TxChain::Am ? 1.0f : 0.0f; }
-        rc = tx_ring(h, &h->d_ra, &h->ra_mask, &h->ra_stride, d.ra);
-        if (!rc && d.rb) rc = dev_alloc(h, &h->d_rb, static_cast<size_t>(h->ra_stride) * h->C);
+        rc = make_ring(h, &h->ra, h->C, d.ra);
+        if (!rc && d.rb) rc = make_ring(h, &h->rb, h->C, d.ra);
         if (!rc) rc = dev_alloc(h, &h->d_an, h->C);
         if (!rc) rc = upload_state(h, h->d_an, an.data(), sizeof(TxAnalogState) * h->C);
     }
@@ -2579,59 +2524,59 @@ void launch_tx_bits(qrl_tx* h, cudaStream_t st, const unsigned char* b, long n, 
 {
     const dim3 g((h->C + 31) / 32);
     switch (h->txm) {
-    case TXM_4FSK: tx_bits_kernel<TXM_4FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
-    case TXM_QPSK: tx_bits_kernel<TXM_QPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
-    case TXM_BPSK: tx_bits_kernel<TXM_BPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
-    case TXM_2FSK: tx_bits_kernel<TXM_2FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
-    case TXM_M17: tx_bits_kernel<TXM_M17><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
-    case TXM_DSSS: tx_bits_kernel<TXM_DSSS><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->d_sym, h->sym_mask, h->sym_stride, sym0); break;
+    case TXM_4FSK: tx_bits_kernel<TXM_4FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
+    case TXM_QPSK: tx_bits_kernel<TXM_QPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
+    case TXM_BPSK: tx_bits_kernel<TXM_BPSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
+    case TXM_2FSK: tx_bits_kernel<TXM_2FSK><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
+    case TXM_M17: tx_bits_kernel<TXM_M17><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
+    case TXM_DSSS: tx_bits_kernel<TXM_DSSS><<<g, 32, 0, st>>>(h->d_bits, h->C, b, n, stride, h->sym, sym0); break;
     }
 }
 // pulse shaping + FM scan: symbol ring -> IF ring
 void launch_shape_fm(qrl_tx* h, cudaStream_t st, long long sym0, long long nsym, int L, int nt, int repeat_only, float pulse_scale, float g1, float g2)
 {
-    tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, st>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, sym0, nsym,
-        L, nt, h->d_arms1, repeat_only, pulse_scale, h->fm_sens, g1, g2, h->d_if, h->if_mask, h->if_stride);
+    tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, st>>>(h->d_bits, h->sym, sym0, nsym,
+        L, nt, h->d_arms1, repeat_only, pulse_scale, h->fm_sens, g1, g2, h->if_);
 }
 // xL interpolator, ring items [m0, m1) -> d_out from output m0 L on
-void launch_interp_generic(qrl_tx* h, const float2* in, unsigned mask, long long stride, long long m0, long long m1, const float* arms,
-                           int L, int NT, float g1, float g2, int apply)
+void launch_interp_generic(qrl_tx* h, Ring<const float2> in, long long m0, long long m1, const float* arms, int L, int NT, float g1, float g2,
+                           int apply)
 {
     const int MT = std::max(1, 4096 / L);
     const size_t smem = sizeof(float) * ((L * NT + 1) & ~1) + sizeof(float2) * (MT + NT);
     interp_fir_ccf_generic_kernel<<<dim3(static_cast<unsigned>((m1 - m0 + MT - 1) / MT), h->C), 256, smem, h->stream>>>(
-        in, mask, stride, m0, m1, arms, L, NT, MT, g1, g2, apply, h->d_out, h->out_stride, m0 * L);
+        in, m0, m1, arms, L, NT, MT, g1, g2, apply, h->d_out, h->out_stride, m0 * L);
 }
 // the FSK chains' final interpolator, IF items [m0, m1) -> d_out from output m0 L2 - out_base on
 void launch_fsk_interp(qrl_tx* h, long long m0, long long m1, long long out_base)
 {
-    if (!fsk_rt(h->L2, h->nt2)) return launch_interp_generic(h, h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    if (!fsk_rt(h->L2, h->nt2)) return launch_interp_generic(h, h->if_, m0, m1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
     constexpr int L = kFskRtL, NT = kFskRtNT, R = 8, G = 16;
     interp_fir_ccf_rt_kernel<L, NT, R, G><<<dim3(static_cast<unsigned>((m1 - m0 + R * G - 1) / (R * G)), h->C), L * G, 0, h->stream>>>(
-        h->d_if, h->if_mask, h->if_stride, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, out_base);
+        h->if_, m0, m1, h->d_arms2, 1.0f, 1.0f, 0, h->d_out, h->out_stride, out_base);
 }
 // rational resampler xL / M, ring to ring: outputs [o0, o1)
-void launch_resamp(qrl_tx* h, const float2* in, unsigned in_mask, long long in_stride, const float* arms, int L, int M, int nt,
-                   long long o0, long long o1, float g1, float g2, int apply, float2* out, unsigned out_mask, long long out_stride)
+void launch_resamp(qrl_tx* h, Ring<const float2> in, const float* arms, int L, int M, int nt, long long o0, long long o1, float g1, float g2,
+                   int apply, Ring<float2> out)
 {
     resamp_ring_to_ring_ccf_kernel<<<grid256(h, o1 - o0), 256, sizeof(float) * L * nt, h->stream>>>(
-        in, in_mask, in_stride, arms, L, M, nt, o0, o1, g1, g2, apply, out, out_mask, out_stride);
+        in, arms, L, M, nt, o0, o1, g1, g2, apply, out);
 }
-// real-tap filter d_cfilt, IF ring -> ring d_rc (NBFM's 50 ksps filter, M17's IF low-pass)
+// real-tap filter d_cfilt, IF ring -> ring rc (NBFM's 50 ksps filter, M17's IF low-pass)
 void launch_if_filter(qrl_tx* h, long long a0, long long a1)
 {
-    fir_ccf_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * h->nt_cfilt, h->stream>>>(h->d_if, h->if_mask, h->if_stride,
-        h->d_rc, h->rc_mask, h->rc_stride, h->d_cfilt, h->nt_cfilt, a0, a1, nullptr, 0, 0, 0);
+    fir_ccf_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * h->nt_cfilt, h->stream>>>(h->if_, h->rc, h->d_cfilt, h->nt_cfilt, a0, a1,
+        nullptr, 0, 0, 0);
 }
-// complex side-band filter d_cfilt, ring d_rs2 -> `out` (SSB, FreeDV)
-void launch_sideband_filter(qrl_tx* h, float2* out, unsigned mask, long long stride, long long a0, long long a1)
+// complex side-band filter d_cfilt, ring rs2 -> `out` (SSB, FreeDV)
+void launch_sideband_filter(qrl_tx* h, Ring<float2> out, long long a0, long long a1)
 {
-    fir_ccc_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(h->d_rs2, h->rc_mask, h->rc_stride,
-        out, mask, stride, h->d_cfilt, h->nt_cfilt, 1.0f, a0, a1, nullptr, 0, 0);
+    fir_ccc_ring_kernel<<<grid256(h, a1 - a0), 256, sizeof(float) * 2 * h->nt_cfilt, h->stream>>>(h->rs2, out, h->d_cfilt, h->nt_cfilt, 1.0f,
+        a0, a1, nullptr, 0, 0);
 }
-void launch_gains(qrl_tx* h, float2* ring, unsigned mask, long long stride, long long a0, long long a1)
+void launch_gains(qrl_tx* h, Ring<float2> ring, long long a0, long long a1)
 {
-    scale2_ring_kernel<<<grid256(h, a1 - a0), 256, 0, h->stream>>>(ring, mask, stride, a0, a1, h->amplif, h->bb_gain);
+    scale2_ring_kernel<<<grid256(h, a1 - a0), 256, 0, h->stream>>>(ring, a0, a1, h->amplif, h->bb_gain);
 }
 // 4FSK: bit chain / pulse shaping + FM scan / x20 interpolator are pipelined slice by slice on three streams (the first two are
 // one-CTA-per-channel recurrences that leave most SMs idle; the interpolator fills them)
@@ -2694,13 +2639,13 @@ void tx_work_psk(qrl_tx* h, const unsigned char* b, long n, long long stride)
 {
     const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n;
     launch_tx_bits(h, h->stream, b, n, stride, sym0);
-    const float2* sym = reinterpret_cast<const float2*>(h->d_sym);
+    const Ring<const float2> sym{ reinterpret_cast<const float2*>(h->sym.d), h->sym.mask, h->sym.stride };     // complex symbols
     if (h->txm == TXM_QPSK && qpsk_rt(h->L1, h->nt1)) {
         constexpr int L = kQpskRtL, NT = kQpskRtNT, MB = 8, MLEN = 64;
         interp_fir_ccf_kernel<L, NT, MB, MLEN><<<dim3(static_cast<unsigned>((nsym + MB * MLEN - 1) / (MB * MLEN)), h->C), L * MB, 0, h->stream>>>(
-            sym, h->sym_mask, h->sym_stride, sym0, sym0 + nsym, h->d_arms1, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, sym0 * L);
+            sym, sym0, sym0 + nsym, h->d_arms1, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, sym0 * L);
     } else {
-        launch_interp_generic(h, sym, h->sym_mask, h->sym_stride, sym0, sym0 + nsym, h->d_arms1, h->L1, h->nt1, h->amplif, h->bb_gain, 1);
+        launch_interp_generic(h, sym, sym0, sym0 + nsym, h->d_arms1, h->L1, h->nt1, h->amplif, h->bb_gain, 1);
     }
     h->launches += 2;
     h->n_out_last = static_cast<long>(nsym * h->L1);
@@ -2714,25 +2659,24 @@ int tx_work_m17_dmr(qrl_tx* h, const unsigned char* b, long n, long long stride)
     h->launches++;
     launch_shape_fm(h, h->stream, sym0, nsym, h->L1, h->nt1, 0, h->pulse_scale, 1.0f, 1.0f);
     if (h->chain == TxChain::Dmr) {
-        tx_delay_ring_kernel<<<grid256(h, m1 - m0), 256, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, h->d_rc, h->rc_mask, h->rc_stride,
-                                                                          m0, m1, h->zi_delay_items);
+        tx_delay_ring_kernel<<<grid256(h, m1 - m0), 256, 0, h->stream>>>(h->if_, h->rc, m0, m1, h->zi_delay_items);
         // the "zero_samples" counters of this call as item ranges (gr_zero_idle_bursts.cpp:61-79: a tag loads the counter, a later
         // one overrides what is left of it, one output is cleared per count)
         std::vector<long long> ranges;
         h->zi.collect(h->C, m0, m1, 0, ranges);
         if (!ranges.empty()) {
             QRL_CK(h->zi.upload(ranges, h->stream));
-            tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride, h->zi.d_ranges);
+            tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->rc, h->zi.d_ranges);
             h->launches++;
         }
     } else {
         launch_if_filter(h, m0, m1);
     }
-    launch_gains(h, h->d_rc, h->rc_mask, h->rc_stride, m0, m1);
+    launch_gains(h, h->rc, m0, m1);
     const long long o0 = (m0 * h->L2 + h->M2 - 1) / h->M2, o1 = (m1 * h->L2 + h->M2 - 1) / h->M2;   // outputs i with floor(i M / L) < m1
     if (o1 - o0 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
-    resamp_ring_ccf_generic_kernel<<<grid256(h, o1 - o0), 256, sizeof(float) * h->L2 * h->nt2, h->stream>>>(h->d_rc, h->rc_mask, h->rc_stride,
-        h->d_arms2, h->L2, h->M2, h->nt2, o0, o1, h->d_out, h->out_stride);
+    resamp_ring_ccf_generic_kernel<<<grid256(h, o1 - o0), 256, sizeof(float) * h->L2 * h->nt2, h->stream>>>(h->rc, h->d_arms2, h->L2, h->M2, h->nt2,
+        o0, o1, h->d_out, h->out_stride);
     h->launches += 4;
     h->n_out_last = static_cast<long>(o1 - o0);
     return QRL_OK;
@@ -2743,28 +2687,28 @@ int tx_work_dsss(qrl_tx* h, const unsigned char* b, long n, long long stride)
     const long long sym0 = h->n_sym, nsym = static_cast<long long>(h->sym_per_item) * n, a0 = sym0 * h->L1, a1 = (sym0 + nsym) * h->L1;
     const long long o0 = (a0 * 50 + 12) / 13, o1 = (a1 * 50 + 12) / 13;
     launch_tx_bits(h, h->stream, b, n, stride, sym0);
-    launch_resamp(h, reinterpret_cast<const float2*>(h->d_sym), h->sym_mask, h->sym_stride, h->d_arms1, h->L1, 1, h->nt1, a0, a1,
-                  h->amplif, h->bb_gain, 1, h->d_if, h->if_mask, h->if_stride);
-    launch_resamp(h, h->d_if, h->if_mask, h->if_stride, h->d_cfilt, 50, 13, h->nt_cfilt, o0, o1, 1.0f, 1.0f, 0, h->d_rc, h->rc_mask, h->rc_stride);
+    const Ring<const float2> chips{ reinterpret_cast<const float2*>(h->sym.d), h->sym.mask, h->sym.stride };
+    launch_resamp(h, chips, h->d_arms1, h->L1, 1, h->nt1, a0, a1, h->amplif, h->bb_gain, 1, h->if_);
+    launch_resamp(h, h->if_, h->d_cfilt, 50, 13, h->nt_cfilt, o0, o1, 1.0f, 1.0f, 0, h->rc);
     if ((o1 - o0) * 50 > h->out_stride) { set_err(h, "qrl_tx_work: output buffer too small"); return QRL_ERANGE; }
-    launch_interp_generic(h, h->d_rc, h->rc_mask, h->rc_stride, o0, o1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+    launch_interp_generic(h, h->rc, o0, o1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
     h->launches += 4;
     h->n_out_last = static_cast<long>((o1 - o0) * 50);
     return QRL_OK;
 }
 void tx_work_nbfm(qrl_tx* h, const float* au, long n, long long stride)
 {
-    tx_nbfm_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->d_ra, h->ra_mask, h->ra_stride,
-        h->d_rb, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->pe_b0, h->pe_b1, h->pe_a1, h->d_arms1, h->nt1,
-        h->d_sym, h->sym_mask, h->sym_stride, h->audio_gain, h->tone_on ? 1 : 0, h->tone_phase, h->tone_inc);
+    tx_nbfm_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->ra,
+        h->rb, h->d_lpf, h->nt_lpf, h->pe_b0, h->pe_b1, h->pe_a1, h->d_arms1, h->nt1,
+        h->sym, h->audio_gain, h->tone_on ? 1 : 0, h->tone_phase, h->tone_inc);
     if (h->tone_on) h->tone_phase += h->tone_inc * static_cast<unsigned>(n);
     const long long r0 = h->n_mid, r1 = ((h->n_audio + n) * 25 + 3) / 4;
     // frequency modulator (Q32 scan) on the 50 ksps stream: "RRC" stage degenerated to a pass-through arm {1}
     launch_shape_fm(h, h->stream, r0, r1 - r0, 1, 1, 1, 1.0f, 1.0f, 1.0f);
     if (r1 > r0) {
         launch_if_filter(h, r0, r1);
-        launch_gains(h, h->d_rc, h->rc_mask, h->rc_stride, r0, r1);
-        launch_interp_generic(h, h->d_rc, h->rc_mask, h->rc_stride, r0, r1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+        launch_gains(h, h->rc, r0, r1);
+        launch_interp_generic(h, h->rc, r0, r1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
     }
     h->launches += 5;
     h->n_out_last = static_cast<long>((r1 - r0) * h->L2);
@@ -2772,53 +2716,49 @@ void tx_work_nbfm(qrl_tx* h, const float* au, long n, long long stride)
 }
 void tx_work_ssb(qrl_tx* h, const float* au, long n, long long stride)
 {
-    tx_ssb_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->d_ra, h->ra_mask, h->ra_stride,
-        h->d_rc, h->rc_mask, h->rc_stride, h->d_lpf, h->nt_lpf, 0.95f, static_cast<float>(1 / (std::sqrt(0.5) / 2)),
-        h->d_rs2, h->rc_mask, h->rc_stride);
+    tx_ssb_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, h->ra, h->rc, h->d_lpf, h->nt_lpf, 0.95f,
+        static_cast<float>(1 / (std::sqrt(0.5) / 2)), h->rs2);
     const long long s0 = h->n_mid, s1 = std::max<long long>(s0, h->n_audio + n - 2);
     if (s1 > s0) {
-        launch_sideband_filter(h, h->d_if, h->if_mask, h->if_stride, s0, s1);
-        launch_gains(h, h->d_if, h->if_mask, h->if_stride, s0, s1);
-        launch_interp_generic(h, h->d_if, h->if_mask, h->if_stride, s0, s1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
+        launch_sideband_filter(h, h->if_, s0, s1);
+        launch_gains(h, h->if_, s0, s1);
+        launch_interp_generic(h, h->if_, s0, s1, h->d_arms2, h->L2, h->nt2, 1.0f, 1.0f, 0);
     }
     h->launches += 4;
     h->n_out_last = static_cast<long>((s1 - s0) * h->L2);
     h->n_mid = s1;
 }
-// AM: audio ring d_ra -> 8 ksps complex ring d_if -> x sps (ring d_rc at the output rate) -> output filter (taps d_cfilt) -> d_out
+// AM: audio ring ra -> 8 ksps complex ring if_ -> x sps (ring rc at the output rate) -> output filter (taps d_cfilt) -> d_out
 int tx_work_am(qrl_tx* h, const float* au, long n, long long stride)
 {
     const long long o0 = h->n_audio * h->L2, o1 = (h->n_audio + n) * h->L2;
-    tx_am_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, 1e-2f, 1e-4f, 1.0f, 1.0f,
-        h->d_ra, h->ra_mask, h->ra_stride, h->d_lpf, h->nt_lpf, h->am_dc, h->d_if, h->if_mask, h->if_stride);
-    launch_resamp(h, h->d_if, h->if_mask, h->if_stride, h->d_arms2, h->L2, 1, h->nt2, o0, o1, h->amplif, h->bb_gain, 1,
-                  h->d_rc, h->rc_mask, h->rc_stride);
+    tx_am_front_kernel<<<h->C, 128, 0, h->stream>>>(h->d_an, au, n, stride, 1e-2f, 1e-4f, 1.0f, 1.0f, h->ra, h->d_lpf, h->nt_lpf, h->am_dc, h->if_);
+    launch_resamp(h, h->if_, h->d_arms2, h->L2, 1, h->nt2, o0, o1, h->amplif, h->bb_gain, 1, h->rc);
     h->launches += 2;
-    if (int rc = launch_fir_ccf_c(h, h->C, h->stream, h->d_rc, h->rc_mask, h->rc_stride, h->d_rs2, h->rc_mask, h->rc_stride,
-                                  h->d_cfilt, h->nt_cfilt, o0, o1, h->d_out, h->out_stride, o0, 0)) return rc;
+    if (int rc = launch_fir_ccf(h, h->C, h->stream, h->rc, h->rs2, h->d_cfilt, h->nt_cfilt, o0, o1, h->d_out, h->out_stride, o0, 0)) return rc;
     h->n_out_last = static_cast<long>(o1 - o0);
     return QRL_OK;
 }
-// FreeDV: int16 modem samples at 8 ksps -> ring d_rs2 -> side-band filter -> ring d_rc -> feedforward AGC -> ring d_if -> x sps -> d_out;
+// FreeDV: int16 modem samples at 8 ksps -> ring rs2 -> side-band filter -> ring rc -> feedforward AGC -> ring if_ -> x sps -> d_out;
 // every stage is one item per thread (no recurrence), all on the handle's stream
 void tx_work_freedv(qrl_tx* h, const short* s, long n, long long stride)
 {
     const long long a0 = h->n_audio, a1 = h->n_audio + n;
     cudaEvent_t pe = h->prof.begin(0, h->stream);
     short_to_complex_ring_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + 255) / 256, 1024)), h->C), 256, 0, h->stream>>>(
-        s, stride, n, static_cast<float>(1.0 / 32765.0), h->d_rs2, h->rc_mask, h->rc_stride, a0);
-    launch_sideband_filter(h, h->d_rc, h->rc_mask, h->rc_stride, a0, a1);
+        s, stride, n, static_cast<float>(1.0 / 32765.0), h->rs2, a0);
+    launch_sideband_filter(h, h->rc, a0, a1);
     h->prof.end(pe);
     constexpr int AN = 512, ATILE = 3584, ANT = 256;
     pe = h->prof.begin(1, h->stream);
     ffagc_kernel<AN, ATILE, ANT><<<dim3(static_cast<unsigned>((n + ATILE - 1) / ATILE), h->C), ANT, 0, h->stream>>>(
-        h->d_rc, h->rc_mask, h->rc_stride, a0, a1, 1.0f, h->d_if, h->if_mask, h->if_stride);
+        h->rc, a0, a1, 1.0f, h->if_);
     h->prof.end(pe);
     // the HBM-write-bound stage (8 B per output sample): register-tiled, x0.98 and x bb_gain fused (the one shape tx_create accepts)
     constexpr int L = 125, NT = 17, R = 8, G = 4;
     pe = h->prof.begin(2, h->stream);
     interp_fir_ccf_rt_kernel<L, NT, R, G><<<dim3(static_cast<unsigned>((n + R * G - 1) / (R * G)), h->C), L * G, 0, h->stream>>>(
-        h->d_if, h->if_mask, h->if_stride, a0, a1, h->d_arms2, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
+        h->if_, a0, a1, h->d_arms2, h->amplif, h->bb_gain, 1, h->d_out, h->out_stride, a0 * L);
     h->prof.end(pe);
     h->launches += 4;
     h->n_out_last = static_cast<long>(n * h->L2);
@@ -3468,8 +3408,8 @@ struct qrl_mmdvm_rx : HandleBase {
     int C = 0, n_rows = 0, nt_arm = 0, nt2 = 0;
     long max_in = 0;
     int* d_rows = nullptr; float* d_arms = nullptr; float* d_taps2 = nullptr;
-    float2 *d_r25 = nullptr, *d_r24 = nullptr, *d_rf = nullptr, *d_in = nullptr;
-    unsigned m25 = 0, m24 = 0; long long s25 = 0, s24 = 0;
+    Ring<float2> r25, r24, rf;     // 25 ksps (multi2) / 250 ksps (single) input, resampler output, channel filter output
+    float2* d_in = nullptr;
     short* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     float* d_rssi = nullptr; long long rssi_stride = 0; int n_rssi_last = 0; long long rssi_b0_last = 0;
     long long n_in = 0, n24 = 0, n_blocks = 0;
@@ -3482,8 +3422,8 @@ struct qrl_mmdvm_tx : HandleBase {
     int* d_rows = nullptr; float* d_arms = nullptr; float* d_taps2 = nullptr; float* d_one = nullptr;
     TxBitState* d_bits = nullptr;
     short* d_in = nullptr;
-    float* d_sym = nullptr; unsigned sym_mask = 0; long long sym_stride = 0;
-    float2 *d_if = nullptr, *d_rf = nullptr; unsigned if_mask = 0; long long if_stride = 0;
+    Ring<float> sym;
+    Ring<float2> if_, rf;          // FM modulator output, channel filter output
     float2* d_lin = nullptr; long long lin_stride = 0;
     float2* d_out = nullptr; long long out_stride = 0; long n_out_last = 0;
     long long n_in = 0, n25 = 0;
@@ -3532,11 +3472,9 @@ int qrl_mmdvm_rx_create(int variant, int n_channels, const int* rows, int n_rows
     if ((rc = upload_floats(h, &h->d_arms, make_arms(ti, h->L, h->nt_arm)))) return fail(rc);
     if ((rc = upload_floats(h, &h->d_taps2, tf))) return fail(rc);
     h->qd_gain = static_cast<float>(24000.0f / (2 * kPi * (h->single ? 10000.0f : 12500.0f)));
-    const unsigned c25 = pow2_at_least(max_in + h->nt_arm + 64), c24 = pow2_at_least(max_in + h->nt2 + 400);
-    h->m25 = c25 - 1; h->s25 = c25; h->m24 = c24 - 1; h->s24 = c24;
-    if ((rc = dev_alloc(h, &h->d_r25, static_cast<size_t>(c25) * h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_r24, static_cast<size_t>(c24) * h->C))) return fail(rc);
-    if ((rc = dev_alloc(h, &h->d_rf, static_cast<size_t>(c24) * h->C))) return fail(rc);
+    if ((rc = make_ring(h, &h->r25, h->C, max_in + h->nt_arm + 64))) return fail(rc);
+    if ((rc = make_ring(h, &h->r24, h->C, max_in + h->nt2 + 400))) return fail(rc);
+    if ((rc = make_ring(h, &h->rf, h->C, max_in + h->nt2 + 400))) return fail(rc);
     h->out_stride = max_in * h->L / h->M + 2;
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->C, false))) return fail(rc);
     h->rssi_stride = h->out_stride / 300 + 2;
@@ -3564,7 +3502,7 @@ int qrl_mmdvm_rx_work(qrl_mmdvm_rx* h, const float* iq, long n, long stride, int
     }
     const int TB = 256;
     mmdvm_gather_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + TB - 1) / TB, 4096)), h->C), TB, 0, h->stream>>>(
-        x, xstride, h->d_rows, n, h->d_r25, h->m25, h->s25, h->n_in);
+        x, xstride, h->d_rows, n, h->r25, h->n_in);
     const long long N = h->n_in + n;
     const long long o0 = h->n24, o1 = (N * h->L + h->M - 1) / h->M;    // outputs o whose newest input floor(M o / L) has arrived
     h->launches++;
@@ -3573,19 +3511,19 @@ int qrl_mmdvm_rx_work(qrl_mmdvm_rx* h, const float* iq, long n, long stride, int
         if (!h->single && h->nt_arm == 35) {       // the reference's filter width (5000 Hz: 819 taps): tiled instance
             const int span_cap = 256 * 25 / 24 + 35 + 4;
             const size_t smem = sizeof(float) * ((24 * 35 + 1) & ~1) + sizeof(float2) * span_cap;
-            resamp_ring_to_ring_tiled_kernel<35><<<g, 256, smem, h->stream>>>(h->d_r25, h->m25, h->s25, h->d_arms, 24, 25, o0, o1, h->d_r24, h->m24, h->s24, span_cap);
+            resamp_ring_to_ring_tiled_kernel<35><<<g, 256, smem, h->stream>>>(h->r25, h->d_arms, 24, 25, o0, o1, h->r24, span_cap);
         } else {
-            resamp_ring_to_ring_ccf_kernel<<<g, TB, sizeof(float) * h->L * h->nt_arm, h->stream>>>(h->d_r25, h->m25, h->s25, h->d_arms, h->L, h->M, h->nt_arm, o0, o1,
-                                                                                                    1.0f, 1.0f, 0, h->d_r24, h->m24, h->s24);
+            resamp_ring_to_ring_ccf_kernel<<<g, TB, sizeof(float) * h->L * h->nt_arm, h->stream>>>(h->r25, h->d_arms, h->L, h->M, h->nt_arm, o0, o1,
+                                                                                                    1.0f, 1.0f, 0, h->r24);
         }
-        { int rc = launch_fir_ccf_c(h, h->C, h->stream, h->d_r24, h->m24, h->s24, h->d_rf, h->m24, h->s24, h->d_taps2, h->nt2, o0, o1, nullptr, 0, 0, 0); if (rc) return rc; h->launches--; }
-        mmdvm_demod_short_kernel<<<g, TB, 0, h->stream>>>(h->d_rf, h->m24, h->s24, o0, o1, h->qd_gain, h->level, h->d_out, h->out_stride);
+        { int rc = launch_fir_ccf(h, h->C, h->stream, h->r24, h->rf, h->d_taps2, h->nt2, o0, o1, nullptr, 0, 0, 0); if (rc) return rc; h->launches--; }
+        mmdvm_demod_short_kernel<<<g, TB, 0, h->stream>>>(h->rf, o0, o1, h->qd_gain, h->level, h->d_out, h->out_stride);
         h->launches += 3;
         const long long b1 = o1 / 300;                                   // complete 300-item blocks so far
         if (b1 > h->n_blocks) {
             const int nb = static_cast<int>(b1 - h->n_blocks);
             // gr_demod_mmdvm tags the resampler's output, gr_demod_mmdvm_multi2 the channel filter's
-            mmdvm_rssi_kernel<<<dim3((nb + 63) / 64, h->C), 64, 0, h->stream>>>(h->single ? h->d_r24 : h->d_rf, h->m24, h->s24, h->n_blocks, nb, h->cal, h->d_rssi, h->rssi_stride);
+            mmdvm_rssi_kernel<<<dim3((nb + 63) / 64, h->C), 64, 0, h->stream>>>(h->single ? h->r24 : h->rf, h->n_blocks, nb, h->cal, h->d_rssi, h->rssi_stride);
             h->launches++;
             h->n_rssi_last = nb; h->rssi_b0_last = h->n_blocks; h->n_blocks = b1;
         }
@@ -3661,11 +3599,9 @@ int qrl_mmdvm_tx_create(int variant, int n_channels, const int* rows, int n_rows
     if ((rc = dev_alloc(h, &h->d_bits, h->C))) return fail(rc);
     { std::vector<TxBitState> st(h->C); for (auto& x : st) { x.scr_reg = 0x7F; x.enc_state = 0; x.diff_prev = 0; x.phase_q = 0; }
       if ((rc = upload_state(h, h->d_bits, st.data(), sizeof(TxBitState) * h->C))) return fail(rc); }
-    { const unsigned cap = pow2_at_least(max_in + 64); h->sym_mask = cap - 1; h->sym_stride = cap;
-      if ((rc = dev_alloc(h, &h->d_sym, static_cast<size_t>(cap) * h->C))) return fail(rc); }
-    { const unsigned cap = pow2_at_least(max_in + std::max(h->nt2, h->nt_arm) + 128); h->if_mask = cap - 1; h->if_stride = cap;
-      if ((rc = dev_alloc(h, &h->d_if, static_cast<size_t>(cap) * h->C))) return fail(rc);
-      if ((rc = dev_alloc(h, &h->d_rf, static_cast<size_t>(cap) * h->C))) return fail(rc); }
+    if ((rc = make_ring(h, &h->sym, h->C, max_in + 64))) return fail(rc);
+    if ((rc = make_ring(h, &h->if_, h->C, max_in + std::max(h->nt2, h->nt_arm) + 128))) return fail(rc);
+    if ((rc = make_ring(h, &h->rf, h->C, max_in + std::max(h->nt2, h->nt_arm) + 128))) return fail(rc);
     h->lin_stride = max_in * h->L / h->M + 4; h->out_stride = h->lin_stride;
     if ((rc = dev_alloc(h, &h->d_lin, static_cast<size_t>(h->lin_stride) * h->C, false))) return fail(rc);
     if ((rc = dev_alloc(h, &h->d_out, static_cast<size_t>(h->out_stride) * h->n_rows))) return fail(rc);      // unused rows stay zero (null_source)
@@ -3698,28 +3634,27 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
     const int TB = 256;
     const long long a0 = h->n_in, a1 = h->n_in + n;
     mmdvm_short_float_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((n + TB - 1) / TB, 4096)), h->C), TB, 0, h->stream>>>(
-        s, sstride, n, h->level, h->d_sym, h->sym_mask, h->sym_stride, a0);
+        s, sstride, n, h->level, h->sym, a0);
     // frequency_modulator_fc: the FM scan kernel with a one-tap "pulse" (x * 1.0 is exact), Q32 phase carried in the state
-    tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->stream>>>(h->d_bits, h->d_sym, h->sym_mask, h->sym_stride, a0, n,
-        1, 1, h->d_one, 0, 1.0f, h->fm_sens, 1.0f, 1.0f, h->d_if, h->if_mask, h->if_stride);
+    tx_shape_fm_kernel<1024, 2><<<h->C, 1024, 0, h->stream>>>(h->d_bits, h->sym, a0, n, 1, 1, h->d_one, 0, 1.0f, h->fm_sens, 1.0f, 1.0f, h->if_);
     if (h->single) {
         // gr_mod_mmdvm.cpp:51-58: gr_zero_idle_bursts(0) between the FM modulator and the filter (items of the 24 ksps stream)
         std::vector<long long> ranges;
         h->zi.collect(h->C, a0, a1, 0, ranges);
         if (!ranges.empty()) {
             QRL_CK(h->zi.upload(ranges, h->stream));
-            tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_if, h->if_mask, h->if_stride, h->zi.d_ranges);
+            tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->if_, h->zi.d_ranges);
             h->launches++;
         }
     }
     dim3 g(static_cast<unsigned>((n + TB - 1) / TB), h->C);
-    { int rc = launch_fir_ccf_c(h, h->C, h->stream, h->d_if, h->if_mask, h->if_stride, h->d_rf, h->if_mask, h->if_stride, h->d_taps2, h->nt2, a0, a1, nullptr, 0, 0, 0); if (rc) return rc; h->launches--; }
-    scale2_ring_kernel<<<g, TB, 0, h->stream>>>(h->d_rf, h->if_mask, h->if_stride, a0, a1, 0.8f, h->single ? h->bb_gain : 1.0f);   // gr_mod_mmdvm: bb_gain here
+    { int rc = launch_fir_ccf(h, h->C, h->stream, h->if_, h->rf, h->d_taps2, h->nt2, a0, a1, nullptr, 0, 0, 0); if (rc) return rc; h->launches--; }
+    scale2_ring_kernel<<<g, TB, 0, h->stream>>>(h->rf, a0, a1, 0.8f, h->single ? h->bb_gain : 1.0f);   // gr_mod_mmdvm: bb_gain here
     const long long o0 = h->n25, o1 = (a1 * h->L + h->M - 1) / h->M;     // outputs i with floor(M i / L) < a1
     if (o1 - o0 > h->lin_stride) { set_err(h, "qrl_mmdvm_tx_work: output buffer too small"); return QRL_ERANGE; }
     if (o1 > o0) {
         dim3 go(static_cast<unsigned>((o1 - o0 + 255) / 256), h->C);
-        resamp_ring_ccf_generic_kernel<<<go, 256, sizeof(float) * h->L * h->nt_arm, h->stream>>>(h->d_rf, h->if_mask, h->if_stride, h->d_arms, h->L, h->M, h->nt_arm, o0, o1,
+        resamp_ring_ccf_generic_kernel<<<go, 256, sizeof(float) * h->L * h->nt_arm, h->stream>>>(h->rf, h->d_arms, h->L, h->M, h->nt_arm, o0, o1,
                                                                                                h->d_lin, h->lin_stride);
         if (!h->single) {
             // gr_mod_mmdvm_multi2.cpp:88,108-117: gr_zero_idle_bursts(0) between the x25/24 resampler and the synthesizer (items of the
@@ -3728,7 +3663,8 @@ int qrl_mmdvm_tx_work(qrl_mmdvm_tx* h, const short* in, long n, long stride, int
             h->zi.collect(h->C, o0, o1, o0, ranges);
             if (!ranges.empty()) {
                 QRL_CK(h->zi.upload(ranges, h->stream));
-                tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(h->d_lin, 0xffffffffu, h->lin_stride, h->zi.d_ranges);
+                tx_zero_ranges_kernel<<<static_cast<unsigned>(ranges.size() / 3), 256, 0, h->stream>>>(
+                    Ring<float2>{ h->d_lin, 0xffffffffu, h->lin_stride }, h->zi.d_ranges);
                 h->launches++;
             }
         }

@@ -14,6 +14,20 @@
 
 namespace qrl {
 
+// A stream ring: [C][capacity] items, capacity a power of two (mask = capacity - 1); item a of channel c sits at
+// d[c * stride + (a & mask)], or at d[((c >> 5) * stride + (a & mask)) * 32 + (c & 31)] when the ring is channel-interleaved.
+// Handles and kernels pass a ring as this one value.  __restrict__ does not carry through a member: a kernel binds
+// `const T* __restrict__ x = ring.d + ...` before it indexes.  agc_costas_kernel, symsync_ext_epilogue_kernel and viterbi_k7_kernel keep
+// (pointer, mask, stride) arguments: with Ring arguments they compiled to other register allocations and ran 3-10 % slower (H100, 700 W).
+template <class T>
+struct Ring {
+    T* d = nullptr;
+    unsigned mask = 0;
+    long long stride = 0;
+    template <class U, class = std::enable_if_t<std::is_same<U, const T>::value>>     // Ring<T> -> Ring<const T>
+    __host__ __device__ operator Ring<U>() const { return { d, mask, stride }; }
+};
+
 // ------------------------------------------------------------------------------------------------
 // device tables (uploaded once per process by qrl_upload_tables)
 // ------------------------------------------------------------------------------------------------
@@ -276,8 +290,7 @@ __global__ void __launch_bounds__(NWARPS * 32)
 fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
                       const float2* __restrict__ hist, int H,
                       const float* __restrict__ taps_padded,   // Q*D floats, zero padded
-                      float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
-                      long long n_in_before, long long k0, long long k1, const RotState* __restrict__ rot = nullptr)
+                      Ring<float2> out_ring, long long n_in_before, long long k0, long long k1, const RotState* __restrict__ rot = nullptr)
 {
     extern __shared__ __align__(128) float2 xs_raw[];   // WC samples
     __shared__ __align__(8) uint64_t fill_bar;
@@ -306,10 +319,10 @@ fir_decim_poly_kernel(const float2* __restrict__ iq, long long iq_stride, long l
         __syncthreads();
     }
 
-    float* outc = reinterpret_cast<float*>(out_ring + static_cast<long long>(c) * ring_stride);
+    float* __restrict__ outc = reinterpret_cast<float*>(out_ring.d + static_cast<long long>(c) * out_ring.stride);
     fir_poly_tile<D, Q, K, NOUT, NWARPS>(xs_raw + win.shift, tap, lane, warp, [&](int i, int comp, float v) {
         const long long k = kbase + i;
-        if (k < k1) outc[2 * (k & ring_mask) + comp] = v;
+        if (k < k1) outc[2 * (k & out_ring.mask) + comp] = v;
     });
 }
 
@@ -322,8 +335,7 @@ __global__ void __launch_bounds__(NTHREADS)
 fir_decim2_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
                   const float2* __restrict__ hist, int H,
                   const float* __restrict__ taps_padded,   // NTP floats
-                  float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
-                  long long n_in_before, long long k0, long long k1)
+                  Ring<float2> out_ring, long long n_in_before, long long k0, long long k1)
 {
     constexpr int D = 2;
     constexpr int NOUT = NTHREADS * K;
@@ -367,11 +379,11 @@ fir_decim2_kernel(const float2* __restrict__ iq, long long iq_stride, long long 
             }
         }
     }
-    float2* outc = out_ring + static_cast<long long>(c) * ring_stride;
+    float2* __restrict__ outc = out_ring.d + static_cast<long long>(c) * out_ring.stride;
 #pragma unroll
     for (int i = 0; i < K; i++) {
         const long long k = kbase + K * t + i;
-        if (k < k1) outc[k & ring_mask] = make_float2(s0[i].x + s1[i].x, s0[i].y + s1[i].y);
+        if (k < k1) outc[k & out_ring.mask] = make_float2(s0[i].x + s1[i].x, s0[i].y + s1[i].y);
     }
 }
 
@@ -385,8 +397,7 @@ __global__ void __launch_bounds__(256)
 fir_resamp_ccf_kernel(const float2* __restrict__ iq, long long iq_stride, long long T,
                       const float2* __restrict__ hist, int H,
                       const float* __restrict__ arms /* [L][NT] */,
-                      float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
-                      long long n_in_before, long long k0, long long k1)
+                      Ring<float2> out_ring, long long n_in_before, long long k0, long long k1)
 {
     constexpr int SPAN = (NOUT * M + L - 1) / L + NT + 1;      // input samples covering NOUT outputs
     extern __shared__ float2 xs_rs[];
@@ -407,7 +418,7 @@ fir_resamp_ccf_kernel(const float2* __restrict__ iq, long long iq_stride, long l
         xs_rs[idx] = v;
     }
     __syncthreads();
-    float2* outc = out_ring + static_cast<long long>(c) * ring_stride;
+    float2* __restrict__ outc = out_ring.d + static_cast<long long>(c) * out_ring.stride;
     for (int o = threadIdx.x; o < NOUT; o += 256) {
         const long long k = kbase + o;
         if (k >= k1) break;
@@ -421,7 +432,7 @@ fir_resamp_ccf_kernel(const float2* __restrict__ iq, long long iq_stride, long l
             re = fmaf(h[j], v.x, re);
             im = fmaf(h[j], v.y, im);
         }
-        outc[k & ring_mask] = make_float2(re, im);
+        outc[k & out_ring.mask] = make_float2(re, im);
     }
 }
 
@@ -432,22 +443,22 @@ fir_resamp_ccf_kernel(const float2* __restrict__ iq, long long iq_stride, long l
 constexpr int kMaxTapsSmem = 4096;
 
 // complex stream, real taps (fft_filter_ccf restated in direct form); optional linear copy (port 0)
-__global__ void fir_ccf_ring_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                                    float2* __restrict__ out, unsigned out_mask, long long out_stride,
+__global__ void fir_ccf_ring_kernel(Ring<const float2> in, Ring<float2> out,
                                     const float* __restrict__ taps, int ntaps, long long a0, long long a1,
                                     float2* __restrict__ lin, long long lin_stride, long long lin_base, int out_interleaved)
 {
+    float2* __restrict__ y_out = out.d;
     extern __shared__ float hs_dyn[];
     for (int i = threadIdx.x; i < ntaps; i += blockDim.x) hs_dyn[i] = taps[i];
     __syncthreads();
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     float2 y = make_float2(0.0f, 0.0f);
-    for (int j = ntaps - 1; j >= 0; j--) ffma2(y, hs_dyn[j], x[(a - j) & in_mask]);
-    if (out_interleaved) out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = y;
-    else out[static_cast<long long>(c) * out_stride + (a & out_mask)] = y;
+    for (int j = ntaps - 1; j >= 0; j--) ffma2(y, hs_dyn[j], x[(a - j) & in.mask]);
+    if (out_interleaved) y_out[(static_cast<long long>(c >> 5) * out.stride + (a & out.mask)) * 32 + (c & 31)] = y;
+    else y_out[static_cast<long long>(c) * out.stride + (a & out.mask)] = y;
     if (lin) lin[static_cast<long long>(c) * lin_stride + (a - lin_base)] = y;
 }
 
@@ -528,11 +539,10 @@ __device__ __forceinline__ void ccf_tile_outputs(const float* hs, const float2* 
 // LDS.64 of a half-warp then hit distinct bank pairs.
 template <int K, int NT>
 __global__ void __launch_bounds__(NT)
-fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                          float2* __restrict__ out, unsigned out_mask, long long out_stride,
-                          const float* __restrict__ taps, int ntaps, long long a0, long long a1,
+fir_ccf_ring_tiled_kernel(Ring<const float2> in, Ring<float2> out, const float* __restrict__ taps, int ntaps, long long a0, long long a1,
                           float2* __restrict__ lin, long long lin_stride, long long lin_base, int out_interleaved)
 {
+    float2* __restrict__ y_out = out.d;
     extern __shared__ __align__(16) float sm_tl[];
     constexpr int TILE = K * NT;
     float* hs = sm_tl;                                                    // ntaps floats (rounded up to even)
@@ -540,10 +550,10 @@ fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long 
     const int c = blockIdx.y;
     const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
     if (tile0 >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
     const int span = TILE + ntaps - 1;
-    for (int i = threadIdx.x; i < span; i += NT) xs[i + (i >> 4)] = x[(tile0 - (ntaps - 1) + i) & in_mask];
+    for (int i = threadIdx.x; i < span; i += NT) xs[i + (i >> 4)] = x[(tile0 - (ntaps - 1) + i) & in.mask];
     __syncthreads();
     const int base = K * threadIdx.x;                  // xs index of the oldest sample of my output 0
     float2 acc[K];
@@ -552,8 +562,8 @@ fir_ccf_ring_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long 
     for (int i = 0; i < K; i++) {
         const long long a = tile0 + base + i;
         if (a >= a1) break;
-        if (out_interleaved) out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc[i];
-        else out[static_cast<long long>(c) * out_stride + (a & out_mask)] = acc[i];
+        if (out_interleaved) y_out[(static_cast<long long>(c >> 5) * out.stride + (a & out.mask)) * 32 + (c & 31)] = acc[i];
+        else y_out[static_cast<long long>(c) * out.stride + (a & out.mask)] = acc[i];
         if (lin) lin[static_cast<long long>(c) * lin_stride + (a - lin_base)] = acc[i];
     }
 }
@@ -629,10 +639,10 @@ __device__ __forceinline__ void fff_tile_outputs(const float* hs, const float* d
 // The CTA first demodulates its tile + ntaps - 1 of history into shared memory, then filters from there.
 template <int K, int NT>
 __global__ void __launch_bounds__(NT)
-qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                            float* __restrict__ out, unsigned out_mask, long long out_stride,
+qdemod_fir_fff_tiled_kernel(Ring<const float2> in, Ring<float> out,
                             const float* __restrict__ taps, int ntaps, float gain, long long a0, long long a1)
 {
+    float* __restrict__ y_out = out.d;
     extern __shared__ __align__(16) float sm_tl[];
     constexpr int TILE = K * NT;
     float* hs = sm_tl;                         // ntaps
@@ -640,7 +650,7 @@ qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, lon
     const int c = blockIdx.y;
     const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * TILE;
     if (tile0 >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     for (int i = threadIdx.x; i < ntaps; i += NT) hs[i] = taps[i];
     const int span = TILE + ntaps - 1;
     for (int i = threadIdx.x; i < span; i += NT) {
@@ -648,8 +658,8 @@ qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, lon
         float d = 0.0f;
         if (n >= 0 && n < a1) {
             float2 prev = make_float2(0.0f, 0.0f);
-            if (n >= 1) prev = x[(n - 1) & in_mask];
-            d = qdemod_sample(x[n & in_mask], prev, gain);
+            if (n >= 1) prev = x[(n - 1) & in.mask];
+            d = qdemod_sample(x[n & in.mask], prev, gain);
         }
         ds[i + (i >> 5)] = d;
     }
@@ -661,7 +671,7 @@ qdemod_fir_fff_tiled_kernel(const float2* __restrict__ in, unsigned in_mask, lon
     for (int i = 0; i < K; i++) {
         const long long a = tile0 + base + i;
         if (a >= a1) break;
-        out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc[i];
+        y_out[(static_cast<long long>(c >> 5) * out.stride + (a & out.mask)) * 32 + (c & 31)] = acc[i];
     }
 }
 
@@ -704,13 +714,12 @@ struct FskFrontendSmem {
 template <int D, int Q, int NOUT1>
 __global__ void __launch_bounds__(FF_NT, 2)
 fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long long T, const float2* __restrict__ hist, int H,
-                       const float* __restrict__ taps1, long long n_in_before, const RotState* __restrict__ rot,
-                       float2* __restrict__ r1, unsigned r1_mask, long long r1_stride,
+                       const float* __restrict__ taps1, long long n_in_before, const RotState* __restrict__ rot, Ring<float2> r1,
                        const float* __restrict__ taps2, int ntaps2, float2* __restrict__ port0, long long port0_stride, long long port0_base,
-                       const float* __restrict__ taps3, int ntaps3, float gain,
-                       float* __restrict__ r4, unsigned r4_mask, long long r4_stride,
+                       const float* __restrict__ taps3, int ntaps3, float gain, Ring<float> r4,
                        long long k0, long long k1, int strip, int C)
 {
+    float* __restrict__ r4w = r4.d;
     constexpr int K = 8, NWARPS = FF_NT / 32, TPC = FF_CH / NOUT1;
     using Win = FirPolyWindow<D, Q, NOUT1>;
     static_assert(FF_CH == K * FF_NT && FF_CH % NOUT1 == 0, "a chunk is one filter pass and whole stage-1 tiles");
@@ -748,11 +757,11 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
     for (int l = threadIdx.x; l < G2; l += FF_NT) y1[l + (l >> 4)] = make_float2(0.0f, 0.0f);
     for (int l = threadIdx.x; l < G3; l += FF_NT) ds[l + (l >> 5)] = 0.0f;
     if (threadIdx.x == 0) y2[0] = make_float2(0.0f, 0.0f);
-    const float2* r1c = r1 + static_cast<long long>(c) * r1_stride;
+    const float2* __restrict__ r1c = r1.d + static_cast<long long>(c) * r1.stride;
     if (first) {
         for (int l = threadIdx.x; l < halo; l += FF_NT) {
             const int li = G2 + l;
-            y1[li + (li >> 4)] = r1c[(v0 + l) & r1_mask];
+            y1[li + (li >> 4)] = r1c[(v0 + l) & r1.mask];
         }
     }
     if (threadIdx.x == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); mbar_fence_init(); }
@@ -770,7 +779,7 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
     };
     if (threadIdx.x == 0) { prefetch(t_lo); prefetch(t_lo + 1); }
     unsigned parity = 0;                                       // bit s: phase of the next completion of bar[s]
-    float2* r1w = r1 + static_cast<long long>(c) * r1_stride;
+    float2* __restrict__ r1w = r1.d + static_cast<long long>(c) * r1.stride;
 
     int t = t_lo;
     for (long long u0 = v0; u0 < b; u0 += FF_CH) {
@@ -796,7 +805,7 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
                 if (k >= b || (first && k < a)) return;
                 const int li = G2 + static_cast<int>(k - u0);
                 reinterpret_cast<float*>(y1 + li + (li >> 4))[comp] = v;
-                if (k >= keep_from) reinterpret_cast<float*>(r1w + (k & r1_mask))[comp] = v;
+                if (k >= keep_from) reinterpret_cast<float*>(r1w + (k & r1.mask))[comp] = v;
             });
             __syncthreads();                                   // window t & 1 consumed
             if (threadIdx.x == 0) prefetch(t + 2);
@@ -831,7 +840,7 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
 #pragma unroll
             for (int i = 0; i < K; i++) {
                 const long long n = u0 + base + i;
-                if (n >= a && n < b) r4[(static_cast<long long>(c >> 5) * r4_stride + (n & r4_mask)) * 32 + (c & 31)] = acc[i];
+                if (n >= a && n < b) r4w[(static_cast<long long>(c >> 5) * r4.stride + (n & r4.mask)) * 32 + (c & 31)] = acc[i];
             }
         }
         __syncthreads();
@@ -845,32 +854,27 @@ fsk_fm_frontend_kernel(const float2* __restrict__ iq, long long iq_stride, long 
 
 // quadrature_demod_cf fused in front of a real FIR (RRC shaping filter): in = complex ring, out = float ring.
 // Each CTA demodulates its tile (+ntaps-1 halo) into shared memory, then filters from there.
-__global__ void qdemod_fir_fff_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                                      float* __restrict__ out, unsigned out_mask, long long out_stride,
-                                      const float* __restrict__ taps, int ntaps, float gain,
-                                      long long a0, long long a1, float* __restrict__ demod_dbg, long long dbg_stride)
+__global__ void qdemod_fir_fff_kernel(Ring<const float2> in, Ring<float> out, const float* __restrict__ taps, int ntaps, float gain,
+                                      long long a0, long long a1)
 {
+    float* __restrict__ y_out = out.d;
     extern __shared__ float sm_dyn[];
     float* hs = sm_dyn;                 // ntaps
     float* ds = sm_dyn + ntaps;         // blockDim.x + ntaps - 1 demodulated samples
     for (int i = threadIdx.x; i < ntaps; i += blockDim.x) hs[i] = taps[i];
     const int c = blockIdx.y;
     const long long tile0 = a0 + static_cast<long long>(blockIdx.x) * blockDim.x;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     const int span = blockDim.x + ntaps - 1;
     for (int i = threadIdx.x; i < span; i += blockDim.x) {
         const long long n = tile0 - (ntaps - 1) + i;       // absolute demod index
         float d = 0.0f;
         if (n >= 0 && n < a1) {
-            const float2 cur = x[n & in_mask];
             float2 prev = make_float2(0.0f, 0.0f);
-            if (n >= 1) prev = x[(n - 1) & in_mask];
-            const float re = cur.x * prev.x + cur.y * prev.y;
-            const float im = cur.y * prev.x - cur.x * prev.y;
-            d = gain * qrl_fast_atan2f(im, re);
+            if (n >= 1) prev = x[(n - 1) & in.mask];
+            d = qdemod_sample(x[n & in.mask], prev, gain);
         }
         ds[i] = d;
-        if (demod_dbg && n >= a0 && n < a1 && i >= ntaps - 1) demod_dbg[static_cast<long long>(c) * dbg_stride + (n - a0)] = d;
     }
     __syncthreads();
     const long long a = tile0 + threadIdx.x;
@@ -879,21 +883,22 @@ __global__ void qdemod_fir_fff_kernel(const float2* __restrict__ in, unsigned in
     const float* p = ds + threadIdx.x + (ntaps - 1);       // newest sample of this output
     for (int j = ntaps - 1; j >= 0; j--) acc = fmaf(hs[j], p[-j], acc);
     // channel-interleaved ring: [c / 32][slot][c % 32]  (one warp of the symbol-sync kernel = one 128-byte row per time step)
-    out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc;
+    y_out[(static_cast<long long>(c >> 5) * out.stride + (a & out.mask)) * 32 + (c & 31)] = acc;
 }
 
 // Channel-interleaved float ring [c / 32][slot][c % 32] -> linear per-channel port buffer [c][a - a0] (gr_demod_dmr's port 3:
 // the symbol filter output, gr_demod_dmr.cpp:103).  grid = (tiles of blockDim.x samples, 32-channel groups), block = (32, ty):
 // reads are whole 128-byte rows of the ring, writes go through a shared-memory transpose so each channel stores runs of 32 floats.
-__global__ void ring_to_port_f32_kernel(const float* __restrict__ ring, unsigned mask, long long stride, int C,
+__global__ void ring_to_port_f32_kernel(Ring<const float> ring, int C,
                                         long long a0, long long a1, float* __restrict__ port, long long port_stride, long long port_off)
 {
+    const float* __restrict__ rg = ring.d;
     __shared__ float tile[32][33];
     const int g = blockIdx.y, lane = threadIdx.x;
     const long long t0 = a0 + static_cast<long long>(blockIdx.x) * 32;
     for (int r = threadIdx.y; r < 32; r += blockDim.y) {
         const long long a = t0 + r;
-        tile[r][lane] = (a < a1) ? ring[(static_cast<long long>(g) * stride + (a & mask)) * 32 + lane] : 0.0f;
+        tile[r][lane] = (a < a1) ? rg[(static_cast<long long>(g) * ring.stride + (a & ring.mask)) * 32 + lane] : 0.0f;
     }
     __syncthreads();
     for (int ch = threadIdx.y; ch < 32; ch += blockDim.y) {
@@ -932,10 +937,10 @@ __device__ __forceinline__ float2 qrl_fir_dot_order_c(const float* __restrict__ 
 // output.  Used for the stage-1 shapes that have no register-tiled instance (WBFM: /5, 41 taps).
 __global__ void __launch_bounds__(128)
 fir_decim_hist_generic_kernel(const float2* __restrict__ iq, long long iq_stride, long long T, const float2* __restrict__ hist, int H,
-                              const float* __restrict__ taps, int ntaps, int D,
-                              float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
+                              const float* __restrict__ taps, int ntaps, int D, Ring<float2> out_ring,
                               long long n_in_before, long long k0, long long k1)
 {
+    float2* __restrict__ y_out = out_ring.d;
     const int c = blockIdx.y;
     const long long k = k0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (k >= k1) return;
@@ -947,7 +952,7 @@ fir_decim_hist_generic_kernel(const float2* __restrict__ iq, long long iq_stride
         if (i >= 0) return i < T ? x[i] : make_float2(0.0f, 0.0f);
         return (H + i >= 0) ? hc[H + i] : make_float2(0.0f, 0.0f);
     });
-    out_ring[static_cast<long long>(c) * ring_stride + (k & ring_mask)] = y;
+    y_out[static_cast<long long>(c) * out_ring.stride + (k & out_ring.mask)] = y;
 }
 
 // Shape-generic rational stage 1 (rational_resampler_ccf(L, M), L > 1): output i takes arm (i M) mod L at input position
@@ -956,9 +961,9 @@ fir_decim_hist_generic_kernel(const float2* __restrict__ iq, long long iq_stride
 __global__ void __launch_bounds__(128)
 fir_resamp_hist_generic_kernel(const float2* __restrict__ iq, long long iq_stride, long long T, const float2* __restrict__ hist, int H,
                                const float* __restrict__ arms /* [L][nt] */, int nt, int L, int M,
-                               float2* __restrict__ out_ring, unsigned ring_mask, long long ring_stride,
-                               long long n_in_before, long long k0, long long k1)
+                               Ring<float2> out_ring, long long n_in_before, long long k0, long long k1)
 {
+    float2* __restrict__ y_out = out_ring.d;
     const int c = blockIdx.y;
     const long long i = k0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= k1) return;
@@ -976,7 +981,7 @@ fir_resamp_hist_generic_kernel(const float2* __restrict__ iq, long long iq_strid
         else v = (H + a >= 0) ? hc[H + a] : make_float2(0.0f, 0.0f);
         re = fmaf(h[k], v.x, re); imv = fmaf(h[k], v.y, imv);
     }
-    out_ring[static_cast<long long>(c) * ring_stride + (i & ring_mask)] = make_float2(re, imv);
+    y_out[static_cast<long long>(c) * out_ring.stride + (i & out_ring.mask)] = make_float2(re, imv);
 }
 
 // Stand-alone batched decimating FIR for any (ntaps, D), zero history: y[k] = sum_j h[j] x[D k - j] in THE FIR order
@@ -1249,8 +1254,7 @@ template <int NMAX>
 __global__ void __launch_bounds__(32)
 fll_kernel(FllParams p, FllState* __restrict__ states, float2* __restrict__ hist_g /* [C][NMAX] rotated-sample window */,
            int C, const float* __restrict__ taps /* lower[2N] | upper[2N] */,
-           const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long avail_total,
-           float2* __restrict__ out, unsigned out_mask, long long out_stride)
+           Ring<const float2> in, long long avail_total, Ring<float2> out)
 {
     __shared__ float2 win[NMAX][32];
     __shared__ float tl[2 * NMAX], tu[2 * NMAX];
@@ -1262,13 +1266,13 @@ fll_kernel(FllParams p, FllState* __restrict__ states, float2* __restrict__ hist
     __syncwarp();
     if (c >= C) return;
     FllState st = states[c];
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    float2* y = out + static_cast<long long>(c) * out_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
+    float2* __restrict__ y = out.d + static_cast<long long>(c) * out.stride;
     int head = static_cast<int>(st.pos & (N - 1));            // slot of the OLDEST sample (N is a power of two)
     for (long long a = st.pos; a < avail_total; a += 8) {
         float2 v[8];
 #pragma unroll
-        for (int j = 0; j < 8; j++) v[j] = (a + j < avail_total) ? x[(a + j) & in_mask] : make_float2(0.0f, 0.0f);
+        for (int j = 0; j < 8; j++) v[j] = (a + j < avail_total) ? x[(a + j) & in.mask] : make_float2(0.0f, 0.0f);
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             if (a + j >= avail_total) break;
@@ -1292,7 +1296,7 @@ fll_kernel(FllParams p, FllState* __restrict__ states, float2* __restrict__ hist
             while (st.phase <= -6.2831854820251465f) st.phase = static_cast<float>(static_cast<double>(st.phase) + 2.0 * 3.14159265358979323846);
             if (st.freq > p.max_freq) st.freq = p.max_freq;
             else if (st.freq < p.min_freq) st.freq = p.min_freq;
-            y[(a + j) & out_mask] = make_float2(orr, oi);
+            y[(a + j) & out.mask] = make_float2(orr, oi);
         }
     }
     st.pos = avail_total;
@@ -1505,10 +1509,9 @@ __device__ __noinline__ float2 symsync_generic_step(float ph)
 // 3 = generic recurrence with the PLAIN Mueller & Mueller detector (gr_demod_dmr.cpp:66; real symbols only) instead of the modified one
 template <int NCOMP, int SLICER, int EPI, int CH, int NST, int NEPI, int LOOPK = LOOP_SYMSYNC, int VAR = 0>
 __global__ void __launch_bounds__(64 + 32 * NEPI)
-symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
-               const float* __restrict__ in, unsigned in_mask, long long in_stride /*slots per group*/, long long avail_total,
+symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C, Ring<const float> in /*slots per group*/, long long avail_total,
                float2* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap,
-               unsigned char* __restrict__ soft_ring, unsigned soft_mask, long long soft_stride, int maxs,
+               Ring<unsigned char> soft_ring, int maxs,
                long long* __restrict__ n_soft_out /* [C] snapshot of the soft-bit write index after this launch */,
                float* __restrict__ ext_scratch = nullptr /* [groups][ext_chunk_cap][maxs + 2][32] (EPI_EXT_*) */,
                int ext_chunk_cap = 0 /* chunks this launch may emit */, int ext_chunk_stride = 0 /* chunks per group in the scratch */,
@@ -1607,14 +1610,14 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
     if (warp == 1) {
         // ------------------------------------------------------------------ TMA producer
         if (lane == 0) {
-            const float* ring = in + static_cast<long long>(g) * in_stride * ROWF;
-            const long long cap = static_cast<long long>(in_mask) + 1;
+            const float* __restrict__ ring = in.d + static_cast<long long>(g) * in.stride * ROWF;
+            const long long cap = static_cast<long long>(in.mask) + 1;
             for (int m = 0; m < nchunks; m++) {
                 const int st = m % NST, u = m / NST;
                 if (u > 0) mbar_wait(&bar_free[st], (u - 1) & 1);
                 const long long w0 = base + static_cast<long long>(m) * STRIDE;
                 float* dst = stage0 + st * CH * ROWF;
-                const long long s0 = w0 & in_mask;
+                const long long s0 = w0 & in.mask;
                 const long long first = (s0 + CH <= cap) ? CH : (cap - s0);
                 fence_proxy_async();
                 mbar_expect_tx(&bar_in[st], CH * ROWF * 4);
@@ -2062,7 +2065,7 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
             n_sym = st.n_sym; n_soft = st.n_soft; costas = st.costas; dp_r = st.dp_r; dp_i = st.dp_i;
             p1cnt = port1_cnt[c];
         }
-        unsigned char* sr = soft_ring + static_cast<long long>(c) * soft_stride;
+        unsigned char* __restrict__ sr = soft_ring.d + static_cast<long long>(c) * soft_ring.stride;
         float2* p1 = port1 + static_cast<long long>(c) * port1_stride;
         for (int m = 0; m < nchunks; m++) {
             const int b = m % NB;
@@ -2115,8 +2118,8 @@ symsync_kernel(SymSyncParams p, SymSyncState* __restrict__ states, int C,
                     sb1 = qrl_soft_u8(o_i, p.soft_scale);
                 }
                 if (p1cnt + s < port1_cap) p1[p1cnt + s] = make_float2(o_r, o_i);
-                if (EPI == EPI_BPSK || EPI == EPI_REAL1) sr[(n_soft + s) & soft_mask] = sb0;
-                else { sr[(n_soft + 2 * s) & soft_mask] = sb0; sr[(n_soft + 2 * s + 1) & soft_mask] = sb1; }
+                if (EPI == EPI_BPSK || EPI == EPI_REAL1) sr[(n_soft + s) & soft_ring.mask] = sb0;
+                else { sr[(n_soft + 2 * s) & soft_ring.mask] = sb0; sr[(n_soft + 2 * s + 1) & soft_ring.mask] = sb1; }
             }
             p1cnt += n; n_soft += ((EPI == EPI_BPSK || EPI == EPI_REAL1) ? 1 : 2) * n; n_sym += n;
             __syncwarp();
@@ -2465,32 +2468,30 @@ struct NbfmParams {
 enum { SQ_MUTED = 0, SQ_ATTACK = 1, SQ_UNMUTED = 2, SQ_DECAY = 3 };
 
 __global__ void __launch_bounds__(128)
-nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
-                  const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long avail_in,
+nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states, Ring<const float2> in, long long avail_in,
                   const float* __restrict__ env_tab,            // sq_ramp + 1 envelope values
-                  float2* __restrict__ gate_ring, unsigned gate_mask, long long gate_stride,
-                  float* __restrict__ dem_ring, unsigned dem_mask, long long dem_stride,
-                  float* __restrict__ res_ring, unsigned res_mask, long long res_stride,
+                  Ring<float2> gate_ring, Ring<float> dem_ring, Ring<float> res_ring,
                   const float* __restrict__ arm_taps,           // [2][nt_arm]
                   const float* __restrict__ audio_taps,
                   float* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap,
                   // NBFM (mode 0) only: when given, the audio filter's output goes to this ring and the de-emphasis runs in
                   // nbfm_deemph_kernel on another stream (its recurrence then overlaps the next slice's squelch recurrence);
                   // aud_snap[c] = audio items produced so far
-                  float* __restrict__ aud_ring = nullptr, unsigned aud_mask = 0, long long aud_stride = 0, long long* __restrict__ aud_snap = nullptr,
+                  Ring<float> aud_ring = {}, long long* __restrict__ aud_snap = nullptr,
                   // NBFM only: the stream between the 2/5 resampler and the audio filter goes through this ring: a plain copy, or
                   // ctcss_squelch_ff (gate: the stream shrinks while the tone is absent) when ct.on (gr_demod_nbfm::set_ctcss)
-                  float* __restrict__ q_ring = nullptr, unsigned q_mask = 0, long long q_stride = 0, NbfmCtcss ct = NbfmCtcss{},
+                  Ring<float> q_ring = {}, NbfmCtcss ct = NbfmCtcss{},
                   const double* __restrict__ c_env_tab = nullptr)
 {
+    float* __restrict__ ar = aud_ring.d;
     const int c = blockIdx.x;
     __shared__ NbfmState st;
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    float2* gr_ = gate_ring + static_cast<long long>(c) * gate_stride;
-    float* dr = dem_ring + static_cast<long long>(c) * dem_stride;
-    float* rr = res_ring + static_cast<long long>(c) * res_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
+    float2* __restrict__ gr_ = gate_ring.d + static_cast<long long>(c) * gate_ring.stride;
+    float* __restrict__ dr = dem_ring.d + static_cast<long long>(c) * dem_ring.stride;
+    float* __restrict__ rr = res_ring.d + static_cast<long long>(c) * res_ring.stride;
     const long long gate0 = st.n_gate;
 
     // ---- 1. squelch (sequential on thread 0; input tiles staged in shared memory by the whole CTA so the
@@ -2510,7 +2511,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
     for (long long tile0 = st.n_in; tile0 < avail_in; tile0 += 2048) {
         const int nt = (avail_in - tile0) < 2048 ? static_cast<int>(avail_in - tile0) : 2048;
         for (int j = threadIdx.x; j < nt; j += blockDim.x) {
-            const float2 v = x[(tile0 + j) & in_mask];
+            const float2 v = __ldg(x + ((tile0 + j) & in.mask));
             xin[j] = v;
             t1s[j] = p.sq_alpha * static_cast<double>(v.x * v.x + v.y * v.y);
         }
@@ -2569,11 +2570,11 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
                         acc = acc + p.b1 * ix1;
                         acc = acc - p.a1 * iy1;
                         ix1 = xin; iy1 = acc;
-                        dr[ng & dem_mask] = static_cast<float>(acc) * p.am_gain;
+                        dr[ng & dem_ring.mask] = static_cast<float>(acc) * p.am_gain;
                         ng++;
                     }
-                } else if (state != SQ_MUTED) { gr_[ng & gate_mask] = make_float2(v.x * env, v.y * env); ng++; }
-                else if (!p.sq_gate) { gr_[ng & gate_mask] = make_float2(0.0f, 0.0f); ng++; }
+                } else if (state != SQ_MUTED) { gr_[ng & gate_ring.mask] = make_float2(v.x * env, v.y * env); ng++; }
+                else if (!p.sq_gate) { gr_[ng & gate_ring.mask] = make_float2(0.0f, 0.0f); ng++; }
             }
             st.pwr = pwr; st.sq_state = state; st.ramped = ramped; st.envelope = env; st.n_gate = ng;
             if (p.mode == 1) { st.agc_gain = agc; st.iir_x1 = ix1; st.iir_y1 = iy1; }
@@ -2584,9 +2585,9 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
             const long long g0 = fast_ng0;
             if (fast_state == SQ_UNMUTED) {
                 const float env = fast_env;
-                for (int j = threadIdx.x; j < n; j += blockDim.x) { const float2 v = xin[j]; gr_[(g0 + j) & gate_mask] = make_float2(v.x * env, v.y * env); }
+                for (int j = threadIdx.x; j < n; j += blockDim.x) { const float2 v = xin[j]; gr_[(g0 + j) & gate_ring.mask] = make_float2(v.x * env, v.y * env); }
             } else if (!p.sq_gate) {
-                for (int j = threadIdx.x; j < n; j += blockDim.x) gr_[(g0 + j) & gate_mask] = make_float2(0.0f, 0.0f);
+                for (int j = threadIdx.x; j < n; j += blockDim.x) gr_[(g0 + j) & gate_ring.mask] = make_float2(0.0f, 0.0f);
             }
         }
         __syncthreads();
@@ -2597,16 +2598,16 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
     const long long gate1 = st.n_gate;
     // ---- 2. quadrature demod over the gated stream (AM: the detector already wrote the 20 ksps stream)
     for (long long n = gate0 + threadIdx.x; n < gate1 && p.mode != 1; n += blockDim.x) {
-        const float2 cur = gr_[n & gate_mask];
+        const float2 cur = gr_[n & gate_ring.mask];
         float2 prev;
         if (n == gate0) prev = make_float2(st.prev_r, st.prev_i);
-        else prev = gr_[(n - 1) & gate_mask];
+        else prev = gr_[(n - 1) & gate_ring.mask];
         const float re = cur.x * prev.x + cur.y * prev.y;
         const float im = cur.y * prev.x - cur.x * prev.y;
-        dr[n & dem_mask] = p.qd_gain * qrl_fast_atan2f(im, re);
+        dr[n & dem_ring.mask] = p.qd_gain * qrl_fast_atan2f(im, re);
     }
     __syncthreads();
-    if (threadIdx.x == 0 && gate1 > gate0 && p.mode != 1) { const float2 l = gr_[(gate1 - 1) & gate_mask]; st.prev_r = l.x; st.prev_i = l.y; }
+    if (threadIdx.x == 0 && gate1 > gate0 && p.mode != 1) { const float2 l = gr_[(gate1 - 1) & gate_ring.mask]; st.prev_r = l.x; st.prev_i = l.y; }
     if (p.mode == 2) {
         // ---- WBFM: x am_gain and de-emphasis IIR over the new demodulated samples (sequential), into the res ring at 200 ksps
         // (tiles through shared memory; b0 x[n] + b1 x[n-1] by all threads, thread 0 keeps the two FP64 operations on the chain)
@@ -2615,7 +2616,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
             double* u = t1s;
             for (long long base = gate0; base < gate1; base += 2048) {
                 const int nb = (gate1 - base) < 2048 ? static_cast<int>(gate1 - base) : 2048;
-                for (int j = threadIdx.x; j < nb; j += blockDim.x) wx[j] = dr[(base + j) & dem_mask] * p.am_gain;
+                for (int j = threadIdx.x; j < nb; j += blockDim.x) wx[j] = dr[(base + j) & dem_ring.mask] * p.am_gain;
                 __syncthreads();
                 const double x1c = st.iir_x1;
                 for (int j = threadIdx.x; j < nb; j += blockDim.x) {
@@ -2632,7 +2633,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
                     st.iir_y1 = y1; st.iir_x1 = static_cast<double>(wx[nb - 1]);
                 }
                 __syncthreads();
-                for (int j = threadIdx.x; j < nb; j += blockDim.x) rr[(base + j) & res_mask] = static_cast<float>(u[j]);
+                for (int j = threadIdx.x; j < nb; j += blockDim.x) rr[(base + j) & res_ring.mask] = static_cast<float>(u[j]);
                 __syncthreads();
             }
         }
@@ -2645,7 +2646,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
             const long long newest = 25 * i;
             const float2 y = qrl_fir_dot_order_c(audio_taps, p.nt_audio, 25, [&](int j) {
                 const long long n = newest - j;
-                return make_float2(n >= 0 ? rr[n & res_mask] : 0.0f, 0.0f);
+                return make_float2(n >= 0 ? rr[n & res_ring.mask] : 0.0f, 0.0f);
             });
             const long long slot = cnt0 + (i - o0);
             if (slot < port1_cap) o[slot] = y.x;
@@ -2668,24 +2669,24 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
         float acc = 0.0f;
         for (int k = p.nt_arm - 1; k >= 0; k--) {
             const long long n = pos - k;
-            const float v = n >= 0 ? dr[n & dem_mask] : 0.0f;
+            const float v = n >= 0 ? dr[n & dem_ring.mask] : 0.0f;
             acc = fmaf(h[k], v, acc);
         }
-        rr[i & res_mask] = acc;
+        rr[i & res_ring.mask] = acc;
     }
     __syncthreads();
     // ---- 3b. NBFM: copy, or tone squelch, into the audio filter's input ring
-    float* qr = q_ring ? q_ring + static_cast<long long>(c) * q_stride : nullptr;
+    float* __restrict__ qr = q_ring.d ? q_ring.d + static_cast<long long>(c) * q_ring.stride : nullptr;
     if (qr) {
         const long long q0 = st.n_q;
         if (!ct.on) {
-            for (long long i = res0 + threadIdx.x; i < res1; i += blockDim.x) qr[(q0 + (i - res0)) & q_mask] = rr[i & res_mask];
+            for (long long i = res0 + threadIdx.x; i < res1; i += blockDim.x) qr[(q0 + (i - res0)) & q_ring.mask] = rr[i & res_ring.mask];
             __syncthreads();
             if (threadIdx.x == 0) st.n_q = q0 + (res1 - res0);
         } else {
             for (long long base = res0; base < res1; base += 2048) {
                 const int nb = (res1 - base) < 2048 ? static_cast<int>(res1 - base) : 2048;
-                for (int j = threadIdx.x; j < nb; j += blockDim.x) aud[j] = rr[(base + j) & res_mask];
+                for (int j = threadIdx.x; j < nb; j += blockDim.x) aud[j] = rr[(base + j) & res_ring.mask];
                 __syncthreads();
                 if (threadIdx.x == 0) {
                     float gl1 = st.gl1, gl2 = st.gl2, gc1 = st.gc1, gc2 = st.gc2, gr1 = st.gr1, gr2 = st.gr2;
@@ -2714,8 +2715,8 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
                         case SQ_ATTACK: env = c_env_tab[++ramped]; if (ramped >= ct.ramp) { state = SQ_UNMUTED; env = 1.0; } break;
                         case SQ_DECAY: env = c_env_tab[--ramped]; if (ramped == 0) state = SQ_MUTED; break;
                         }
-                        if (state != SQ_MUTED) { qr[nq & q_mask] = static_cast<float>(static_cast<double>(xv) * env); nq++; }
-                        else if (!ct.gate) { qr[nq & q_mask] = 0.0f; nq++; }
+                        if (state != SQ_MUTED) { qr[nq & q_ring.mask] = static_cast<float>(static_cast<double>(xv) * env); nq++; }
+                        else if (!ct.gate) { qr[nq & q_ring.mask] = 0.0f; nq++; }
                     }
                     st.gl1 = gl1; st.gl2 = gl2; st.gc1 = gc1; st.gc2 = gc2; st.gr1 = gr1; st.gr2 = gr2;
                     st.g_processed = proc; st.c_mute = mute; st.c_state = state; st.c_ramped = ramped; st.c_env = env; st.n_q = nq;
@@ -2727,7 +2728,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
     }
     // ---- 4. audio low-pass (direct form), into shared staging for the IIR
     const float* fsrc = qr ? qr : rr;                               // the filter's input stream and its length so far
-    const unsigned fmask = qr ? q_mask : res_mask;
+    const unsigned fmask = qr ? q_ring.mask : res_ring.mask;
     const long long fend = qr ? st.n_q : res1;
     const long long aud0 = st.n_aud;
     const int n_aud = static_cast<int>(fend - aud0);                // one output per input item
@@ -2742,11 +2743,11 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
                 acc = fmaf(audio_taps[k], v, acc);
             }
             aud[j] = acc;
-            if (aud_ring && p.mode == 0) aud_ring[static_cast<long long>(c) * aud_stride + (a & aud_mask)] = acc;
+            if (ar && p.mode == 0) ar[static_cast<long long>(c) * aud_ring.stride + (a & aud_ring.mask)] = acc;
         }
         __syncthreads();
         // ---- 5. de-emphasis IIR (double) + output gain (sequential)
-        if (aud_ring && p.mode == 0) {
+        if (ar && p.mode == 0) {
             // split form: nbfm_deemph_kernel does it
         } else if (p.mode == 1) {
             const int cnt0 = port1_cnt[c];
@@ -2790,7 +2791,7 @@ nbfm_audio_kernel(NbfmParams p, NbfmState* __restrict__ states,
 struct NbfmDeemphState { double iir_x1, iir_y1; long long n_done; };
 __global__ void __launch_bounds__(128)
 nbfm_deemph_kernel(double b0, double b1, double a1, float out_gain, NbfmDeemphState* __restrict__ states,
-                   const float* __restrict__ aud_ring, unsigned aud_mask, long long aud_stride, const long long* __restrict__ aud_snap,
+                   Ring<const float> aud_ring, const long long* __restrict__ aud_snap,
                    float* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap)
 {
     const int c = blockIdx.x;
@@ -2800,11 +2801,11 @@ nbfm_deemph_kernel(double b0, double b1, double a1, float out_gain, NbfmDeemphSt
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
     const long long a0 = st.n_done, a1n = aud_snap[c];
-    const float* ar = aud_ring + static_cast<long long>(c) * aud_stride;
+    const float* __restrict__ ar = aud_ring.d + static_cast<long long>(c) * aud_ring.stride;
     float* o = port1 + static_cast<long long>(c) * port1_stride;
     for (long long base = a0; base < a1n; base += 2048) {
         const int nb = (a1n - base) < 2048 ? static_cast<int>(a1n - base) : 2048;
-        for (int j = threadIdx.x; j < nb; j += blockDim.x) aud[j] = ar[(base + j) & aud_mask];
+        for (int j = threadIdx.x; j < nb; j += blockDim.x) aud[j] = ar[(base + j) & aud_ring.mask];
         __syncthreads();
         const double x1c = st.iir_x1;
         for (int j = threadIdx.x; j < nb; j += blockDim.x) {
@@ -2831,28 +2832,28 @@ nbfm_deemph_kernel(double b0, double b1, double a1, float out_gain, NbfmDeemphSt
 }
 
 // complex stream, COMPLEX taps (fft_filter_ccc restated in direct form), optional input gain (multiply_const_cc in front)
-__global__ void fir_ccc_ring_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                                    float2* __restrict__ out, unsigned out_mask, long long out_stride,
+__global__ void fir_ccc_ring_kernel(Ring<const float2> in, Ring<float2> out,
                                     const float* __restrict__ taps_c /* interleaved */, int ntaps, float in_gain,
                                     long long a0, long long a1, float2* __restrict__ lin, long long lin_stride, long long lin_base)
 {
+    float2* __restrict__ y_out = out.d;
     extern __shared__ float hs_dyn[];
     for (int i = threadIdx.x; i < 2 * ntaps; i += blockDim.x) hs_dyn[i] = taps_c[i];
     __syncthreads();
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     float re = 0.0f, im = 0.0f;
     for (int j = ntaps - 1; j >= 0; j--) {
-        float2 v = x[(a - j) & in_mask];
+        float2 v = x[(a - j) & in.mask];
         v.x = v.x * in_gain; v.y = v.y * in_gain;
         const float hr = hs_dyn[2 * j], hi = hs_dyn[2 * j + 1];
         re = fmaf(hr, v.x, re); re = fmaf(-hi, v.y, re);
         im = fmaf(hr, v.y, im); im = fmaf(hi, v.x, im);
     }
     const float2 y = make_float2(re, im);
-    out[static_cast<long long>(c) * out_stride + (a & out_mask)] = y;
+    y_out[static_cast<long long>(c) * out.stride + (a & out.mask)] = y;
     if (lin) lin[static_cast<long long>(c) * lin_stride + (a - lin_base)] = y;
 }
 
@@ -2873,27 +2874,24 @@ struct SsbParams {
 };
 
 __global__ void __launch_bounds__(128)
-ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
-                 const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long avail_in,
-                 float2* __restrict__ clip_ring, unsigned clip_mask, long long clip_stride,
-                 float* __restrict__ str_ring, unsigned str_mask, long long str_stride,
-                 const float* __restrict__ audio_taps,
+ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states, Ring<const float2> in, long long avail_in, Ring<float2> clip_ring,
+                 Ring<float> str_ring, const float* __restrict__ audio_taps,
                  float* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap)
 {
     const int c = blockIdx.x;
     __shared__ SsbState st;
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    float2* cr = clip_ring + static_cast<long long>(c) * clip_stride;
-    float* sr = str_ring + static_cast<long long>(c) * str_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
+    float2* __restrict__ cr = clip_ring.d + static_cast<long long>(c) * clip_ring.stride;
+    float* __restrict__ sr = str_ring.d + static_cast<long long>(c) * str_ring.stride;
     const long long gate0 = st.n_gate;
     __syncthreads();      // every thread holds its copy of gate0 before thread 0 advances st.n_gate at the end of step 1
     // ---- 1. squelch + AGC (sequential); the AGC output is parked in the clip ring, clipped in place in step 2
     if (threadIdx.x == 0) {
         double pwr = st.pwr; int state = st.sq_state; float gain = st.gain; long long ng = st.n_gate;
         for (long long a = st.n_in; a < avail_in; a++) {
-            const float2 v = x[a & in_mask];
+            const float2 v = x[a & in.mask];
             const float mag2 = v.x * v.x + v.y * v.y;
             pwr = p.sq_alpha * static_cast<double>(mag2) + (1.0 - p.sq_alpha) * pwr;
             const bool mute = pwr < p.sq_threshold;
@@ -2906,7 +2904,7 @@ ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
                 gain = gain - tmp * rate;
                 if (gain < 0.0f) gain = 10e-5f;
                 if (p.max_gain > 0.0f && gain > p.max_gain) gain = p.max_gain;
-                cr[ng & clip_mask] = make_float2(orr, oi);
+                cr[ng & clip_ring.mask] = make_float2(orr, oi);
                 ng++;
             }
         }
@@ -2916,13 +2914,13 @@ ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
     const long long gate1 = st.n_gate;
     // ---- 2. clipper: magnitude limited to `clip`, phase kept (fast_atan2f + sincos)
     for (long long n = gate0 + threadIdx.x; n < gate1; n += blockDim.x) {
-        const float2 v = cr[n & clip_mask];
+        const float2 v = cr[n & clip_ring.mask];
         const float mag = sqrtf(v.x * v.x + v.y * v.y);
         const float ph = qrl_fast_atan2f(v.y, v.x);
         const float cl = mag < p.clip ? mag : p.clip;
         float sn, cs;
         qrl_sincosf(ph, sn, cs);
-        cr[n & clip_mask] = make_float2(cs * cl, sn * cl);
+        cr[n & clip_ring.mask] = make_float2(cs * cl, sn * cl);
     }
     __syncthreads();
     // ---- 3. stretcher: gain from the 5-point envelope maximum around n (needs n+2), real part x out_gain
@@ -2931,14 +2929,14 @@ ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
     for (long long n = str0 + threadIdx.x; n < str1; n += blockDim.x) {
         auto env = [&](long long k) -> float {
             if (k < 0) return 0.0f;
-            const float2 v = cr[k & clip_mask];
+            const float2 v = cr[k & clip_ring.mask];
             return sqrtf(v.x * v.x + v.y * v.y);
         };
         float h = env(n);
         h = fmaxf(h, env(n - 2)); h = fmaxf(h, env(n - 1)); h = fmaxf(h, env(n + 1)); h = fmaxf(h, env(n + 2));
         h = h * p.emax; h = fmaxf(h, 1.0f); h = h - 1.0f; h = h * 2.0f; h = h + 1.0f;
-        const float re = cr[n & clip_mask].x / h;
-        sr[n & str_mask] = re * p.out_gain;
+        const float re = cr[n & clip_ring.mask].x / h;
+        sr[n & str_ring.mask] = re * p.out_gain;
     }
     __syncthreads();
     // ---- 4. audio band-pass (direct form), one output per stretcher output
@@ -2950,7 +2948,7 @@ ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
         float acc = 0.0f;
         for (int k = p.nt_audio - 1; k >= 0; k--) {
             const long long n = a - k;
-            const float v = n >= 0 ? sr[n & str_mask] : 0.0f;
+            const float v = n >= 0 ? sr[n & str_ring.mask] : 0.0f;
             acc = fmaf(audio_taps[k], v, acc);
         }
         const long long idx = cnt0 + (a - aud0);
@@ -2972,24 +2970,25 @@ ssb_audio_kernel(SsbParams p, SsbState* __restrict__ states,
 // one thread per sample, channel-major rings.
 // ------------------------------------------------------------------------------------------------
 template <int NB>
-__global__ void fsk_bank_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
+__global__ void fsk_bank_kernel(Ring<const float2> in,
                                 const float* __restrict__ taps_c /* [NB][2*ntaps] */, int ntaps, long long a0, long long a1,
-                                float* __restrict__ out /* float2 ring (NB=4) or float ring (NB=2) */, unsigned out_mask, long long out_stride)
+                                Ring<float> out /* float2 ring (NB=4) or float ring (NB=2) */)
 {
+    float* __restrict__ y_out = out.d;
     extern __shared__ float hs_dyn[];
     for (int i = threadIdx.x; i < NB * 2 * ntaps; i += blockDim.x) hs_dyn[i] = taps_c[i];
     __syncthreads();
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     float m[NB];
 #pragma unroll
     for (int b = 0; b < NB; b++) {
         const float* h = hs_dyn + b * 2 * ntaps;
         float re = 0.0f, im = 0.0f;
         for (int j = ntaps - 1; j >= 0; j--) {
-            const float2 v = x[(a - j) & in_mask];
+            const float2 v = x[(a - j) & in.mask];
             re = fmaf(h[2 * j], v.x, re); re = fmaf(-h[2 * j + 1], v.y, re);
             im = fmaf(h[2 * j], v.y, im); im = fmaf(h[2 * j + 1], v.x, im);
         }
@@ -3002,29 +3001,29 @@ __global__ void fsk_bank_kernel(const float2* __restrict__ in, unsigned in_mask,
         else if ((m[1] > m[0]) && (m[1] > m[2]) && (m[1] > m[3])) { orr = N; oi = P; }
         else if ((m[2] > m[1]) && (m[2] > m[0]) && (m[2] > m[3])) { orr = P; oi = P; }
         else if ((m[3] > m[1]) && (m[3] > m[0]) && (m[3] > m[2])) { orr = P; oi = N; }
-        reinterpret_cast<float2*>(out)[static_cast<long long>(c) * out_stride + (a & out_mask)] = make_float2(orr, oi);
+        reinterpret_cast<float2*>(y_out)[static_cast<long long>(c) * out.stride + (a & out.mask)] = make_float2(orr, oi);
     } else {
         const float q = m[0] / m[1];
         const float t = fmaxf(fminf(q, 2.0f), 0.0f);          // NaN (0/0 at start-up) -> the rail, like the oracle
-        out[static_cast<long long>(c) * out_stride + (a & out_mask)] = t + -1.0f;
+        y_out[static_cast<long long>(c) * out.stride + (a & out.mask)] = t + -1.0f;
     }
 }
 
 // float stream, real taps (fft_filter_fff direct form): channel-major ring in, channel-interleaved ring out
-__global__ void fir_fff_ring_kernel(const float* __restrict__ in, unsigned in_mask, long long in_stride,
-                                    float* __restrict__ out, unsigned out_mask, long long out_stride,
+__global__ void fir_fff_ring_kernel(Ring<const float> in, Ring<float> out,
                                     const float* __restrict__ taps, int ntaps, long long a0, long long a1)
 {
+    float* __restrict__ y_out = out.d;
     extern __shared__ float hs_dyn[];
     for (int i = threadIdx.x; i < ntaps; i += blockDim.x) hs_dyn[i] = taps[i];
     __syncthreads();
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
-    const float* x = in + static_cast<long long>(c) * in_stride;
+    const float* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     float acc = 0.0f;
-    for (int j = ntaps - 1; j >= 0; j--) acc = fmaf(hs_dyn[j], x[(a - j) & in_mask], acc);
-    out[(static_cast<long long>(c >> 5) * out_stride + (a & out_mask)) * 32 + (c & 31)] = acc;
+    for (int j = ntaps - 1; j >= 0; j--) acc = fmaf(hs_dyn[j], x[(a - j) & in.mask], acc);
+    y_out[(static_cast<long long>(c >> 5) * out.stride + (a & out.mask)) * 32 + (c & 31)] = acc;
 }
 
 // Front-end rotator (gr_demod_base's rotator_cc, carrier offset) as a pass of its own: out[c][n] = qrl_rotate(rs[c], n_abs0 + n,
@@ -3450,8 +3449,9 @@ enum { TXM_4FSK = 0, TXM_QPSK = 1, TXM_BPSK = 2, TXM_2FSK = 3, TXM_M17 = 4, TXM_
 // map {2,3,1,0} -> chunks_to_symbols {-1.5 .. 1.5}: 4 symbols per input byte
 template <int MODE>
 __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const unsigned char* __restrict__ bytes, long long n, long long stride,
-                               float* __restrict__ sym_ring /* float or float2 */, unsigned sym_mask, long long sym_stride, long long sym0)
+                               Ring<float> sym_ring /* float or float2 */, long long sym0)
 {
+    float* __restrict__ sym = sym_ring.d;
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     TxBitState st = states[c];
@@ -3464,7 +3464,7 @@ __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const uns
             for (int k = 3; k >= 0; k--) {
                 const unsigned dibit = (byte >> (2 * k)) & 3u;
                 const unsigned chunk = (0x1Eu >> (2 * dibit)) & 3u;           // map {2,3,1,0}, two bits per entry
-                sym_ring[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = -1.5f + static_cast<float>(chunk);
+                sym[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = -1.5f + static_cast<float>(chunk);
                 si++;
             }
             continue;
@@ -3485,7 +3485,7 @@ __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const uns
 #pragma unroll
                 for (int q = 0; q < 13; q++) {
                     const unsigned chip = ((0x1F35u >> (12 - q)) & 1u) ^ bit;      // {1,1,1,1,1,0,0,1,1,0,1,0,1}, first chip = MSB
-                    reinterpret_cast<float2*>(sym_ring)[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = make_float2(chip ? 1.0f : -1.0f, 0.0f);
+                    reinterpret_cast<float2*>(sym)[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = make_float2(chip ? 1.0f : -1.0f, 0.0f);
                     si++;
                 }
             }
@@ -3496,8 +3496,8 @@ __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const uns
 #pragma unroll
             for (int k = 15; k >= 0; k--) {
                 const float lv = ((coded >> k) & 1u) ? 1.0f : -1.0f;
-                if (MODE == TXM_BPSK) reinterpret_cast<float2*>(sym_ring)[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = make_float2(lv, 0.0f);
-                else sym_ring[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = lv;
+                if (MODE == TXM_BPSK) reinterpret_cast<float2*>(sym)[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = make_float2(lv, 0.0f);
+                else sym[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = lv;
                 si++;
             }
             continue;
@@ -3510,9 +3510,9 @@ __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const uns
                 st.diff_prev = (chunk + st.diff_prev) & 3u;
                 const float qr = (st.diff_prev >= 2u) ? 0.707f : -0.707f;
                 const float qi = (st.diff_prev == 1u || st.diff_prev == 2u) ? 0.707f : -0.707f;
-                reinterpret_cast<float2*>(sym_ring)[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = make_float2(qr, qi);
+                reinterpret_cast<float2*>(sym)[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = make_float2(qr, qi);
             } else {
-                sym_ring[static_cast<long long>(c) * sym_stride + (si & sym_mask)] = -1.5f + static_cast<float>(chunk);
+                sym[static_cast<long long>(c) * sym_ring.stride + (si & sym_ring.mask)] = -1.5f + static_cast<float>(chunk);
             }
             si++;
         }
@@ -3526,14 +3526,13 @@ __global__ void tx_bits_kernel(TxBitState* __restrict__ states, int C, const uns
 // per-channel phase is a prefix sum: one CTA per channel scans its samples block by block.
 template <int NTHREADS, int ITEMS>
 __global__ void __launch_bounds__(NTHREADS)
-tx_shape_fm_kernel(TxBitState* __restrict__ states, const float* __restrict__ sym_ring, unsigned sym_mask, long long sym_stride,
+tx_shape_fm_kernel(TxBitState* __restrict__ states, Ring<const float> sym_ring,
                    long long sym0, long long nsym, int L, int nt_arm, const float* __restrict__ arms /* [L][nt_arm] */, int repeat_only,
-                   float pulse_scale, float fm_sens, float amplif, float bb_gain,
-                   float2* __restrict__ if_ring, unsigned if_mask, long long if_stride)
+                   float pulse_scale, float fm_sens, float amplif, float bb_gain, Ring<float2> if_ring)
 {
     const int c = blockIdx.x;
-    const float* sy = sym_ring + static_cast<long long>(c) * sym_stride;
-    float2* o = if_ring + static_cast<long long>(c) * if_stride;
+    const float* __restrict__ sy = sym_ring.d + static_cast<long long>(c) * sym_ring.stride;
+    float2* __restrict__ o = if_ring.d + static_cast<long long>(c) * if_ring.stride;
     __shared__ unsigned warp_sums[NTHREADS / 32];
     __shared__ unsigned carry;
     if (threadIdx.x == 0) carry = states[c].phase_q;
@@ -3550,11 +3549,11 @@ tx_shape_fm_kernel(TxBitState* __restrict__ states, const float* __restrict__ sy
             if (a < n1) {
                 const long long m = a / L; const int ph = static_cast<int>(a - m * L);
                 float x;
-                if (repeat_only) x = sy[m & sym_mask];
+                if (repeat_only) x = sy[m & sym_ring.mask];
                 else {
                     const float* h = arms + ph * nt_arm;
                     float acc = 0.0f;
-                    for (int k = nt_arm - 1; k >= 0; k--) acc = fmaf(h[k], sy[(m - k) & sym_mask], acc);
+                    for (int k = nt_arm - 1; k >= 0; k--) acc = fmaf(h[k], sy[(m - k) & sym_ring.mask], acc);
                     x = acc * pulse_scale;
                 }
                 const float finc = fm_sens * x;
@@ -3587,7 +3586,7 @@ tx_shape_fm_kernel(TxBitState* __restrict__ states, const float* __restrict__ sy
                 const float cs = d_sine_tab[2 * ci] * static_cast<float>(uc >> 1) + d_sine_tab[2 * ci + 1];
                 float re = cs * amplif, im = sn * amplif;
                 re = re * bb_gain; im = im * bb_gain;
-                o[a & if_mask] = make_float2(re, im);
+                o[a & if_ring.mask] = make_float2(re, im);
             }
         }
         __syncthreads();
@@ -3602,7 +3601,7 @@ tx_shape_fm_kernel(TxBitState* __restrict__ states, const float* __restrict__ sy
 // (one shared-memory load per m), 2 NT FFMA per output sample; L*MB threads keep every lane busy.
 template <int L, int NT, int MB, int MLEN>
 __global__ void __launch_bounds__(L * MB)
-interp_fir_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride, long long m0, long long m1,
+interp_fir_ccf_kernel(Ring<const float2> in_ring, long long m0, long long m1,
                       const float* __restrict__ arms /* [L][NT] */, float post_gain1, float post_gain2, int apply_gain,
                       float2* __restrict__ out, long long out_stride, long long out_base /* absolute output index of out[c][0] */)
 {
@@ -3611,10 +3610,10 @@ interp_fir_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long
     const int c = blockIdx.y;
     const long long tile0 = m0 + static_cast<long long>(blockIdx.x) * (MB * MLEN);
     if (tile0 >= m1) return;
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     for (int i = threadIdx.x; i < MB * MLEN + NT - 1; i += L * MB) {
         const long long m = tile0 - (NT - 1) + i;
-        xs[i] = (m < m1) ? x[m & in_mask] : make_float2(0.0f, 0.0f);
+        xs[i] = (m < m1) ? x[m & in_ring.mask] : make_float2(0.0f, 0.0f);
     }
     __syncthreads();
     const int p = threadIdx.x % L, mb = threadIdx.x / L;
@@ -3649,7 +3648,7 @@ interp_fir_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long
 // for the LSU -- and keeping the taps resident across tiles costs an occupancy step (64 registers); the one-tile form below stays)
 template <int L, int NT, int R, int G>
 __global__ void __launch_bounds__(L * G)
-interp_fir_ccf_rt_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride, long long m0, long long m1,
+interp_fir_ccf_rt_kernel(Ring<const float2> in_ring, long long m0, long long m1,
                          const float* __restrict__ arms /* [L][NT] */, float post_gain1, float post_gain2, int apply_gain,
                          float2* __restrict__ out, long long out_stride, long long out_base)
 {
@@ -3658,10 +3657,10 @@ interp_fir_ccf_rt_kernel(const float2* __restrict__ in_ring, unsigned in_mask, l
     const int c = blockIdx.y;
     const long long tile0 = m0 + static_cast<long long>(blockIdx.x) * TM;
     if (tile0 >= m1) return;
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     for (int i = threadIdx.x; i < TM + NT - 1; i += L * G) {
         const long long m = tile0 - (NT - 1) + i;
-        xs[i] = (m < m1) ? x[m & in_mask] : make_float2(0.0f, 0.0f);
+        xs[i] = (m < m1) ? x[m & in_ring.mask] : make_float2(0.0f, 0.0f);
     }
     __syncthreads();
     const int p = threadIdx.x % L, q = threadIdx.x / L;
@@ -3694,7 +3693,7 @@ interp_fir_ccf_rt_kernel(const float2* __restrict__ in_ring, unsigned in_mask, l
 // Shape-generic interpolating FIR (any L, NT): one thread per output sample, arm taps and the input window in shared
 // memory.  Used for the TX shapes that have no register-tiled instance (QPSK x100/x500, BPSK x250/x500, 2FSK x10 ...).
 __global__ void __launch_bounds__(256)
-interp_fir_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride, long long m0, long long m1,
+interp_fir_ccf_generic_kernel(Ring<const float2> in_ring, long long m0, long long m1,
                               const float* __restrict__ arms /* [L][NT] */, int L, int NT, int MT /* m per CTA */,
                               float post_gain1, float post_gain2, int apply_gain,
                               float2* __restrict__ out, long long out_stride, long long out_base)
@@ -3706,10 +3705,10 @@ interp_fir_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_ma
     const long long tile0 = m0 + static_cast<long long>(blockIdx.x) * MT;
     if (tile0 >= m1) return;
     for (int i = threadIdx.x; i < L * NT; i += 256) hs[i] = arms[i];
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     for (int i = threadIdx.x; i < MT + NT - 1; i += 256) {
         const long long m = tile0 - (NT - 1) + i;
-        xs[i] = (m < m1) ? x[m & in_mask] : make_float2(0.0f, 0.0f);
+        xs[i] = (m < m1) ? x[m & in_ring.mask] : make_float2(0.0f, 0.0f);
     }
     __syncthreads();
     float2* oc = out + static_cast<long long>(c) * out_stride;
@@ -3731,7 +3730,7 @@ interp_fir_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_ma
 // output i takes arm (i M) mod L at ring position floor(i M / L), arms[p][k] = taps[p + k L], plain oldest-first accumulation (the
 // oracle's order for L > 1).  One thread per output sample, the arm table in shared memory; consecutive outputs share their inputs.
 __global__ void __launch_bounds__(256)
-resamp_ring_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride,
+resamp_ring_ccf_generic_kernel(Ring<const float2> in_ring,
                                const float* __restrict__ arms /* [L][NT] */, int L, int M, int NT, long long o0, long long o1,
                                float2* __restrict__ out, long long out_stride)
 {
@@ -3744,10 +3743,10 @@ resamp_ring_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_m
     const long long im = i * M;
     const long long newest = im / L;                                      // absolute index of the newest input sample
     const float* h = sm_rr + static_cast<int>(im - newest * L) * NT;
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     float re = 0.0f, imv = 0.0f;
     for (int k = NT - 1; k >= 0; k--) {
-        const float2 v = x[(newest - k) & in_mask];                       // before the first sample: the zero-initialised top of the ring
+        const float2 v = x[(newest - k) & in_ring.mask];                       // before the first sample: the zero-initialised top of the ring
         re = fmaf(h[k], v.x, re); imv = fmaf(h[k], v.y, imv);
     }
     out[static_cast<long long>(c) * out_stride + (i - o0)] = make_float2(re, imv);
@@ -3756,10 +3755,11 @@ resamp_ring_ccf_generic_kernel(const float2* __restrict__ in_ring, unsigned in_m
 // the same resampler writing a ring (a later stage needs the history across calls), with the two multiply_const_cc gains behind it
 // when apply_gain is set (gr_mod_dsss.cpp:83-86: x25 pulse shaping -> x0.65 -> x bb_gain -> x50 / 13)
 __global__ void __launch_bounds__(256)
-resamp_ring_to_ring_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride,
+resamp_ring_to_ring_ccf_kernel(Ring<const float2> in_ring,
                                const float* __restrict__ arms /* [L][NT] */, int L, int M, int NT, long long o0, long long o1,
-                               float g1, float g2, int apply_gain, float2* __restrict__ out_ring, unsigned out_mask, long long out_stride)
+                               float g1, float g2, int apply_gain, Ring<float2> out_ring)
 {
+    float2* __restrict__ y_out = out_ring.d;
     extern __shared__ float sm_r2r[];
     for (int i = threadIdx.x; i < L * NT; i += 256) sm_r2r[i] = arms[i];
     __syncthreads();
@@ -3769,15 +3769,15 @@ resamp_ring_to_ring_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_m
     const long long im = i * M;
     const long long newest = im / L;
     const float* h = sm_r2r + static_cast<int>(im - newest * L) * NT;
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     float re = 0.0f, imv = 0.0f;
     for (int k = NT - 1; k >= 0; k--) {
         const long long a = newest - k;
-        const float2 v = a >= 0 ? x[a & in_mask] : make_float2(0.0f, 0.0f);
+        const float2 v = a >= 0 ? x[a & in_ring.mask] : make_float2(0.0f, 0.0f);
         re = fmaf(h[k], v.x, re); imv = fmaf(h[k], v.y, imv);
     }
     if (apply_gain) { re = re * g1; imv = imv * g1; re = re * g2; imv = imv * g2; }
-    out_ring[static_cast<long long>(c) * out_stride + (i & out_mask)] = make_float2(re, imv);
+    y_out[static_cast<long long>(c) * out_ring.stride + (i & out_ring.mask)] = make_float2(re, imv);
 }
 
 // Tiled form of resamp_ring_to_ring_ccf_kernel for M >= L (a decimating rational resampler, gr_demod_mmdvm_multi2's 24 / 25): a CTA takes
@@ -3786,10 +3786,11 @@ resamp_ring_to_ring_ccf_kernel(const float2* __restrict__ in_ring, unsigned in_m
 // per tap).  Same taps, same order (oldest first) as the generic kernel: bit-identical.
 template <int NT>
 __global__ void __launch_bounds__(256)
-resamp_ring_to_ring_tiled_kernel(const float2* __restrict__ in_ring, unsigned in_mask, long long in_stride,
+resamp_ring_to_ring_tiled_kernel(Ring<const float2> in_ring,
                                  const float* __restrict__ arms /* [L][NT] */, int L, int M, long long o0, long long o1,
-                                 float2* __restrict__ out_ring, unsigned out_mask, long long out_stride, int span_cap)
+                                 Ring<float2> out_ring, int span_cap)
 {
+    float2* __restrict__ y_out = out_ring.d;
     extern __shared__ float sm_rt[];
     float* hs = sm_rt;                                               // L * NT
     float2* xs = reinterpret_cast<float2*>(sm_rt + ((L * NT + 1) & ~1));
@@ -3800,10 +3801,10 @@ resamp_ring_to_ring_tiled_kernel(const float2* __restrict__ in_ring, unsigned in
     const long long first = (ob * M) / L - (NT - 1), last = ((oe - 1) * M) / L;      // input span of this CTA
     const int span = static_cast<int>(last - first + 1);
     for (int i = threadIdx.x; i < L * NT; i += 256) hs[i] = arms[i];
-    const float2* x = in_ring + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in_ring.d + static_cast<long long>(c) * in_ring.stride;
     for (int i = threadIdx.x; i < span && i < span_cap; i += 256) {
         const long long a = first + i;
-        xs[i] = a >= 0 ? x[a & in_mask] : make_float2(0.0f, 0.0f);
+        xs[i] = a >= 0 ? x[a & in_ring.mask] : make_float2(0.0f, 0.0f);
     }
     __syncthreads();
     const long long o = ob + threadIdx.x;
@@ -3814,7 +3815,7 @@ resamp_ring_to_ring_tiled_kernel(const float2* __restrict__ in_ring, unsigned in
     float re = 0.0f, imv = 0.0f;
 #pragma unroll
     for (int k = NT - 1; k >= 0; k--) { const float2 v = w[-k]; re = fmaf(h[k], v.x, re); imv = fmaf(h[k], v.y, imv); }
-    out_ring[static_cast<long long>(c) * out_stride + (o & out_mask)] = make_float2(re, imv);
+    y_out[static_cast<long long>(c) * out_ring.stride + (o & out_ring.mask)] = make_float2(re, imv);
 }
 
 // ================================================================================================
@@ -3826,26 +3827,26 @@ struct TxAnalogState { long long n_in, n_rs, n_str; double iir_x1, iir_y1; float
 // NBFM: audio LPF -> x0.99 -> pre-emphasis IIR (double) -> rational_resampler_fff(25,4) -> float ring (FM input)
 __global__ void __launch_bounds__(128)
 tx_nbfm_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict__ audio, long long n, long long a_stride,
-                     float* __restrict__ ra, unsigned ra_mask, long long ra_stride,      // audio ring
-                     float* __restrict__ rb, unsigned rb_mask, long long rb_stride,      // filtered + pre-emphasised
+                     Ring<float> ra,      // audio ring
+                     Ring<float> rb,      // filtered + pre-emphasised
                      const float* __restrict__ lpf, int nt_lpf, double b0, double b1, double a1,
                      const float* __restrict__ arms /* [25][nt_arm] */, int nt_arm,
-                     float* __restrict__ rs_out, unsigned rs_mask, long long rs_stride,
+                     Ring<float> rs_out,
                      float audio_gain, int tone_on, unsigned tone_phase0, unsigned tone_inc)      // gr_mod_nbfm::set_ctcss: gain + CTCSS tone
 {
     const int c = blockIdx.x;
     __shared__ TxAnalogState st;
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
-    float* A = ra + static_cast<long long>(c) * ra_stride;
-    float* B = rb + static_cast<long long>(c) * rb_stride;
-    float* R = rs_out + static_cast<long long>(c) * rs_stride;
+    float* __restrict__ A = ra.d + static_cast<long long>(c) * ra.stride;
+    float* __restrict__ B = rb.d + static_cast<long long>(c) * rb.stride;
+    float* __restrict__ R = rs_out.d + static_cast<long long>(c) * rs_out.stride;
     const long long a0 = st.n_in, a1n = st.n_in + n;
-    for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) A[a & ra_mask] = audio[static_cast<long long>(c) * a_stride + (a - a0)];
+    for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) A[a & ra.mask] = audio[static_cast<long long>(c) * a_stride + (a - a0)];
     __syncthreads();
     for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) {
         float acc = 0.0f;
-        for (int k = nt_lpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(lpf[k], m >= 0 ? A[m & ra_mask] : 0.0f, acc); }
+        for (int k = nt_lpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(lpf[k], m >= 0 ? A[m & ra.mask] : 0.0f, acc); }
         float v = acc * audio_gain;                                   // multiply_const_ff(0.99 / 0.98 / 0.85)
         if (tone_on) {
             // add_ff with sig_source_f(8000, cos, f, 0.15) = fxpt_nco: (float)(fxpt::cos(phase) * 0.15); phase of this call's sample j
@@ -3855,18 +3856,18 @@ tx_nbfm_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict
             const float cs = d_sine_tab[2 * ci] * static_cast<float>(uc >> 1) + d_sine_tab[2 * ci + 1];
             v = v + static_cast<float>(static_cast<double>(cs) * 0.15);
         }
-        B[a & rb_mask] = v;
+        B[a & rb.mask] = v;
     }
     __syncthreads();
     if (threadIdx.x == 0) {
         double x1 = st.iir_x1, y1 = st.iir_y1;
         for (long long a = a0; a < a1n; a++) {
-            const double xin = static_cast<double>(B[a & rb_mask]);
+            const double xin = static_cast<double>(B[a & rb.mask]);
             double acc = b0 * xin;
             acc = acc + b1 * x1;
             acc = acc - a1 * y1;
             x1 = xin; y1 = acc;
-            B[a & rb_mask] = static_cast<float>(acc);
+            B[a & rb.mask] = static_cast<float>(acc);
         }
         st.iir_x1 = x1; st.iir_y1 = y1;
     }
@@ -3877,8 +3878,8 @@ tx_nbfm_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict
         const long long pos = (4 * i) / 25;
         const float* h = arms + static_cast<int>((4 * i) % 25) * nt_arm;
         float acc = 0.0f;
-        for (int k = nt_arm - 1; k >= 0; k--) { const long long m = pos - k; acc = fmaf(h[k], m >= 0 ? B[m & rb_mask] : 0.0f, acc); }
-        R[i & rs_mask] = acc;
+        for (int k = nt_arm - 1; k >= 0; k--) { const long long m = pos - k; acc = fmaf(h[k], m >= 0 ? B[m & rb.mask] : 0.0f, acc); }
+        R[i & rs_out.mask] = acc;
     }
     __syncthreads();
     if (threadIdx.x == 0) { st.n_in = a1n; st.n_rs = r1; states[c] = st; }
@@ -3886,41 +3887,38 @@ tx_nbfm_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict
 
 // SSB: audio band-pass -> float_to_complex -> cessb::clipper_cc(0.95) -> cessb::stretcher_cc -> complex ring
 __global__ void __launch_bounds__(128)
-tx_ssb_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict__ audio, long long n, long long a_stride,
-                    float* __restrict__ ra, unsigned ra_mask, long long ra_stride,
-                    float2* __restrict__ rclip, unsigned rc_mask, long long rc_stride,
-                    const float* __restrict__ bpf, int nt_bpf, float clip, float emax,
-                    float2* __restrict__ rstr, unsigned rs_mask, long long rs_stride)
+tx_ssb_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict__ audio, long long n, long long a_stride, Ring<float> ra,
+                    Ring<float2> rclip, const float* __restrict__ bpf, int nt_bpf, float clip, float emax, Ring<float2> rstr)
 {
     const int c = blockIdx.x;
     __shared__ TxAnalogState st;
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
-    float* A = ra + static_cast<long long>(c) * ra_stride;
-    float2* Cc = rclip + static_cast<long long>(c) * rc_stride;
-    float2* S = rstr + static_cast<long long>(c) * rs_stride;
+    float* __restrict__ A = ra.d + static_cast<long long>(c) * ra.stride;
+    float2* __restrict__ Cc = rclip.d + static_cast<long long>(c) * rclip.stride;
+    float2* __restrict__ S = rstr.d + static_cast<long long>(c) * rstr.stride;
     const long long a0 = st.n_in, a1n = st.n_in + n;
-    for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) A[a & ra_mask] = audio[static_cast<long long>(c) * a_stride + (a - a0)];
+    for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) A[a & ra.mask] = audio[static_cast<long long>(c) * a_stride + (a - a0)];
     __syncthreads();
     for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) {
         float acc = 0.0f;
-        for (int k = nt_bpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(bpf[k], m >= 0 ? A[m & ra_mask] : 0.0f, acc); }
+        for (int k = nt_bpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(bpf[k], m >= 0 ? A[m & ra.mask] : 0.0f, acc); }
         const float mag = sqrtf(acc * acc + 0.0f * 0.0f);
         const float ph = qrl_fast_atan2f(0.0f, acc);
         const float cl = mag < clip ? mag : clip;
         float sn, cs;
         qrl_sincosf(ph, sn, cs);
-        Cc[a & rc_mask] = make_float2(cs * cl, sn * cl);
+        Cc[a & rclip.mask] = make_float2(cs * cl, sn * cl);
     }
     __syncthreads();
     const long long s0 = st.n_str, s1 = a1n >= 2 ? a1n - 2 : 0;
     for (long long k = s0 + threadIdx.x; k < s1; k += blockDim.x) {
-        auto env = [&](long long j) -> float { if (j < 0) return 0.0f; const float2 v = Cc[j & rc_mask]; return sqrtf(v.x * v.x + v.y * v.y); };
+        auto env = [&](long long j) -> float { if (j < 0) return 0.0f; const float2 v = Cc[j & rclip.mask]; return sqrtf(v.x * v.x + v.y * v.y); };
         float h = env(k);
         h = fmaxf(h, env(k - 2)); h = fmaxf(h, env(k - 1)); h = fmaxf(h, env(k + 1)); h = fmaxf(h, env(k + 2));
         h = h * emax; h = fmaxf(h, 1.0f); h = h - 1.0f; h = h * 2.0f; h = h + 1.0f;
-        const float2 v = Cc[k & rc_mask];
-        S[k & rs_mask] = make_float2(v.x / h, v.y / h);
+        const float2 v = Cc[k & rclip.mask];
+        S[k & rstr.mask] = make_float2(v.x / h, v.y / h);
     }
     __syncthreads();
     if (threadIdx.x == 0) { st.n_in = a1n; st.n_str = s1 > s0 ? s1 : s0; states[c] = st; }
@@ -3931,15 +3929,14 @@ tx_ssb_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict_
 __global__ void __launch_bounds__(128)
 tx_am_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict__ audio, long long n, long long a_stride,
                    float attack, float decay, float ref, float max_gain,
-                   float* __restrict__ ra, unsigned ra_mask, long long ra_stride, const float* __restrict__ bpf, int nt_bpf, float dc,
-                   float2* __restrict__ rsym, unsigned rs_mask, long long rs_stride)
+                   Ring<float> ra, const float* __restrict__ bpf, int nt_bpf, float dc, Ring<float2> rsym)
 {
     const int c = blockIdx.x;
     __shared__ TxAnalogState st;
     if (threadIdx.x == 0) st = states[c];
     __syncthreads();
-    float* A = ra + static_cast<long long>(c) * ra_stride;
-    float2* S = rsym + static_cast<long long>(c) * rs_stride;
+    float* __restrict__ A = ra.d + static_cast<long long>(c) * ra.stride;
+    float2* __restrict__ S = rsym.d + static_cast<long long>(c) * rsym.stride;
     const long long a0 = st.n_in, a1n = st.n_in + n;
     if (threadIdx.x == 0) {
         float gain = st.agc;
@@ -3953,29 +3950,30 @@ tx_am_front_kernel(TxAnalogState* __restrict__ states, const float* __restrict__
             if (max_gain > 0.0f && gain > max_gain) gain = max_gain;
             float v = out < -0.98f ? -0.98f : (out > 0.98f ? 0.98f : out);
             v = v * 0.95f;
-            A[(a0 + i) & ra_mask] = v;
+            A[(a0 + i) & ra.mask] = v;
         }
         st.agc = gain;
     }
     __syncthreads();
     for (long long a = a0 + threadIdx.x; a < a1n; a += blockDim.x) {
         float acc = 0.0f;
-        for (int k = nt_bpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(bpf[k], m >= 0 ? A[m & ra_mask] : 0.0f, acc); }
-        S[a & rs_mask] = make_float2(acc + dc, 0.0f);
+        for (int k = nt_bpf - 1; k >= 0; k--) { const long long m = a - k; acc = fmaf(bpf[k], m >= 0 ? A[m & ra.mask] : 0.0f, acc); }
+        S[a & rsym.mask] = make_float2(acc + dc, 0.0f);
     }
     __syncthreads();
     if (threadIdx.x == 0) { st.n_in = a1n; states[c] = st; }
 }
 
 // in-place x g1 x g2 on a channel-major complex ring segment (multiply_const_cc twice)
-__global__ void scale2_ring_kernel(float2* __restrict__ ring, unsigned mask, long long stride, long long a0, long long a1, float g1, float g2)
+__global__ void scale2_ring_kernel(Ring<float2> ring, long long a0, long long a1, float g1, float g2)
 {
+    float2* __restrict__ rg = ring.d;
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
-    float2 v = ring[static_cast<long long>(c) * stride + (a & mask)];
+    float2 v = rg[static_cast<long long>(c) * ring.stride + (a & ring.mask)];
     v.x = v.x * g1; v.y = v.y * g1; v.x = v.x * g2; v.y = v.y * g2;
-    ring[static_cast<long long>(c) * stride + (a & mask)] = v;
+    rg[static_cast<long long>(c) * ring.stride + (a & ring.mask)] = v;
 }
 
 // ================================================================================================
@@ -4009,15 +4007,13 @@ struct DsssParams {
 constexpr int kDsssChunk = 1024;
 
 __global__ void __launch_bounds__(256)
-dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
-                  const float2* __restrict__ r1, unsigned r1_mask, long long r1_stride, long long k1,
+dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states, Ring<const float2> r1, long long k1,
                   const float* __restrict__ arms /* [13][nt_arm] */, const float* __restrict__ taps2, const float2* __restrict__ dtaps_rev,
-                  float2* __restrict__ ra, float2* __restrict__ rc, unsigned ring_mask, long long ring_stride,
-                  float2* __restrict__ rd, unsigned rd_mask, long long rd_stride,
-                  float2* __restrict__ port0, long long port0_stride, long long o_call0,
+                  Ring<float2> ra, Ring<float2> rc, Ring<float2> rd, float2* __restrict__ port0, long long port0_stride, long long o_call0,
                   float2* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap,
-                  unsigned char* __restrict__ soft_ring, unsigned soft_mask, long long soft_stride, long long* __restrict__ n_soft_out)
+                  Ring<unsigned char> soft_ring, long long* __restrict__ n_soft_out)
 {
+    unsigned char* __restrict__ sr = soft_ring.d;
     __shared__ DsssState st;
     __shared__ float s_arms[13 * 8], s_t2[64];
     __shared__ float2 s_dt[640];
@@ -4029,10 +4025,10 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
     for (int i = tid; i < p.nt2; i += 256) s_t2[i] = taps2[i];
     for (int i = tid; i < p.ntaps; i += 256) s_dt[i] = dtaps_rev[i];
     __syncthreads();
-    const float2* x1 = r1 + static_cast<long long>(c) * r1_stride;
-    float2* xa = ra + static_cast<long long>(c) * ring_stride;
-    float2* xc = rc + static_cast<long long>(c) * ring_stride;
-    float2* xd = rd + static_cast<long long>(c) * rd_stride;
+    const float2* __restrict__ x1 = r1.d + static_cast<long long>(c) * r1.stride;
+    float2* __restrict__ xa = ra.d + static_cast<long long>(c) * ra.stride;
+    float2* __restrict__ xc = rc.d + static_cast<long long>(c) * rc.stride;
+    float2* __restrict__ xd = rd.d + static_cast<long long>(c) * rd.stride;
     const long long o0 = st.o_n;
     const long long o1 = (k1 * 13 + 49) / 50;                    // outputs o whose newest input floor(50 o / 13) has arrived
     // ---- A: rational resampler 13 / 50 (arm (50 o) mod 13 at input floor(50 o / 13), oldest tap first)
@@ -4042,16 +4038,16 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
         float re = 0.0f, imv = 0.0f;
         for (int k = p.nt_arm - 1; k >= 0; k--) {
             const long long a = newest - k;
-            const float2 v = a >= 0 ? x1[a & r1_mask] : make_float2(0.0f, 0.0f);
+            const float2 v = a >= 0 ? x1[a & r1.mask] : make_float2(0.0f, 0.0f);
             re = fmaf(hh[k], v.x, re); imv = fmaf(hh[k], v.y, imv);
         }
-        xa[o & ring_mask] = make_float2(re, imv);
+        xa[o & ra.mask] = make_float2(re, imv);
     }
     __syncthreads();
     // ---- B: frequency / phase lock (per-item recurrence) over shared-memory chunks
     for (long long b0 = o0; b0 < o1; b0 += kDsssChunk) {
         const int n = static_cast<int>(o1 - b0 < kDsssChunk ? o1 - b0 : kDsssChunk);
-        for (int i = tid; i < n; i += 256) s_buf[i] = xa[(b0 + i) & ring_mask];
+        for (int i = tid; i < n; i += 256) s_buf[i] = xa[(b0 + i) & ra.mask];
         __syncthreads();
         if (tid == 0) {
             LoopState pll = st.pll;
@@ -4063,7 +4059,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
             st.pll = pll;
         }
         __syncthreads();
-        for (int i = tid; i < n; i += 256) xa[(b0 + i) & ring_mask] = s_buf[i];
+        for (int i = tid; i < n; i += 256) xa[(b0 + i) & ra.mask] = s_buf[i];
         __syncthreads();
     }
     // ---- C: low-pass -> port 0 and the AGC's input
@@ -4071,17 +4067,17 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
         float re = 0.0f, imv = 0.0f;
         for (int k = p.nt2 - 1; k >= 0; k--) {
             const long long a = o - k;
-            const float2 v = a >= 0 ? xa[a & ring_mask] : make_float2(0.0f, 0.0f);
+            const float2 v = a >= 0 ? xa[a & ra.mask] : make_float2(0.0f, 0.0f);
             re = fmaf(s_t2[k], v.x, re); imv = fmaf(s_t2[k], v.y, imv);
         }
-        xc[o & ring_mask] = make_float2(re, imv);
+        xc[o & rc.mask] = make_float2(re, imv);
         if (o - o_call0 < port0_stride) port0[static_cast<long long>(c) * port0_stride + (o - o_call0)] = make_float2(re, imv);
     }
     __syncthreads();
     // ---- D: agc2_cc::scale (signed rate compare, see agc_costas_kernel)
     for (long long b0 = o0; b0 < o1; b0 += kDsssChunk) {
         const int n = static_cast<int>(o1 - b0 < kDsssChunk ? o1 - b0 : kDsssChunk);
-        for (int i = tid; i < n; i += 256) s_buf[i] = xc[(b0 + i) & ring_mask];
+        for (int i = tid; i < n; i += 256) s_buf[i] = xc[(b0 + i) & rc.mask];
         __syncthreads();
         if (tid == 0) {
             float gain = st.agc;
@@ -4097,7 +4093,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
             st.agc = gain;
         }
         __syncthreads();
-        for (int i = tid; i < n; i += 256) xc[(b0 + i) & ring_mask] = s_buf[i];
+        for (int i = tid; i < n; i += 256) xc[(b0 + i) & rc.mask] = s_buf[i];
         __syncthreads();
     }
     // ---- E: despreader.  Symbol m needs items up to m N + (ntaps - N) - 1.
@@ -4108,7 +4104,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
         const long long w0 = m * p.N - 2LL * p.N + 1;
         for (int i = tid; i < wlen; i += 256) {
             const long long a = w0 + i;
-            s_buf[i] = a >= 0 ? xc[a & ring_mask] : make_float2(0.0f, 0.0f);
+            s_buf[i] = a >= 0 ? xc[a & rc.mask] : make_float2(0.0f, 0.0f);
         }
         __syncthreads();
         float best = 0.0f; int bj = 0x7fffffff; float2 bv = make_float2(0.0f, 0.0f);
@@ -4133,7 +4129,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
         }
         if (tid == 0) {
             const float sc = 2.0f / static_cast<float>(p.N);
-            xd[m & rd_mask] = s_mag[0] > 0.0f ? make_float2(s_val[0].x * sc, s_val[0].y * sc) : make_float2(0.0f * sc, 0.0f * sc);
+            xd[m & rd.mask] = s_mag[0] > 0.0f ? make_float2(s_val[0].x * sc, s_val[0].y * sc) : make_float2(0.0f * sc, 0.0f * sc);
         }
         __syncthreads();
     }
@@ -4149,7 +4145,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
             const float* tt = d_mmse_tab + imu * 8;
             float yr = 0.0f, yi = 0.0f;
             for (int i = 0; i < 8; i++) {
-                const float2 v = xd[(st.cr_ii + i) & rd_mask];
+                const float2 v = xd[(st.cr_ii + i) & rd.mask];
                 yr = fmaf(tt[7 - i], v.x, yr); yi = fmaf(tt[7 - i], v.y, yi);
             }
             st.p2r = st.p1r; st.p2i = st.p1i; st.p1r = st.p0r; st.p1i = st.p0i; st.p0r = yr; st.p0i = yi;
@@ -4170,7 +4166,7 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
             qrl_costas_step(st.costas, p.costas_alpha, p.costas_beta, 2, false, yr, yi, cr, ci);
             if (cnt < port1_cap) port1[static_cast<long long>(c) * port1_stride + cnt] = make_float2(cr, ci);
             cnt++;
-            soft_ring[static_cast<long long>(c) * soft_stride + (st.n_soft & soft_mask)] = qrl_soft_u8(cr, p.soft_scale);
+            sr[static_cast<long long>(c) * soft_ring.stride + (st.n_soft & soft_ring.mask)] = qrl_soft_u8(cr, p.soft_scale);
             st.n_soft++; st.n_sym++;
         }
         port1_cnt[c] = cnt < port1_cap ? cnt : port1_cap;
@@ -4185,23 +4181,24 @@ dsss_chain_kernel(DsssParams p, DsssState* __restrict__ states,
 // ================================================================================================
 // rows of a [n_rows][in_stride] slab (the channelizer's output) -> per-channel input ring (the resampler's history lives there)
 __global__ void mmdvm_gather_kernel(const float2* __restrict__ in, long long in_stride, const int* __restrict__ rows, long long n,
-                                    float2* __restrict__ ring, unsigned mask, long long stride, long long a0)
+                                    Ring<float2> ring, long long a0)
 {
+    float2* __restrict__ rg = ring.d;
     const int c = blockIdx.y;
     const float2* src = in + static_cast<long long>(rows[c]) * in_stride;
     for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x)
-        ring[static_cast<long long>(c) * stride + ((a0 + i) & mask)] = src[i];
+        rg[static_cast<long long>(c) * ring.stride + ((a0 + i) & ring.mask)] = src[i];
 }
 // quadrature_demod_cf(gain) -> x level (multiply_const_ff) -> float_to_short(1, 32767) = volk_32f_s32f_convert_16i: x scale, clip, rintf
-__global__ void mmdvm_demod_short_kernel(const float2* __restrict__ ring, unsigned mask, long long stride, long long o0, long long o1,
+__global__ void mmdvm_demod_short_kernel(Ring<const float2> ring, long long o0, long long o1,
                                          float gain, float level, short* __restrict__ out, long long out_stride)
 {
     const int c = blockIdx.y;
     const long long o = o0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (o >= o1) return;
-    const float2* x = ring + static_cast<long long>(c) * stride;
-    const float2 a = x[o & mask];
-    const float2 p = o > 0 ? x[(o - 1) & mask] : make_float2(0.0f, 0.0f);
+    const float2* __restrict__ x = ring.d + static_cast<long long>(c) * ring.stride;
+    const float2 a = x[o & ring.mask];
+    const float2 p = o > 0 ? x[(o - 1) & ring.mask] : make_float2(0.0f, 0.0f);
     const float re = a.x * p.x + a.y * p.y;                              // x[n] * conj(x[n-1])
     const float im = a.y * p.x - a.x * p.y;
     float v = gain * qrl_fast_atan2f(im, re);
@@ -4211,17 +4208,17 @@ __global__ void mmdvm_demod_short_kernel(const float2* __restrict__ ring, unsign
     out[static_cast<long long>(c) * out_stride + (o - o0)] = static_cast<short>(rintf(v));
 }
 // rssi_tag_block (rssi_tag_block.cpp:42-63): one value per 300 items, the block's own sequential float sum of (|x|^2)^2
-__global__ void mmdvm_rssi_kernel(const float2* __restrict__ ring, unsigned mask, long long stride, long long b0, int nblocks, float cal,
+__global__ void mmdvm_rssi_kernel(Ring<const float2> ring, long long b0, int nblocks, float cal,
                                   float* __restrict__ db, long long db_stride)
 {
     const int c = blockIdx.y;
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= nblocks) return;
-    const float2* x = ring + static_cast<long long>(c) * stride;
+    const float2* __restrict__ x = ring.d + static_cast<long long>(c) * ring.stride;
     const long long base = (b0 + j) * 300;
     float sum = 0.0f;
     for (int i = 0; i < 300; i++) {
-        const float2 v = x[(base + i) & mask];
+        const float2 v = x[(base + i) & ring.mask];
         const float pwr = v.x * v.x + v.y * v.y;
         sum = sum + pwr * pwr;
     }
@@ -4230,14 +4227,15 @@ __global__ void mmdvm_rssi_kernel(const float2* __restrict__ ring, unsigned mask
 }
 // short_to_float(1, 32767) = volk_16i_s32f_convert_32f (SIMD form: x (float)(1 / 32767)) -> x level -> the FM modulator's input ring
 __global__ void mmdvm_short_float_kernel(const short* __restrict__ in, long long in_stride, long long n, float level,
-                                         float* __restrict__ ring, unsigned mask, long long stride, long long a0)
+                                         Ring<float> ring, long long a0)
 {
+    float* __restrict__ rg = ring.d;
     const int c = blockIdx.y;
     const float inv = static_cast<float>(1.0 / 32767.0);
     for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         float v = static_cast<float>(in[static_cast<long long>(c) * in_stride + i]) * inv;
         v = v * level;
-        ring[static_cast<long long>(c) * stride + ((a0 + i) & mask)] = v;
+        rg[static_cast<long long>(c) * ring.stride + ((a0 + i) & ring.mask)] = v;
     }
 }
 // per-channel linear rows -> rows of the synthesizer's [n_rows][stride] input slab
@@ -4316,22 +4314,23 @@ __global__ void sc8_to_fc32_kernel(const char2* __restrict__ in, long long in_st
 // gr_zero_idle_bursts (gr_zero_idle_bursts.cpp:45-82) as two ring passes.  (1) the sync block's history: out[a] = in[a - delay_items]
 // (zero before the stream began); (2) the "zero_samples" counter: the host has turned the tags of this call into [begin, end) item
 // ranges per channel (qrl_tx_work), one CTA per range clears them.
-__global__ void tx_delay_ring_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride,
-                                     float2* __restrict__ out, unsigned out_mask, long long out_stride,
-                                     long long a0, long long a1, long long delay_items)
+__global__ void tx_delay_ring_kernel(Ring<const float2> in, Ring<float2> out, long long a0, long long a1, long long delay_items)
 {
+    float2* __restrict__ y_out = out.d;
+    const float2* __restrict__ x_in = in.d;
     const int c = blockIdx.y;
     const long long a = a0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (a >= a1) return;
     const long long s = a - delay_items;
     float2 v = make_float2(0.0f, 0.0f);
-    if (s >= 0) v = in[static_cast<long long>(c) * in_stride + (s & in_mask)];
-    out[static_cast<long long>(c) * out_stride + (a & out_mask)] = v;
+    if (s >= 0) v = x_in[static_cast<long long>(c) * in.stride + (s & in.mask)];
+    y_out[static_cast<long long>(c) * out.stride + (a & out.mask)] = v;
 }
-__global__ void tx_zero_ranges_kernel(float2* __restrict__ ring, unsigned mask, long long stride, const long long* __restrict__ ranges)
+__global__ void tx_zero_ranges_kernel(Ring<float2> ring, const long long* __restrict__ ranges)
 {
+    float2* __restrict__ rg = ring.d;
     const long long c = ranges[3 * blockIdx.x], a0 = ranges[3 * blockIdx.x + 1], a1 = ranges[3 * blockIdx.x + 2];
-    for (long long a = a0 + threadIdx.x; a < a1; a += blockDim.x) ring[c * stride + (a & mask)] = make_float2(0.0f, 0.0f);
+    for (long long a = a0 + threadIdx.x; a < a1; a += blockDim.x) rg[c * ring.stride + (a & ring.mask)] = make_float2(0.0f, 0.0f);
 }
 
 // ================================================================================================
@@ -4345,9 +4344,8 @@ struct FreedvRxParams { float attack, decay, ref, max_gain; int nt_audio; };
 // shared-memory chunks; the fabsf form of the AM chain) into a float ring, then over the CTA band_pass_2(1, 8000, 200, 3500, 200, 90) in direct form (oldest tap
 // first) -> x0.1 -> float_to_short(1, 32768) (x scale, clip, rintf) -> port 1 (int16 modem samples for freedv_rx_ss)
 __global__ void __launch_bounds__(128)
-freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
-                      const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long avail_in,
-                      float* __restrict__ agc_ring, unsigned agc_mask, long long agc_stride, const float* __restrict__ audio_taps,
+freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states, Ring<const float2> in, long long avail_in,
+                      Ring<float> agc_ring, const float* __restrict__ audio_taps,
                       short* __restrict__ port1, long long port1_stride, int* __restrict__ port1_cnt, int port1_cap)
 {
     extern __shared__ float fdv_taps[];
@@ -4359,8 +4357,8 @@ freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
     const long long a0 = st.n_in;
     const int cnt0 = port1_cnt[c];
     __syncthreads();      // every thread holds a0 before thread 0 advances st.n_in
-    const float2* x = in + static_cast<long long>(c) * in_stride;
-    float* g = agc_ring + static_cast<long long>(c) * agc_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
+    float* __restrict__ g = agc_ring.d + static_cast<long long>(c) * agc_ring.stride;
     // the recurrence walks shared-memory chunks: the CTA stages the real parts, thread 0 runs the gain over them in place, the CTA
     // stores the AGC output (one global round trip per chunk instead of one per sample on the dependent chain)
     constexpr int CHUNK = 1024;
@@ -4368,7 +4366,7 @@ freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
     float gain = st.gain;
     for (long long b0 = a0; b0 < avail_in; b0 += CHUNK) {
         const int nb = static_cast<int>(avail_in - b0 < CHUNK ? avail_in - b0 : CHUNK);
-        for (int j = threadIdx.x; j < nb; j += blockDim.x) buf[j] = x[(b0 + j) & in_mask].x;
+        for (int j = threadIdx.x; j < nb; j += blockDim.x) buf[j] = x[(b0 + j) & in.mask].x;
         __syncthreads();
         if (threadIdx.x == 0) {
             for (int j = 0; j < nb; j++) {
@@ -4382,7 +4380,7 @@ freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
             }
         }
         __syncthreads();
-        for (int j = threadIdx.x; j < nb; j += blockDim.x) g[(b0 + j) & agc_mask] = buf[j];
+        for (int j = threadIdx.x; j < nb; j += blockDim.x) g[(b0 + j) & agc_ring.mask] = buf[j];
         __syncthreads();
     }
     if (threadIdx.x == 0) { st.gain = gain; st.n_in = avail_in; }
@@ -4392,7 +4390,7 @@ freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
         float acc = 0.0f;
         for (int k = p.nt_audio - 1; k >= 0; k--) {
             const long long n = a - k;
-            acc = fmaf(fdv_taps[k], n >= 0 ? g[n & agc_mask] : 0.0f, acc);
+            acc = fmaf(fdv_taps[k], n >= 0 ? g[n & agc_ring.mask] : 0.0f, acc);
         }
         float v = acc * 0.1f;
         v = v * 32768.0f;
@@ -4409,12 +4407,13 @@ freedv_rx_tail_kernel(FreedvRxParams p, FreedvRxState* __restrict__ states,
 
 // TX front: int16 modem samples -> short_to_float(1, scale) (x (float)(1 / scale)) -> float_to_complex -> complex ring at absolute a0..
 __global__ void short_to_complex_ring_kernel(const short* __restrict__ in, long long in_stride, long long n, float inv,
-                                             float2* __restrict__ ring, unsigned mask, long long stride, long long a0)
+                                             Ring<float2> ring, long long a0)
 {
+    float2* __restrict__ rg = ring.d;
     const int c = blockIdx.y;
     for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         const float v = static_cast<float>(in[static_cast<long long>(c) * in_stride + i]) * inv;
-        ring[static_cast<long long>(c) * stride + ((a0 + i) & mask)] = make_float2(v, 0.0f);
+        rg[static_cast<long long>(c) * ring.stride + ((a0 + i) & ring.mask)] = make_float2(v, 0.0f);
     }
 }
 
@@ -4425,8 +4424,7 @@ __global__ void short_to_complex_ring_kernel(const short* __restrict__ in, long 
 // Each thread scans CH consecutive items, then combines the chunk totals of its block.  Max is exact, so the order does not matter.
 template <int N, int TILE, int NT>
 __global__ void __launch_bounds__(NT)
-ffagc_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_stride, long long m0, long long m1, float ref,
-             float2* __restrict__ out, unsigned out_mask, long long out_stride)
+ffagc_kernel(Ring<const float2> in, long long m0, long long m1, float ref, Ring<float2> out)
 {
     constexpr int SPAN = TILE + N;                  // local item i = absolute input tile0 - (N - 1) + i; the last item is padding
     constexpr int CH = SPAN / NT;                   // items per thread
@@ -4436,11 +4434,11 @@ ffagc_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_strid
     const int c = blockIdx.y;
     const long long tile0 = m0 + static_cast<long long>(blockIdx.x) * TILE;
     const long long s0 = tile0 - (N - 1);
-    const float2* x = in + static_cast<long long>(c) * in_stride;
+    const float2* __restrict__ x = in.d + static_cast<long long>(c) * in.stride;
     for (int i = threadIdx.x; i < SPAN; i += NT) {
         const long long a = s0 + i;
         float e = 0.0f;                             // envelopes are >= 0: 0 is neutral (history and the items past m1)
-        if (a >= 0 && a < m1) { const float2 v = x[a & in_mask]; e = fmaxf(fabsf(v.x), fabsf(v.y)); }
+        if (a >= 0 && a < m1) { const float2 v = x[a & in.mask]; e = fmaxf(fabsf(v.x), fabsf(v.y)); }
         pre[i] = e;
     }
     __syncthreads();
@@ -4461,15 +4459,15 @@ ffagc_kernel(const float2* __restrict__ in, unsigned in_mask, long long in_strid
 #pragma unroll
     for (int j = 0; j < CH; j++) { pre[b + j] = fmaxf(pl[j], before); suf[b + j] = fmaxf(sl[j], after); }
     __syncthreads();
-    float2* o = out + static_cast<long long>(c) * out_stride;
+    float2* __restrict__ o = out.d + static_cast<long long>(c) * out.stride;
     for (int i = threadIdx.x; i < TILE; i += NT) {
         const long long m = tile0 + i;
         if (m >= m1) break;
         const float mx = fmaxf(fmaxf(suf[i], pre[i + N - 1]), 1e-4f);
         const float gain = ref / mx;
         const long long a = m - (N - 1);
-        const float2 v = a >= 0 ? x[a & in_mask] : make_float2(0.0f, 0.0f);
-        o[m & out_mask] = make_float2(v.x * gain, v.y * gain);
+        const float2 v = a >= 0 ? x[a & in.mask] : make_float2(0.0f, 0.0f);
+        o[m & out.mask] = make_float2(v.x * gain, v.y * gain);
     }
 }
 

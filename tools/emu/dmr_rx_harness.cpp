@@ -53,6 +53,8 @@ int main(int argc, char** argv)
     const unsigned r2_cap = pow2_at_least(n1max + ntaps3 + 64), r4_cap = pow2_at_least(2 * n1max + 600);
     std::vector<float2> r2((size_t)r2_cap * C, float2{ 0, 0 });
     std::vector<float> r4((size_t)r4_cap * groups * 32, 0.0f);
+    const Ring<float2> r2_ring{ r2.data(), r2_cap - 1, r2_cap };
+    const Ring<float> r4_ring{ r4.data(), r4_cap - 1, r4_cap };
     std::vector<float> scratch((size_t)groups * ss_chunk_cap * (maxs + 2) * 32, 0.0f);
     std::vector<int> hdr((size_t)groups * 128, 0);
     const long port0_cap = n1max, port1_cap = n1max / std::max(1, sym_sps - 1) + 64, port2_cap = 2 * port1_cap + 160;
@@ -60,6 +62,7 @@ int main(int argc, char** argv)
     std::vector<unsigned char> port2((size_t)port2_cap * C), soft(64);
     std::vector<float> port3((size_t)port0_cap * C);
     std::vector<int> port1_cnt(C), port2_cnt(C);
+    const Ring<unsigned char> soft_ring{ soft.data(), 63, 64 };
     std::vector<long long> nsoft(C);
     std::vector<SymSyncState> ss(C);
     for (auto& s : ss) { memset(&s, 0, sizeof s); s.avg_period = ssp.sps; s.inst_period = ssp.sps; s.mu = 0.0f; }
@@ -76,16 +79,16 @@ int main(int argc, char** argv)
             const int TB = 256;
             dim3 gtile((unsigned)((n_new + TB - 1) / TB), C);
             emu::launch(gtile, dim3(TB), sizeof(float) * (2 * ntaps3 + TB), [&] {
-                qdemod_fir_fff_kernel(r2.data(), r2_cap - 1, r2_cap, r4.data(), r4_cap - 1, r4_cap, taps3.data(), ntaps3, qd_gain, k0, k1, nullptr, 0); });
+                qdemod_fir_fff_kernel(r2_ring, r4_ring, taps3.data(), ntaps3, qd_gain, k0, k1); });
             emu::launch(dim3((unsigned)((n_new + 31) / 32), groups), dim3(32, 8), 0, [&] {
-                ring_to_port_f32_kernel(r4.data(), r4_cap - 1, r4_cap, C, k0, k1, port3.data(), port0_cap, 0); });
+                ring_to_port_f32_kernel(r4_ring, C, k0, k1, port3.data(), port0_cap, 0); });
         }
         const size_t smem = sizeof(float) * (NST * CH * 32 + SYMSYNC_TAB_FLOATS + 2 * (maxs + 2) * 32) + sizeof(int) * 64;
         const int chunk_bound = (int)std::min<long long>(ss_chunk_cap, n_new / symsync_stride(CH, ssp.lookahead) + 3);
         emu::launch(dim3(groups), dim3(96), smem, [&] {
             symsync_kernel<1, SL_RECT4, EPI_EXT_4FSK_FM, CH, NST, 1, LOOP_SYMSYNC, 3>(
-                ssp, ss.data(), C, r4.data(), r4_cap - 1, r4_cap, k1, port1.data(), port1_cap, port1_cnt.data(), (int)port1_cap,
-                soft.data(), 63, 64, maxs, nsoft.data(), scratch.data(), chunk_bound, (int)ss_chunk_cap, hdr.data()); });
+                ssp, ss.data(), C, r4_ring, k1, port1.data(), port1_cap, port1_cnt.data(), (int)port1_cap,
+                soft_ring, maxs, nsoft.data(), scratch.data(), chunk_bound, (int)ss_chunk_cap, hdr.data()); });
         if (chunk_bound > 0)
             emu::launch(dim3(chunk_bound, groups), dim3(32, 8), 0, [&] {
                 symsync_ext_epilogue_kernel<1>(ssp, C, scratch.data(), (int)ss_chunk_cap, maxs, hdr.data(), port1.data(), port1_cap, (int)port1_cap,

@@ -49,6 +49,8 @@ int main(int argc, char** argv)
     const unsigned sym_cap = pow2_at_least(max_sym + 64), if_cap = pow2_at_least(max_sym * L1 + 128), rc_cap = pow2_at_least(max_sym * L1 + 512 + nt2);
     std::vector<float> sym((size_t)sym_cap * C, 0.0f);
     std::vector<float2> ifr((size_t)if_cap * C, float2{ 0, 0 }), rc((size_t)rc_cap * C, float2{ 0, 0 });
+    const Ring<float> sym_ring{ sym.data(), sym_cap - 1, sym_cap };
+    const Ring<float2> if_ring{ ifr.data(), if_cap - 1, if_cap }, rc_ring{ rc.data(), rc_cap - 1, rc_cap };
     const long long out_stride = (4LL * max_items * L1 * L2 + M2 - 1) / M2 + 8;
     std::vector<float2> out((size_t)out_stride * C), all((size_t)out_stride * C);
     std::vector<TxBitState> st(C, TxBitState{ 0x7F, 0, 0, 0 });
@@ -61,20 +63,20 @@ int main(int argc, char** argv)
         const unsigned char* b = data.data() + edges[e];
         const long long sym0 = n_sym, nsym = 4LL * n;
         emu::launch(dim3((C + 31) / 32), dim3(32), 0, [&] {
-            tx_bits_kernel<TXM_M17>(st.data(), C, b, n, max_items, sym.data(), sym_cap - 1, sym_cap, sym0); });
+            tx_bits_kernel<TXM_M17>(st.data(), C, b, n, max_items, sym_ring, sym0); });
         emu::launch(dim3(C), dim3(1024), 0, [&] {
-            tx_shape_fm_kernel<1024, 2>(st.data(), sym.data(), sym_cap - 1, sym_cap, sym0, nsym, L1, nt1, arms1.data(), 0, pulse_scale, fm_sens,
-                                        1.0f, 1.0f, ifr.data(), if_cap - 1, if_cap); });
+            tx_shape_fm_kernel<1024, 2>(st.data(), sym_ring, sym0, nsym, L1, nt1, arms1.data(), 0, pulse_scale, fm_sens,
+                                        1.0f, 1.0f, if_ring); });
         const long long m0 = sym0 * L1, m1 = (sym0 + nsym) * L1;
         const int TB = 256;
         dim3 g((unsigned)((m1 - m0 + TB - 1) / TB), C);
         emu::launch(g, dim3(TB), sizeof(float) * nt_cfilt, [&] {
-            fir_ccf_ring_kernel(ifr.data(), if_cap - 1, if_cap, rc.data(), rc_cap - 1, rc_cap, cfilt.data(), nt_cfilt, m0, m1, nullptr, 0, 0, 0); });
-        emu::launch(g, dim3(TB), 0, [&] { scale2_ring_kernel(rc.data(), rc_cap - 1, rc_cap, m0, m1, amplif, bb_gain); });
+            fir_ccf_ring_kernel(if_ring, rc_ring, cfilt.data(), nt_cfilt, m0, m1, nullptr, 0, 0, 0); });
+        emu::launch(g, dim3(TB), 0, [&] { scale2_ring_kernel(rc_ring, m0, m1, amplif, bb_gain); });
         const long long o0 = (m0 * L2 + M2 - 1) / M2, o1 = (m1 * L2 + M2 - 1) / M2;
         if (o1 - o0 > out_stride) return 4;
         emu::launch(dim3((unsigned)((o1 - o0 + 255) / 256), C), dim3(256), sizeof(float) * L2 * nt2, [&] {
-            resamp_ring_ccf_generic_kernel(rc.data(), rc_cap - 1, rc_cap, arms2.data(), L2, M2, nt2, o0, o1, out.data(), out_stride); });
+            resamp_ring_ccf_generic_kernel(rc_ring, arms2.data(), L2, M2, nt2, o0, o1, out.data(), out_stride); });
         for (int c = 0; c < C; c++)
             for (long long i = 0; i < o1 - o0; i++) all[(size_t)c * out_stride + total_out + i] = out[(size_t)c * out_stride + i];
         total_out += o1 - o0;

@@ -25,7 +25,7 @@ int main()
         std::vector<float> port((size_t)C * port_stride, -1.0f);
         if (a1 > a0)
             emu::launch(dim3((unsigned)((a1 - a0 + 31) / 32), groups), dim3(32, 8), 0, [&] {
-                qrl::ring_to_port_f32_kernel(ring.data(), cap - 1, cap, C, a0, a1, port.data(), port_stride, off); });
+                qrl::ring_to_port_f32_kernel(qrl::Ring<const float>{ ring.data(), cap - 1, cap }, C, a0, a1, port.data(), port_stride, off); });
         for (int c = 0; c < C; c++)
             for (long long i = 0; i < port_stride; i++) {
                 const long long a = a0 + (i - off);
